@@ -31,6 +31,9 @@ extern "C" {
 #define TQ_ERR_UNSUPPORTED (-4)
 #define TQ_ERR_OOM (-5)
 #define TQ_ERR_CORRUPT (-6)
+/* A TQ_OP_BOOL query (tile engine only) has a 1024-doc tile of a segment whose postings, summed over its clauses, exceed the
+ * largest tile buffer (12288 pairs), so even a repeat of the query alone cannot hold it.  Split the query or the segment. */
+#define TQ_ERR_TILE_CAPACITY (-7)
 
 /* schema::IndexRecordOption (src/schema/index_record_option.rs): decides the skip record
  * size 5 / 8 / 12 bytes (src/postings/skip.rs:205-253). */
@@ -168,7 +171,7 @@ typedef struct {
   uint64_t tile_postings;       /* postings decoded and scored by k_score_lists (every distinct list once) */
   uint64_t tile_list_bytes;     /* bytes of those lists' postings ranges (skip data + packed blocks + VInt tails) */
   uint64_t tile_scratch_bytes;  /* HBM scratch of the pair arrays, tile indexes and samples */
-  uint64_t tile_fallbacks;      /* 1 if the run overflowed a tile engine buffer and was repeated on the per-query kernels */
+  uint64_t tile_fallbacks;      /* 1 if the run overflowed a tile engine buffer and was repeated (TQ_OP_BOOL on the tile engine, the rest on the per-query kernels) */
   uint64_t tile_counters[8];    /* cumulative, with TQ_TILE_COUNTERS=1: (query, tile) pairs seen / skipped / light / heavy,
                                    essential postings applied, docs completed, docs at or above the threshold;
                                    [7] (always): dynamic shared memory bytes of a k_tile CTA of the last prepared group */
@@ -275,7 +278,7 @@ int tq_batch_results_pack_dev(tq_batch*, uint32_t* packed_dev);
 /* tq_batch_results_pack_dev without the wait: the copies are enqueued behind the run on the batch's stream, so that pack, all-gather,
  * merge and the NEXT batch's run can all be queued before the host waits for this batch (two batches in flight per GPU).
  * packed_dev holds 3 * nq * k_max + nq + 4 words; the last four are the run's overflow flags -- non-zero on any shard: take
- * tq_batch_results_pack_dev instead (it repeats an overflowed run on the per-query kernels). */
+ * tq_batch_results_pack_dev instead (it repeats an overflowed run: TQ_OP_BOOL queries on the tile engine with capacities that hold them, the rest on the per-query kernels). */
 int tq_batch_results_pack_dev_async(tq_batch*, uint32_t* packed_dev);
 int tq_merge_topk_packed_dev(tq_ctx*, void* cuda_stream, uint32_t n_lists, uint32_t nq, uint32_t stride, uint32_t k,
                              const uint32_t* packed_dev, size_t pitch_words, uint32_t* out_packed_dev);

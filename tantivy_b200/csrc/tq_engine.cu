@@ -157,7 +157,7 @@ struct tq_ctx {
 
 constexpr int kTileRounds = 4;  // launches of k_tile per run: the sample launch + three exact ones
 
-// Deep copy of a batch's queries (only kept when the tile engine runs them: an overflowing run is repeated on the per-query kernels).
+// Deep copy of a batch's queries (only kept when the tile engine runs them: an overflowing run is repeated, see finalize_run).
 struct OwnedQueries {
   std::vector<tq_query> q;
   std::vector<tq_term_seg> ts;
@@ -188,7 +188,8 @@ struct tq_batch {
   DevBuf tile_dev;  // pair arrays, tile indexes, samples, flags of the tile engine
   uint32_t* flags_pin = nullptr;  // [0] tile buffer overflow, [1] candidate region overflow (read back after the last phase)
   size_t tile_zero_off = 0, tile_zero_bytes = 0, tile_flags_off = 0;
-  bool finalized = false, is_fallback = false, last_round_sampled = false;
+  bool finalized = false, last_round_sampled = false;
+  int repeat = 0;  // 0: a caller's batch; 1, 2: the repeat of an overflowed run (batch_prepare_impl)
   PinBuf pin;      // staged descriptors (H2D source)
   DevBuf dev;      // descriptors on device
   DevBuf scratch;  // qstate + candidates + results
@@ -910,7 +911,7 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, const SegPlan* pl
 
 }  // namespace
 
-static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, bool force_legacy, tq_batch** out);
+static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int repeat, tq_batch** out);
 
 extern "C" {
 
@@ -925,12 +926,15 @@ void tq_batch_destroy(tq_batch* b) {
 }
 
 int tq_batch_prepare(tq_ctx* c, const tq_query* queries, size_t nq, tq_batch** out) {
-  return batch_prepare_impl(c, queries, nq, false, out);
+  return batch_prepare_impl(c, queries, nq, 0, out);
 }
 
 }  // extern "C"
 
-static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, bool force_legacy, tq_batch** out) {
+// repeat (finalize_run): 0 = a caller's batch.  1 = the repeat of an overflowed run: TERM / AND / OR / phrase queries take the
+// per-query kernels; TQ_OP_BOOL queries stay on the tile engine with candidate regions as large as their postings and the largest
+// tile buffer.  2 = as 1, but every TQ_OP_BOOL query in a tile group of its own.
+static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int repeat, tq_batch** out) {
   if (!c || !out || (!queries && nq)) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
   TQ_CUDA(cudaSetDevice(c->device));
   tq_batch* b = acquire_batch(c);
@@ -944,7 +948,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
   b->n_spans = 0;
   b->groups.clear();
   b->owned = OwnedQueries{};
-  b->is_fallback = force_legacy;
+  b->repeat = repeat;
 
   std::vector<QList> qlists;
   std::vector<QSeg> qsegs;
@@ -965,7 +969,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
   uint32_t strip_cached_max = 0, or_max_lists = 0, phrase_ct = 2;
   std::vector<TileGroupBuild> tgroups;
   std::vector<size_t> q_cands(nq, 0);
-  const bool tile_on = c->tile != 0 && !force_legacy;
+  const bool tile_on = c->tile != 0 && repeat == 0;
   const uint64_t tile_pair_budget = (uint64_t)c->tile_scratch_mb * (1u << 20) / 8u;
   uint64_t tile_pairs_total = 0;
   // Single-term queries ride along on the tile engine when the batch has multi-term queries whose decoded lists they share
@@ -987,7 +991,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
       if (q.k == 0 || q.k > TQ_MAX_K) return fail(TQ_ERR_INVALID_ARGUMENT, "k must be in 1..TQ_MAX_K");
       if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
       const bool is_bool = q.op == TQ_OP_BOOL;
-      if (is_bool && (!tile_on || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
+      if (is_bool && (c->tile == 0 || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
       if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_PHRASE && !is_bool) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
       if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
       if (!q.weight || (!q.avg_fieldnorm && !q.tf_cache) || (!q.term_segs && q.n_term_segs)) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
@@ -1106,8 +1110,9 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
       }
       // ---- route: the shared-decode tile engine, or the per-query kernels -------------------------------------------------
       bool on_tile = false;
-      if (tile_on && (((c->tile_ops >> op) & 1u) || op == TQ_OP_BOOL) && (op != TQ_OP_TERM || terms_on_tile) && n_plans) {
-        if (tgroups.empty()) tgroups.emplace_back();
+      const bool to_tile = repeat ? op == TQ_OP_BOOL : tile_on && (((c->tile_ops >> op) & 1u) || op == TQ_OP_BOOL) && (op != TQ_OP_TERM || terms_on_tile);
+      if (to_tile && n_plans) {
+        if (tgroups.empty() || (repeat == 2 && !tgroups.back().segs.empty())) tgroups.emplace_back();
         // wide unions: every query brings its clause words, work-list entries and (mostly distinct) lists into the CTA's shared
         // memory; smaller groups keep two CTAs per SM (configs[4]: 1.64 s -> 1.05 s per 512 20-term queries on 500M docs)
         const uint32_t max_q = q.n_terms > 8 ? std::min(c->tile_max_queries, c->tile_wide_queries) : c->tile_max_queries;
@@ -1121,9 +1126,12 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
           tile_pairs_total += tile_admit(tgroups.back(), (uint32_t)qi, op, plans.data(), n_plans);
           on_tile = true;
           // every doc at or above the running threshold is handed over: the sample launch and the k_theta passes keep that
-          // near k; a query that still overflows sends the batch to the per-query kernels (flags[1])
+          // near k; a query that still overflows has the run repeated (flags[1], finalize_run).  A query hands each doc over at
+          // most once (every tile once per run, a doc once per (query, tile): by its first posting in the driving clauses), so
+          // its postings bound its candidates: the region of a repeat cannot overflow.
           const uint32_t cand_floor = c->tile_cand_floor;  // (test hook: tiny regions overflow)
-          q_cands[qi] += (size_t)std::min<uint64_t>(q_postings, std::max<uint64_t>((cand_floor >= 8192 ? 128ull : 1ull) * q.k, cand_floor));
+          q_cands[qi] += repeat ? (size_t)q_postings
+                                : (size_t)std::min<uint64_t>(q_postings, std::max<uint64_t>((cand_floor >= 8192 ? 128ull : 1ull) * q.k, cand_floor));
         }
       }
       if (on_tile) continue;
@@ -1309,6 +1317,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
     gs.p_cap = (uint32_t)std::min<double>(kTileMaxPairs, std::max(1024.0, dens_max * kTile * 1.25 + 192.0));
     gs.p_cap = (gs.p_cap + 63u) & ~63u;
     if (c->tile_pcap_hook) gs.p_cap = c->tile_pcap_hook;  // (test hook: overflowing tiles)
+    if (repeat) gs.p_cap = kTileMaxPairs;  // the repeat of an overflowed run: the largest tile buffer there is
     // Launches: [0] samples scores on a spread of short tile runs, [1..3] are exact and cover every tile once.
     const uint32_t target = std::max(1u, c->tile_units);
     const uint32_t sample_div = std::max<uint32_t>(2u, c->tile_sample_div);
@@ -1482,7 +1491,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, boo
     b->groups.push_back(run);
   }
   (void)tix_cursor;
-  if (!b->groups.empty()) {  // the queries are kept: an overflowing run is repeated on the per-query kernels
+  if (!b->groups.empty()) {  // the queries are kept: an overflowing run is repeated (finalize_run)
     OwnedQueries& o = b->owned;
     o.q.assign(queries, queries + nq);
     size_t n_ts = 0, n_t = 0;
@@ -1725,29 +1734,42 @@ static int run_phase(tq_batch* b, int phase) {
   return TQ_OK;
 }
 
-// After the last phase: wait for the stream; a run whose tile engine overflowed (a tile with more pairs than its buffer, or a
-// query with more candidates than its region) is repeated on the per-query kernels and its rows replace ours.  Exactness
-// never depends on the fast path's capacity guesses.
+// After the last phase: wait for the stream.  A run whose tile engine overflowed (a tile with more pairs than its buffer, or a
+// query with more candidates than its region) is repeated and the repeat's rows replace ours, query by query.  In the repeat
+// TERM / AND / OR / phrase queries take the per-query kernels, which have no such capacities; TQ_OP_BOOL queries, which have no
+// per-query kernel, run on the tile engine again with regions that cannot overflow and the largest tile buffer (level 1).  If
+// that buffer overflows too, they run once more in tile groups of one query each (level 2); a tile whose postings do not fit
+// the buffer even for one query fails with TQ_ERR_TILE_CAPACITY.  Exactness never depends on the fast path's capacity guesses.
 static int finalize_run(tq_batch* b) {
   if (!b->ran) return fail(TQ_ERR_INVALID_ARGUMENT, "batch has not run");
   if (b->finalized) return TQ_OK;
   TQ_CUDA(cudaStreamSynchronize(b->stream));
   b->finalized = true;
-  if (b->groups.empty() || b->is_fallback) return TQ_OK;
-  if (b->flags_pin[0] == 0 && b->flags_pin[1] == 0) return TQ_OK;
+  if (b->groups.empty()) return TQ_OK;
+  const bool pairs_over = b->flags_pin[0] != 0, cands_over = b->flags_pin[1] != 0;
+  if (!pairs_over && !cands_over) return TQ_OK;
+  if (b->repeat == 2 && pairs_over)
+    return fail(TQ_ERR_TILE_CAPACITY, "a TQ_OP_BOOL query has a 1024-doc tile whose postings exceed the tile buffer (12288 pairs) "
+                                      "even in a tile group of its own: split the query or the segment");
+  if (b->repeat && cands_over) return fail(TQ_ERR_CUDA, "a repeated TQ_OP_BOOL query overflowed a candidate region sized by its postings");
+  int level = pairs_over ? 2 : 1;
   tq_batch* fb = nullptr;
-  int rc = batch_prepare_impl(b->ctx, b->owned.q.data(), b->owned.q.size(), true, &fb);
-  if (rc != TQ_OK) return rc;
-  rc = tq_batch_run(fb);
-  if (rc == TQ_OK) {
-    cudaError_t e = cudaStreamSynchronize(fb->stream);
-    if (e == cudaSuccess && fb->res_bytes == b->res_bytes)
-      e = cudaMemcpyAsync(b->scratch.p + b->res_off, fb->scratch.p + fb->res_off, b->res_bytes, cudaMemcpyDeviceToDevice, b->stream);
+  int rc = batch_prepare_impl(b->ctx, b->owned.q.data(), b->owned.q.size(), std::max(level, b->repeat + 1), &fb);
+  if (rc == TQ_OK) rc = tq_batch_run(fb);
+  if (rc == TQ_OK) rc = finalize_run(fb);  // (a level-1 repeat whose buffer overflowed repeats itself at level 2)
+  if (rc == TQ_OK && fb->nq != b->nq) rc = fail(TQ_ERR_CUDA, "repeat batch holds other queries");
+  if (rc == TQ_OK && b->nq) {
+    const size_t width = (size_t)std::min(b->kmax, fb->kmax) * 4, dp = (size_t)b->kmax * 4, sp = (size_t)fb->kmax * 4;
+    const BatchParams& D = b->params;
+    const BatchParams& S = fb->params;
+    cudaError_t e = cudaMemcpy2DAsync(D.res_scores, dp, S.res_scores, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(D.res_segs, dp, S.res_segs, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(D.res_docs, dp, S.res_docs, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(D.res_counts, S.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
     if (e != cudaSuccess) rc = fail(TQ_ERR_CUDA, cudaGetErrorString(e));
-    else if (fb->res_bytes != b->res_bytes) rc = fail(TQ_ERR_CUDA, "fallback batch layout differs");
   }
-  tq_batch_destroy(fb);
+  if (fb) tq_batch_destroy(fb);
   b->stats.tile_fallbacks = 1;
   return rc;
 }
@@ -1949,7 +1971,7 @@ int tq_batch_results_pack_dev(tq_batch* b, uint32_t* packed_dev) {
 // sharded caller can queue pack -> all-gather -> merge -> the next batch's run and only then wait for this one (two batches in
 // flight).  packed_dev holds 3 * nq * k_max + nq + 4 words; the last four are the run's overflow flags -- all zero: the rows are
 // final; anything else: the tile engine overflowed a buffer and the caller must take tq_batch_results_pack_dev (which repeats the
-// run on the per-query kernels) instead.  The flags travel with the rows, so every shard sees every shard's.
+// run, see finalize_run) instead.  The flags travel with the rows, so every shard sees every shard's.
 int tq_batch_results_pack_dev_async(tq_batch* b, uint32_t* packed_dev) {
   if (!b || !b->ran) return fail(TQ_ERR_INVALID_ARGUMENT, "batch has not run");
   if (!packed_dev) return fail(TQ_ERR_INVALID_ARGUMENT, "null output");
@@ -1960,7 +1982,7 @@ int tq_batch_results_pack_dev_async(tq_batch* b, uint32_t* packed_dev) {
   TQ_CUDA(cudaMemcpyAsync(packed_dev + 2 * rows, b->params.res_docs, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
   TQ_CUDA(cudaMemcpyAsync(packed_dev + 3 * rows, b->params.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream));
   uint32_t* flags = packed_dev + 3 * rows + b->nq;
-  if (!b->groups.empty() && !b->is_fallback && !b->finalized)
+  if (!b->groups.empty() && !b->finalized)
     TQ_CUDA(cudaMemcpyAsync(flags, b->tile_dev.p + b->tile_flags_off, 16, cudaMemcpyDeviceToDevice, b->stream));
   else
     TQ_CUDA(cudaMemsetAsync(flags, 0, 16, b->stream));  // (per-query kernels cannot overflow; a finalized run has been repaired already)

@@ -273,7 +273,7 @@ class CrossGpuMerger:
     def complete(self, batch, rows_to_host=True):
         """Waits for a batch queued with run() + finish_async().  Returns the merged rows as numpy (see fetch_host) when
         rows_to_host, else None.  If ANY rank's tile engine overflowed a buffer, every rank repeats the hand-over on the
-        waiting path (tq_batch_results_pack_dev repeats an overflowed run on the per-query kernels): same collectives on all ranks."""
+        waiting path (tq_batch_results_pack_dev repeats an overflowed run): same collectives on all ranks."""
         batch.results_dev()  # waits for the batch's stream; an overflowed run of THIS rank is repaired here
         ext, _ = self._stream(batch)
         with self.torch.cuda.stream(ext):

@@ -7,7 +7,8 @@ import os
 import numpy as np
 
 from oracle import tq_oracle as O
-from tantivy_b200._abi import TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_TERM, TQ_RECORD_FREQS, QueryBatch
+from tantivy_b200._abi import (TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT, TQ_OCCUR_SHOULD, TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_TERM,
+                               TQ_RECORD_FREQS, TQ_TERM_IGNORE_FREQ, QueryBatch)
 
 GOLDEN = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "reference_fixtures.json")))
 
@@ -67,12 +68,12 @@ def searcher_stats(segments):
 
 
 def make_query(op, segments, terms, k, boost=1.0):
-    """terms = list of term ordinals (same ordinal in every segment)."""
+    """terms = list of term ordinals (same ordinal in every segment); boost = one value, or one per clause."""
     n_docs, avg = searcher_stats(segments)
     weights, term_segs = [], []
     for clause, t in enumerate(terms):
         df = sum(s.terms[t][0] for s in segments)
-        weights.append(O.bm25_weight(df, n_docs, boost))
+        weights.append(O.bm25_weight(df, n_docs, boost[clause] if isinstance(boost, (list, tuple)) else boost))
         for s in segments:
             if s.terms[t][0] > 0:
                 term_segs.append(s.term_seg(t, clause))
@@ -106,6 +107,125 @@ def bool_query(q, occurs, groups=None, msm=0):
         q["term_group"] = groups
     q["min_should_match"] = msm
     return q
+
+
+BOOL_BOOSTS = (1.0, 0.0, -1.5, 1e4)
+BOOL_KS = (1, 10, 128, 129, 1000)
+
+
+def random_bool_shapes(rng, n, n_terms, n_wide=3):
+    """n seeded random TQ_OP_BOOL shapes over the term ordinals 0..n_terms-1, each a dict of terms, occurs, groups, msm, flags,
+    boosts and k.  1-12 clauses (the first n_wide shapes: 32); MUST clauses in groups of 1-4 (group ids in random order over the
+    clauses); minimum_should_match 0..n_should+1; TQ_TERM_IGNORE_FREQ on about a fifth of the clauses; per clause a boost of
+    BOOL_BOOSTS; k of BOOL_KS.  Every eighth shape is a conjunction of single-clause MUST groups.  Shape i repeats a term by i % 4: not at all / in two MUST groups / twice in one MUST group /
+    as a SHOULD and a MUST_NOT clause."""
+    shapes = []
+    for i in range(n):
+        n_cl = 32 if i < n_wide else int(rng.integers(1, 13))
+        occ = [int(o) for o in rng.choice([TQ_OCCUR_SHOULD, TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT], size=n_cl, p=[0.45, 0.35, 0.2])]
+        terms = [int(t) for t in rng.integers(0, n_terms, size=n_cl)]
+        repeat = i % 4
+        pure = i % 8 == 4  # every clause a MUST group of its own, all reading freqs: block_wand_intersection from four on
+        if pure:
+            occ = [TQ_OCCUR_MUST] * n_cl
+        if repeat == 3 and n_cl >= 2:  # the same term as SHOULD and as MUST_NOT
+            a, b = (int(x) for x in rng.choice(n_cl, size=2, replace=False))
+            occ[a], occ[b], terms[b] = TQ_OCCUR_SHOULD, TQ_OCCUR_MUST_NOT, terms[a]
+        if repeat in (1, 2) and occ.count(TQ_OCCUR_MUST) < 2 and n_cl >= 2:
+            for c in rng.choice(n_cl, size=2, replace=False):
+                occ[int(c)] = TQ_OCCUR_MUST
+        must = [c for c in range(n_cl) if occ[c] == TQ_OCCUR_MUST]
+        sizes = []
+        while sum(sizes) < len(must):
+            sizes.append(min(int(rng.integers(1, 5)), len(must) - sum(sizes)))
+        if pure:
+            sizes = [1] * len(must)
+        if repeat == 1 and len(sizes) == 1 and sizes[0] >= 2:  # two groups are needed
+            sizes = [1, sizes[0] - 1]
+        if repeat == 2 and len(sizes) >= 2 and max(sizes) < 2:  # a group of two is needed
+            sizes = [2] + sizes[2:]
+        ids = rng.permutation(len(sizes)) + 1
+        order = rng.permutation(must)
+        groups = [0] * n_cl
+        pos = 0
+        for g, sz in zip(ids, sizes):
+            for c in order[pos:pos + sz]:
+                groups[int(c)] = int(g)
+            pos += sz
+        members = {}
+        for c in must:
+            members.setdefault(groups[c], []).append(c)
+        ms = list(members.values())
+        if repeat == 1 and len(ms) >= 2:  # one term in two MUST groups
+            terms[ms[1][0]] = terms[ms[0][0]]
+        if repeat == 2:  # one term twice in one MUST group
+            big = [m for m in ms if len(m) >= 2]
+            if big:
+                terms[big[0][1]] = terms[big[0][0]]
+        n_should = occ.count(TQ_OCCUR_SHOULD)
+        shapes.append(dict(terms=terms, occurs=occ, groups=groups, msm=int(rng.integers(0, n_should + 2)),
+                           flags=[TQ_TERM_IGNORE_FREQ if rng.random() < 0.2 and not pure else 0 for _ in range(n_cl)],
+                           boosts=[float(b) for b in rng.choice(BOOL_BOOSTS, size=n_cl, p=[0.7, 0.1, 0.1, 0.1])],
+                           k=int(rng.choice(BOOL_KS))))
+    return shapes
+
+
+def shape_query(q, shape):
+    """The TQ_OP_BOOL query of a shape, from a make_query / SynthIndex.query dict of its terms (weights already boosted)."""
+    q = bool_query(q, shape["occurs"], shape["groups"], shape["msm"])
+    q["term_flags"] = list(shape["flags"])
+    return q
+
+
+def bool_shape_query(segments, shape):
+    return shape_query(make_query(TQ_OP_OR, segments, shape["terms"], shape["k"], boost=list(shape["boosts"])), shape)
+
+
+def bool_branches(q, segment_ord, basic=False):
+    """Which way BooleanWeight::complex_scorer (boolean_weight.rs:236-431) goes for TQ_OP_BOOL query q on one segment, restated
+    from the reference's code: a set of labels.  Clauses without postings in the segment are EmptyScorers and drop out;
+    basic = the segment's field is indexed without freqs."""
+    occ, grp = q["term_occur"], q.get("term_group")
+    n = len(occ)
+    flags = q.get("term_flags") or [0] * n
+    present = {ts[0] for ts in q["term_segs"] if ts[1] == segment_ord and ts[3] > 0}
+    groups = {}
+    for c in range(n):
+        if occ[c] == TQ_OCCUR_MUST:
+            g = groups.setdefault(grp[c] if grp is not None else 256 + c, [])
+            if c in present:
+                g.append(c)
+    if any(not g for g in groups.values()):
+        return {"empty_must"}
+    groups = list(groups.values())
+    should = [c for c in range(n) if occ[c] == TQ_OCCUR_SHOULD and c in present]
+    must_not = [c for c in range(n) if occ[c] == TQ_OCCUR_MUST_NOT and c in present]
+    m = int(q.get("min_should_match", 0))
+    if m > len(should):
+        return {"msm_gt_n"}
+    out = set()
+    if m >= 2 and m == len(should):  # the SHOULD clauses become MUST clauses
+        out.add("msm_eq_n")
+        groups += [[c] for c in should]
+        should, m = [], 0
+    if not should:
+        if not groups:
+            return {"nothing"}
+        out.add("must_only")
+    elif m == 0:
+        out.add("optional_with_must" if groups else "optional_without_must")
+    else:
+        out.add("required_union" if m == 1 else "required_disjunction")
+    if must_not:
+        out.add("exclude_1" if len(must_not) == 1 else "exclude_many")
+    if len(groups) >= 4:  # block_wand_intersection: MUST TermScorers reading freqs and nothing else (:312-340)
+        seq = not should and not must_not and all(len(g) == 1 and not basic and not (flags[g[0]] & TQ_TERM_IGNORE_FREQ) for g in groups)
+        out.add("groups4_sequential" if seq else "groups4_intersection")
+    return out
+
+
+BOOL_BRANCHES = {"empty_must", "msm_gt_n", "msm_eq_n", "optional_with_must", "optional_without_must", "required_union",
+                 "required_disjunction", "exclude_1", "exclude_many", "groups4_sequential", "groups4_intersection"}
 
 
 def hits(result, i=0):

@@ -5,10 +5,11 @@ import numpy as np
 import pytest
 
 from oracle import tq_oracle as O
-from tantivy_b200._abi import (TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_TERM, TQ_RECORD_BASIC, TQ_RECORD_FREQS,
-                               TQ_RECORD_FREQS_POSITIONS, QueryBatch)
+from tantivy_b200._abi import (TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT, TQ_OCCUR_SHOULD, TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_TERM,
+                               TQ_RECORD_BASIC, TQ_RECORD_FREQS, TQ_RECORD_FREQS_POSITIONS, QueryBatch)
 from tests import score_model as M
-from tests.helpers import BOOL_SHAPES, OracleSegment, bool_query, hits, make_query
+from tests.helpers import (BOOL_BOOSTS, BOOL_BRANCHES, BOOL_KS, BOOL_SHAPES, OracleSegment, bool_branches, bool_query, bool_shape_query,
+                          hits, make_query, random_bool_shapes)
 
 
 def _pair(lists, lengths, segment_ord=0, alive=None, record_option=TQ_RECORD_FREQS, max_doc=None):
@@ -230,3 +231,63 @@ def test_must_not_without_postings_in_one_segment(dense):
     # neither order alone gives these rows: the segments follow different rules
     assert rows != M.search(msegs, q, terms, intersection_order=True)
     assert rows != M.search(msegs, q, terms, intersection_order=False)
+
+
+# ---- random mixed boolean shapes: every branch of complex_scorer ---------------------------------------------------------
+def _random_bool_case(seed, n_queries):
+    rng = np.random.default_rng(seed)
+    osegs, msegs = _random_pairs(rng, 3, 8, deletes=True)
+    osegs[0].terms[6] = (0, 0, 0)  # terms without postings in some segments: EmptyScorers there
+    osegs[1].terms[3] = (0, 0, 0)
+    osegs[1].terms[7] = (0, 0, 0)
+    osegs[2].terms[1] = (0, 0, 0)
+    shapes = random_bool_shapes(rng, n_queries, 8)
+    return osegs, msegs, shapes, [bool_shape_query(osegs, sh) for sh in shapes]
+
+
+def test_random_boolean_shapes_match_the_oracle():
+    """Several hundred seeded random TQ_OP_BOOL shapes (repeated terms, msm 0..n+1, boosts 0 / -1.5 / 1e4, TQ_TERM_IGNORE_FREQ,
+    32 clauses) over three segments with deletes and absent terms: model == oracle for the rows and for Count, and together
+    the shapes take every branch of complex_scorer."""
+    osegs, msegs, shapes, queries = _random_bool_case(4242, 360)
+    seen = set()
+    for q in queries:
+        for s in osegs:
+            seen |= bool_branches(q, s.segment_ord)
+    assert BOOL_BRANCHES <= seen, BOOL_BRANCHES - seen
+    _assert_model_is_oracle(osegs, msegs, queries, [sh["terms"] for sh in shapes])
+    ix = O.OracleIndex()
+    for s in osegs:
+        s.register(ix)
+    counts = ix.count_batch(QueryBatch(queries))
+    assert [M.count(msegs, q, sh["terms"]) for q, sh in zip(queries, shapes)] == list(counts)
+    assert sum(1 for c in counts if c) > len(queries) // 3  # (not a vacuous comparison)
+
+
+def test_random_boolean_shapes_cover_the_generator():
+    """The generator makes what its callers rely on: 1-12 and 32 clauses, MUST groups of 1-4, msm up to n_should + 1, each
+    repeated-term pattern, every boost and k."""
+    shapes = random_bool_shapes(np.random.default_rng(4242), 360, 8)
+    assert {len(s["terms"]) for s in shapes} == set(range(1, 13)) | {32}
+    sizes = set()
+    pats = set()
+    for s in shapes:
+        groups = {}
+        for c, (o, g) in enumerate(zip(s["occurs"], s["groups"])):
+            if o == TQ_OCCUR_MUST:
+                groups.setdefault(g, []).append(s["terms"][c])
+        sizes |= {len(m) for m in groups.values()}
+        if any(len(set(m)) < len(m) for m in groups.values()):
+            pats.add("twice in one group")
+        firsts = [set(m) for m in groups.values()]
+        if any(a & b for i, a in enumerate(firsts) for b in firsts[i + 1:]):
+            pats.add("in two groups")
+        should = {t for t, o in zip(s["terms"], s["occurs"]) if o == TQ_OCCUR_SHOULD}
+        if should & {t for t, o in zip(s["terms"], s["occurs"]) if o == TQ_OCCUR_MUST_NOT}:
+            pats.add("should and must_not")
+    assert sizes == {1, 2, 3, 4}
+    assert pats == {"twice in one group", "in two groups", "should and must_not"}
+    assert any(s["msm"] == s["occurs"].count(TQ_OCCUR_SHOULD) + 1 for s in shapes)
+    assert {b for s in shapes for b in s["boosts"]} == set(BOOL_BOOSTS)
+    assert {s["k"] for s in shapes} == set(BOOL_KS)
+    assert any(f for s in shapes for f in s["flags"])
