@@ -63,6 +63,33 @@ struct PinBuf {
   void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
 
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Descriptors for the device: arrays placed back to back at 256-byte alignment.  reserve() sizes a pinned buffer and a device
+// buffer of that layout (device pointers are valid from then on), copy() fills the pinned one, one H2D copy of `bytes` the other.
+struct Staging {
+  struct Part { size_t off; const void* src; size_t n; };
+  std::vector<Part> parts;
+  size_t bytes = 0;
+  uint8_t *host = nullptr, *dev = nullptr;  // set by reserve
+  size_t add(const void* src, size_t n) {  // src null: space only (device-only data, or filled through on_host)
+    parts.push_back(Part{bytes, src, n});
+    const size_t off = bytes;
+    bytes = align256(bytes + n);
+    return off;
+  }
+  template <class T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size() * sizeof(T)); }
+  cudaError_t reserve(PinBuf& pin, DevBuf& d) {
+    cudaError_t e = pin.ensure(bytes + 256);
+    if (e == cudaSuccess) e = d.ensure(bytes + 256);
+    host = pin.p; dev = d.p;
+    return e;
+  }
+  void copy() const { for (const Part& p : parts) if (p.src && p.n) memcpy(host + p.off, p.src, p.n); }
+  template <class T> T* on_host(size_t off) const { return reinterpret_cast<T*>(host + off); }
+  template <class T> T* on_device(size_t off) const { return reinterpret_cast<T*>(dev + off); }
+};
+
 struct ListKey {
   uint32_t segment_ord, field;
   uint64_t postings_start;  // bit 63: the table was built with term frequencies ignored (TQ_TERM_IGNORE_FREQ)
@@ -152,10 +179,26 @@ struct tq_ctx {
   uint64_t tile_smem_last = 0;
   uint32_t tile_cand_floor = 32768, tile_max_dens_x1000 = 0, tile_pcap_hook = 0, tile_big_min = 6, tile_units = 0;
   uint32_t target_units = 0;  // CTAs a batch's per-query units aim for (4 x 32 per SM)
-  uint32_t or_prune = 1, or_strip = 1, or_pipe = 1, strip_prune = 1, strip_sample_div = 32, strip_sample_div2 = 8, strip_sample_div3 = 2, strip_ne_div = 8, strip_ne_div2 = 64;
+  uint32_t or_prune = 0, or_strip = 1, or_pipe = 1, strip_prune = 1, strip_sample_div = 32, strip_sample_div2 = 8, strip_sample_div3 = 2, strip_ne_div = 8, strip_ne_div2 = 64;
 };
 
 constexpr int kTileRounds = 4;  // launches of k_tile per run: the sample launch + three exact ones
+
+// Unit classes of the per-query kernels: the order of tq_batch::n_units / unit_base and of the batch's Unit array.
+enum UnitClass : int {
+  UC_TERM = TQ_OP_TERM, UC_AND = TQ_OP_AND, UC_OR_WINDOW = TQ_OP_OR,  // k_term, k_and, k_or / k_or_pipe
+  UC_STRIP, UC_STRIP_ROUND1, UC_STRIP_ROUND2, UC_STRIP_ROUND3,        // k_or_strip: main launch (last phase), threshold rounds (phases 0..2)
+  UC_PHRASE, UC_CLASSES                                               // k_phrase
+};
+
+// Appends n elements at src to v and points at the copy (null stays null).  v's capacity must hold them: earlier copies stay put.
+template <class T>
+static const T* keep(std::vector<T>& v, const T* src, size_t n) {
+  if (!src) return nullptr;
+  const size_t at = v.size();
+  v.insert(v.end(), src, src + n);
+  return v.data() + at;
+}
 
 // Deep copy of a batch's queries (only kept when the tile engine runs them: an overflowing run is repeated, see finalize_run).
 struct OwnedQueries {
@@ -165,6 +208,27 @@ struct OwnedQueries {
   std::vector<uint8_t> flags;
   std::vector<tq_term_pos> tp;
   std::vector<uint32_t> toff;
+  void assign(const tq_query* queries, size_t nq) {
+    size_t n_ts = 0, n_t = 0, n_cache = 0;
+    for (size_t qi = 0; qi < nq; ++qi) {
+      n_ts += queries[qi].n_term_segs;
+      n_t += queries[qi].n_terms;
+      if (queries[qi].tf_cache) n_cache += 256 * (size_t)queries[qi].n_terms;
+    }
+    ts.reserve(n_ts); tp.reserve(n_ts);
+    w.reserve(n_t); avg.reserve(n_t); flags.reserve(n_t); toff.reserve(n_t);
+    cache.reserve(n_cache);
+    q.assign(queries, queries + nq);
+    for (tq_query& d : q) {
+      d.term_segs = keep(ts, d.term_segs, d.n_term_segs);
+      d.term_pos = keep(tp, d.term_pos, d.n_term_segs);
+      d.weight = keep(w, d.weight, d.n_terms);
+      d.avg_fieldnorm = keep(avg, d.avg_fieldnorm, d.n_terms);
+      d.tf_cache = keep(cache, d.tf_cache, 256 * (size_t)d.n_terms);
+      d.term_flags = keep(flags, d.term_flags, d.n_terms);
+      d.term_offset = keep(toff, d.term_offset, d.n_terms);
+    }
+  }
 };
 
 struct tq_batch {
@@ -197,8 +261,7 @@ struct tq_batch {
   BatchParams params{};
   size_t desc_bytes = 0;
   uint32_t nq = 0, kmax = 0;
-  uint32_t n_units[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // term, and, or (window kernel), or (strip kernel), strip threshold rounds 1..3, phrase
-  uint32_t unit_base[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  uint32_t n_units[UC_CLASSES] = {}, unit_base[UC_CLASSES] = {};  // per UnitClass
   uint32_t phrase_ct = 2;                 // most terms of a phrase in the batch (k_phrase's candidate stride)
   const PhraseAux* phrase_aux = nullptr;  // device: per clause of the batch's phrase queries (parallel to qlists)
   uint32_t strip_cached_max = 0;
@@ -206,6 +269,7 @@ struct tq_batch {
   size_t qinit_off = 0;
   int next_phase = 0;  // of the current run (0: none started)
   size_t qstate_off = 0, cands_off = 0, res_off = 0, res_bytes = 0, n_cands = 0;
+  struct { size_t scores, segs, docs, counts; } res_at{};  // the result columns inside the res_bytes at res_off (and in res_pin)
   tq_stats stats{};
   bool ran = false;
 };
@@ -556,7 +620,7 @@ int get_list(tq_ctx* c, const tq_term_seg& ts, bool ignore_freq, std::vector<Pen
 int flush_builds(tq_ctx* c, std::vector<PendingBuild>& pending, uint64_t* built) {
   if (pending.empty()) return TQ_OK;
   const size_t n = pending.size();
-  struct Fail { tq_ctx* c; std::vector<PendingBuild>& p; bool ok = false; ~Fail() { if (!ok) rollback_builds(c, p); } } guard{c, pending};
+  PendingScope guard{c, pending};
   TQ_CUDA(c->build_pin.ensure(n * (sizeof(ListDesc) + sizeof(BuildJob) + 4)));
   TQ_CUDA(c->build_dev.ensure(n * (sizeof(ListDesc) + sizeof(BuildJob) + 4)));
   ListDesc* hd = reinterpret_cast<ListDesc*>(c->build_pin.p);
@@ -574,7 +638,6 @@ int flush_builds(tq_ctx* c, std::vector<PendingBuild>& pending, uint64_t* built)
   for (size_t i = 0; i < n; ++i)
     if (hs[i] != 0) return fail(TQ_ERR_CORRUPT, "posting list bytes are not a valid tantivy posting list");
   *built += n;
-  guard.ok = true;
   pending.clear();
   return TQ_OK;
 }
@@ -628,7 +691,7 @@ int get_pos(tq_ctx* c, const tq_term_seg& ts, const tq_term_pos& tp, std::vector
 int flush_pos_builds(tq_ctx* c, std::vector<PendingPos>& pending) {
   if (pending.empty()) return TQ_OK;
   const size_t n = pending.size();
-  struct Fail { tq_ctx* c; std::vector<PendingPos>& p; bool ok = false; ~Fail() { if (!ok) rollback_pos(c, p); } } guard{c, pending};
+  PendingPosScope guard{c, pending};
   TQ_CUDA(c->build_pin.ensure(n * (sizeof(PosJob) + 4)));
   TQ_CUDA(c->build_dev.ensure(n * (sizeof(PosJob) + 4)));
   PosJob* hj = reinterpret_cast<PosJob*>(c->build_pin.p);
@@ -644,14 +707,9 @@ int flush_pos_builds(tq_ctx* c, std::vector<PendingPos>& pending) {
     if (hs[i] == 2) return fail(TQ_ERR_OOM, "the segment's position-table pool is exhausted");
     if (hs[i] != 0) return fail(TQ_ERR_CORRUPT, "position bytes are not a valid tantivy position stream");
   }
-  guard.ok = true;
   pending.clear();
   return TQ_OK;
 }
-
-struct CacheKey {
-  std::vector<float> table;
-};
 
 }  // namespace
 
@@ -689,6 +747,50 @@ static void collect_times(tq_batch* b) {
   b->stats.tile_ms = by_kind[SPAN_TILE];
   b->stats.theta_ms = by_kind[SPAN_THETA];
   b->stats.phrase_ms = by_kind[SPAN_PHRASE];
+}
+
+// The run's kernel times into its stats, and its stats into the context's (tq_get_stats).
+static void publish_stats(tq_batch* b) {
+  collect_times(b);
+  std::lock_guard<std::mutex> g(b->ctx->mu);
+  b->ctx->stats = b->stats;
+}
+
+// Enqueues a copy of src's result rows (the first min(k_max, stride) of each) and counts into device arrays of row stride `stride`.
+static cudaError_t copy_rows(const tq_batch* src, cudaStream_t stream, float* scores, uint32_t* segs, uint32_t* docs, uint32_t* counts, size_t stride) {
+  const BatchParams& S = src->params;
+  const size_t dp = stride * 4, sp = (size_t)src->kmax * 4, width = std::min(dp, sp);
+  auto rows = [&](void* d, const void* s) {  // (one plain copy when both sides have the same stride)
+    return dp == sp ? cudaMemcpyAsync(d, s, sp * src->nq, cudaMemcpyDeviceToDevice, stream)
+                    : cudaMemcpy2DAsync(d, dp, s, sp, width, src->nq, cudaMemcpyDeviceToDevice, stream);
+  };
+  cudaError_t e = rows(scores, S.res_scores);
+  if (e == cudaSuccess) e = rows(segs, S.res_segs);
+  if (e == cudaSuccess) e = rows(docs, S.res_docs);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(counts, S.res_counts, (size_t)src->nq * 4, cudaMemcpyDeviceToDevice, stream);
+  return e;
+}
+
+// One Count kernel over (query, segment) pairs: stages their clause words (list ids, or BOOL structure words with list ids), the
+// pairs, the units and zeroed per-query counters, runs `kernel` and adds the counts to out_counts.
+template <class Params, class Seg>
+static int count_on_device(tq_batch* b, const std::vector<uint32_t>& words, const std::vector<Seg>& segs, const std::vector<Unit>& units,
+                           size_t nq, uint64_t* out_counts, void (*kernel)(Params)) {
+  const std::vector<unsigned long long> zeros(nq, 0);
+  Staging st;
+  const size_t o_w = st.add(words), o_s = st.add(segs), o_u = st.add(units), o_c = st.add(zeros);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  const Params P{b->ctx->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const Seg>(o_s), st.on_device<const Unit>(o_u),
+                 st.on_device<unsigned long long>(o_c)};
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  kernel<<<(unsigned)units.size(), kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  TQ_CUDA(cudaMemcpyAsync(b->pin.p + o_c, b->dev.p + o_c, nq * 8, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  const unsigned long long* dc = st.on_host<const unsigned long long>(o_c);
+  for (size_t qi = 0; qi < nq; ++qi) out_counts[qi] += dc[qi];
+  return TQ_OK;
 }
 
 static tq_batch* acquire_batch(tq_ctx* c) {
@@ -753,6 +855,88 @@ struct TileGroupBuild {
   uint64_t list_bytes = 0;                         // postings-range bytes of the distinct lists
 };
 
+// A tile group as the device reads it: slots in their final order, TSegs, TQuerys, clause words, the units of its launches and
+// the score chunks of k_score_lists.
+struct GroupStage {
+  std::vector<TSlot> slots;
+  std::vector<TSeg> segs;
+  std::vector<TQuery> queries;
+  std::vector<uint16_t> clauses;
+  std::vector<TUnit> units[kTileRounds];
+  std::vector<SChunk> chunks;
+  uint32_t max_slots = 1, p_cap = 1024, max_big = 1, max_queries = 1, max_clause_words = 0, max_clauses = 1;
+  size_t tix_words = 0;
+};
+
+// A (query, segment) of the per-query kernels, beside its QSeg: its unit class, the blocks / windows / tiles its units cover, and
+// whether it is a strip pair with a threshold sample pass (MaxScore can then skip its dense clauses).
+struct SegWork { UnitClass cls; uint32_t total; bool sample; };
+
+// The plan of one batch: what the stages of batch_prepare_impl hand on to each other.
+struct BatchPlan {
+  const tq_query* queries = nullptr;
+  size_t nq = 0;
+  int repeat = 0;
+  bool terms_on_tile = false;
+  std::vector<DQuery> dq;
+  std::vector<size_t> q_cands;                          // candidate-region size per query
+  std::vector<float> caches;                            // n_caches * 256
+  std::unordered_map<uint32_t, uint32_t> cache_by_avg;  // avg bits -> cache idx
+  uint32_t last_avg_bits = 0, last_avg_idx = 0xFFFFFFFFu;
+  std::vector<PendingBuild> pending;
+  std::vector<PendingPos> pending_pos;
+  std::vector<const tq_term_seg*> order;  // reused from query to query
+  std::vector<SegPlan> plans;             // the current query's, n_plans live entries (reused from query to query)
+  size_t n_plans = 0;
+  // per-query kernels
+  std::vector<QList> qlists;
+  std::vector<QSeg> qsegs;
+  std::vector<SegWork> work;    // parallel to qsegs
+  std::vector<PhraseAux> qaux;  // parallel to qlists once a phrase query shows up
+  std::vector<Unit> units[UC_CLASSES];
+  uint32_t n_qsegs_op[4] = {0, 0, 0, 0};  // (query, segment) pairs of k_term, k_and + k_phrase, the window kernels, k_or_strip
+  uint32_t strip_cached_max = 0, or_max_lists = 0, phrase_ct = 2;
+  // tile engine
+  std::vector<TileGroupBuild> tgroups;
+  std::vector<GroupStage> gstage;  // parallel to tgroups
+  uint64_t tile_pairs_total = 0, pair_cursor = 0, tile_postings = 0, tile_units = 0;
+  size_t tix_total_words = 0, tile_bytes = 0;
+  // totals
+  uint64_t built = 0, alg_bytes = 0, postings = 0, op_bytes[3] = {0, 0, 0};
+  uint32_t kmax = 1;
+  size_t n_cands = 0;
+};
+
+// Calls f(lists, n) per segment on the query's (clause, segment) lists with postings, by (segment, clause); stops at the first error.
+template <class F>
+int for_each_segment(const tq_query& q, std::vector<const tq_term_seg*>& order, F&& f) {
+  order.clear();
+  for (uint32_t i = 0; i < q.n_term_segs; ++i) {
+    if (q.term_segs[i].term_idx >= q.n_terms) return fail(TQ_ERR_INVALID_ARGUMENT, "term_idx out of range");
+    if (q.term_segs[i].doc_freq) order.push_back(&q.term_segs[i]);
+  }
+  std::stable_sort(order.begin(), order.end(), [](const tq_term_seg* a, const tq_term_seg* b) {
+    return a->segment_ord != b->segment_ord ? a->segment_ord < b->segment_ord : a->term_idx < b->term_idx;
+  });
+  for (size_t i = 0, j; i < order.size(); i = j) {
+    for (j = i + 1; j < order.size() && order[j]->segment_ord == order[i]->segment_ord; ++j) {}
+    const int rc = f(order.data() + i, j - i);
+    if (rc != TQ_OK) return rc;
+  }
+  return TQ_OK;
+}
+
+// Maps the clause entries of TQ_OP_BOOL structure words (layout: bool_structure) in place; header words and group lengths stay.
+template <class W, class Map>
+void map_bool_clauses(W* w, size_t n, Map map) {
+  size_t x = 4;
+  for (uint32_t g = 0; g < w[0]; ++g) {
+    const size_t len = w[x++];
+    for (size_t e = 0; e < len; ++e, ++x) w[x] = (W)map(w[x]);
+  }
+  for (; x < n; ++x) w[x] = (W)map(w[x]);
+}
+
 // BooleanWeight::complex_scorer for ONE segment (boolean_weight.rs:236-431), term leaves only: `here` = the clauses that have
 // postings in the segment (term_idx / doc_freq / weight per entry).  Clauses without postings are EmptyScorers -- removed before
 // anything is counted; an empty MUST group empties the query in this segment.  Writes
@@ -812,41 +996,23 @@ int bool_structure(const tq_query& q, const uint32_t* term_idx, const uint32_t* 
   return 1;
 }
 
-// Would the group still satisfy k_tile's limits with this query added?  Returns the number of NEW pair elements, or -1.
-int64_t tile_admit_cost(const TileGroupBuild& g, const SegPlan* plans, size_t n_plans, uint32_t max_dens_x1000, uint32_t max_slots, uint32_t max_queries) {
-  int64_t new_pairs = 0;
-  for (size_t pi = 0; pi < n_plans; ++pi) {
-    const SegPlan& sp = plans[pi];
-    auto it = g.seg_of.find(sp.segment_ord);
-    const TileGroupBuild::SegB* sb = it == g.seg_of.end() ? nullptr : &g.segs[it->second];
-    if (sb && sb->queries.size() + 1 > max_queries) return -1;
-    size_t n_slots = sb ? sb->slots.size() : 0;
-    double dens = sb ? sb->dens : 0.0;
-    for (auto& h : sp.here) {
-      const bool found = sb && g.find_slot(*sb, h.second) != kNoSlot;
-      if (!found) {
-        ++n_slots;
-        dens += (double)h.first / std::max(1u, sp.seg->max_doc);
-        new_pairs += ((int64_t)h.first + 127) / 128 * 128;
-      }
-    }
-    if (n_slots > max_slots) return -1;
-    if (dens * kTile * 1.5 + 256.0 > (double)kTileMaxPairs || (max_dens_x1000 && dens * 1000.0 > max_dens_x1000)) return -1;
-  }
-  return new_pairs;
-}
-
-// Cheap sufficient test (every clause counted as a new list): most queries pass it and skip the exact cost.
-bool tile_admit_surely_fits(const TileGroupBuild& g, const SegPlan* plans, size_t n_plans, uint32_t max_dens_x1000, uint32_t max_slots, uint32_t max_queries) {
+// Would the group still satisfy k_tile's limits with this query added?  exact = false counts every clause as a new list: a cheap
+// sufficient test that most queries pass.  exact = true: a clause whose list already has a slot in the group adds nothing.
+bool tile_fits(const tq_ctx* c, const TileGroupBuild& g, const SegPlan* plans, size_t n_plans, uint32_t max_queries, bool exact) {
   for (size_t pi = 0; pi < n_plans; ++pi) {
     const SegPlan& sp = plans[pi];
     auto it = g.seg_of.find(sp.segment_ord);
     const TileGroupBuild::SegB* sb = it == g.seg_of.end() ? nullptr : &g.segs[it->second];
     if (sb && sb->queries.size() + 1 > max_queries) return false;
+    size_t n_slots = sb ? sb->slots.size() : 0;
     double dens = sb ? sb->dens : 0.0;
-    for (auto& h : sp.here) dens += (double)h.first / std::max(1u, sp.seg->max_doc);
-    if ((sb ? sb->slots.size() : 0) + sp.here.size() > max_slots) return false;
-    if (dens * kTile * 1.5 + 256.0 > (double)kTileMaxPairs || (max_dens_x1000 && dens * 1000.0 > max_dens_x1000)) return false;
+    for (auto& h : sp.here) {
+      if (exact && sb && g.find_slot(*sb, h.second) != kNoSlot) continue;
+      ++n_slots;
+      dens += (double)h.first / std::max(1u, sp.seg->max_doc);
+    }
+    if (n_slots > c->tile_max_slots) return false;
+    if (dens * kTile * 1.5 + 256.0 > (double)kTileMaxPairs || (c->tile_max_dens_x1000 && dens * 1000.0 > c->tile_max_dens_x1000)) return false;
   }
   return true;
 }
@@ -894,360 +1060,283 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, const SegPlan* pl
       if (op != TQ_OP_BOOL) sb.clauses.push_back((uint16_t)slot);
     }
     if (op == TQ_OP_BOOL) {  // the structure words stay, the clause indices become slots
-      const std::vector<uint16_t>& w = sp.bool_words;
-      size_t x = 0;
-      for (int k = 0; k < 4; ++k) sb.clauses.push_back(w[x++]);
-      for (uint32_t g = 0; g < w[0]; ++g) {
-        const uint16_t len = w[x++];
-        sb.clauses.push_back(len);
-        for (uint16_t e = 0; e < len; ++e) sb.clauses.push_back(slot_of_here[w[x++]]);
-      }
-      while (x < w.size()) sb.clauses.push_back(slot_of_here[w[x++]]);
+      const size_t at = sb.clauses.size();
+      sb.clauses.insert(sb.clauses.end(), sp.bool_words.begin(), sp.bool_words.end());
+      map_bool_clauses(sb.clauses.data() + at, sp.bool_words.size(), [&](uint16_t a) { return slot_of_here[a]; });
     }
     sb.queries.push_back(tq);
   }
   return g.pairs - pairs_before;
 }
 
-}  // namespace
+// tq_stats' bytes_term / bytes_and / bytes_or class of a query shape: phrases count as AND, mixed boolean queries as OR.
+int bytes_class(int op) { return op == TQ_OP_PHRASE ? TQ_OP_AND : (op == TQ_OP_BOOL ? TQ_OP_OR : op); }
 
-static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int repeat, tq_batch** out);
-
-extern "C" {
-
-void tq_batch_destroy(tq_batch* b) {
-  if (!b) return;
-  cudaSetDevice(b->ctx->device);
-  cudaStreamSynchronize(b->stream);
-  b->next_phase = 0;
-  b->ran = false;
-  std::lock_guard<std::mutex> g(b->ctx->mu);
-  b->ctx->pool.push_back(b);  // buffers are recycled by the next batch
-}
-
-int tq_batch_prepare(tq_ctx* c, const tq_query* queries, size_t nq, tq_batch** out) {
-  return batch_prepare_impl(c, queries, nq, 0, out);
-}
-
-}  // extern "C"
-
-// repeat (finalize_run): 0 = a caller's batch.  1 = the repeat of an overflowed run: TERM / AND / OR / phrase queries take the
-// per-query kernels; TQ_OP_BOOL queries stay on the tile engine with candidate regions as large as their postings and the largest
-// tile buffer.  2 = as 1, but every TQ_OP_BOOL query in a tile group of its own.
-static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int repeat, tq_batch** out) {
-  if (!c || !out || (!queries && nq)) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
-  TQ_CUDA(cudaSetDevice(c->device));
-  tq_batch* b = acquire_batch(c);
-  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
-  struct Guard { tq_batch* b; bool ok = false; ~Guard() { if (!ok) tq_batch_destroy(b); } } guard{b};
-  b->ran = false;
-  b->finalized = false;
-  b->next_phase = 0;  // a recycled batch may have been abandoned in the middle of a phased run
-  b->nq = (uint32_t)nq;
-  b->stats = tq_stats{};
-  b->n_spans = 0;
-  b->groups.clear();
-  b->owned = OwnedQueries{};
-  b->repeat = repeat;
-
-  std::vector<QList> qlists;
-  std::vector<QSeg> qsegs;
-  std::vector<Unit> units[8];
-  std::vector<PhraseAux> qaux;  // parallel to qlists once a phrase query shows up
-  std::vector<PendingPos> pending_pos;
-  std::vector<DQuery> dq(nq);
-  std::vector<float> caches;  // n_caches * 256
-  std::unordered_map<uint32_t, uint32_t> cache_by_avg;  // avg bits -> cache idx
-  std::vector<PendingBuild> pending;
-  uint64_t built = 0, alg_bytes = 0, postings = 0, op_bytes[3] = {0, 0, 0};
-  uint32_t kmax = 1;
-  size_t n_cands = 0;
-  std::vector<int> qseg_op;
-  std::vector<uint32_t> qseg_total;
-  uint32_t n_qsegs_op[4] = {0, 0, 0, 0};
-  std::vector<char> qseg_sample;  // strip pairs that get a threshold sample pass (MaxScore can then skip their dense clauses)
-  uint32_t strip_cached_max = 0, or_max_lists = 0, phrase_ct = 2;
-  std::vector<TileGroupBuild> tgroups;
-  std::vector<size_t> q_cands(nq, 0);
-  const bool tile_on = c->tile != 0 && repeat == 0;
-  const uint64_t tile_pair_budget = (uint64_t)c->tile_scratch_mb * (1u << 20) / 8u;
-  uint64_t tile_pairs_total = 0;
-  // Single-term queries ride along on the tile engine when the batch has multi-term queries whose decoded lists they share
-  // (mixed workload: 32.6 K q/s against 28.6 K with them on k_term); a batch of nothing but single-term queries has nothing to
-  // share and streams its lists through k_term (configs[0]: 1.39 M q/s against 0.49 M).  TQ_TILE_TERMS: 0 never, 1 always, 2 this rule.
-  bool terms_on_tile = c->tile_terms == 1;
-  if (c->tile_terms >= 2)
-    for (size_t qi = 0; qi < nq && !terms_on_tile; ++qi)
-      terms_on_tile = queries[qi].n_terms >= 2 && queries[qi].op != TQ_OP_PHRASE;
-  {
-    std::lock_guard<std::mutex> g(c->mu);
-    PendingScope pending_scope{c, pending};  // an early error return leaves no half-built list in the cache
-    PendingPosScope pending_pos_scope{c, pending_pos};
-    std::vector<const tq_term_seg*> order;
-    std::vector<SegPlan> plans;  // reused from query to query (n_plans live entries)
-    uint32_t last_avg_bits = 0, last_avg_idx = 0xFFFFFFFFu;
-    for (size_t qi = 0; qi < nq; ++qi) {
-      const tq_query& q = queries[qi];
-      if (q.k == 0 || q.k > TQ_MAX_K) return fail(TQ_ERR_INVALID_ARGUMENT, "k must be in 1..TQ_MAX_K");
-      if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
-      const bool is_bool = q.op == TQ_OP_BOOL;
-      if (is_bool && (c->tile == 0 || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
-      if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_PHRASE && !is_bool) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
-      if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
-      if (!q.weight || (!q.avg_fieldnorm && !q.tf_cache) || (!q.term_segs && q.n_term_segs)) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
-      const bool is_phrase = q.op == TQ_OP_PHRASE;
-      if (is_phrase) {
-        if (q.n_terms < 2 || q.n_terms > TQ_MAX_PHRASE_TERMS) return fail(TQ_ERR_UNSUPPORTED, "a phrase takes 2..TQ_MAX_PHRASE_TERMS terms on the device path");
-        // slop: two terms take intersection_count_with_slop on the device; three and more carry per-position slops through
-        // growing buffers (intersection_count_with_carrying_slop, phrase_scorer.rs:236-345) and stay on the reference's CPU path
-        if (q.slop != 0 && q.n_terms != 2) return fail(TQ_ERR_UNSUPPORTED, "phrase slop with more than two terms stays on the reference's CPU path");
-        if ((!q.term_pos && q.n_term_segs) || !q.term_offset) return fail(TQ_ERR_INVALID_ARGUMENT, "a phrase needs term_pos and term_offset");
-      }
-      kmax = std::max(kmax, q.k);
-      alg_bytes += 12ull * q.k;
-      op_bytes[is_phrase ? TQ_OP_AND : (is_bool ? TQ_OP_OR : (q.n_terms == 1 ? TQ_OP_TERM : q.op))] += 12ull * q.k;
-      // tf-norm tables of this query's clauses
-      uint32_t cache_idx[TQ_MAX_TERMS];
-      for (uint32_t t = 0; t < q.n_terms; ++t) {
-        if (q.tf_cache) {
-          cache_idx[t] = (uint32_t)(caches.size() / 256);
-          caches.insert(caches.end(), q.tf_cache + 256 * (size_t)t, q.tf_cache + 256 * (size_t)(t + 1));
-        } else {
-          uint32_t bits;
-          memcpy(&bits, &q.avg_fieldnorm[t], 4);
-          if (bits == last_avg_bits && last_avg_idx != 0xFFFFFFFFu) { cache_idx[t] = last_avg_idx; continue; }  // (nearly always the same field)
-          auto it = cache_by_avg.find(bits);
-          if (it == cache_by_avg.end()) {
-            float tab[256];
-            bm25_tf_cache(q.avg_fieldnorm[t], tab);
-            it = cache_by_avg.emplace(bits, (uint32_t)(caches.size() / 256)).first;
-            caches.insert(caches.end(), tab, tab + 256);
-          }
-          cache_idx[t] = it->second;
-          last_avg_bits = bits; last_avg_idx = it->second;
-        }
-      }
-      // effective shape: an AND / OR of one clause is that clause (boolean_weight.rs:57-68, block_wand_union.rs:154-157)
-      const int op = is_phrase ? TQ_OP_PHRASE : (is_bool ? TQ_OP_BOOL : (q.n_terms == 1 ? TQ_OP_TERM : q.op));
-      dq[qi].k = q.k;
-      dq[qi].op = (uint32_t)op;
-      // group the (clause, segment) lists by segment
-      order.clear();
-      for (uint32_t i = 0; i < q.n_term_segs; ++i) {
-        if (q.term_segs[i].term_idx >= q.n_terms) return fail(TQ_ERR_INVALID_ARGUMENT, "term_idx out of range");
-        if (q.term_segs[i].doc_freq) order.push_back(&q.term_segs[i]);
-      }
-      std::stable_sort(order.begin(), order.end(), [](const tq_term_seg* a, const tq_term_seg* b) {
-        return a->segment_ord != b->segment_ord ? a->segment_ord < b->segment_ord : a->term_idx < b->term_idx;
-      });
-      size_t n_plans = 0;
-      uint64_t q_postings = 0;
-      for (size_t i = 0; i < order.size();) {
-        size_t j = i;
-        while (j < order.size() && order[j]->segment_ord == order[i]->segment_ord) ++j;
-        // lists of this (query, segment), clause order
-        const size_t n_here = j - i;
-        bool dup = false;
-        for (size_t a = i + 1; a < j; ++a) dup |= order[a]->term_idx == order[a - 1]->term_idx;
-        if (dup) return fail(TQ_ERR_INVALID_ARGUMENT, "duplicate (term_idx, segment_ord)");
-        if ((op == TQ_OP_AND || op == TQ_OP_PHRASE) && n_here != q.n_terms) { i = j; continue; }  // a clause is absent: empty intersection
-        if (n_plans == plans.size()) plans.emplace_back();
-        SegPlan& sp = plans[n_plans++];
-        sp.here.clear();
-        sp.term_idx.clear();
-        sp.uniform_fn = true;
-        sp.no_freq = 0;
-        sp.segment_ord = order[i]->segment_ord;
-        for (size_t a = i; a < j; ++a) {
-          uint32_t id;
-          const bool ignore_freq = q.term_flags && (q.term_flags[order[a]->term_idx] & TQ_TERM_IGNORE_FREQ);
-          int rc = get_list(c, *order[a], ignore_freq, pending, &id, &sp.seg);
-          if (rc != TQ_OK) return rc;
-          if (ignore_freq || sp.seg->record_option == TQ_RECORD_BASIC) sp.no_freq |= 1u << (a - i);
-          if (a == i) sp.fn0 = sp.seg->d_fieldnorm; else sp.uniform_fn &= (sp.seg->d_fieldnorm == sp.fn0);
-          QList ql{id, q.weight[is_phrase ? 0 : order[a]->term_idx], cache_idx[is_phrase ? 0 : order[a]->term_idx], 0};
-          if (is_phrase) {  // the clause's position table; QList.pad carries its id to the aux array below
-            if (sp.seg->record_option != TQ_RECORD_FREQS_POSITIONS) return fail(TQ_ERR_INVALID_ARGUMENT, "phrase query on a field without positions");
-            rc = get_pos(c, *order[a], q.term_pos[order[a] - q.term_segs], pending_pos, &ql.pad);
-            if (rc != TQ_OK) return rc;
-          }
-          sp.here.push_back(SegPlan::Clause{order[a]->doc_freq, ql, (uint32_t)(order[a]->postings_end - order[a]->postings_start)});
-          sp.term_idx.push_back(order[a]->term_idx);
-          alg_bytes += (order[a]->postings_end - order[a]->postings_start) + order[a]->doc_freq;
-          op_bytes[is_phrase ? TQ_OP_AND : (is_bool ? TQ_OP_OR : op)] += (order[a]->postings_end - order[a]->postings_start) + order[a]->doc_freq;
-          postings += order[a]->doc_freq;
-          q_postings += order[a]->doc_freq;
-        }
-        if (op == TQ_OP_PHRASE) {
-          // PhraseScorer keeps its terms by ascending size_hint (intersection.rs:40-52); every clause carries
-          // (max_offset - its offset), the shift that lines the terms' positions up (phrase_scorer.rs:349-398)
-          uint32_t max_offset = 0;
-          for (uint32_t t = 0; t < q.n_terms; ++t) max_offset = std::max(max_offset, q.term_offset[t]);
-          for (size_t a = 0; a < sp.here.size(); ++a) sp.here[a].range_len = max_offset - q.term_offset[sp.term_idx[a]];  // (range_len is free here)
-          std::stable_sort(sp.here.begin(), sp.here.end(), [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.first < b.first; });
-        }
-        if (op == TQ_OP_AND)  // leader = rarest, then ascending doc_freq; stable (block_wand_intersection.rs:27)
-          std::stable_sort(sp.here.begin(), sp.here.end(), [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.first < b.first; });
-        if (op == TQ_OP_OR)
-          // Canonical union order = descending Bm25Weight.weight, ties in clause order (the reference's own order is
-          // data dependent, block_wand_union.rs:205-208): the f32 sum is taken in this order, and the clauses with the
-          // smallest score bounds form a suffix, which is what the MaxScore splits of k_tile / k_or_strip need.
-          std::stable_sort(sp.here.begin(), sp.here.end(), [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.second.weight > b.second.weight; });
-        sp.prunable = true;
-        for (auto& h : sp.here) sp.prunable = sp.prunable && std::isfinite(h.second.weight) && h.second.weight >= 0.0f;
-        // an AND reaches block_wand_intersection only when every term reads freqs (boolean_weight.rs:318-340); the two orders
-        // differ from the fourth scorer on, so fewer keep the kernels' plain loop
-        sp.intersection_order = op == TQ_OP_AND && sp.no_freq != 0 && sp.here.size() >= 4;
-        if (op == TQ_OP_BOOL) {
-          uint32_t dfs[TQ_MAX_TERMS];
-          float ws[TQ_MAX_TERMS];
-          for (size_t a = 0; a < sp.here.size(); ++a) { dfs[a] = sp.here[a].first; ws[a] = sp.here[a].second.weight; }
-          const int st = bool_structure(q, sp.term_idx.data(), dfs, ws, sp.here.size(), sp.no_freq, sp.bool_words, &sp.intersection_order);
-          if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
-          if (st == 0) { --n_plans; i = j; continue; }
-        }
-        i = j;
-      }
-      // ---- route: the shared-decode tile engine, or the per-query kernels -------------------------------------------------
-      bool on_tile = false;
-      const bool to_tile = repeat ? op == TQ_OP_BOOL : tile_on && (((c->tile_ops >> op) & 1u) || op == TQ_OP_BOOL) && (op != TQ_OP_TERM || terms_on_tile);
-      if (to_tile && n_plans) {
-        if (tgroups.empty() || (repeat == 2 && !tgroups.back().segs.empty())) tgroups.emplace_back();
-        // wide unions: every query brings its clause words, work-list entries and (mostly distinct) lists into the CTA's shared
-        // memory; smaller groups keep two CTAs per SM (configs[4]: 1.64 s -> 1.05 s per 512 20-term queries on 500M docs)
-        const uint32_t max_q = q.n_terms > 8 ? std::min(c->tile_max_queries, c->tile_wide_queries) : c->tile_max_queries;
-        bool fits = tile_admit_surely_fits(tgroups.back(), plans.data(), n_plans, c->tile_max_dens_x1000, c->tile_max_slots, max_q);
-        if (!fits) fits = tile_admit_cost(tgroups.back(), plans.data(), n_plans, c->tile_max_dens_x1000, c->tile_max_slots, max_q) >= 0;
-        if (!fits && !tgroups.back().segs.empty()) {  // the current group is full: open the next one
-          TileGroupBuild fresh;
-          if (tile_admit_cost(fresh, plans.data(), n_plans, c->tile_max_dens_x1000, c->tile_max_slots, max_q) >= 0) { tgroups.emplace_back(); fits = true; }
-        }
-        if (fits && tile_pairs_total + q_postings + 128ull * n_plans * q.n_terms <= tile_pair_budget) {
-          tile_pairs_total += tile_admit(tgroups.back(), (uint32_t)qi, op, plans.data(), n_plans);
-          on_tile = true;
-          // every doc at or above the running threshold is handed over: the sample launch and the k_theta passes keep that
-          // near k; a query that still overflows has the run repeated (flags[1], finalize_run).  A query hands each doc over at
-          // most once (every tile once per run, a doc once per (query, tile): by its first posting in the driving clauses), so
-          // its postings bound its candidates: the region of a repeat cannot overflow.
-          const uint32_t cand_floor = c->tile_cand_floor;  // (test hook: tiny regions overflow)
-          q_cands[qi] += repeat ? (size_t)q_postings
-                                : (size_t)std::min<uint64_t>(q_postings, std::max<uint64_t>((cand_floor >= 8192 ? 128ull : 1ull) * q.k, cand_floor));
-        }
-      }
-      if (on_tile) continue;
-      if (op == TQ_OP_BOOL && n_plans) return fail(TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL query does not fit the tile engine's buffers (split the batch / raise TQ_TILE_SCRATCH_MB)");
-      for (size_t pi = 0; pi < n_plans; ++pi) {
-        SegPlan& sp = plans[pi];
-        auto& here = sp.here;
-        QSeg qs;
-        memset(&qs, 0, sizeof(qs));
-        qs.query = (uint32_t)qi;
-        qs.lists_base = (uint32_t)qlists.size();
-        qs.segment_ord = sp.segment_ord;
-        qs.max_doc = sp.seg->max_doc;
-        qs.alive = sp.seg->d_alive;
-        qs.fieldnorm = sp.uniform_fn ? sp.fn0 : nullptr;
-        const bool prunable = sp.prunable && op != TQ_OP_TERM;
-        qs.flags = (sp.uniform_fn ? 1u : 0u) | (prunable ? 2u : 0u) | (sp.intersection_order ? 4u : 0u);
-        int unit_class = op == TQ_OP_PHRASE ? 7 : op;
-        if (op == TQ_OP_PHRASE) {
-          if (qaux.size() < qlists.size()) qaux.resize(qlists.size(), PhraseAux{0, 0, 0});
-          for (auto& h : here) { qaux.push_back(PhraseAux{h.second.pad, h.range_len, q.slop}); h.second.pad = 0; }
-          phrase_ct = std::max<uint32_t>(phrase_ct, (uint32_t)here.size());
-        }
-        if (op == TQ_OP_OR && c->or_strip && q.k <= kStripMaxK && here.size() <= kStripMaxLists) {
-          // strip kernel: clauses with less than one block per kWin-doc window keep their current block decoded in shared memory
-          uint32_t n_thin = 0;
-          static const uint64_t thin_mult = env_u32("TQ_STRIP_THIN_MULT", 1u);
-          auto is_thin = [&](uint32_t df) { return (uint64_t)df * (kWin / 128u) < (uint64_t)qs.max_doc * thin_mult; };
-          for (auto& h : here) if (is_thin(h.first)) ++n_thin;
-          if (n_thin <= kMaxCached) {
-            uint32_t slot = 0;
-            for (auto& h : here) h.second.pad = is_thin(h.first) ? (1u | (slot++ << 1)) : 0u;
-            strip_cached_max = std::max(strip_cached_max, n_thin);
-            unit_class = 3;
-          }
-        }
-        if (unit_class == TQ_OP_OR) or_max_lists = std::max<uint32_t>(or_max_lists, (uint32_t)here.size());
-        for (auto& h : here) qlists.push_back(h.second);
-        qs.n_lists = (uint32_t)here.size();
-        const uint32_t lead_total = here[0].first / 128u + ((here[0].first % 128u) ? 1u : 0u);
-        qsegs.push_back(qs);
-        qseg_op.push_back(unit_class);
-        {
-          bool any_thick = false;
-          for (auto& h : here) any_thick = any_thick || (uint64_t)h.first * std::max(c->strip_ne_div, c->strip_ne_div2) >= qs.max_doc;
-          qseg_sample.push_back(unit_class == 3 && prunable && any_thick);
-        }
-        qseg_total.push_back(unit_class == 3 ? (qs.max_doc + kWin - 1) / kWin : (op == TQ_OP_OR ? (qs.max_doc + kTileDocs - 1) / kTileDocs : lead_total));
-        ++n_qsegs_op[unit_class == 7 ? TQ_OP_AND : unit_class];
-      }
-    }
-    // Work units. A unit is one CTA's share of a (query, segment). With few (query, segment) pairs in the
-    // batch every pair is cut into many units (latency); with many, units grow so that a CTA's local
-    // top-k threshold gets tight and few candidates reach k_final (throughput).
-    const uint32_t target_units = c->target_units;
-    for (size_t s = 0; s < qsegs.size(); ++s) {
-      const int op = qseg_op[s];
-      const uint32_t total = qseg_total[s];
-      const uint32_t min_per = op == TQ_OP_TERM ? c->term_blocks_per_unit : ((op == TQ_OP_AND || op == 7) ? c->and_blocks_per_unit : (op == 3 ? kStripWarps * 64u : c->or_tiles_per_unit));
-      const uint32_t n_same = n_qsegs_op[op == 7 ? TQ_OP_AND : op];
-      const uint32_t want_units = std::max<uint32_t>(1u, (target_units + n_same - 1) / n_same);
-      const uint32_t per = std::max<uint32_t>(min_per, (total + want_units - 1) / want_units);
-      const uint32_t k = dq[qsegs[s].query].k;
-      // Threshold sample: the first 1/sample_div of a strip pair's windows run in a launch of their own; the exact k-th
-      // best score over all sampled windows of the query (k_theta) then seeds the threshold of the main launch, whose
-      // MaxScore split drops the dense clauses from the first window on.  Nothing is scored twice.
-      uint32_t first = 0;
-      if (op == 3 && qseg_sample[s] && c->strip_sample_div > 1 && total >= 8u * c->strip_sample_div) {
-        const uint32_t cut1 = std::max<uint32_t>(kStripWarps, total / c->strip_sample_div);
-        const uint32_t cut2 = c->strip_sample_div2 > 1 && c->strip_sample_div2 < c->strip_sample_div ? std::max(cut1, total / c->strip_sample_div2) : cut1;
-        const uint32_t cut3 = c->strip_sample_div3 > 1 && c->strip_sample_div3 < c->strip_sample_div2 ? std::max(cut2, total / c->strip_sample_div3) : cut2;
-        const uint32_t cuts[4] = {0, cut1, cut2, cut3};
-        for (int r = 0; r < 3; ++r)  // round r covers [cuts[r], cuts[r+1]); a k_theta pass follows each round
-          for (uint32_t b0 = cuts[r]; b0 < cuts[r + 1]; b0 += per) {
-            units[4 + r].push_back(Unit{(uint32_t)s, b0, std::min(cuts[r + 1], b0 + per), 0});
-            q_cands[qsegs[s].query] += (size_t)kStripWarps * k;
-          }
-        first = cut3;
-      }
-      for (uint32_t b0 = first; b0 < total; b0 += per) {
-        units[op].push_back(Unit{(uint32_t)s, b0, std::min(total, b0 + per), 0});
-        q_cands[qsegs[s].query] += op == 3 ? (size_t)kStripWarps * k : 2u * (size_t)k;  // what one unit may hand over
-      }
-    }
-    for (size_t qi = 0; qi < nq; ++qi) {
-      dq[qi].cand_base = (uint32_t)n_cands;
-      dq[qi].cand_cap = (uint32_t)q_cands[qi];
-      n_cands += q_cands[qi];
-      if (n_cands > 0xFFFFFFF0ull) return fail(TQ_ERR_UNSUPPORTED, "batch too large: split it");
-    }
-    int rc = flush_builds(c, pending, &built);
-    if (rc == TQ_OK) rc = flush_pos_builds(c, pending_pos);
-    if (rc != TQ_OK) return rc;
+int validate_query(const tq_ctx* c, const tq_query& q) {
+  if (q.k == 0 || q.k > TQ_MAX_K) return fail(TQ_ERR_INVALID_ARGUMENT, "k must be in 1..TQ_MAX_K");
+  if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
+  const bool is_bool = q.op == TQ_OP_BOOL;
+  if (is_bool && (c->tile == 0 || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
+  if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_PHRASE && !is_bool) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
+  if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
+  if (!q.weight || (!q.avg_fieldnorm && !q.tf_cache) || (!q.term_segs && q.n_term_segs)) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
+  if (q.op == TQ_OP_PHRASE) {
+    if (q.n_terms < 2 || q.n_terms > TQ_MAX_PHRASE_TERMS) return fail(TQ_ERR_UNSUPPORTED, "a phrase takes 2..TQ_MAX_PHRASE_TERMS terms on the device path");
+    // slop: two terms take intersection_count_with_slop on the device; three and more carry per-position slops through
+    // growing buffers (intersection_count_with_carrying_slop, phrase_scorer.rs:236-345) and stay on the reference's CPU path
+    if (q.slop != 0 && q.n_terms != 2) return fail(TQ_ERR_UNSUPPORTED, "phrase slop with more than two terms stays on the reference's CPU path");
+    if ((!q.term_pos && q.n_term_segs) || !q.term_offset) return fail(TQ_ERR_INVALID_ARGUMENT, "a phrase needs term_pos and term_offset");
   }
-  if (caches.empty()) caches.resize(256, 0.0f);
-  if (!qaux.empty() && qaux.size() < qlists.size()) qaux.resize(qlists.size(), PhraseAux{0, 0, 0});
+  return TQ_OK;
+}
 
-  // ---- tile groups: slot order, pair bases, score chunks, tile ranges of the launches -------------------------------------------
-  struct GroupStage {
-    std::vector<TSlot> slots;
-    std::vector<TSeg> segs;
-    std::vector<TQuery> queries;
-    std::vector<uint16_t> clauses;
-    std::vector<TUnit> units[kTileRounds];
-    std::vector<SChunk> chunks;
-    uint32_t max_slots = 1, p_cap = 1024, max_big = 1, max_queries = 1, max_clause_words = 0, max_clauses = 1;
-    size_t tix_words = 0;
-  };
-  std::vector<GroupStage> gstage(tgroups.size());
-  uint64_t pair_cursor = 0;
-  size_t tix_total_words = 0;
-  uint64_t tile_postings = 0, tile_units = 0;
+// The tf-norm table of every clause: its own rows of tf_cache, or the batch's table of its avg_fieldnorm.
+void tf_tables(BatchPlan& pl, const tq_query& q, uint32_t* cache_idx) {
+  for (uint32_t t = 0; t < q.n_terms; ++t) {
+    if (q.tf_cache) {
+      cache_idx[t] = (uint32_t)(pl.caches.size() / 256);
+      pl.caches.insert(pl.caches.end(), q.tf_cache + 256 * (size_t)t, q.tf_cache + 256 * (size_t)(t + 1));
+      continue;
+    }
+    uint32_t bits;
+    memcpy(&bits, &q.avg_fieldnorm[t], 4);
+    if (bits == pl.last_avg_bits && pl.last_avg_idx != 0xFFFFFFFFu) { cache_idx[t] = pl.last_avg_idx; continue; }  // (nearly always the same field)
+    auto it = pl.cache_by_avg.find(bits);
+    if (it == pl.cache_by_avg.end()) {
+      float tab[256];
+      bm25_tf_cache(q.avg_fieldnorm[t], tab);
+      it = pl.cache_by_avg.emplace(bits, (uint32_t)(pl.caches.size() / 256)).first;
+      pl.caches.insert(pl.caches.end(), tab, tab + 256);
+    }
+    cache_idx[t] = it->second;
+    pl.last_avg_bits = bits;
+    pl.last_avg_idx = it->second;
+  }
+}
+
+// The query's SegPlans (pl.plans[0, n_plans)): one per segment that can match, clauses in evaluation order.  ctx->mu held.
+int plan_segments(tq_ctx* c, BatchPlan& pl, const tq_query& q, int op, const uint32_t* cache_idx, uint64_t* q_postings) {
+  const bool is_phrase = op == TQ_OP_PHRASE;
+  pl.n_plans = 0;
+  return for_each_segment(q, pl.order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
+    for (size_t a = 1; a < n_here; ++a)
+      if (ts[a]->term_idx == ts[a - 1]->term_idx) return fail(TQ_ERR_INVALID_ARGUMENT, "duplicate (term_idx, segment_ord)");
+    if ((op == TQ_OP_AND || is_phrase) && n_here != q.n_terms) return TQ_OK;  // a clause is absent: empty intersection
+    if (pl.n_plans == pl.plans.size()) pl.plans.emplace_back();
+    SegPlan& sp = pl.plans[pl.n_plans++];
+    sp.here.clear();
+    sp.term_idx.clear();
+    sp.uniform_fn = true;
+    sp.no_freq = 0;
+    sp.segment_ord = ts[0]->segment_ord;
+    for (size_t a = 0; a < n_here; ++a) {
+      const tq_term_seg& t = *ts[a];
+      uint32_t id;
+      const bool ignore_freq = q.term_flags && (q.term_flags[t.term_idx] & TQ_TERM_IGNORE_FREQ);
+      int rc = get_list(c, t, ignore_freq, pl.pending, &id, &sp.seg);
+      if (rc != TQ_OK) return rc;
+      if (ignore_freq || sp.seg->record_option == TQ_RECORD_BASIC) sp.no_freq |= 1u << a;
+      if (a == 0) sp.fn0 = sp.seg->d_fieldnorm; else sp.uniform_fn &= (sp.seg->d_fieldnorm == sp.fn0);
+      const uint32_t tw = is_phrase ? 0 : t.term_idx;
+      QList ql{id, q.weight[tw], cache_idx[tw], 0};
+      if (is_phrase) {  // the clause's position table; QList.pad carries its id to the aux array (append_qsegs)
+        if (sp.seg->record_option != TQ_RECORD_FREQS_POSITIONS) return fail(TQ_ERR_INVALID_ARGUMENT, "phrase query on a field without positions");
+        rc = get_pos(c, t, q.term_pos[ts[a] - q.term_segs], pl.pending_pos, &ql.pad);
+        if (rc != TQ_OK) return rc;
+      }
+      const uint64_t range = t.postings_end - t.postings_start;
+      sp.here.push_back(SegPlan::Clause{t.doc_freq, ql, (uint32_t)range});
+      sp.term_idx.push_back(t.term_idx);
+      pl.alg_bytes += range + t.doc_freq;
+      pl.op_bytes[bytes_class(op)] += range + t.doc_freq;
+      pl.postings += t.doc_freq;
+      *q_postings += t.doc_freq;
+    }
+    auto by_doc_freq = [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.first < b.first; };
+    if (is_phrase) {
+      // PhraseScorer keeps its terms by ascending size_hint (intersection.rs:40-52); every clause carries
+      // (max_offset - its offset), the shift that lines the terms' positions up (phrase_scorer.rs:349-398)
+      uint32_t max_offset = 0;
+      for (uint32_t t = 0; t < q.n_terms; ++t) max_offset = std::max(max_offset, q.term_offset[t]);
+      for (size_t a = 0; a < sp.here.size(); ++a) sp.here[a].range_len = max_offset - q.term_offset[sp.term_idx[a]];  // (range_len is free here)
+      std::stable_sort(sp.here.begin(), sp.here.end(), by_doc_freq);
+    }
+    if (op == TQ_OP_AND)  // leader = rarest, then ascending doc_freq; stable (block_wand_intersection.rs:27)
+      std::stable_sort(sp.here.begin(), sp.here.end(), by_doc_freq);
+    if (op == TQ_OP_OR)
+      // Canonical union order = descending Bm25Weight.weight, ties in clause order (the reference's own order is
+      // data dependent, block_wand_union.rs:205-208): the f32 sum is taken in this order, and the clauses with the
+      // smallest score bounds form a suffix, which is what the MaxScore splits of k_tile / k_or_strip need.
+      std::stable_sort(sp.here.begin(), sp.here.end(), [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.second.weight > b.second.weight; });
+    sp.prunable = true;
+    for (auto& h : sp.here) sp.prunable = sp.prunable && std::isfinite(h.second.weight) && h.second.weight >= 0.0f;
+    // an AND reaches block_wand_intersection only when every term reads freqs (boolean_weight.rs:318-340); the two orders
+    // differ from the fourth scorer on, so fewer keep the kernels' plain loop
+    sp.intersection_order = op == TQ_OP_AND && sp.no_freq != 0 && sp.here.size() >= 4;
+    if (op == TQ_OP_BOOL) {
+      uint32_t dfs[TQ_MAX_TERMS];
+      float ws[TQ_MAX_TERMS];
+      for (size_t a = 0; a < sp.here.size(); ++a) { dfs[a] = sp.here[a].first; ws[a] = sp.here[a].second.weight; }
+      const int st = bool_structure(q, sp.term_idx.data(), dfs, ws, sp.here.size(), sp.no_freq, sp.bool_words, &sp.intersection_order);
+      if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
+      if (st == 0) --pl.n_plans;
+    }
+    return TQ_OK;
+  });
+}
+
+// Puts query qi into a tile group if the tile engine takes it and it fits; false: it runs on the per-query kernels.
+bool route_to_tile(const tq_ctx* c, BatchPlan& pl, size_t qi, int op, uint64_t q_postings) {
+  const tq_query& q = pl.queries[qi];
+  const bool to_tile = pl.repeat ? op == TQ_OP_BOOL
+                                 : c->tile != 0 && (((c->tile_ops >> op) & 1u) || op == TQ_OP_BOOL) && (op != TQ_OP_TERM || pl.terms_on_tile);
+  if (!to_tile || !pl.n_plans) return false;
+  std::vector<TileGroupBuild>& tg = pl.tgroups;
+  if (tg.empty() || (pl.repeat == 2 && !tg.back().segs.empty())) tg.emplace_back();
+  // wide unions: every query brings its clause words, work-list entries and (mostly distinct) lists into the CTA's shared
+  // memory; smaller groups keep two CTAs per SM (configs[4]: 1.64 s -> 1.05 s per 512 20-term queries on 500M docs)
+  const uint32_t max_q = q.n_terms > 8 ? std::min(c->tile_max_queries, c->tile_wide_queries) : c->tile_max_queries;
+  const SegPlan* plans = pl.plans.data();
+  bool fits = tile_fits(c, tg.back(), plans, pl.n_plans, max_q, false) || tile_fits(c, tg.back(), plans, pl.n_plans, max_q, true);
+  if (!fits && !tg.back().segs.empty() && tile_fits(c, TileGroupBuild{}, plans, pl.n_plans, max_q, false)) {  // the current group is full: open the next one
+    tg.emplace_back();
+    fits = true;
+  }
+  const uint64_t tile_pair_budget = (uint64_t)c->tile_scratch_mb * (1u << 20) / 8u;
+  if (!fits || pl.tile_pairs_total + q_postings + 128ull * pl.n_plans * q.n_terms > tile_pair_budget) return false;
+  pl.tile_pairs_total += tile_admit(tg.back(), (uint32_t)qi, op, plans, pl.n_plans);
+  // every doc at or above the running threshold is handed over: the sample launch and the k_theta passes keep that
+  // near k; a query that still overflows has the run repeated (flags[1], finalize_run).  A query hands each doc over at
+  // most once (every tile once per run, a doc once per (query, tile): by its first posting in the driving clauses), so
+  // its postings bound its candidates: the region of a repeat cannot overflow.
+  const uint32_t cand_floor = c->tile_cand_floor;  // (test hook: tiny regions overflow)
+  pl.q_cands[qi] += pl.repeat ? (size_t)q_postings
+                              : (size_t)std::min<uint64_t>(q_postings, std::max<uint64_t>((cand_floor >= 8192 ? 128ull : 1ull) * q.k, cand_floor));
+  return true;
+}
+
+// The (query, segment) pairs of query qi on the per-query kernels: QSeg, clause lists, unit class.
+void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
+  const tq_query& q = pl.queries[qi];
+  for (size_t pi = 0; pi < pl.n_plans; ++pi) {
+    SegPlan& sp = pl.plans[pi];
+    auto& here = sp.here;
+    QSeg qs;
+    memset(&qs, 0, sizeof(qs));
+    qs.query = (uint32_t)qi;
+    qs.lists_base = (uint32_t)pl.qlists.size();
+    qs.segment_ord = sp.segment_ord;
+    qs.max_doc = sp.seg->max_doc;
+    qs.alive = sp.seg->d_alive;
+    qs.fieldnorm = sp.uniform_fn ? sp.fn0 : nullptr;
+    const bool prunable = sp.prunable && op != TQ_OP_TERM;
+    qs.flags = (sp.uniform_fn ? 1u : 0u) | (prunable ? 2u : 0u) | (sp.intersection_order ? 4u : 0u);
+    UnitClass cls = op == TQ_OP_PHRASE ? UC_PHRASE : (UnitClass)op;
+    if (op == TQ_OP_PHRASE) {
+      if (pl.qaux.size() < pl.qlists.size()) pl.qaux.resize(pl.qlists.size(), PhraseAux{0, 0, 0});
+      for (auto& h : here) { pl.qaux.push_back(PhraseAux{h.second.pad, h.range_len, q.slop}); h.second.pad = 0; }
+      pl.phrase_ct = std::max<uint32_t>(pl.phrase_ct, (uint32_t)here.size());
+    }
+    if (op == TQ_OP_OR && c->or_strip && q.k <= kStripMaxK && here.size() <= kStripMaxLists) {
+      // strip kernel: clauses with less than one block per kWin-doc window keep their current block decoded in shared memory
+      uint32_t n_thin = 0;
+      static const uint64_t thin_mult = env_u32("TQ_STRIP_THIN_MULT", 1u);
+      auto is_thin = [&](uint32_t df) { return (uint64_t)df * (kWin / 128u) < (uint64_t)qs.max_doc * thin_mult; };
+      for (auto& h : here) if (is_thin(h.first)) ++n_thin;
+      if (n_thin <= kMaxCached) {
+        uint32_t slot = 0;
+        for (auto& h : here) h.second.pad = is_thin(h.first) ? (1u | (slot++ << 1)) : 0u;
+        pl.strip_cached_max = std::max(pl.strip_cached_max, n_thin);
+        cls = UC_STRIP;
+      }
+    }
+    if (cls == UC_OR_WINDOW) pl.or_max_lists = std::max<uint32_t>(pl.or_max_lists, (uint32_t)here.size());
+    for (auto& h : here) pl.qlists.push_back(h.second);
+    qs.n_lists = (uint32_t)here.size();
+    const uint32_t lead_total = here[0].first / 128u + ((here[0].first % 128u) ? 1u : 0u);
+    pl.qsegs.push_back(qs);
+    bool any_thick = false;
+    for (auto& h : here) any_thick = any_thick || (uint64_t)h.first * std::max(c->strip_ne_div, c->strip_ne_div2) >= qs.max_doc;
+    const uint32_t total = cls == UC_STRIP ? (qs.max_doc + kWin - 1) / kWin : (op == TQ_OP_OR ? (qs.max_doc + kTileDocs - 1) / kTileDocs : lead_total);
+    pl.work.push_back(SegWork{cls, total, cls == UC_STRIP && prunable && any_thick});
+    ++pl.n_qsegs_op[cls == UC_PHRASE ? UC_AND : cls];
+  }
+}
+
+// Validates query qi and plans it: into a tile group, or onto the per-query kernels.  ctx->mu held.
+int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi) {
+  const tq_query& q = pl.queries[qi];
+  int rc = validate_query(c, q);
+  if (rc != TQ_OK) return rc;
+  // effective shape: an AND / OR of one clause is that clause (boolean_weight.rs:57-68, block_wand_union.rs:154-157)
+  const int op = q.op == TQ_OP_PHRASE ? TQ_OP_PHRASE : (q.op == TQ_OP_BOOL ? TQ_OP_BOOL : (q.n_terms == 1 ? TQ_OP_TERM : q.op));
+  pl.kmax = std::max(pl.kmax, q.k);
+  pl.alg_bytes += 12ull * q.k;
+  pl.op_bytes[bytes_class(op)] += 12ull * q.k;
+  uint32_t cache_idx[TQ_MAX_TERMS];
+  tf_tables(pl, q, cache_idx);
+  pl.dq[qi].k = q.k;
+  pl.dq[qi].op = (uint32_t)op;
+  uint64_t q_postings = 0;
+  rc = plan_segments(c, pl, q, op, cache_idx, &q_postings);
+  if (rc != TQ_OK) return rc;
+  if (route_to_tile(c, pl, qi, op, q_postings)) return TQ_OK;
+  if (op == TQ_OP_BOOL && pl.n_plans) return fail(TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL query does not fit the tile engine's buffers (split the batch / raise TQ_TILE_SCRATCH_MB)");
+  append_qsegs(c, pl, qi, op);
+  return TQ_OK;
+}
+
+// Work units. A unit is one CTA's share of a (query, segment). With few (query, segment) pairs in the
+// batch every pair is cut into many units (latency); with many, units grow so that a CTA's local
+// top-k threshold gets tight and few candidates reach k_final (throughput).  Then the candidate regions follow.
+int cut_units(const tq_ctx* c, BatchPlan& pl) {
+  const uint32_t target_units = c->target_units;
+  for (size_t s = 0; s < pl.qsegs.size(); ++s) {
+    const SegWork& w = pl.work[s];
+    const uint32_t total = w.total;
+    const uint32_t min_per = w.cls == UC_TERM ? c->term_blocks_per_unit
+                             : ((w.cls == UC_AND || w.cls == UC_PHRASE) ? c->and_blocks_per_unit : (w.cls == UC_STRIP ? kStripWarps * 64u : c->or_tiles_per_unit));
+    const uint32_t n_same = pl.n_qsegs_op[w.cls == UC_PHRASE ? UC_AND : w.cls];
+    const uint32_t want_units = std::max<uint32_t>(1u, (target_units + n_same - 1) / n_same);
+    const uint32_t per = std::max<uint32_t>(min_per, (total + want_units - 1) / want_units);
+    const uint32_t query = pl.qsegs[s].query, k = pl.dq[query].k;
+    // Threshold sample: the first 1/sample_div of a strip pair's windows run in a launch of their own; the exact k-th
+    // best score over all sampled windows of the query (k_theta) then seeds the threshold of the main launch, whose
+    // MaxScore split drops the dense clauses from the first window on.  Nothing is scored twice.
+    uint32_t first = 0;
+    if (w.cls == UC_STRIP && w.sample && c->strip_sample_div > 1 && total >= 8u * c->strip_sample_div) {
+      const uint32_t cut1 = std::max<uint32_t>(kStripWarps, total / c->strip_sample_div);
+      const uint32_t cut2 = c->strip_sample_div2 > 1 && c->strip_sample_div2 < c->strip_sample_div ? std::max(cut1, total / c->strip_sample_div2) : cut1;
+      const uint32_t cut3 = c->strip_sample_div3 > 1 && c->strip_sample_div3 < c->strip_sample_div2 ? std::max(cut2, total / c->strip_sample_div3) : cut2;
+      const uint32_t cuts[4] = {0, cut1, cut2, cut3};
+      for (int r = 0; r < 3; ++r)  // round r covers [cuts[r], cuts[r+1]); a k_theta pass follows each round
+        for (uint32_t b0 = cuts[r]; b0 < cuts[r + 1]; b0 += per) {
+          pl.units[UC_STRIP_ROUND1 + r].push_back(Unit{(uint32_t)s, b0, std::min(cuts[r + 1], b0 + per), 0});
+          pl.q_cands[query] += (size_t)kStripWarps * k;
+        }
+      first = cut3;
+    }
+    for (uint32_t b0 = first; b0 < total; b0 += per) {
+      pl.units[w.cls].push_back(Unit{(uint32_t)s, b0, std::min(total, b0 + per), 0});
+      pl.q_cands[query] += w.cls == UC_STRIP ? (size_t)kStripWarps * k : 2u * (size_t)k;  // what one unit may hand over
+    }
+  }
+  for (size_t qi = 0; qi < pl.nq; ++qi) {
+    pl.dq[qi].cand_base = (uint32_t)pl.n_cands;
+    pl.dq[qi].cand_cap = (uint32_t)pl.q_cands[qi];
+    pl.n_cands += pl.q_cands[qi];
+    if (pl.n_cands > 0xFFFFFFF0ull) return fail(TQ_ERR_UNSUPPORTED, "batch too large: split it");
+  }
+  return TQ_OK;
+}
+
+// Tile groups: slot order, pair bases, score chunks, tile ranges of the launches.
+int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
+  pl.gstage.resize(pl.tgroups.size());
   const uint32_t big_min = c->tile_big_min;
-  for (size_t gi = 0; gi < tgroups.size(); ++gi) {
-    TileGroupBuild& tg = tgroups[gi];
-    GroupStage& gs = gstage[gi];
+  for (size_t gi = 0; gi < pl.tgroups.size(); ++gi) {
+    TileGroupBuild& tg = pl.tgroups[gi];
+    GroupStage& gs = pl.gstage[gi];
     double dens_max = 0;
     uint64_t tiles_total = 0;
     uint32_t kmax_g = 1;
@@ -1273,38 +1362,32 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
       for (uint32_t i = 0; i < perm.size(); ++i) {
         TSlot sl = sb.slots[perm[i]];
         sl.tseg = (uint32_t)gs.segs.size();
-        sl.pair_base = (uint32_t)pair_cursor;
+        sl.pair_base = (uint32_t)pl.pair_cursor;
         if (is_big(sl) && n_big < kTileMaxBig) sl.big = n_big++;  // (the densest ones: the order above is by descending doc_freq)
         const uint32_t n_total = sl.doc_freq / 128u + ((sl.doc_freq % 128u) ? 1u : 0u);
         for (uint32_t b0 = 0; b0 < n_total; b0 += 64u) gs.chunks.push_back(SChunk{(uint32_t)gs.slots.size(), b0, std::min(n_total, b0 + 64u)});
-        pair_cursor += ((uint64_t)sl.doc_freq + 127) / 128 * 128;
-        tile_postings += sl.doc_freq;
+        pl.pair_cursor += ((uint64_t)sl.doc_freq + 127) / 128 * 128;
+        pl.tile_postings += sl.doc_freq;
         gs.slots.push_back(sl);
       }
       G.n_big = n_big;
-      G.tix = reinterpret_cast<uint32_t*>(tix_total_words + gs.tix_words);  // offset for now, rebased below
+      G.tix = reinterpret_cast<uint32_t*>(pl.tix_total_words + gs.tix_words);  // offset for now, rebased in lay_out
       gs.tix_words += (size_t)(G.n_tiles + 1) * n_big;
       const uint32_t clause_shift = (uint32_t)gs.clauses.size();
       G.clause_base = clause_shift;
       G.n_clause_words = (uint32_t)sb.clauses.size();
       gs.max_clause_words = std::max(gs.max_clause_words, G.n_clause_words);
+      gs.clauses.insert(gs.clauses.end(), sb.clauses.begin(), sb.clauses.end());
       for (auto& tq : sb.queries) {
         TQuery t2 = tq;
         t2.clause_base += clause_shift;
         gs.queries.push_back(t2);
-        kmax_g = std::max(kmax_g, dq[tq.query].k);
+        kmax_g = std::max(kmax_g, pl.dq[tq.query].k);
         gs.max_clauses = std::max<uint32_t>(gs.max_clauses, tq.n_clauses);
-      }
-      {  // clause slots follow the permutation (the structure words of TQ_OP_BOOL queries do not)
-        const size_t c0 = gs.clauses.size();
-        for (uint16_t cl : sb.clauses) gs.clauses.push_back(cl);
-        for (auto& tq : sb.queries) {
-          uint16_t* w = gs.clauses.data() + c0 + tq.clause_base;
-          if (tq.op != kTileOpBool) { for (uint32_t e = 0; e < tq.n_clauses; ++e) w[e] = (uint16_t)new_of[w[e]]; continue; }
-          size_t x = 4;
-          for (uint32_t g = 0; g < w[0]; ++g) { const uint16_t len = w[x++]; for (uint16_t e = 0; e < len; ++e, ++x) w[x] = (uint16_t)new_of[w[x]]; }
-          for (; x < tq.n_clauses; ++x) w[x] = (uint16_t)new_of[w[x]];
-        }
+        // clause slots follow the permutation (the structure words of TQ_OP_BOOL queries do not)
+        uint16_t* w = gs.clauses.data() + t2.clause_base;
+        if (tq.op == kTileOpBool) map_bool_clauses(w, tq.n_clauses, [&](uint16_t s) { return new_of[s]; });
+        else for (uint32_t e = 0; e < tq.n_clauses; ++e) w[e] = (uint16_t)new_of[w[e]];
       }
       gs.max_slots = std::max(gs.max_slots, G.n_slots);
       gs.max_big = std::max(gs.max_big, G.n_big);
@@ -1313,11 +1396,11 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
       tiles_total += sb.t_hi - sb.t_lo;
       gs.segs.push_back(G);
     }
-    tix_total_words += gs.tix_words;
+    pl.tix_total_words += gs.tix_words;
     gs.p_cap = (uint32_t)std::min<double>(kTileMaxPairs, std::max(1024.0, dens_max * kTile * 1.25 + 192.0));
     gs.p_cap = (gs.p_cap + 63u) & ~63u;
     if (c->tile_pcap_hook) gs.p_cap = c->tile_pcap_hook;  // (test hook: overflowing tiles)
-    if (repeat) gs.p_cap = kTileMaxPairs;  // the repeat of an overflowed run: the largest tile buffer there is
+    if (pl.repeat) gs.p_cap = kTileMaxPairs;  // the repeat of an overflowed run: the largest tile buffer there is
     // Launches: [0] samples scores on a spread of short tile runs, [1..3] are exact and cover every tile once.
     const uint32_t target = std::max(1u, c->tile_units);
     const uint32_t sample_div = std::max<uint32_t>(2u, c->tile_sample_div);
@@ -1348,125 +1431,98 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
         for (uint32_t t0 = cuts[r]; t0 < cuts[r + 1]; t0 += per) gs.units[1 + r].push_back(TUnit{si, tl + t0, tl + std::min(cuts[r + 1], t0 + per), 0});
       }
     }
-    for (int r = 0; r < kTileRounds; ++r) tile_units += gs.units[r].size();
+    for (int r = 0; r < kTileRounds; ++r) pl.tile_units += gs.units[r].size();
   }
-  if (pair_cursor > 0xFFFFFF00ull) return fail(TQ_ERR_UNSUPPORTED, "batch decodes more than 4G postings: split it");
+  if (pl.pair_cursor > 0xFFFFFF00ull) return fail(TQ_ERR_UNSUPPORTED, "batch decodes more than 4G postings: split it");
+  return TQ_OK;
+}
 
-  // ---- stage descriptors -------------------------------------------------------------------------
-  auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t off = 0;
-  const size_t o_caches = off; off = align(off + caches.size() * 4);
-  const size_t n_caches = caches.size() / 256;
-  const size_t o_tftab = off; off = align(off + n_caches * kTfRows * 256 * 4);  // device only (built by k_build_tf_tables)
-  const size_t o_qlists = off; off = align(off + qlists.size() * sizeof(QList));
-  const size_t o_qsegs = off; off = align(off + qsegs.size() * sizeof(QSeg));
-  const size_t o_qaux = off; off = align(off + qaux.size() * sizeof(PhraseAux));
-  const size_t n_units_total = units[0].size() + units[1].size() + units[2].size() + units[3].size() + units[4].size() + units[5].size() + units[6].size() + units[7].size();
-  b->strip_cached_max = strip_cached_max;
-  b->or_max_lists = or_max_lists;
-  b->phrase_ct = std::min<uint32_t>(phrase_ct, kPhraseMaxTerms);
-  const size_t o_units = off; off = align(off + n_units_total * sizeof(Unit));
-  const size_t o_queries = off; off = align(off + dq.size() * sizeof(DQuery));
-  const size_t o_qinit = off; off = align(off + std::max<size_t>(nq, 1) * sizeof(QState));  // per-run initial state (threshold keys)
-  struct GroupOff { size_t slots, segs, queries, clauses, units, chunks; };
-  std::vector<GroupOff> goff(gstage.size());
-  for (size_t gi = 0; gi < gstage.size(); ++gi) {
-    GroupStage& gs = gstage[gi];
-    size_t nu = 0;
-    for (int r = 0; r < kTileRounds; ++r) nu += gs.units[r].size();
-    goff[gi].slots = off; off = align(off + gs.slots.size() * sizeof(TSlot));
-    goff[gi].segs = off; off = align(off + gs.segs.size() * sizeof(TSeg));
-    goff[gi].queries = off; off = align(off + gs.queries.size() * sizeof(TQuery));
-    goff[gi].clauses = off; off = align(off + gs.clauses.size() * 2);
-    goff[gi].units = off; off = align(off + nu * sizeof(TUnit));
-    goff[gi].chunks = off; off = align(off + gs.chunks.size() * sizeof(SChunk));
+// One array of units out of per-class lists; class i starts at base[i] and has n[i] units.
+template <class U, size_t N>
+std::vector<U> concat_units(const std::vector<U> (&by_class)[N], uint32_t* base, uint32_t* n) {
+  std::vector<U> all;
+  for (size_t i = 0; i < N; ++i) {
+    base[i] = (uint32_t)all.size();
+    n[i] = (uint32_t)by_class[i].size();
+    all.insert(all.end(), by_class[i].begin(), by_class[i].end());
   }
-  b->desc_bytes = off;
-  TQ_CUDA(b->pin.ensure(off + 256));
-  TQ_CUDA(b->dev.ensure(off + 256));
+  return all;
+}
+
+// Stages the descriptors, sizes the tile and run scratch, fills BatchParams / TileParams, starts the upload and tf-table build.
+int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
+  if (pl.caches.empty()) pl.caches.resize(256, 0.0f);
+  if (!pl.qaux.empty() && pl.qaux.size() < pl.qlists.size()) pl.qaux.resize(pl.qlists.size(), PhraseAux{0, 0, 0});
+  const size_t nq = pl.nq, nq1 = std::max<size_t>(nq, 1), n_caches = pl.caches.size() / 256;
+  const std::vector<Unit> units = concat_units(pl.units, b->unit_base, b->n_units);
+  Staging st;
+  const size_t o_caches = st.add(pl.caches);
+  const size_t o_tftab = st.add(nullptr, n_caches * kTfRows * 256 * 4);  // device only (built by k_build_tf_tables)
+  const size_t o_qlists = st.add(pl.qlists), o_qsegs = st.add(pl.qsegs), o_qaux = st.add(pl.qaux), o_units = st.add(units);
+  const size_t o_queries = st.add(pl.dq);
+  const size_t o_qinit = st.add(nullptr, nq1 * sizeof(QState));  // per-run initial state (threshold keys), filled below
+  struct GroupOff { size_t slots, segs, queries, clauses, units, chunks; };
+  std::vector<GroupOff> goff(pl.gstage.size());
+  std::vector<std::vector<TUnit>> gunits(pl.gstage.size());
+  b->groups.resize(pl.gstage.size());
+  for (size_t gi = 0; gi < pl.gstage.size(); ++gi) {
+    const GroupStage& gs = pl.gstage[gi];
+    gunits[gi] = concat_units(gs.units, b->groups[gi].unit_base, b->groups[gi].n_units);
+    goff[gi] = GroupOff{st.add(gs.slots), st.add(gs.segs), st.add(gs.queries), st.add(gs.clauses), st.add(gunits[gi]), st.add(gs.chunks)};
+  }
+  b->desc_bytes = st.bytes;
+  TQ_CUDA(st.reserve(b->pin, b->dev));
 
   // ---- tile scratch: pair arrays | tile indexes | samples | sample counts | flags + counters --------------------------------
   uint32_t sample_cap = 0;
-  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0, tile_bytes = 0;
-  if (!gstage.empty()) {
+  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0;
+  if (!pl.gstage.empty()) {
     uint64_t sample_units_tiles = 0;
-    for (auto& gs : gstage) for (auto& u : gs.units[0]) sample_units_tiles += u.t1 - u.t0;
+    for (auto& gs : pl.gstage) for (auto& u : gs.units[0]) sample_units_tiles += u.t1 - u.t0;
     sample_cap = (uint32_t)std::min<uint64_t>(1u << 16, std::max<uint64_t>(256, sample_units_tiles * 8u));
     size_t so2 = 0;
-    to_docs = so2; so2 = align(so2 + (size_t)pair_cursor * 4);
-    to_scores = so2; so2 = align(so2 + (size_t)pair_cursor * 4);
-    to_tix = so2; so2 = align(so2 + tix_total_words * 4);
-    to_samples = so2; so2 = align(so2 + (size_t)std::max<size_t>(nq, 1) * sample_cap * 4);
-    to_scount = so2; so2 = align(so2 + std::max<size_t>(nq, 1) * 4);
-    to_flags = so2; so2 = align(so2 + 256);
-    tile_bytes = so2;
-    TQ_CUDA(b->tile_dev.ensure(tile_bytes));
+    to_docs = so2; so2 = align256(so2 + (size_t)pl.pair_cursor * 4);
+    to_scores = so2; so2 = align256(so2 + (size_t)pl.pair_cursor * 4);
+    to_tix = so2; so2 = align256(so2 + pl.tix_total_words * 4);
+    to_samples = so2; so2 = align256(so2 + nq1 * sample_cap * 4);
+    to_scount = so2; so2 = align256(so2 + nq1 * 4);
+    to_flags = so2; so2 = align256(so2 + 256);
+    pl.tile_bytes = so2;
+    TQ_CUDA(b->tile_dev.ensure(pl.tile_bytes));
   }
   b->tile_zero_off = to_scount;
-  b->tile_zero_bytes = gstage.empty() ? 0 : (to_flags + 256 - to_scount);
+  b->tile_zero_bytes = pl.gstage.empty() ? 0 : (to_flags + 256 - to_scount);
   b->tile_flags_off = to_flags;
+  for (auto& gs : pl.gstage)  // rebase the tile-index offsets to device addresses
+    for (auto& G : gs.segs) G.tix = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_tix) + reinterpret_cast<size_t>(G.tix);
 
-  memcpy(b->pin.p + o_caches, caches.data(), caches.size() * 4);
-  if (!qlists.empty()) memcpy(b->pin.p + o_qlists, qlists.data(), qlists.size() * sizeof(QList));
-  if (!qsegs.empty()) memcpy(b->pin.p + o_qsegs, qsegs.data(), qsegs.size() * sizeof(QSeg));
-  if (!qaux.empty()) memcpy(b->pin.p + o_qaux, qaux.data(), qaux.size() * sizeof(PhraseAux));
-  b->phrase_aux = reinterpret_cast<const PhraseAux*>(b->dev.p + o_qaux);
-  {
-    Unit* u = reinterpret_cast<Unit*>(b->pin.p + o_units);
-    uint32_t base = 0;
-    for (int op = 0; op < 8; ++op) {
-      b->unit_base[op] = base;
-      b->n_units[op] = (uint32_t)units[op].size();
-      if (!units[op].empty()) memcpy(u + base, units[op].data(), units[op].size() * sizeof(Unit));
-      base += (uint32_t)units[op].size();
-    }
-  }
-  if (!dq.empty()) memcpy(b->pin.p + o_queries, dq.data(), dq.size() * sizeof(DQuery));
-  {
-    QState* qi0 = reinterpret_cast<QState*>(b->pin.p + o_qinit);
-    for (size_t qi = 0; qi < std::max<size_t>(nq, 1); ++qi) {
-      qi0[qi].theta = 0; qi0[qi].cand_count = 0;
-      if (qi < nq && (queries[qi].flags & TQ_QUERY_HAS_THRESHOLD)) {
-        // collect score > threshold: the smallest accepted key is the next representable score (NaN: no filter)
-        float th = queries[qi].threshold;
-        if (th == 0.0f) th = 0.0f;  // -0.0 and +0.0 are the same threshold
-        if (th == th) { const uint32_t key = host_score_key(th); qi0[qi].theta = key == 0xFFFFFFFFu ? key : key + 1u; }
-      }
+  st.copy();
+  QState* qi0 = st.on_host<QState>(o_qinit);
+  for (size_t qi = 0; qi < nq1; ++qi) {
+    qi0[qi].theta = 0; qi0[qi].cand_count = 0;
+    if (qi < nq && (pl.queries[qi].flags & TQ_QUERY_HAS_THRESHOLD)) {
+      // collect score > threshold: the smallest accepted key is the next representable score (NaN: no filter)
+      float th = pl.queries[qi].threshold;
+      if (th == 0.0f) th = 0.0f;  // -0.0 and +0.0 are the same threshold
+      if (th == th) { const uint32_t key = host_score_key(th); qi0[qi].theta = key == 0xFFFFFFFFu ? key : key + 1u; }
     }
   }
   b->qinit_off = o_qinit;
-  size_t tix_cursor = 0;
-  for (size_t gi = 0; gi < gstage.size(); ++gi) {
-    GroupStage& gs = gstage[gi];
-    tq_batch::TileGroup run;
-    for (auto& G : gs.segs) {  // rebase the tile-index offsets to device addresses
-      const size_t w = reinterpret_cast<size_t>(G.tix);
-      G.tix = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_tix) + w;
-    }
-    tix_cursor += gs.tix_words;
-    if (!gs.slots.empty()) memcpy(b->pin.p + goff[gi].slots, gs.slots.data(), gs.slots.size() * sizeof(TSlot));
-    if (!gs.segs.empty()) memcpy(b->pin.p + goff[gi].segs, gs.segs.data(), gs.segs.size() * sizeof(TSeg));
-    if (!gs.queries.empty()) memcpy(b->pin.p + goff[gi].queries, gs.queries.data(), gs.queries.size() * sizeof(TQuery));
-    if (!gs.clauses.empty()) memcpy(b->pin.p + goff[gi].clauses, gs.clauses.data(), gs.clauses.size() * 2);
-    {
-      TUnit* u = reinterpret_cast<TUnit*>(b->pin.p + goff[gi].units);
-      uint32_t base = 0;
-      for (int r = 0; r < kTileRounds; ++r) {
-        run.unit_base[r] = base;
-        run.n_units[r] = (uint32_t)gs.units[r].size();
-        if (!gs.units[r].empty()) memcpy(u + base, gs.units[r].data(), gs.units[r].size() * sizeof(TUnit));
-        base += (uint32_t)gs.units[r].size();
-      }
-    }
-    if (!gs.chunks.empty()) memcpy(b->pin.p + goff[gi].chunks, gs.chunks.data(), gs.chunks.size() * sizeof(SChunk));
+  b->phrase_aux = st.on_device<const PhraseAux>(o_qaux);
+  b->strip_cached_max = pl.strip_cached_max;
+  b->or_max_lists = pl.or_max_lists;
+  b->phrase_ct = std::min<uint32_t>(pl.phrase_ct, kPhraseMaxTerms);
+  for (size_t gi = 0; gi < pl.gstage.size(); ++gi) {
+    const GroupStage& gs = pl.gstage[gi];
+    tq_batch::TileGroup& run = b->groups[gi];
     run.n_chunks = (uint32_t)gs.chunks.size();
     TileParams& TP = run.params;
-    TP.slots = reinterpret_cast<const TSlot*>(b->dev.p + goff[gi].slots);
-    TP.segs = reinterpret_cast<const TSeg*>(b->dev.p + goff[gi].segs);
-    TP.queries = reinterpret_cast<const TQuery*>(b->dev.p + goff[gi].queries);
-    TP.clauses = reinterpret_cast<const uint16_t*>(b->dev.p + goff[gi].clauses);
-    TP.units = reinterpret_cast<const TUnit*>(b->dev.p + goff[gi].units);
-    TP.chunks = reinterpret_cast<const SChunk*>(b->dev.p + goff[gi].chunks);
+    TP.slots = st.on_device<const TSlot>(goff[gi].slots);
+    TP.segs = st.on_device<const TSeg>(goff[gi].segs);
+    TP.queries = st.on_device<const TQuery>(goff[gi].queries);
+    TP.clauses = st.on_device<const uint16_t>(goff[gi].clauses);
+    TP.units = st.on_device<const TUnit>(goff[gi].units);
+    TP.chunks = st.on_device<const SChunk>(goff[gi].chunks);
     TP.p_docs = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_docs);
     TP.p_scores = reinterpret_cast<float*>(b->tile_dev.p + to_scores);
     TP.samples = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_samples);
@@ -1488,79 +1544,38 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
     run.smem = tile_smem_bytes(gs.p_cap, gs.max_slots, TP.max_big, TP.max_queries, TP.seg_cap, TP.cl_cap, TP.n_win);
     c->tile_smem_last = run.smem;
     if (run.smem > 200u * 1024u) return fail(TQ_ERR_UNSUPPORTED, "tile group needs more shared memory than an SM has");
-    b->groups.push_back(run);
-  }
-  (void)tix_cursor;
-  if (!b->groups.empty()) {  // the queries are kept: an overflowing run is repeated (finalize_run)
-    OwnedQueries& o = b->owned;
-    o.q.assign(queries, queries + nq);
-    size_t n_ts = 0, n_t = 0;
-    for (size_t qi = 0; qi < nq; ++qi) { n_ts += queries[qi].n_term_segs; n_t += queries[qi].n_terms; }
-    o.ts.reserve(n_ts); o.w.reserve(n_t); o.avg.reserve(n_t); o.flags.reserve(n_t);
-    size_t n_cache = 0;
-    for (size_t qi = 0; qi < nq; ++qi) if (queries[qi].tf_cache) n_cache += 256 * (size_t)queries[qi].n_terms;
-    o.cache.reserve(n_cache);
-    o.tp.reserve(n_ts); o.toff.reserve(n_t);
-    for (size_t qi = 0; qi < nq; ++qi) {
-      const tq_query& q = queries[qi];
-      tq_query& d = o.q[qi];
-      d.term_pos = nullptr;
-      if (q.term_pos) { d.term_pos = reinterpret_cast<const tq_term_pos*>(o.tp.size() + 1); o.tp.insert(o.tp.end(), q.term_pos, q.term_pos + q.n_term_segs); }
-      d.term_offset = nullptr;
-      if (q.term_offset) { d.term_offset = reinterpret_cast<const uint32_t*>(o.toff.size() + 1); o.toff.insert(o.toff.end(), q.term_offset, q.term_offset + q.n_terms); }
-      d.term_segs = reinterpret_cast<const tq_term_seg*>(o.ts.size());  // offsets for now (the vectors do not move again: reserved)
-      o.ts.insert(o.ts.end(), q.term_segs, q.term_segs + q.n_term_segs);
-      d.weight = reinterpret_cast<const float*>(o.w.size());
-      o.w.insert(o.w.end(), q.weight, q.weight + q.n_terms);
-      d.avg_fieldnorm = nullptr;
-      if (q.avg_fieldnorm) { d.avg_fieldnorm = reinterpret_cast<const float*>(o.avg.size() + 1); o.avg.insert(o.avg.end(), q.avg_fieldnorm, q.avg_fieldnorm + q.n_terms); }
-      d.tf_cache = nullptr;
-      if (q.tf_cache) { d.tf_cache = reinterpret_cast<const float*>(o.cache.size() + 1); o.cache.insert(o.cache.end(), q.tf_cache, q.tf_cache + 256 * (size_t)q.n_terms); }
-      d.term_flags = nullptr;
-      if (q.term_flags) { d.term_flags = reinterpret_cast<const uint8_t*>(o.flags.size() + 1); o.flags.insert(o.flags.end(), q.term_flags, q.term_flags + q.n_terms); }
-    }
-    for (size_t qi = 0; qi < nq; ++qi) {
-      tq_query& d = o.q[qi];
-      d.term_segs = o.ts.data() + reinterpret_cast<size_t>(d.term_segs);
-      d.weight = o.w.data() + reinterpret_cast<size_t>(d.weight);
-      if (d.avg_fieldnorm) d.avg_fieldnorm = o.avg.data() + (reinterpret_cast<size_t>(d.avg_fieldnorm) - 1);
-      if (d.tf_cache) d.tf_cache = o.cache.data() + (reinterpret_cast<size_t>(d.tf_cache) - 1);
-      if (d.term_flags) d.term_flags = o.flags.data() + (reinterpret_cast<size_t>(d.term_flags) - 1);
-      if (d.term_pos) d.term_pos = o.tp.data() + (reinterpret_cast<size_t>(d.term_pos) - 1);
-      if (d.term_offset) d.term_offset = o.toff.data() + (reinterpret_cast<size_t>(d.term_offset) - 1);
-    }
   }
 
   // ---- scratch: qstate | candidates | results ------------------------------------------------------
-  b->kmax = kmax;
-  b->n_cands = n_cands;
+  b->kmax = pl.kmax;
+  b->n_cands = pl.n_cands;
   size_t so = 0;
-  b->qstate_off = so; so = align(so + std::max<size_t>(nq, 1) * sizeof(QState));
-  b->cands_off = so; so = align(so + std::max<size_t>(n_cands, 1) * sizeof(Cand));
+  b->qstate_off = so; so = align256(so + nq1 * sizeof(QState));
+  b->cands_off = so; so = align256(so + std::max<size_t>(pl.n_cands, 1) * sizeof(Cand));
   b->res_off = so;
-  const size_t rows = std::max<size_t>(nq, 1) * kmax;
-  const size_t o_rs = 0, o_rg = align(rows * 4), o_rd = o_rg + align(rows * 4), o_rc = o_rd + align(rows * 4);
-  b->res_bytes = o_rc + align(std::max<size_t>(nq, 1) * 4);
+  const size_t col = align256(nq1 * pl.kmax * 4);
+  b->res_at = {0, col, 2 * col, 3 * col};
+  b->res_bytes = b->res_at.counts + align256(nq1 * 4);
   so += b->res_bytes;
   TQ_CUDA(b->scratch.ensure(so));
   TQ_CUDA(b->res_pin.ensure(b->res_bytes));
 
   BatchParams& P = b->params;
   P.lists = c->d_lists;
-  P.caches = reinterpret_cast<const float*>(b->dev.p + o_caches);
-  P.tf_tables = reinterpret_cast<const float*>(b->dev.p + o_tftab);
-  P.qlists = reinterpret_cast<const QList*>(b->dev.p + o_qlists);
-  P.qsegs = reinterpret_cast<const QSeg*>(b->dev.p + o_qsegs);
-  P.units = reinterpret_cast<const Unit*>(b->dev.p + o_units);
-  P.queries = reinterpret_cast<const DQuery*>(b->dev.p + o_queries);
+  P.caches = st.on_device<const float>(o_caches);
+  P.tf_tables = st.on_device<const float>(o_tftab);
+  P.qlists = st.on_device<const QList>(o_qlists);
+  P.qsegs = st.on_device<const QSeg>(o_qsegs);
+  P.units = st.on_device<const Unit>(o_units);
+  P.queries = st.on_device<const DQuery>(o_queries);
   P.qstate = reinterpret_cast<QState*>(b->scratch.p + b->qstate_off);
   P.cands = reinterpret_cast<Cand*>(b->scratch.p + b->cands_off);
   uint8_t* r = b->scratch.p + b->res_off;
-  P.res_scores = reinterpret_cast<float*>(r + o_rs);
-  P.res_segs = reinterpret_cast<uint32_t*>(r + o_rg);
-  P.res_docs = reinterpret_cast<uint32_t*>(r + o_rd);
-  P.res_counts = reinterpret_cast<uint32_t*>(r + o_rc);
-  P.res_stride = kmax;
+  P.res_scores = reinterpret_cast<float*>(r + b->res_at.scores);
+  P.res_segs = reinterpret_cast<uint32_t*>(r + b->res_at.segs);
+  P.res_docs = reinterpret_cast<uint32_t*>(r + b->res_at.docs);
+  P.res_counts = reinterpret_cast<uint32_t*>(r + b->res_at.counts);
+  P.res_stride = pl.kmax;
   P.n_queries = (uint32_t)nq;
   P.counters = c->d_counters;
   P.or_prune = c->or_prune;
@@ -1571,28 +1586,96 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
 
   TQ_CUDA(cudaEventRecord(b->ev_start, b->stream));
   TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, b->desc_bytes, cudaMemcpyHostToDevice, b->stream));
+  const unsigned n = (unsigned)(n_caches * kTfRows * 256);
+  k_build_tf_tables<<<(n + 255) / 256, 256, 0, b->stream>>>(P.caches, st.on_device<float>(o_tftab), (uint32_t)n_caches);
+  TQ_CUDA(cudaGetLastError());
+  return TQ_OK;
+}
+
+}  // namespace
+
+// repeat (finalize_run): 0 = a caller's batch.  1 = the repeat of an overflowed run: TERM / AND / OR / phrase queries take the
+// per-query kernels; TQ_OP_BOOL queries stay on the tile engine with candidate regions as large as their postings and the largest
+// tile buffer.  2 = as 1, but every TQ_OP_BOOL query in a tile group of its own.
+static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int repeat, tq_batch** out) {
+  if (!c || !out || (!queries && nq)) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; bool ok = false; ~Guard() { if (!ok) tq_batch_destroy(b); } } guard{b};
+  b->ran = false;
+  b->finalized = false;
+  b->next_phase = 0;  // a recycled batch may have been abandoned in the middle of a phased run
+  b->nq = (uint32_t)nq;
+  b->stats = tq_stats{};
+  b->n_spans = 0;
+  b->groups.clear();
+  b->owned = OwnedQueries{};
+  b->repeat = repeat;
+
+  BatchPlan pl{queries, nq, repeat};
+  pl.dq.resize(nq);
+  pl.q_cands.assign(nq, 0);
+  // Single-term queries ride along on the tile engine when the batch has multi-term queries whose decoded lists they share
+  // (mixed workload: 32.6 K q/s against 28.6 K with them on k_term); a batch of nothing but single-term queries has nothing to
+  // share and streams its lists through k_term (configs[0]: 1.39 M q/s against 0.49 M).  TQ_TILE_TERMS: 0 never, 1 always, 2 this rule.
+  pl.terms_on_tile = c->tile_terms == 1;
+  if (c->tile_terms >= 2)
+    for (size_t qi = 0; qi < nq && !pl.terms_on_tile; ++qi)
+      pl.terms_on_tile = queries[qi].n_terms >= 2 && queries[qi].op != TQ_OP_PHRASE;
   {
-    const unsigned n = (unsigned)(n_caches * kTfRows * 256);
-    k_build_tf_tables<<<(n + 255) / 256, 256, 0, b->stream>>>(P.caches, reinterpret_cast<float*>(b->dev.p + o_tftab), (uint32_t)n_caches);
-    TQ_CUDA(cudaGetLastError());
+    std::lock_guard<std::mutex> g(c->mu);
+    PendingScope pending_scope{c, pl.pending};  // an early error return leaves no half-built list in the cache
+    PendingPosScope pending_pos_scope{c, pl.pending_pos};
+    int rc = TQ_OK;
+    for (size_t qi = 0; qi < nq && rc == TQ_OK; ++qi) rc = plan_query(c, pl, qi);
+    if (rc == TQ_OK) rc = cut_units(c, pl);
+    if (rc == TQ_OK) rc = flush_builds(c, pl.pending, &pl.built);
+    if (rc == TQ_OK) rc = flush_pos_builds(c, pl.pending_pos);
+    if (rc != TQ_OK) return rc;
   }
-  b->stats.lists_built = built;
-  b->stats.units = n_units_total + tile_units;
+  int rc = stage_tile_groups(c, pl);
+  if (rc == TQ_OK && !pl.tgroups.empty()) b->owned.assign(queries, nq);  // the queries are kept: an overflowing run is repeated (finalize_run)
+  if (rc == TQ_OK) rc = lay_out(c, b, pl);
+  if (rc != TQ_OK) return rc;
+
+  const uint32_t* nu = b->n_units;
+  const uint64_t strip_units = (uint64_t)nu[UC_STRIP] + nu[UC_STRIP_ROUND1] + nu[UC_STRIP_ROUND2] + nu[UC_STRIP_ROUND3];
+  b->stats.lists_built = pl.built;
+  b->stats.units = nu[UC_TERM] + nu[UC_AND] + nu[UC_OR_WINDOW] + strip_units + nu[UC_PHRASE] + pl.tile_units;
   b->stats.h2d_bytes = b->desc_bytes;
-  b->stats.algorithmic_bytes = alg_bytes;
-  b->stats.postings = postings;
-  b->stats.units_term = units[0].size(); b->stats.units_and = units[1].size(); b->stats.units_or = units[2].size() + units[3].size() + units[4].size() + units[5].size() + units[6].size(); b->stats.units_or_strip = units[3].size() + units[4].size() + units[5].size() + units[6].size();
-  b->stats.bytes_term = op_bytes[0]; b->stats.bytes_and = op_bytes[1]; b->stats.bytes_or = op_bytes[2];
-  b->stats.units_tile = tile_units;
-  b->stats.units_phrase = units[7].size();
+  b->stats.algorithmic_bytes = pl.alg_bytes;
+  b->stats.postings = pl.postings;
+  b->stats.units_term = nu[UC_TERM]; b->stats.units_and = nu[UC_AND]; b->stats.units_or = nu[UC_OR_WINDOW] + strip_units; b->stats.units_or_strip = strip_units;
+  b->stats.bytes_term = pl.op_bytes[0]; b->stats.bytes_and = pl.op_bytes[1]; b->stats.bytes_or = pl.op_bytes[2];
+  b->stats.units_tile = pl.tile_units;
+  b->stats.units_phrase = nu[UC_PHRASE];
   b->stats.tile_groups = b->groups.size();
-  b->stats.tile_postings = tile_postings;
-  for (auto& tg : tgroups) b->stats.tile_list_bytes += tg.list_bytes;
-  b->stats.tile_scratch_bytes = tile_bytes;
+  b->stats.tile_postings = pl.tile_postings;
+  for (auto& tg : pl.tgroups) b->stats.tile_list_bytes += tg.list_bytes;
+  b->stats.tile_scratch_bytes = pl.tile_bytes;
   guard.ok = true;
   *out = b;
   return TQ_OK;
 }
+
+extern "C" {
+
+void tq_batch_destroy(tq_batch* b) {
+  if (!b) return;
+  cudaSetDevice(b->ctx->device);
+  cudaStreamSynchronize(b->stream);
+  b->next_phase = 0;
+  b->ran = false;
+  std::lock_guard<std::mutex> g(b->ctx->mu);
+  b->ctx->pool.push_back(b);  // buffers are recycled by the next batch
+}
+
+int tq_batch_prepare(tq_ctx* c, const tq_query* queries, size_t nq, tq_batch** out) {
+  return batch_prepare_impl(c, queries, nq, 0, out);
+}
+
+}  // extern "C"
 
 // Phases of a run: 0 = term / AND / window-union kernels + the decode-and-score pass and the sample launch of the tile engine
 // + the strips' first threshold round, 1 and 2 = the next (exact) tile launches / threshold rounds, 3 = the last tile launch,
@@ -1628,17 +1711,17 @@ static int run_phase(tq_batch* b, int phase) {
     TQ_CUDA(cudaMemcpyAsync(P.qstate, b->dev.p + b->qinit_off, std::max<size_t>(b->nq, 1) * sizeof(QState), cudaMemcpyDeviceToDevice, b->stream));
     if (tiles) TQ_CUDA(cudaMemsetAsync(b->tile_dev.p + b->tile_zero_off, 0, b->tile_zero_bytes, b->stream));
     TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
-    if (b->n_units[TQ_OP_TERM]) {
+    if (b->n_units[UC_TERM]) {
       const int sp = span_begin(b, SPAN_TERM);
-      k_term<<<b->n_units[TQ_OP_TERM], kThreads, 0, b->stream>>>(P, b->unit_base[TQ_OP_TERM]); ++launches;
+      k_term<<<b->n_units[UC_TERM], kThreads, 0, b->stream>>>(P, b->unit_base[UC_TERM]); ++launches;
       span_end(b, sp);
     }
-    if (b->n_units[TQ_OP_AND]) {
+    if (b->n_units[UC_AND]) {
       const int sp = span_begin(b, SPAN_AND);
-      k_and<<<b->n_units[TQ_OP_AND], kThreads, 0, b->stream>>>(P, b->unit_base[TQ_OP_AND]); ++launches;
+      k_and<<<b->n_units[UC_AND], kThreads, 0, b->stream>>>(P, b->unit_base[UC_AND]); ++launches;
       span_end(b, sp);
     }
-    if (b->n_units[7]) {
+    if (b->n_units[UC_PHRASE]) {
       // phrase queries share nothing with the tile engine's launches (their own candidate regions; k_theta and the key export
       // skip them) and k_phrase waits on dependent position loads most of the time: it runs on a second stream next to them
       const bool aside = tiles && b->ctx->phrase_side;
@@ -1648,20 +1731,20 @@ static int run_phase(tq_batch* b, int phase) {
         TQ_CUDA(cudaStreamWaitEvent(b->side, b->ev_side0, 0));
       }
       const int sp = span_begin(b, SPAN_PHRASE, on);
-      k_phrase<<<b->n_units[7], kPhraseThreads, phrase_smem_bytes(b->phrase_ct), on>>>(P, b->ctx->d_pos_descs, b->phrase_aux, b->unit_base[7], b->phrase_ct); ++launches;
+      k_phrase<<<b->n_units[UC_PHRASE], kPhraseThreads, phrase_smem_bytes(b->phrase_ct), on>>>(P, b->ctx->d_pos_descs, b->phrase_aux, b->unit_base[UC_PHRASE], b->phrase_ct); ++launches;
       span_end(b, sp, on);
       if (aside) {
         TQ_CUDA(cudaEventRecord(b->ev_side1, b->side));
         b->side_pending = true;
       }
     }
-    if (b->n_units[TQ_OP_OR]) {
+    if (b->n_units[UC_OR_WINDOW]) {
       const int sp = span_begin(b, SPAN_OR);
       // window unions: the TMA/mbarrier pipeline when every union has few enough clauses for its tables, else the plain kernel
       if (b->ctx->or_pipe && b->or_max_lists <= kPipeMaxLists && !b->ctx->or_prune)
-        k_or_pipe<<<b->n_units[TQ_OP_OR], kPipeThreads, pipe_smem_bytes(), b->stream>>>(P, b->unit_base[TQ_OP_OR]);
+        k_or_pipe<<<b->n_units[UC_OR_WINDOW], kPipeThreads, pipe_smem_bytes(), b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);
       else
-        k_or<<<b->n_units[TQ_OP_OR], kThreads, kOrDynSmem, b->stream>>>(P, b->unit_base[TQ_OP_OR]);
+        k_or<<<b->n_units[UC_OR_WINDOW], kThreads, kOrDynSmem, b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);
       ++launches;
       span_end(b, sp);
     }
@@ -1679,9 +1762,8 @@ static int run_phase(tq_batch* b, int phase) {
     if (tiles) {
       const int rc = launch_tile_round(b, phase, &launches);
       if (rc != TQ_OK) return rc;
-      if (phase == 0 && (kTileRounds == kPhases + 0)) {}  // (rounds 1..3 belong to phases 1..3)
     }
-    const int r = 4 + phase;
+    const int r = UC_STRIP_ROUND1 + phase;
     if (b->n_units[r]) {
       const int sp = span_begin(b, SPAN_OR);
       k_or_strip<<<b->n_units[r], kStripThreads, strip_smem_bytes(b->strip_cached_max), b->stream>>>(P, b->unit_base[r], b->strip_cached_max);
@@ -1713,9 +1795,9 @@ static int run_phase(tq_batch* b, int phase) {
     const int rc = launch_tile_round(b, kTileRounds - 1, &launches);
     if (rc != TQ_OK) return rc;
   }
-  if (b->n_units[3]) {
+  if (b->n_units[UC_STRIP]) {
     const int sp = span_begin(b, SPAN_OR);
-    k_or_strip<<<b->n_units[3], kStripThreads, strip_smem_bytes(b->strip_cached_max), b->stream>>>(P, b->unit_base[3], b->strip_cached_max); ++launches;
+    k_or_strip<<<b->n_units[UC_STRIP], kStripThreads, strip_smem_bytes(b->strip_cached_max), b->stream>>>(P, b->unit_base[UC_STRIP], b->strip_cached_max); ++launches;
     span_end(b, sp);
   }
   TQ_CUDA(cudaGetLastError());
@@ -1759,13 +1841,8 @@ static int finalize_run(tq_batch* b) {
   if (rc == TQ_OK) rc = finalize_run(fb);  // (a level-1 repeat whose buffer overflowed repeats itself at level 2)
   if (rc == TQ_OK && fb->nq != b->nq) rc = fail(TQ_ERR_CUDA, "repeat batch holds other queries");
   if (rc == TQ_OK && b->nq) {
-    const size_t width = (size_t)std::min(b->kmax, fb->kmax) * 4, dp = (size_t)b->kmax * 4, sp = (size_t)fb->kmax * 4;
     const BatchParams& D = b->params;
-    const BatchParams& S = fb->params;
-    cudaError_t e = cudaMemcpy2DAsync(D.res_scores, dp, S.res_scores, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
-    if (e == cudaSuccess) e = cudaMemcpy2DAsync(D.res_segs, dp, S.res_segs, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
-    if (e == cudaSuccess) e = cudaMemcpy2DAsync(D.res_docs, dp, S.res_docs, sp, width, b->nq, cudaMemcpyDeviceToDevice, b->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(D.res_counts, S.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream);
+    cudaError_t e = copy_rows(fb, b->stream, D.res_scores, D.res_segs, D.res_docs, D.res_counts, b->kmax);
     if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
     if (e != cudaSuccess) rc = fail(TQ_ERR_CUDA, cudaGetErrorString(e));
   }
@@ -1853,9 +1930,7 @@ int tq_batch_results_dev(tq_batch* b, const float** scores_dev, const uint32_t**
   if (doc_dev) *doc_dev = b->params.res_docs;
   if (count_dev) *count_dev = b->params.res_counts;
   if (stride) *stride = b->kmax;
-  collect_times(b);
-  std::lock_guard<std::mutex> g(b->ctx->mu);
-  b->ctx->stats = b->stats;
+  publish_stats(b);
   return TQ_OK;
 }
 
@@ -1864,15 +1939,9 @@ int tq_batch_results_copy_dev(tq_batch* b, float* scores_dev, uint32_t* segment_
   if (!scores_dev || !segment_ord_dev || !doc_dev || !count_dev) return fail(TQ_ERR_INVALID_ARGUMENT, "null output");
   TQ_CUDA(cudaSetDevice(b->ctx->device));
   { const int rc = finalize_run(b); if (rc != TQ_OK) return rc; }
-  const size_t rows = (size_t)b->nq * b->kmax * 4;
-  TQ_CUDA(cudaMemcpyAsync(scores_dev, b->params.res_scores, rows, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(segment_ord_dev, b->params.res_segs, rows, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(doc_dev, b->params.res_docs, rows, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(count_dev, b->params.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream));
+  TQ_CUDA(copy_rows(b, b->stream, scores_dev, segment_ord_dev, doc_dev, count_dev, b->kmax));
   TQ_CUDA(cudaStreamSynchronize(b->stream));
-  collect_times(b);
-  std::lock_guard<std::mutex> g(b->ctx->mu);
-  b->ctx->stats = b->stats;
+  publish_stats(b);
   return TQ_OK;
 }
 
@@ -1884,12 +1953,10 @@ int tq_batch_fetch(tq_batch* b, uint32_t out_stride, float* out_scores, uint32_t
   TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, b->scratch.p + b->res_off, b->res_bytes, cudaMemcpyDeviceToHost, b->stream));
   TQ_CUDA(cudaEventRecord(b->ev_end, b->stream));
   TQ_CUDA(cudaStreamSynchronize(b->stream));
-  const size_t rows = std::max<size_t>(b->nq, 1) * b->kmax;
-  auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const float* rs = reinterpret_cast<const float*>(b->res_pin.p);
-  const uint32_t* rg = reinterpret_cast<const uint32_t*>(b->res_pin.p + align(rows * 4));
-  const uint32_t* rd = reinterpret_cast<const uint32_t*>(b->res_pin.p + 2 * align(rows * 4));
-  const uint32_t* rc = reinterpret_cast<const uint32_t*>(b->res_pin.p + 3 * align(rows * 4));
+  const float* rs = reinterpret_cast<const float*>(b->res_pin.p + b->res_at.scores);
+  const uint32_t* rg = reinterpret_cast<const uint32_t*>(b->res_pin.p + b->res_at.segs);
+  const uint32_t* rd = reinterpret_cast<const uint32_t*>(b->res_pin.p + b->res_at.docs);
+  const uint32_t* rc = reinterpret_cast<const uint32_t*>(b->res_pin.p + b->res_at.counts);
   for (uint32_t q = 0; q < b->nq; ++q) {
     const uint32_t n = std::min(std::min(rc[q], b->kmax), out_stride);
     out_count[q] = rc[q];
@@ -1897,12 +1964,10 @@ int tq_batch_fetch(tq_batch* b, uint32_t out_stride, float* out_scores, uint32_t
     memcpy(out_segment_ord + (size_t)q * out_stride, rg + (size_t)q * b->kmax, n * 4);
     memcpy(out_doc + (size_t)q * out_stride, rd + (size_t)q * b->kmax, n * 4);
   }
-  collect_times(b);
   float ms = 0;
   if (cudaEventElapsedTime(&ms, b->ev_start, b->ev_end) == cudaSuccess) b->stats.total_ms = ms;
   b->stats.d2h_bytes = b->res_bytes;
-  std::lock_guard<std::mutex> g(b->ctx->mu);
-  b->ctx->stats = b->stats;
+  publish_stats(b);
   return TQ_OK;
 }
 
@@ -1957,13 +2022,8 @@ int tq_batch_results_pack_dev(tq_batch* b, uint32_t* packed_dev) {
   TQ_CUDA(cudaSetDevice(b->ctx->device));
   { const int rc = finalize_run(b); if (rc != TQ_OK) return rc; }
   const size_t rows = (size_t)b->nq * b->kmax;
-  TQ_CUDA(cudaMemcpyAsync(packed_dev, b->params.res_scores, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + rows, b->params.res_segs, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + 2 * rows, b->params.res_docs, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + 3 * rows, b->params.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream));
-  collect_times(b);
-  std::lock_guard<std::mutex> g(b->ctx->mu);
-  b->ctx->stats = b->stats;
+  TQ_CUDA(copy_rows(b, b->stream, reinterpret_cast<float*>(packed_dev), packed_dev + rows, packed_dev + 2 * rows, packed_dev + 3 * rows, b->kmax));
+  publish_stats(b);
   return TQ_OK;
 }
 
@@ -1977,10 +2037,7 @@ int tq_batch_results_pack_dev_async(tq_batch* b, uint32_t* packed_dev) {
   if (!packed_dev) return fail(TQ_ERR_INVALID_ARGUMENT, "null output");
   TQ_CUDA(cudaSetDevice(b->ctx->device));
   const size_t rows = (size_t)b->nq * b->kmax;
-  TQ_CUDA(cudaMemcpyAsync(packed_dev, b->params.res_scores, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + rows, b->params.res_segs, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + 2 * rows, b->params.res_docs, rows * 4, cudaMemcpyDeviceToDevice, b->stream));
-  TQ_CUDA(cudaMemcpyAsync(packed_dev + 3 * rows, b->params.res_counts, (size_t)b->nq * 4, cudaMemcpyDeviceToDevice, b->stream));
+  TQ_CUDA(copy_rows(b, b->stream, reinterpret_cast<float*>(packed_dev), packed_dev + rows, packed_dev + 2 * rows, packed_dev + 3 * rows, b->kmax));
   uint32_t* flags = packed_dev + 3 * rows + b->nq;
   if (!b->groups.empty() && !b->finalized)
     TQ_CUDA(cudaMemcpyAsync(flags, b->tile_dev.p + b->tile_flags_off, 16, cudaMemcpyDeviceToDevice, b->stream));
@@ -2017,56 +2074,41 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
       if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
       if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
       if (q.op == TQ_OP_BOOL && (!q.term_occur || !q.weight)) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_BOOL needs term_occur and weights");
-      order.clear();
-      for (uint32_t i = 0; i < q.n_term_segs; ++i) {
-        if (q.term_segs[i].term_idx >= q.n_terms) return fail(TQ_ERR_INVALID_ARGUMENT, "term_idx out of range");
-        if (q.term_segs[i].doc_freq) order.push_back(&q.term_segs[i]);
-      }
-      std::stable_sort(order.begin(), order.end(), [](const tq_term_seg* a, const tq_term_seg* b) {
-        return a->segment_ord != b->segment_ord ? a->segment_ord < b->segment_ord : a->term_idx < b->term_idx;
-      });
-      for (size_t i = 0; i < order.size();) {
-        size_t j = i;
-        while (j < order.size() && order[j]->segment_ord == order[i]->segment_ord) ++j;
-        const uint32_t n_here = (uint32_t)(j - i);
+      const int rc = for_each_segment(q, order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
         if (q.op == TQ_OP_BOOL) {  // mixed shapes: the structure of this segment, with list ids in place of the clause indices
           uint32_t tix_[TQ_MAX_TERMS], dfs_[TQ_MAX_TERMS], ids_[TQ_MAX_TERMS];
           float ws_[TQ_MAX_TERMS];
           const Segment* seg = nullptr;
-          for (size_t a = i; a < j; ++a) {
-            int rc = get_list(c, *order[a], false, pending, &ids_[a - i], &seg);
+          for (size_t a = 0; a < n_here; ++a) {
+            int rc = get_list(c, *ts[a], false, pending, &ids_[a], &seg);
             if (rc != TQ_OK) return rc;
-            tix_[a - i] = order[a]->term_idx; dfs_[a - i] = order[a]->doc_freq; ws_[a - i] = q.weight[order[a]->term_idx];
+            tix_[a] = ts[a]->term_idx; dfs_[a] = ts[a]->doc_freq; ws_[a] = q.weight[ts[a]->term_idx];
           }
           std::vector<uint16_t> words;
           bool io_unused;  // (a count adds no scores)
           const int st = bool_structure(q, tix_, dfs_, ws_, n_here, 0u, words, &io_unused);
           if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
-          if (st > 0) {
-            CountBoolSeg bs{};
-            bs.query = (uint32_t)qi; bs.words_base = (uint32_t)bool_words.size(); bs.max_doc = seg->max_doc; bs.alive = seg->d_alive;
-            size_t x = 0;
-            for (int k4 = 0; k4 < 4; ++k4) bool_words.push_back(words[x++]);
-            for (uint32_t g2 = 0; g2 < words[0]; ++g2) { const uint16_t len = words[x++]; bool_words.push_back(len); for (uint16_t e = 0; e < len; ++e) bool_words.push_back(ids_[words[x++]]); }
-            while (x < words.size()) bool_words.push_back(ids_[words[x++]]);
-            const uint32_t tiles = (bs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-            for (uint32_t t0 = 0; t0 < tiles; t0 += per) bool_units.push_back(Unit{(uint32_t)bool_segs.size(), t0, std::min(tiles, t0 + per), 0});
-            bool_segs.push_back(bs);
-          }
-          i = j;
-          continue;
+          if (st == 0) return TQ_OK;
+          CountBoolSeg bs{};
+          bs.query = (uint32_t)qi; bs.words_base = (uint32_t)bool_words.size(); bs.max_doc = seg->max_doc; bs.alive = seg->d_alive;
+          bool_words.insert(bool_words.end(), words.begin(), words.end());
+          map_bool_clauses(bool_words.data() + bs.words_base, words.size(), [&](uint32_t a) { return ids_[a]; });
+          const uint32_t tiles = (bs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
+          for (uint32_t t0 = 0; t0 < tiles; t0 += per) bool_units.push_back(Unit{(uint32_t)bool_segs.size(), t0, std::min(tiles, t0 + per), 0});
+          bool_segs.push_back(bs);
+          return TQ_OK;
         }
-        if (q.op == TQ_OP_AND && n_here < q.n_terms) { i = j; continue; }  // a clause without postings: empty intersection
+        if (q.op == TQ_OP_AND && n_here < q.n_terms) return TQ_OK;  // a clause without postings: empty intersection
         CountSeg cs{};
-        cs.query = (uint32_t)qi; cs.lists_base = (uint32_t)list_ids.size(); cs.n_lists = n_here; cs.op = (uint32_t)q.op;
+        cs.query = (uint32_t)qi; cs.lists_base = (uint32_t)list_ids.size(); cs.n_lists = (uint32_t)n_here; cs.op = (uint32_t)q.op;
         const Segment* seg = nullptr;
         uint64_t df_single = 0;
-        for (size_t a = i; a < j; ++a) {
+        for (size_t a = 0; a < n_here; ++a) {
           uint32_t id;
-          int rc = get_list(c, *order[a], false, pending, &id, &seg);
+          int rc = get_list(c, *ts[a], false, pending, &id, &seg);
           if (rc != TQ_OK) return rc;
           list_ids.push_back(id);
-          df_single = order[a]->doc_freq;
+          df_single = ts[a]->doc_freq;
         }
         cs.max_doc = seg->max_doc;
         cs.alive = seg->d_alive;
@@ -2078,66 +2120,19 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
           for (uint32_t t0 = 0; t0 < tiles; t0 += per) units.push_back(Unit{(uint32_t)segs.size(), t0, std::min(tiles, t0 + per), 0});
           segs.push_back(cs);
         }
-        i = j;
-      }
+        return TQ_OK;
+      });
+      if (rc != TQ_OK) return rc;
     }
     int rc = flush_builds(c, pending, &built);
     if (rc != TQ_OK) return rc;
   }
   if (!bool_units.empty()) {  // mixed boolean shapes: their own kernel, counts added to out_counts
-    auto align2 = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    size_t o2 = 0;
-    const size_t o_w = o2; o2 = align2(o2 + bool_words.size() * 4);
-    const size_t o_s = o2; o2 = align2(o2 + bool_segs.size() * sizeof(CountBoolSeg));
-    const size_t o_u = o2; o2 = align2(o2 + bool_units.size() * sizeof(Unit));
-    const size_t o_c = o2; o2 = align2(o2 + nq * 8);
-    TQ_CUDA(b->pin.ensure(o2 + 256));
-    TQ_CUDA(b->dev.ensure(o2 + 256));
-    memcpy(b->pin.p + o_w, bool_words.data(), bool_words.size() * 4);
-    memcpy(b->pin.p + o_s, bool_segs.data(), bool_segs.size() * sizeof(CountBoolSeg));
-    memcpy(b->pin.p + o_u, bool_units.data(), bool_units.size() * sizeof(Unit));
-    memset(b->pin.p + o_c, 0, nq * 8);
-    TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, o2, cudaMemcpyHostToDevice, b->stream));
-    CountBoolParams BP;
-    BP.lists = c->d_lists;
-    BP.words = reinterpret_cast<const uint32_t*>(b->dev.p + o_w);
-    BP.segs = reinterpret_cast<const CountBoolSeg*>(b->dev.p + o_s);
-    BP.units = reinterpret_cast<const Unit*>(b->dev.p + o_u);
-    BP.counts = reinterpret_cast<unsigned long long*>(b->dev.p + o_c);
-    k_count_bool<<<(unsigned)bool_units.size(), kThreads, 0, b->stream>>>(BP);
-    TQ_CUDA(cudaGetLastError());
-    TQ_CUDA(cudaMemcpyAsync(b->pin.p + o_c, b->dev.p + o_c, nq * 8, cudaMemcpyDeviceToHost, b->stream));
-    TQ_CUDA(cudaStreamSynchronize(b->stream));
-    const unsigned long long* dc = reinterpret_cast<const unsigned long long*>(b->pin.p + o_c);
-    for (size_t qi = 0; qi < nq; ++qi) out_counts[qi] += dc[qi];
+    const int rc = count_on_device(b, bool_words, bool_segs, bool_units, nq, out_counts, k_count_bool);
+    if (rc != TQ_OK) return rc;
   }
   if (units.empty()) return TQ_OK;
-  auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t off = 0;
-  const size_t o_ids = off; off = align(off + list_ids.size() * 4);
-  const size_t o_segs = off; off = align(off + segs.size() * sizeof(CountSeg));
-  const size_t o_units = off; off = align(off + units.size() * sizeof(Unit));
-  const size_t o_counts = off; off = align(off + nq * 8);
-  TQ_CUDA(b->pin.ensure(off + 256));
-  TQ_CUDA(b->dev.ensure(off + 256));
-  memcpy(b->pin.p + o_ids, list_ids.data(), list_ids.size() * 4);
-  memcpy(b->pin.p + o_segs, segs.data(), segs.size() * sizeof(CountSeg));
-  memcpy(b->pin.p + o_units, units.data(), units.size() * sizeof(Unit));
-  memset(b->pin.p + o_counts, 0, nq * 8);
-  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, off, cudaMemcpyHostToDevice, b->stream));
-  CountParams P;
-  P.lists = c->d_lists;
-  P.list_ids = reinterpret_cast<const uint32_t*>(b->dev.p + o_ids);
-  P.segs = reinterpret_cast<const CountSeg*>(b->dev.p + o_segs);
-  P.units = reinterpret_cast<const Unit*>(b->dev.p + o_units);
-  P.counts = reinterpret_cast<unsigned long long*>(b->dev.p + o_counts);
-  k_count<<<(unsigned)units.size(), kThreads, 0, b->stream>>>(P);
-  TQ_CUDA(cudaGetLastError());
-  TQ_CUDA(cudaMemcpyAsync(b->pin.p + o_counts, b->dev.p + o_counts, nq * 8, cudaMemcpyDeviceToHost, b->stream));
-  TQ_CUDA(cudaStreamSynchronize(b->stream));
-  const unsigned long long* dc = reinterpret_cast<const unsigned long long*>(b->pin.p + o_counts);
-  for (size_t qi = 0; qi < nq; ++qi) out_counts[qi] += dc[qi];
-  return TQ_OK;
+  return count_on_device(b, list_ids, segs, units, nq, out_counts, k_count);
 }
 
 // ---- codec-level access ---------------------------------------------------------------------------
