@@ -168,7 +168,7 @@ struct tq_ctx {
   std::vector<tq_batch*> pool;
   tq_stats stats{};
   uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit;
-  unsigned long long* d_counters = nullptr;  // [0..8) k_or / k_or_strip window routes, [8..16) k_tile diagnostics
+  unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 16, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
   uint32_t tile_ops = 7;  // bit per TQ_OP_*: which query shapes the tile engine takes
   uint32_t tile_seg_cap_hook = 0;
@@ -179,7 +179,6 @@ struct tq_ctx {
   uint64_t tile_smem_last = 0;
   uint32_t tile_cand_floor = 32768, tile_max_dens_x1000 = 0, tile_pcap_hook = 0, tile_big_min = 6, tile_units = 0;
   uint32_t target_units = 0;  // CTAs a batch's per-query units aim for (4 x 32 per SM)
-  uint32_t or_prune = 0, or_strip = 1, or_pipe = 1, strip_prune = 1, strip_sample_div = 32, strip_sample_div2 = 8, strip_sample_div3 = 2, strip_ne_div = 8, strip_ne_div2 = 64;
 };
 
 constexpr int kTileRounds = 4;  // launches of k_tile per run: the sample launch + three exact ones
@@ -314,15 +313,6 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->term_blocks_per_unit = env_u32("TQ_TERM_BLOCKS_PER_UNIT", 512);
   c->and_blocks_per_unit = env_u32("TQ_AND_BLOCKS_PER_UNIT", 128);
   c->or_tiles_per_unit = env_u32("TQ_OR_TILES_PER_UNIT", 16);
-  c->or_strip = env_u32("TQ_OR_STRIP", 1);
-  c->or_pipe = env_u32("TQ_OR_PIPE", 1);
-  c->strip_sample_div = env_u32("TQ_STRIP_SAMPLE_DIV", 32);  // share of a pair's windows in the threshold sample (0/1: off)
-  c->strip_sample_div2 = env_u32("TQ_STRIP_SAMPLE_DIV2", 8);  // second sample round ends at this share (0/1: one round only)
-  c->strip_sample_div3 = env_u32("TQ_STRIP_SAMPLE_DIV3", 2);  // third round: up to half of the windows
-  c->strip_ne_div = env_u32("TQ_STRIP_NE_DIV", 8);
-  c->strip_ne_div2 = env_u32("TQ_STRIP_NE_DIV2", 64);
-  c->strip_prune = env_u32("TQ_STRIP_PRUNE", 1);  // MaxScore split inside k_or_strip (exact)
-  c->or_prune = env_u32("TQ_OR_PRUNE", 0);  // MaxScore route: exact, but only pays off for small k / rare terms
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -1237,11 +1227,10 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
       for (auto& h : here) { pl.qaux.push_back(PhraseAux{h.second.pad, h.range_len, q.slop}); h.second.pad = 0; }
       pl.phrase_ct = std::max<uint32_t>(pl.phrase_ct, (uint32_t)here.size());
     }
-    if (op == TQ_OP_OR && c->or_strip && q.k <= kStripMaxK && here.size() <= kStripMaxLists) {
+    if (op == TQ_OP_OR && q.k <= kStripMaxK && here.size() <= kStripMaxLists) {
       // strip kernel: clauses with less than one block per kWin-doc window keep their current block decoded in shared memory
       uint32_t n_thin = 0;
-      static const uint64_t thin_mult = env_u32("TQ_STRIP_THIN_MULT", 1u);
-      auto is_thin = [&](uint32_t df) { return (uint64_t)df * (kWin / 128u) < (uint64_t)qs.max_doc * thin_mult; };
+      auto is_thin = [&](uint32_t df) { return (uint64_t)df * (kWin / 128u) < (uint64_t)qs.max_doc; };
       for (auto& h : here) if (is_thin(h.first)) ++n_thin;
       if (n_thin <= kMaxCached) {
         uint32_t slot = 0;
@@ -1256,7 +1245,7 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
     const uint32_t lead_total = here[0].first / 128u + ((here[0].first % 128u) ? 1u : 0u);
     pl.qsegs.push_back(qs);
     bool any_thick = false;
-    for (auto& h : here) any_thick = any_thick || (uint64_t)h.first * std::max(c->strip_ne_div, c->strip_ne_div2) >= qs.max_doc;
+    for (auto& h : here) any_thick = any_thick || (uint64_t)h.first * kStripNeDiv2 >= qs.max_doc;
     const uint32_t total = cls == UC_STRIP ? (qs.max_doc + kWin - 1) / kWin : (op == TQ_OP_OR ? (qs.max_doc + kTileDocs - 1) / kTileDocs : lead_total);
     pl.work.push_back(SegWork{cls, total, cls == UC_STRIP && prunable && any_thick});
     ++pl.n_qsegs_op[cls == UC_PHRASE ? UC_AND : cls];
@@ -1304,10 +1293,10 @@ int cut_units(const tq_ctx* c, BatchPlan& pl) {
     // best score over all sampled windows of the query (k_theta) then seeds the threshold of the main launch, whose
     // MaxScore split drops the dense clauses from the first window on.  Nothing is scored twice.
     uint32_t first = 0;
-    if (w.cls == UC_STRIP && w.sample && c->strip_sample_div > 1 && total >= 8u * c->strip_sample_div) {
-      const uint32_t cut1 = std::max<uint32_t>(kStripWarps, total / c->strip_sample_div);
-      const uint32_t cut2 = c->strip_sample_div2 > 1 && c->strip_sample_div2 < c->strip_sample_div ? std::max(cut1, total / c->strip_sample_div2) : cut1;
-      const uint32_t cut3 = c->strip_sample_div3 > 1 && c->strip_sample_div3 < c->strip_sample_div2 ? std::max(cut2, total / c->strip_sample_div3) : cut2;
+    if (w.cls == UC_STRIP && w.sample && total >= 8u * kStripSampleDiv) {
+      const uint32_t cut1 = std::max<uint32_t>(kStripWarps, total / kStripSampleDiv);
+      const uint32_t cut2 = std::max(cut1, total / kStripSampleDiv2);
+      const uint32_t cut3 = std::max(cut2, total / kStripSampleDiv3);
       const uint32_t cuts[4] = {0, cut1, cut2, cut3};
       for (int r = 0; r < 3; ++r)  // round r covers [cuts[r], cuts[r+1]); a k_theta pass follows each round
         for (uint32_t b0 = cuts[r]; b0 < cuts[r + 1]; b0 += per) {
@@ -1578,10 +1567,6 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
   P.res_stride = pl.kmax;
   P.n_queries = (uint32_t)nq;
   P.counters = c->d_counters;
-  P.or_prune = c->or_prune;
-  P.strip_prune = c->strip_prune;
-  P.strip_ne_div = c->strip_ne_div;
-  P.strip_ne_div2 = c->strip_ne_div2;
   P.ovf = b->groups.empty() ? nullptr : reinterpret_cast<uint32_t*>(b->tile_dev.p + to_flags) + 1;
 
   TQ_CUDA(cudaEventRecord(b->ev_start, b->stream));
@@ -1741,7 +1726,7 @@ static int run_phase(tq_batch* b, int phase) {
     if (b->n_units[UC_OR_WINDOW]) {
       const int sp = span_begin(b, SPAN_OR);
       // window unions: the TMA/mbarrier pipeline when every union has few enough clauses for its tables, else the plain kernel
-      if (b->ctx->or_pipe && b->or_max_lists <= kPipeMaxLists && !b->ctx->or_prune)
+      if (b->or_max_lists <= kPipeMaxLists)
         k_or_pipe<<<b->n_units[UC_OR_WINDOW], kPipeThreads, pipe_smem_bytes(), b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);
       else
         k_or<<<b->n_units[UC_OR_WINDOW], kThreads, kOrDynSmem, b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);

@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(kThreads) k_term(const BatchParams P, uint32_t
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) { s_top.count = 0; s_top.theta = (unsigned long long)qs->theta << 32; }
   __syncthreads();
-  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, P.counters, 0u, (unsigned)kThreads};
+  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, 0u, (unsigned)kThreads};
   BlockFetch f;
   if (U.begin + warp < U.end) fetch_issue(L, U.begin + warp, lane, f);
   for (uint32_t r = U.begin; r < U.end; r += kWarps) {
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(kThreads) k_and(const BatchParams P, uint32_t 
   uint32_t* dec = s_dec[warp];
   if (threadIdx.x == 0) { s_top.count = 0; s_top.theta = (unsigned long long)qs->theta << 32; }
   __syncthreads();
-  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, P.counters, 0u, (unsigned)kThreads};
+  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, 0u, (unsigned)kThreads};
   // MaxScore for the conjunction (exact): a leader doc whose own score plus the secondaries' bounds (score < weight)
   // cannot reach the threshold is dropped BEFORE its secondary blocks are looked up and decoded -- the lookups are
   // what this kernel spends its time on (block_wand_intersection.rs:60-120 prunes on block maxima for the same reason).
@@ -385,49 +385,38 @@ __global__ void __launch_bounds__(kThreads) k_and(const BatchParams P, uint32_t 
 // A slot holding -0.0f has not been touched: -0.0 + s == 0.0 + s bit for bit for every s except
 // s == -0.0 (SumCombiner starts from 0.0, score_combiner.rs:39-57).
 //
-// Two ways through a window of kTileDocs doc ids:
-//  * exhaustive: every clause's blocks are decoded and added in clause order, then the window is harvested;
-//  * MaxScore-pruned (once the threshold is high enough): clauses whose maximum scores add up to less
-//    than the threshold are "non-essential" (find_pivot_doc's prefix, block_wand_union.rs:16-43). Only the
-//    essential clauses are decoded; a doc is "promising" if its essential score plus the non-essential
-//    bound can reach the threshold, and only promising docs get their exact clause-ordered score.
-//    Every doc that is skipped provably scores below the threshold, so the result set is unchanged.
-constexpr uint32_t kTouchedCap = 2048;
-constexpr uint32_t kPromisingCap = 64;
-
+// A window of kTileDocs doc ids is skipped when no clause has a block in it, or when even the sum of all clause
+// maxima cannot reach the threshold.  Otherwise every clause's blocks are decoded and added in clause order, then
+// the window is harvested.
 struct OrShared {
   uint32_t blo[2][32], bhi[2][32];  // per clause: block range overlapping the tile (double buffered)
   uint32_t cur[32];                 // per clause: search cursor
   uint32_t any[2];
   uint32_t npass;
-  float prefix[33];      // prefix[i] = sum of the i smallest clause maxima
-  uint8_t order[32];     // clause ordinals by ascending maximum score
-  uint32_t ne_mask;      // non-essential clauses for the current threshold
-  float ne_bound;        // upper bound of their joint contribution
-  uint32_t mode;         // 0 skip, 1 exhaustive, 2 pruned
-  uint32_t touched_n, p_n, overflow;
-  uint16_t touched[kTouchedCap];
-  uint16_t plist[kPromisingCap];
-  uint32_t pbits[kTileDocs / 32];
+  float bound;                      // sum of the clause maxima x 1.00001: no doc can score more
+  uint32_t run;                     // the current window is accumulated and harvested
 };
+
+// Blocks of a posting list that overlap doc ids [lo, hi), searched from block `from`: returns how many, starting at
+// `first`, the first block whose last doc is >= lo (n when there is none; the next window's search starts there).
+__device__ __forceinline__ uint32_t window_blocks(const uint32_t* last_doc, uint32_t n, uint32_t from, uint32_t lo, uint32_t hi,
+                                                  uint32_t lane, uint32_t& first) {
+  first = first_block_ge(last_doc, from, n, lo, lane);
+  if (first >= n) return 0;
+  // the last block that can hold a doc < hi is the first one whose last doc is >= hi-1
+  const uint32_t last = first_block_ge(last_doc, first, n, hi - 1u, lane);
+  return (last < n ? last : n - 1u) - first + 1u;
+}
 
 __device__ __forceinline__ void or_tile_ranges(const BatchParams& P, const QSeg& S, OrShared& sh, int buf, uint32_t tile,
                                                uint32_t warp, uint32_t lane) {
   const uint32_t lo = tile * kTileDocs;
   const uint32_t hi = min(lo + kTileDocs, S.max_doc);
   for (uint32_t t = warp; t < S.n_lists; t += kWarps) {
-    const QList ql = P.qlists[S.lists_base + t];
-    const uint32_t* last_doc = P.lists[ql.list_id].last_doc;
-    const uint32_t n_total = P.lists[ql.list_id].n_total;
-    uint32_t blo = 1, bhi = 0;
-    const uint32_t j_lo = first_block_ge(last_doc, sh.cur[t], n_total, lo, lane);
-    if (j_lo < n_total) {
-      // the last block that can hold a doc < hi is the first one whose last doc is >= hi-1
-      uint32_t j_hi = first_block_ge(last_doc, j_lo, n_total, hi - 1u, lane);
-      if (j_hi >= n_total) j_hi = n_total - 1u;
-      blo = j_lo; bhi = j_hi;
-    }
-    if (lane == 0) { sh.blo[buf][t] = blo; sh.bhi[buf][t] = bhi; sh.cur[t] = j_lo; if (blo <= bhi) sh.any[buf] = 1; }
+    const ListDesc& L = P.lists[P.qlists[S.lists_base + t].list_id];
+    uint32_t first;
+    const uint32_t cnt = window_blocks(L.last_doc, L.n_total, sh.cur[t], lo, hi, lane, first);
+    if (lane == 0) { sh.blo[buf][t] = cnt ? first : 1u; sh.bhi[buf][t] = cnt ? first + cnt - 1u : 0u; sh.cur[t] = first; if (cnt) sh.any[buf] = 1; }
   }
 }
 
@@ -446,6 +435,70 @@ __device__ __forceinline__ void or_next_item(const OrShared& sh, int buf, uint32
   }
 }
 
+// Harvest of the window [lo, lo + kTileDocs) by the threads of T: count what passes, then push in one go when it
+// fits; every score slot is reset to -0.0.  A float compare against the threshold score rejects nearly every slot
+// (untouched slots hold -0.0, which is below any positive threshold); the exact key test runs only on the survivors.
+// *npass is a shared pass count, 0 on entry and on return.
+__device__ __forceinline__ void or_harvest(const TopK& T, float* s_acc, const QSeg& S, uint32_t lo, uint32_t k,
+                                           unsigned int* theta_global, uint32_t* npass, uint32_t lane) {
+  const float neg_zero = __uint_as_float(0x80000000u);
+  const unsigned long long theta = *T.theta;
+  const float theta_f = threshold_score((uint32_t)(theta >> 32));
+  uint32_t passmask = 0;
+#pragma unroll 1
+  for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
+    const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
+    const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
+    if (v.x >= theta_f || v.y >= theta_f || v.z >= theta_f || v.w >= theta_f) {
+      const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const uint32_t d = lo + idx + c;
+        bool pass = vv[c] >= theta_f && __float_as_uint(vv[c]) != 0x80000000u && make_key(vv[c], d) >= theta;
+        if (pass && S.alive) pass = is_alive(S.alive, d);
+        passmask |= pass ? (1u << (j * 4 + c)) : 0u;
+      }
+    }
+  }
+  const uint32_t wsum = __reduce_add_sync(kFull, (uint32_t)__popc(passmask));
+  if (lane == 0 && wsum) atomicAdd(npass, wsum);
+  topk_sync(T);
+  const bool fits = *T.count + *npass <= kCap;
+  topk_sync(T);  // every thread has read the count before anyone starts pushing (the branch must be uniform)
+  if (threadIdx.x == 0) *npass = 0;
+  if (fits) {
+#pragma unroll 1
+    for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
+      const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
+      const uint32_t sub = (passmask >> (j * 4)) & 15u;
+      if (__ballot_sync(kFull, sub != 0)) {
+        const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int c = 0; c < 4; ++c) topk_push(T, (sub >> c) & 1u, make_key(vv[c], lo + idx + c), lane);
+      }
+      *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
+    }
+    topk_round_end(T, k, theta_global);
+  } else {  // cold start: more survivors than the buffer holds; go in rounds with compaction between
+    topk_round_end(T, k, theta_global);  // leaves at most kCap - kRoundMargin keys
+#pragma unroll 1
+    for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
+      const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
+      const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
+      const float vv[4] = {v.x, v.y, v.z, v.w};
+      const unsigned long long th = *T.theta;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const unsigned long long key = make_key(vv[c], lo + idx + c);
+        topk_push(T, ((passmask >> (j * 4 + c)) & 1u) && key >= th, key, lane);
+      }
+      *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
+      topk_round_end(T, k, theta_global);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_t unit_base) {
   extern __shared__ __align__(16) float s_acc[];                  // [kTileDocs]
   uint8_t* s_fn = reinterpret_cast<uint8_t*>(s_acc + kTileDocs);  // [kTileDocs]
@@ -459,25 +512,25 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
   const float neg_zero = __uint_as_float(0x80000000u);
   const bool staged_fn = (S.flags & 1u) && S.fieldnorm != nullptr;
   for (uint32_t i = threadIdx.x; i < kTileDocs; i += kThreads) s_acc[i] = neg_zero;
-  for (uint32_t i = threadIdx.x; i < kTileDocs / 32; i += kThreads) sh.pbits[i] = 0;
   if (threadIdx.x < 32) sh.cur[threadIdx.x] = 0;
   if (threadIdx.x == 0) {
     s_top.count = 0; s_top.theta = (unsigned long long)qs->theta << 32;
-    sh.any[0] = sh.any[1] = 0; sh.npass = 0; sh.touched_n = 0; sh.p_n = 0; sh.overflow = 0;
-    // clauses by ascending maximum score; a clause can add at most its weight (tf/(tf+norm) < 1, bm25.rs:170-175)
+    sh.any[0] = sh.any[1] = 0; sh.npass = 0;
+    // a clause can add at most its weight (tf/(tf+norm) < 1, bm25.rs:170-175); the maxima are added in ascending order
     float mx[32];
-    for (uint32_t t = 0; t < S.n_lists; ++t) { mx[t] = fmaxf(P.qlists[S.lists_base + t].weight, 0.0f); sh.order[t] = (uint8_t)t; }
+    for (uint32_t t = 0; t < S.n_lists; ++t) mx[t] = fmaxf(P.qlists[S.lists_base + t].weight, 0.0f);
     for (uint32_t i = 1; i < S.n_lists; ++i) {
-      const uint8_t o = sh.order[i];
+      const float m = mx[i];
       uint32_t j = i;
-      while (j > 0 && mx[sh.order[j - 1]] > mx[o]) { sh.order[j] = sh.order[j - 1]; --j; }
-      sh.order[j] = o;
+      while (j > 0 && mx[j - 1] > m) { mx[j] = mx[j - 1]; --j; }
+      mx[j] = m;
     }
-    sh.prefix[0] = 0.0f;
-    for (uint32_t i = 0; i < S.n_lists; ++i) sh.prefix[i + 1] = sh.prefix[i] + mx[sh.order[i]];
+    float sum = 0.0f;
+    for (uint32_t i = 0; i < S.n_lists; ++i) sum += mx[i];
+    sh.bound = sum * 1.00001f;  // f32 sums of up to 32 terms differ by < 4e-6 relative
   }
   __syncthreads();
-  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, P.counters, 0u, (unsigned)kThreads};
+  const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, 0u, (unsigned)kThreads};
   or_tile_ranges(P, S, sh, 0, U.begin, warp, lane);
   unsigned int theta_g_seen = 0;  // thread 0: query-wide threshold sampled one window ago
   __syncthreads();
@@ -485,152 +538,17 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
     const int buf = (int)((tile - U.begin) & 1u);
     const uint32_t lo = tile * kTileDocs;
     const uint32_t hi = min(lo + kTileDocs, S.max_doc);
-    // ---- decide how to go through this window ------------------------------------------------------
     if (threadIdx.x == 0) {
       const unsigned long long g = (unsigned long long)theta_g_seen << 32;
       if (g > s_top.theta) s_top.theta = g;
       theta_g_seen = *(volatile unsigned int*)&qs->theta;  // consumed at the next window
-      const float theta_f = threshold_score((uint32_t)(s_top.theta >> 32));
-      uint32_t n_ne = 0, mask = 0;
-      while (n_ne < S.n_lists && sh.prefix[n_ne + 1] * 1.00001f < theta_f) { mask |= 1u << sh.order[n_ne]; ++n_ne; }
-      sh.ne_mask = mask;
-      sh.ne_bound = sh.prefix[n_ne] * 1.00001f;  // f32 sums of up to 32 terms differ by < 4e-6 relative
-      if (!P.or_prune && n_ne != S.n_lists) { n_ne = 0; sh.ne_mask = 0; sh.ne_bound = 0.0f; }
-      sh.mode = (!sh.any[buf] || n_ne == S.n_lists) ? 0u : (n_ne == 0 ? 1u : 2u);  // all non-essential: nothing here can enter the top-k
-      atomicAdd(&P.counters[sh.mode == 0 ? 0 : (sh.mode == 1 ? 1 : 2)], 1ull);
+      sh.run = sh.any[buf] && sh.bound >= threshold_score((uint32_t)(s_top.theta >> 32));
     }
     __syncthreads();
-    uint32_t mode = sh.mode;
-    const unsigned long long theta = *T.theta;
-    const float theta_f = threshold_score((uint32_t)(theta >> 32));
+    const bool run = sh.run != 0;
 
-    if (mode == 2) {
-      // ---- pruned, stage 1: essential clauses only, order-free estimate ---------------------------
-      const uint32_t ne_mask = sh.ne_mask;
-      uint32_t rr = 0;
-      for (uint32_t t = 0; t < S.n_lists; ++t) {
-        if ((ne_mask >> t) & 1u) continue;
-        const uint32_t blo = sh.blo[buf][t], bhi = sh.bhi[buf][t];
-        if (blo > bhi) continue;
-        const uint32_t nb = bhi - blo + 1u;
-        const QList ql = P.qlists[S.lists_base + t];
-        const ListDesc L = P.lists[ql.list_id];
-        const Scorer scr = make_scorer(P, ql);
-        for (uint32_t b = blo + ((warp + kWarps - (rr & (kWarps - 1))) & (kWarps - 1)); b <= bhi; b += kWarps) {
-          uint32_t doc[4], tf[4];
-          decode_block(L, b, lane, doc, tf);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            if (doc[i] >= lo && doc[i] < hi) {
-              const uint32_t slot = doc[i] - lo;
-              const float sc = bm25_score(scr, L.fieldnorm, doc[i], tf[i]);
-              const float old = atomicAdd(&s_acc[slot], sc);
-              if (__float_as_uint(old) == 0x80000000u) {
-                const uint32_t idx = atomicAdd(&sh.touched_n, 1u);
-                if (idx < kTouchedCap) sh.touched[idx] = (uint16_t)slot; else sh.overflow = 1;
-              }
-            }
-          }
-        }
-        rr += nb;
-      }
-      __syncthreads();
-      if (sh.overflow) {  // too many essential postings for the list: clean up and take the exhaustive route
-        if (threadIdx.x == 0) atomicAdd(&P.counters[4], 1ull);
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < kTileDocs; i += kThreads) s_acc[i] = neg_zero;
-        if (threadIdx.x == 0) { sh.touched_n = 0; sh.overflow = 0; }
-        mode = 1;
-        __syncthreads();
-      } else {
-        // which touched docs could still reach the threshold once the non-essential clauses are added
-        const uint32_t n_touched = sh.touched_n;
-        const float ne_bound = sh.ne_bound;
-        for (uint32_t i = threadIdx.x; i < n_touched; i += kThreads) {
-          const uint32_t slot = sh.touched[i];
-          const float est = s_acc[slot];
-          s_acc[slot] = neg_zero;
-          if (est + fabsf(est) * 1e-5f + ne_bound >= theta_f) {
-            const uint32_t j = atomicAdd(&sh.p_n, 1u);
-            if (j < kPromisingCap) { sh.plist[j] = (uint16_t)slot; atomicOr(&sh.pbits[slot >> 5], 1u << (slot & 31u)); }
-            else sh.overflow = 1;
-          }
-        }
-        __syncthreads();
-        const uint32_t p_n = sh.p_n;
-        const bool too_many = sh.overflow != 0;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-          atomicAdd(&P.counters[7], (unsigned long long)sh.touched_n);
-          atomicAdd(&P.counters[too_many ? 5 : (p_n == 0 ? 3 : 6)], too_many ? 1ull : (p_n == 0 ? 1ull : (unsigned long long)p_n));
-          sh.touched_n = 0; sh.overflow = 0;
-        }
-        if (too_many) {
-          for (uint32_t i = threadIdx.x; i < kTileDocs / 32; i += kThreads) sh.pbits[i] = 0;
-          if (threadIdx.x == 0) sh.p_n = 0;
-          mode = 1;
-          __syncthreads();
-        } else if (p_n == 0) {
-          mode = 0;
-        } else {
-          // ---- pruned, stage 2: exact clause-ordered score of the promising docs only -------------------
-          for (uint32_t tt = 0; tt < S.n_lists; ++tt) {
-            const uint32_t blo = sh.blo[buf][tt], bhi = sh.bhi[buf][tt];
-            if (blo <= bhi) {
-              const QList ql = P.qlists[S.lists_base + tt];
-              const ListDesc L = P.lists[ql.list_id];
-              const Scorer scr = make_scorer(P, ql);
-              for (uint32_t b = blo + warp; b <= bhi; b += kWarps) {
-                // does this block's doc range hold a promising doc?
-                const uint32_t last = __ldg(L.last_doc + b);
-                const uint32_t prev = b ? __ldg(L.last_doc + b - 1) : 0u;
-                bool mine = false;
-                for (uint32_t i = lane; i < p_n; i += 32) {
-                  const uint32_t d = lo + sh.plist[i];
-                  mine |= (d <= last) && (b == 0 || d > prev);
-                }
-                if (__ballot_sync(kFull, mine) == 0) continue;
-                uint32_t doc[4], tf[4];
-                decode_block(L, b, lane, doc, tf);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  if (doc[i] >= lo && doc[i] < hi) {
-                    const uint32_t slot = doc[i] - lo;
-                    if ((sh.pbits[slot >> 5] >> (slot & 31u)) & 1u) {
-                      const float sc = bm25_score(scr, L.fieldnorm, doc[i], tf[i]);
-                      s_acc[slot] = __fadd_rn(s_acc[slot], sc);
-                    }
-                  }
-                }
-              }
-            }
-            __syncthreads();  // clause order is the f32 summation order
-          }
-          for (uint32_t base = 0; base < p_n; base += kThreads) {
-            const uint32_t i = base + threadIdx.x;
-            bool pass = false;
-            unsigned long long key = 0;
-            if (i < p_n) {
-              const uint32_t slot = sh.plist[i];
-              const float v = s_acc[slot];
-              s_acc[slot] = neg_zero;
-              sh.pbits[slot >> 5] = 0;  // every bit of that word belongs to a promising slot being reset
-              const uint32_t d = lo + slot;
-              key = make_key(v, d);
-              pass = __float_as_uint(v) != 0x80000000u && key >= theta;
-              if (pass && S.alive) pass = is_alive(S.alive, d);
-            }
-            topk_push(T, pass, key, lane);
-          }
-          if (threadIdx.x == 0) sh.p_n = 0;
-          topk_round_end(T, Q.k, &qs->theta);
-          mode = 3;  // done
-        }
-      }
-    }
-
-    if (mode == 1) {
-      // ---- exhaustive accumulate -----------------------------------------------------------------------
+    if (run) {
+      // ---- accumulate ----------------------------------------------------------------------------------
       // fieldnorm bytes of the window: one coalesced 16-byte row per thread pair instead of a byte gather per posting
       if (staged_fn) {
         const uint4* src = reinterpret_cast<const uint4*>(S.fieldnorm + lo);
@@ -680,68 +598,8 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
       or_tile_ranges(P, S, sh, buf ^ 1, tile + 1, warp, lane);
     }
 
-    if (mode == 1) {
-      // harvest: count what passes, then push in one go when it fits.
-      // A float compare against the threshold score rejects nearly every slot (untouched slots hold
-      // -0.0, which is below any positive threshold); the exact key test runs only on the survivors.
-      uint32_t passmask = 0;
-#pragma unroll 1
-      for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-        const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-        const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-        if (v.x >= theta_f || v.y >= theta_f || v.z >= theta_f || v.w >= theta_f) {
-          const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint32_t d = lo + idx + c;
-            bool pass = vv[c] >= theta_f && __float_as_uint(vv[c]) != 0x80000000u && make_key(vv[c], d) >= theta;
-            if (pass && S.alive) pass = is_alive(S.alive, d);
-            passmask |= pass ? (1u << (j * 4 + c)) : 0u;
-          }
-        }
-      }
-      const uint32_t wsum = __reduce_add_sync(kFull, (uint32_t)__popc(passmask));
-      if (lane == 0 && wsum) atomicAdd(&sh.npass, wsum);
-      __syncthreads();
-      const uint32_t npass = sh.npass;
-      const bool fits = *T.count + npass <= kCap;
-      __syncthreads();
-      if (fits) {
-#pragma unroll 1
-        for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-          const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-          const uint32_t sub = (passmask >> (j * 4)) & 15u;
-          if (__ballot_sync(kFull, sub != 0)) {
-            const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int c = 0; c < 4; ++c) topk_push(T, (sub >> c) & 1u, make_key(vv[c], lo + idx + c), lane);
-          }
-          *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-        }
-        if (threadIdx.x == 0) sh.npass = 0;
-        topk_round_end(T, Q.k, &qs->theta);
-      } else {  // cold start: more survivors than the buffer holds; go in rounds with compaction between
-        if (threadIdx.x == 0) sh.npass = 0;
-        topk_round_end(T, Q.k, &qs->theta);  // leaves at most kCap - kRoundMargin keys
-#pragma unroll 1
-        for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-          const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-          const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-          const float vv[4] = {v.x, v.y, v.z, v.w};
-          const unsigned long long th = *T.theta;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const unsigned long long key = make_key(vv[c], lo + idx + c);
-            topk_push(T, ((passmask >> (j * 4 + c)) & 1u) && key >= th, key, lane);
-          }
-          *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-          topk_round_end(T, Q.k, &qs->theta);
-        }
-      }
-    } else {
-      __syncthreads();
-    }
+    if (run) or_harvest(T, s_acc, S, lo, Q.k, &qs->theta, &sh.npass, lane);
+    else __syncthreads();
   }
   topk_flush(T, Q, qs, P.cands, S.segment_ord);
 }
@@ -755,7 +613,8 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
 //    16-byte block records gives position and record, the packed vectors follow (2 dependent loads);
 //  * thinner clauses keep their current block DECODED AND SCORED in shared memory (docs + scores); a window only
 //    looks at it when the block's next unread doc falls inside the window, so a block is decoded once per strip.
-// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or.
+// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or_pipe, or
+// k_or for more than kPipeMaxLists clauses.
 #ifndef TQ_KWIN
 #define TQ_KWIN 1024
 #endif
@@ -766,6 +625,14 @@ constexpr uint32_t kStripWarps = 4;
 constexpr uint32_t kStripThreads = kStripWarps * 32;
 constexpr uint32_t kStripMaxLists = 8;
 constexpr uint32_t kStripMaxK = 128;
+// MaxScore split: a clause with at least one posting per kStripNeDiv docs may turn non-essential; in a union without
+// such a clause, the densest one may still go under the looser bound kStripNeDiv2.
+constexpr uint32_t kStripNeDiv = 8;
+constexpr uint32_t kStripNeDiv2 = 64;
+// Threshold sample: the three sample launches of a (query, segment) end at 1/32, 1/8 and 1/2 of its windows.
+constexpr uint32_t kStripSampleDiv = 32;
+constexpr uint32_t kStripSampleDiv2 = 8;
+constexpr uint32_t kStripSampleDiv3 = 2;
 constexpr uint32_t kNoDoc = 0xFFFFFFFFu;
 
 struct StripWarpFixed {  // per warp, dynamic shared memory; followed by n_cached x StripCache
@@ -897,7 +764,7 @@ __global__ void __launch_bounds__(kStripThreads) k_or_strip(const BatchParams P,
   const uint32_t w_end = U.begin + (uint32_t)(((unsigned long long)n_win * (warp + 1)) / kStripWarps);
   for (uint32_t i = lane; i < kWin; i += 32) W.acc[i] = neg_zero;
   const bool staged_fn = (S.flags & 1u) && S.fieldnorm != nullptr;
-  const bool prunable = (S.flags & 2u) != 0 && P.strip_prune != 0;  // every weight finite and >= 0
+  const bool prunable = (S.flags & 2u) != 0;  // every weight finite and >= 0
   uint32_t thick_mask = 0;
   uint32_t n_e_min = 0;  // only the thick clauses at the end of the list may turn non-essential: thin ones are cheap to
                          // apply and every clause kept essential tightens the cold-window test
@@ -922,11 +789,11 @@ __global__ void __launch_bounds__(kStripThreads) k_or_strip(const BatchParams P,
       }
     }
     __syncwarp();
-    {  // a clause may turn non-essential when it has at least one posting per ne_div docs (thick clauses: 1 per 8)
+    {  // a clause may turn non-essential when it has at least one posting per kStripNeDiv docs
       n_e_min = S.n_lists;
-      while (n_e_min > 0 && (unsigned long long)s_list[n_e_min - 1u].doc_freq * P.strip_ne_div >= S.max_doc) --n_e_min;
-      // no such clause: the single densest one may still go if it is dense enough to matter (strip_ne_div2)
-      if (n_e_min == S.n_lists && n_e_min > 1 && (unsigned long long)s_list[n_e_min - 1u].doc_freq * P.strip_ne_div2 >= S.max_doc) --n_e_min;
+      while (n_e_min > 0 && (unsigned long long)s_list[n_e_min - 1u].doc_freq * kStripNeDiv >= S.max_doc) --n_e_min;
+      // no such clause: the single densest one may still go if it is dense enough to matter (kStripNeDiv2)
+      if (n_e_min == S.n_lists && n_e_min > 1 && (unsigned long long)s_list[n_e_min - 1u].doc_freq * kStripNeDiv2 >= S.max_doc) --n_e_min;
     }
     // ---- the windows ---------------------------------------------------------------------------------------
     uint32_t since_refresh = 0;
@@ -1202,6 +1069,7 @@ struct PipeShared {
   uint2 desc[kPipeSlots];  // .x meta (0xFFFFFFFF: VInt tail, no bytes), .y last doc of the previous block, low bit of block index in... see below
   uint32_t blk[kPipeSlots]; // block ordinal (needed for the tail pseudo block)
   PipeWindow win[2];
+  uint32_t npass;           // consumers: pass count of the harvest
 };
 __host__ __device__ constexpr size_t pipe_smem_bytes() {
   return kTileDocs * sizeof(float) + 2 * kTileDocs + kPipeSlots * kPipeSlotBytes;
@@ -1261,6 +1129,7 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
     for (uint32_t i = 0; i < 2; ++i) { mbar_init(&ps.win_full[i], 1); mbar_init(&ps.win_empty[i], kWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     s_top.count = 0; s_top.theta = (unsigned long long)qs->theta << 32;
+    ps.npass = 0;
   }
   for (uint32_t i = threadIdx.x; i < kTileDocs; i += kPipeThreads) s_acc[i] = neg_zero;
   __syncthreads();
@@ -1268,7 +1137,7 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
 
   if (warp == kWarps) {
     // =========================== producer ======================================================================
-    __shared__ uint32_t p_cur[kPipeMaxLists], p_blo[kPipeMaxLists], p_cnt[kPipeMaxLists];
+    __shared__ uint32_t p_cur[kPipeMaxLists], p_cnt[kPipeMaxLists];  // per clause: first block of the window, block count
     if (lane < kPipeMaxLists) p_cur[lane] = 0;
     __syncwarp();
     uint32_t n_item = 0;  // ring item counter
@@ -1281,15 +1150,10 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
       uint32_t total = 0;
       for (uint32_t t = 0; t < S.n_lists; ++t) {
         const ListDesc& L = s_list[t];
-        uint32_t blo = 0, cnt = 0;
-        const uint32_t j_lo = first_block_ge(L.last_doc, p_cur[t], L.n_total, lo, lane);
-        if (j_lo < L.n_total) {
-          uint32_t j_hi = first_block_ge(L.last_doc, j_lo, L.n_total, hi - 1u, lane);
-          if (j_hi >= L.n_total) j_hi = L.n_total - 1u;
-          blo = j_lo; cnt = j_hi - j_lo + 1u;
-        }
+        uint32_t first;
+        const uint32_t cnt = window_blocks(L.last_doc, L.n_total, p_cur[t], lo, hi, lane, first);
         __syncwarp();
-        if (lane == 0) { p_cur[t] = j_lo; p_blo[t] = blo; p_cnt[t] = cnt; }
+        if (lane == 0) { p_cur[t] = first; p_cnt[t] = cnt; }
         total += cnt;
       }
       __syncwarp();
@@ -1311,7 +1175,7 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
       __syncwarp();
       for (uint32_t t = 0; t < S.n_lists; ++t) {
         const ListDesc& L = s_list[t];
-        const uint32_t cnt = p_cnt[t], blo = p_blo[t];
+        const uint32_t cnt = p_cnt[t], blo = p_cur[t];
         // 16 blocks per step, one lane per block.  A slot frees up only when the consumers have added a whole BATCH,
         // and that batch may contain blocks of this very step, so a lane must never make another lane wait: every
         // lane polls its slot once per turn and issues the moment it is free.
@@ -1349,7 +1213,7 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
     }
   } else {
     // =========================== consumers =====================================================================
-    const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, P.counters, 1u, (unsigned)kThreads};
+    const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, 1u, (unsigned)kThreads};
     unsigned int theta_g_seen = 0;
     for (uint32_t wi = 0; wi < n_windows; ++wi) {
       const uint32_t buf = wi & 1u;
@@ -1434,65 +1298,7 @@ __global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P
             pipe_consumer_sync();  // clause order is the f32 summation order
           }
         }
-        // ---- harvest (same as k_or, consumers only) -----------------------------------------------------------
-        const unsigned long long theta = *T.theta;
-        const float theta_f = threshold_score((uint32_t)(theta >> 32));
-        uint32_t passmask = 0;
-#pragma unroll 1
-        for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-          const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-          const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-          if (v.x >= theta_f || v.y >= theta_f || v.z >= theta_f || v.w >= theta_f) {
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const uint32_t dd = lo + idx + c;
-              bool pass = vv[c] >= theta_f && __float_as_uint(vv[c]) != 0x80000000u && make_key(vv[c], dd) >= theta;
-              if (pass && S.alive) pass = is_alive(S.alive, dd);
-              passmask |= pass ? (1u << (j * 4 + c)) : 0u;
-            }
-          }
-        }
-        // room check: the buffer keeps at most kCap - kRoundMargin keys between windows, a window adds at most... see below
-        const uint32_t wsum = __reduce_add_sync(kFull, (uint32_t)__popc(passmask));
-        __shared__ uint32_t s_npass;
-        if (threadIdx.x == 0) s_npass = 0;
-        pipe_consumer_sync();
-        if (lane == 0 && wsum) atomicAdd(&s_npass, wsum);
-        pipe_consumer_sync();
-        const bool fits = *T.count + s_npass <= kCap;
-        pipe_consumer_sync();  // every consumer has read the count before anyone starts pushing (the branch must be uniform)
-        if (fits) {
-#pragma unroll 1
-          for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-            const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-            const uint32_t sub = (passmask >> (j * 4)) & 15u;
-            if (__ballot_sync(kFull, sub != 0)) {
-              const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-              const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-              for (int c = 0; c < 4; ++c) topk_push(T, (sub >> c) & 1u, make_key(vv[c], lo + idx + c), lane);
-            }
-            *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-          }
-          topk_round_end(T, Q.k, &qs->theta);
-        } else {  // cold start: go in rounds with compaction between
-          topk_round_end(T, Q.k, &qs->theta);
-#pragma unroll 1
-          for (int j = 0; j < (int)(kTileDocs / (kThreads * 4)); ++j) {
-            const uint32_t idx = (j * kThreads + threadIdx.x) * 4;
-            const float4 v = *reinterpret_cast<const float4*>(s_acc + idx);
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-            const unsigned long long th = *T.theta;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const unsigned long long key = make_key(vv[c], lo + idx + c);
-              topk_push(T, ((passmask >> (j * 4 + c)) & 1u) && key >= th, key, lane);
-            }
-            *reinterpret_cast<float4*>(s_acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-            topk_round_end(T, Q.k, &qs->theta);
-          }
-        }
+        or_harvest(T, s_acc, S, lo, Q.k, &qs->theta, &ps.npass, lane);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&ps.win_empty[buf]);  // this warp no longer reads the window's table or fieldnorms

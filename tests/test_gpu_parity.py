@@ -371,11 +371,25 @@ def test_synth_mixed_batch(ctx, synth):
     assert_same(g, c, qb.nq)
     st = ctx.stats()
     assert st["units"] > 0 and st["kernel_launches"] >= 3 and st["algorithmic_bytes"] > 0
+    if ctx.engine == "legacy":
+        # or_windows counts k_or_strip's windows alone ([1] exhaustive, [2] hot, [3] cold, [5] bytes read): the k = 100
+        # unions above are strip unions
+        w = st["or_windows"]
+        assert w[1] + w[2] + w[3] > 0 and w[5] > 0 and [w[i] for i in (0, 4, 6, 7)] == [0, 0, 0, 0]
+        # with k > 128 the unions take k_or_pipe; neither it nor the compactions of the term and AND CTAs count there
+        queries = [ix.query(TQ_OP_TERM, [0], 10, segment_base=base), ix.query(TQ_OP_AND, [0, 1], 10, segment_base=base),
+                   ix.query(TQ_OP_OR, [0, 1], 256, segment_base=base), ix.query(TQ_OP_OR, [0, 1, 2, 3, 4, 5], 1000, segment_base=base)]
+        qb = QueryBatch(queries)
+        assert_same(ctx.search_batch(qb), oi.search_batch(qb, mode=0, n_threads=8), qb.nq)
+        st = ctx.stats()
+        assert st["units_or"] > 0 and st["units_or_strip"] == 0
+        assert st["or_windows"] == w
 
 
 def test_synth_union_pruning_is_exact(ctx, synth):
-    """Unions of dense and rare terms with small k make k_or switch to its MaxScore-pruned route after
-    the first windows; the result must stay identical to the exhaustive oracle, hit for hit."""
+    """Unions of dense and rare terms with small k: once the threshold is high enough, k_tile (tile engine) and
+    k_or_strip (per-query kernels) skip the docs that cannot reach it; the result must stay identical to the
+    exhaustive oracle, hit for hit."""
     ix, oi, base = synth
     queries = []
     for k in (1, 3, 10, 50):
