@@ -169,11 +169,12 @@ typedef struct {
   uint64_t tile_groups;         /* query groups evaluated together (one decode-and-score pass each) */
   uint64_t tile_postings;       /* postings decoded and scored by k_score_lists (every distinct list once) */
   uint64_t tile_list_bytes;     /* bytes of those lists' postings ranges (skip data + packed blocks + VInt tails) */
-  uint64_t tile_scratch_bytes;  /* HBM scratch of the pair arrays, tile indexes and samples */
+  uint64_t tile_scratch_bytes;  /* HBM scratch of the pair arrays, tile indexes, samples and k_tile's sparse-slot cursors */
   uint64_t tile_fallbacks;      /* 1 if the run overflowed a tile engine buffer and was repeated (TQ_OP_BOOL on the tile engine, the rest on the per-query kernels) */
   uint64_t tile_counters[8];    /* cumulative, with TQ_TILE_COUNTERS=1: (query, tile) pairs seen / skipped / light / heavy,
                                    essential postings applied, docs completed, docs at or above the threshold;
                                    [7] (always): dynamic shared memory bytes of a k_tile CTA of the last prepared group */
+  uint64_t tile_ctas_per_sm;    /* k_tile CTAs an SM holds at once in the exact launches of the last prepared group (occupancy API) */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */

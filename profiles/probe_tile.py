@@ -40,7 +40,7 @@ for i in range(steps + 2):
     print(json.dumps({"step": i, "prepare_ms": round(1e3 * (t1 - t0), 2), "run_ms": round(1e3 * (t2 - t1), 2),
                       **{k: round(st[k], 3) for k in keys}, "launches": st["kernel_launches"], "units_tile": st["units_tile"],
                       "tile_postings": st["tile_postings"], "scratch_MB": st["tile_scratch_bytes"] >> 20, "fallback": st["tile_fallbacks"],
-                      "groups": st["tile_groups"], "smem": int(c1[7]),
+                      "groups": st["tile_groups"], "smem": int(c1[7]), "tile_ctas_per_sm": st["tile_ctas_per_sm"],
                       "counters(pairs,skip,light,heavy,ess,compl,pass)": (c1 - c0)[:7].tolist()}), flush=True)
     c0 = c1
     bt.close()

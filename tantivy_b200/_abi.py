@@ -119,6 +119,7 @@ class Stats(C.Structure):
         ("tile_scratch_bytes", C.c_uint64),
         ("tile_fallbacks", C.c_uint64),
         ("tile_counters", C.c_uint64 * 8),
+        ("tile_ctas_per_sm", C.c_uint64),
     ]
 
 

@@ -176,7 +176,7 @@ struct tq_ctx {
   uint32_t phrase_side = 1;
   uint32_t tile_terms = 2;
   uint32_t tile_max_slots = kTileMaxSlots, tile_max_queries = kTileMaxQueries, tile_wide_queries = 256;
-  uint64_t tile_smem_last = 0;
+  uint64_t tile_smem_last = 0, tile_ctas_last = 0;
   uint32_t tile_cand_floor = 32768, tile_max_dens_x1000 = 0, tile_pcap_hook = 0, tile_big_min = 6, tile_units = 0;
   uint32_t target_units = 0;  // CTAs a batch's per-query units aim for (4 x 32 per SM)
 };
@@ -327,7 +327,7 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->tile_max_dens_x1000 = env_u32("TQ_TILE_MAX_DENS_X1000", 0);  // test hook: cap on a group's pairs per 1000 docs (forces several groups)
   c->tile_pcap_hook = env_u32("TQ_TILE_PCAP", 0);            // test hook: tile buffer size (forces overflowing tiles)
   c->tile_seg_cap_hook = env_u32("TQ_TILE_SEG_CAP", 0);      // test hook: entries of the per-tile work list (forces extra routing rounds)
-  c->tile_max_slots = std::min<uint32_t>(kTileMaxSlots, std::max<uint32_t>(64u, env_u32("TQ_TILE_MAX_SLOTS", kTileMaxSlots)));  // distinct lists of one segment per group (shared memory per CTA grows by 20 B per list)
+  c->tile_max_slots = std::min<uint32_t>(kTileMaxSlots, std::max<uint32_t>(64u, env_u32("TQ_TILE_MAX_SLOTS", kTileMaxSlots)));  // distinct lists of one segment per group (shared memory per CTA grows by 12 B per list)
   c->tile_max_queries = std::min<uint32_t>(kTileMaxQueries, std::max<uint32_t>(1u, env_u32("TQ_TILE_MAX_QUERIES", kTileMaxQueries)));  // queries of one segment per group
   c->tile_wide_queries = std::max<uint32_t>(1u, env_u32("TQ_TILE_WIDE_QUERIES", 256));  // ... for queries of more than 8 terms
   c->tile_terms = env_u32("TQ_TILE_TERMS", 2);               // single-term queries on the tile engine: 0 never, 1 always, 2 when the batch has multi-term queries
@@ -348,7 +348,11 @@ int tq_ctx_create(int device, tq_ctx** out) {
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kOrDynSmem);
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pipe_smem_bytes());
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)strip_smem_bytes(kMaxCached));
-  if (err == cudaSuccess) err = cudaFuncSetAttribute(k_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  // k_tile's occupancy is bound by shared memory: ask for the largest carveout so that the SM's full 228 KB is there to share
+  for (auto kern : {k_tile<false, false>, k_tile<false, true>, k_tile<true, false>, k_tile<true, true>}) {
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+  }
   if (err != cudaSuccess) { delete c; return fail(TQ_ERR_CUDA, cudaGetErrorString(err)); }
   *out = c;
   return TQ_OK;
@@ -400,6 +404,7 @@ int tq_get_stats(tq_ctx* c, tq_stats* out) {
   if (cudaMemcpy(h, c->d_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
     for (int i = 0; i < 8; ++i) { out->or_windows[i] = h[i]; out->tile_counters[i] = h[8 + i]; }
   out->tile_counters[7] = c->tile_smem_last;
+  out->tile_ctas_per_sm = c->tile_ctas_last;
   return TQ_OK;
 }
 
@@ -1464,7 +1469,7 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
 
   // ---- tile scratch: pair arrays | tile indexes | samples | sample counts | flags + counters --------------------------------
   uint32_t sample_cap = 0;
-  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0;
+  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0, to_cursors = 0;
   if (!pl.gstage.empty()) {
     uint64_t sample_units_tiles = 0;
     for (auto& gs : pl.gstage) for (auto& u : gs.units[0]) sample_units_tiles += u.t1 - u.t0;
@@ -1476,6 +1481,10 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     to_samples = so2; so2 = align256(so2 + nq1 * sample_cap * 4);
     to_scount = so2; so2 = align256(so2 + nq1 * 4);
     to_flags = so2; so2 = align256(so2 + 256);
+    size_t cursors = 0;  // k_tile's sparse-slot cursors: max_slots per CTA of the largest launch (launches of a batch run one after another)
+    for (auto& gs : pl.gstage)
+      for (auto& u : gs.units) cursors = std::max<size_t>(cursors, u.size() * gs.max_slots);
+    to_cursors = so2; so2 = align256(so2 + cursors * sizeof(uint2));
     pl.tile_bytes = so2;
     TQ_CUDA(b->tile_dev.ensure(pl.tile_bytes));
   }
@@ -1518,6 +1527,7 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     TP.sample_count = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_scount);
     TP.flags = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_flags);
     TP.counters = c->tile_counters ? c->d_counters + 8 : nullptr;
+    TP.cursors = reinterpret_cast<uint2*>(b->tile_dev.p + to_cursors);
     TP.sample_cap = sample_cap;
     TP.p_cap = gs.p_cap;
     TP.max_slots = gs.max_slots;
@@ -1533,6 +1543,9 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     run.smem = tile_smem_bytes(gs.p_cap, gs.max_slots, TP.max_big, TP.max_queries, TP.seg_cap, TP.cl_cap, TP.n_win);
     c->tile_smem_last = run.smem;
     if (run.smem > 200u * 1024u) return fail(TQ_ERR_UNSUPPORTED, "tile group needs more shared memory than an SM has");
+    int ctas = 0;
+    TQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k_tile<false, false>, kTileThreads, run.smem));
+    c->tile_ctas_last = (uint64_t)ctas;
   }
 
   // ---- scratch: qstate | candidates | results ------------------------------------------------------
@@ -1675,7 +1688,9 @@ static int launch_tile_round(tq_batch* b, int r, uint64_t* launches) {
   const int sp = span_begin(b, SPAN_TILE);
   for (auto& g : b->groups) {
     if (!g.n_units[r]) continue;
-    k_tile<<<g.n_units[r], kTileThreads, g.smem, b->stream>>>(b->params, g.params, g.unit_base[r], r == 0 ? 1u : 0u);
+    const bool counters = g.params.counters != nullptr;
+    auto kern = r == 0 ? (counters ? k_tile<true, true> : k_tile<true, false>) : (counters ? k_tile<false, true> : k_tile<false, false>);
+    kern<<<g.n_units[r], kTileThreads, g.smem, b->stream>>>(b->params, g.params, g.unit_base[r]);
     ++*launches;
   }
   span_end(b, sp);

@@ -101,6 +101,8 @@ struct TileParams {
   uint32_t* flags;         // [0]: a tile held more pairs than p_cap (the batch is re-run on the per-query kernels)
   unsigned long long* counters;  // [8] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
                                  //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold
+                                 //     (null: the launch runs k_tile<*, false>)
+  uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
   uint32_t sample_cap;
   uint32_t p_cap;      // pairs of one tile that fit in shared memory
   uint32_t max_slots;  // largest n_slots of any segment of the group
@@ -267,7 +269,9 @@ struct TileTQ {
   uint8_t n_clauses;
   uint8_t op_flags;      // op [0:2) | Intersection order << 5 | phrase << 6 | prunable << 7
 };
-struct TileSeg { uint16_t q, clause, start, len; };  // postings [start, start + len) of one essential clause of flat pair q
+// one essential clause of flat pair q: its postings in the tile are the slot's staged range (s_info of cl[clause]; the sample
+// launch takes at most kSampleSeg of them)
+struct TileSeg { uint16_t q, clause; };
 
 // Union: the doc at tile offset `off`, met as posting p of essential clause c.  Exact score in the canonical order, or nothing when
 // the bounds show it cannot reach the threshold.  Returns true when `sum` is a complete score.
@@ -377,33 +381,39 @@ __device__ __forceinline__ bool tile_eval_bool(const TileView& V, const uint16_t
 }
 
 constexpr uint32_t kTileStageWords = 2u * kTileMaxBig + kTileWarps * 17u;
-// Shared memory of a k_tile CTA: the work list (TileQ records + segments) and two windows for the rare heavy pairs ...
+// Shared memory of a k_tile CTA: the work list (TileQ records + segments), and in the same bytes the windows of the rare heavy
+// pairs (stage B3 starts after the last B2 of the tile) ...
 __host__ __device__ constexpr size_t tile_union_bytes(uint32_t max_queries, uint32_t seg_cap, uint32_t n_win) {
   // (the segment list doubles as stage A's scratch: never smaller than kTileStageWords words)
   const size_t seg_bytes = (size_t)seg_cap * sizeof(TileSeg) > kTileStageWords * 4u ? (size_t)seg_cap * sizeof(TileSeg) : kTileStageWords * 4u;
-  return ((size_t)n_win * kTile * 4 + (size_t)max_queries * sizeof(TileQ) + seg_bytes + 15) & ~(size_t)15;
+  const size_t list_bytes = (size_t)max_queries * sizeof(TileQ) + seg_bytes, win_bytes = (size_t)n_win * kTile * 4;
+  return ((list_bytes > win_bytes ? list_bytes : win_bytes) + 15) & ~(size_t)15;
 }
+// (the sparse slots' cursors are not on chip: TileParams::cursors)
 __host__ __device__ constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries, uint32_t seg_cap,
                                                       uint32_t cl_cap, uint32_t n_win, uint32_t has_phrase = 0) {
-  return (size_t)p_cap * 4 + tile_union_bytes(max_queries, seg_cap, n_win) + (size_t)max_slots * 20 + (size_t)max_big * 128 +
+  return (size_t)p_cap * 4 + tile_union_bytes(max_queries, seg_cap, n_win) + (size_t)max_slots * 12 + (size_t)max_big * 128 +
          (size_t)max_queries * sizeof(TileTQ) + (size_t)max_big * 64 + (size_t)p_cap * 2 + (size_t)max_queries * 2 + (size_t)cl_cap * 2 + 64 +
          (has_phrase ? (size_t)max_slots * 4 + 8 : 0);
 }
 
-__global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, const TileParams TP, uint32_t unit_base, uint32_t sample_mode) {
+// One instantiation per launch kind, so that each compiles only what it runs: kSample = the sample launch (threshold samples
+// instead of candidates), kCounters = TQ_TILE_COUNTERS diagnostics.  The exact launches without counters do ~90 % of the
+// work; they must fit 64 registers so that four CTAs share an SM.
+template <bool kSample, bool kCounters>
+__global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_tile(const BatchParams P, const TileParams TP, uint32_t unit_base) {
+  constexpr bool sample_mode = kSample;
   extern __shared__ __align__(16) unsigned char s_dyn[];
   float* s_score = reinterpret_cast<float*>(s_dyn);                            // [p_cap]
   unsigned char* s_union = reinterpret_cast<unsigned char*>(s_score + TP.p_cap);
   const size_t union_bytes = tile_union_bytes(TP.max_queries, TP.seg_cap, TP.n_win);
   const uint32_t n_win = TP.n_win;
-  float* s_acc = reinterpret_cast<float*>(s_union);                            // [n_win][kTile] windows of the heavy pairs
-  TileQ* s_q = reinterpret_cast<TileQ*>(s_acc + n_win * kTile);                // [max_queries] flat pairs of this tile
+  TileQ* s_q = reinterpret_cast<TileQ*>(s_union);                              // [max_queries] flat pairs of this tile (B1, B2)
   TileSeg* s_seg = reinterpret_cast<TileSeg*>(s_q + TP.max_queries);           // [seg_cap]
+  float* s_acc = reinterpret_cast<float*>(s_union);                            // [n_win][kTile] windows of the heavy pairs (B3)
   uint32_t* s_info = reinterpret_cast<uint32_t*>(s_union + union_bytes);       // [max_slots]
   float* s_max = reinterpret_cast<float*>(s_info + TP.max_slots);              // [max_slots] largest score of the slot in this tile (>= 0)
-  uint32_t* s_cur = reinterpret_cast<uint32_t*>(s_max + TP.max_slots);         // [max_slots] small slots: first pair not staged yet
-  uint32_t* s_nxt = s_cur + TP.max_slots;                                      // [max_slots] ... and its doc (0xFFFFFFFF: list exhausted)
-  uint32_t* s_mask = s_nxt + TP.max_slots;                                     // [max_slots] stripe masks of the sparse slots
+  uint32_t* s_mask = reinterpret_cast<uint32_t*>(s_max + TP.max_slots);        // [max_slots] stripe masks of the sparse slots
   uint32_t* s_bits = s_mask + TP.max_slots;                                    // [max_big][32]
   TileTQ* s_tq = reinterpret_cast<TileTQ*>(s_bits + TP.max_big * 32u);         // [max_queries] this segment's queries
   uint16_t* s_rank = reinterpret_cast<uint16_t*>(s_tq + TP.max_queries);       // [max_big][32]
@@ -427,8 +437,10 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const float neg_zero = __uint_as_float(0x80000000u);
   const TileView V{s_off, s_score, s_info, s_bits, s_rank, s_mask, G.n_big};
-  for (uint32_t i = tid; i < n_win * kTile; i += kTileThreads) s_acc[i] = neg_zero;
-  if (tid < 8) s_stat[tid] = 0ull;
+  // sparse slots: (first pair not staged yet, its doc or 0xFFFFFFFF once the list is exhausted), this CTA's share of the
+  // launch's cursor scratch; slot s is always walked by the same thread, so no barrier guards it
+  uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
+  if (kCounters && tid < 8) s_stat[tid] = 0ull;
   if (tid < kTileMaxQueries / 32u) s_defer[tid] = 0u;
   // the segment's queries and their clause slots are read for every tile: keep them on chip (clause_base becomes an index into cl0)
   const bool cl_staged = G.n_clause_words <= TP.cl_cap;
@@ -470,10 +482,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const uint32_t s = s0 + (uint32_t)j * kTileThreads;
-      if (s < G.n_slots) {
-        s_cur[s] = a[j];
-        s_nxt[s] = a[j] < df[j] ? __ldg(d[j] + a[j]) : 0xFFFFFFFFu;
-      }
+      if (s < G.n_slots) cursor[s] = make_uint2(a[j], a[j] < df[j] ? __ldg(d[j] + a[j]) : 0xFFFFFFFFu);
     }
   }
   __syncthreads();
@@ -555,8 +564,11 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
         }
       }
     }
+    uint2 next_cur = G.n_big + tid < G.n_slots ? cursor[G.n_big + tid] : make_uint2(0u, 0u);
     for (uint32_t s = G.n_big + tid; s < G.n_slots; s += kTileThreads) {  // sparse lists: one thread walks its cursor
-      uint32_t nd = s_nxt[s];
+      const uint2 cs = next_cur;
+      if (s + kTileThreads < G.n_slots) next_cur = cursor[s + kTileThreads];  // (in flight while this slot is staged)
+      uint32_t nd = cs.y;
       if (nd >= hi) {
         s_info[s] = 0u; s_max[s] = 0.0f; s_mask[s] = 0u;
         continue;
@@ -564,7 +576,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
       const TSlot sl = slots[s];
       const uint32_t* __restrict__ d = TP.p_docs + sl.pair_base;
       const float* __restrict__ sc = TP.p_scores + sl.pair_base;
-      const uint32_t cur = s_cur[s];
+      const uint32_t cur = cs.x;
       // the pair at the cursor belongs to this tile (nd < hi); fetch it and the next three, docs and scores, in ONE round trip
       uint32_t d4[4];
       float v4[4];
@@ -592,8 +604,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
       } else {
         nd = d4[n];
       }
-      s_cur[s] = cur + n;
-      s_nxt[s] = nd;
+      cursor[s] = make_uint2(cur + n, nd);
       if (nd < hi + kTile) {  // the next tile reads this list again: start its pairs on their way to L2 now
         asm volatile("prefetch.global.L2 [%0];" ::"l"(d + cur + n));
         asm volatile("prefetch.global.L2 [%0];" ::"l"(sc + cur + n));
@@ -732,20 +743,14 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
           const uint32_t qslot = atomicAdd(&s_nflat, 1u);
           s_q[qslot] = rec;
           uint32_t w = sb;
-          const uint32_t len_cap = sample_mode ? kSampleSeg : 0xFFFFu;
           if (op == kTileOpBool) {
-            for (uint32_t e = 0; e < b_dn; ++e) {
-              const uint32_t info = s_info[cl[b_d0 + e]];
-              if (info >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)(b_d0 + e), (uint16_t)(info & 0xFFFFu), (uint16_t)min(info >> 16, len_cap)};
-            }
+            for (uint32_t e = 0; e < b_dn; ++e)
+              if (s_info[cl[b_d0 + e]] >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)(b_d0 + e)};
           } else if (op == kTileOpAnd) {
-            const uint32_t info = s_info[cl[rec_ne]];
-            s_seg[w] = TileSeg{(uint16_t)qslot, (uint16_t)rec_ne, (uint16_t)(info & 0xFFFFu), (uint16_t)min(info >> 16, len_cap)};
+            s_seg[w] = TileSeg{(uint16_t)qslot, (uint16_t)rec_ne};
           } else {
-            for (uint32_t c = 0; c < rec_ne; ++c) {
-              const uint32_t info = s_info[cl[c]];
-              if (info >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)c, (uint16_t)(info & 0xFFFFu), (uint16_t)min(info >> 16, len_cap)};
-            }
+            for (uint32_t c = 0; c < rec_ne; ++c)
+              if (s_info[cl[c]] >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)c};
           }
           ++st_flat;
           st_ess += cnt;
@@ -764,25 +769,31 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
         sbase = __shfl_sync(kFull, sbase, 0);
         if (sbase >= n_seg) break;
         // 32 segments, one per lane; their postings are dealt to the lanes 32 at a time (load-balanced expansion)
-        TileSeg mine = TileSeg{0, 0, 0, 0};
-        if (sbase + lane < n_seg) mine = s_seg[sbase + lane];
-        const uint32_t incl = warp_incl_scan((uint32_t)mine.len, lane);
+        uint32_t m_len = 0, m_qc = 0, m_start = 0;  // the lane's segment: postings [m_start, m_start + m_len), q | clause << 16
+        if (sbase + lane < n_seg) {
+          const TileSeg sg = s_seg[sbase + lane];
+          const uint32_t info = s_info[cl0[s_tq[s_q[sg.q].qi].clause_base + sg.clause]];
+          m_qc = sg.q | ((uint32_t)sg.clause << 16);
+          m_start = info & 0xFFFFu;
+          m_len = sample_mode ? min(info >> 16, kSampleSeg) : info >> 16;
+        }
+        const uint32_t incl = warp_incl_scan(m_len, lane);
         const uint32_t total = __shfl_sync(kFull, incl, 31);
-        const uint32_t excl = incl - mine.len;
+        const uint32_t excl = incl - m_len;
+        const uint32_t m_pbase = m_start - excl;  // (mod 2^32) the pair index of the chunk item ibase + lane is m_pbase + ibase + lane
         for (uint32_t ibase = 0; ibase < total; ibase += 32u) {
           const uint32_t item = ibase + lane;
           // the segment of item `ibase + lane`: every listed segment holds a posting, so segment numbers grow by one at each
           // start; (segments that start before this chunk) - 1 + (starts at or before the lane's item)
           const uint32_t rel = excl - ibase;  // (wraps for segments that start before the chunk)
-          const uint32_t starts = __reduce_or_sync(kFull, (mine.len && rel < 32u) ? (1u << rel) : 0u);
-          const uint32_t earlier = (uint32_t)__popc(__ballot_sync(kFull, mine.len && excl < ibase));
+          const uint32_t starts = __reduce_or_sync(kFull, (m_len && rel < 32u) ? (1u << rel) : 0u);
+          const uint32_t earlier = (uint32_t)__popc(__ballot_sync(kFull, m_len && excl < ibase));
           const uint32_t j = earlier - 1u + (uint32_t)__popc(starts & (0xFFFFFFFFu >> (31u - lane)));
-          const uint32_t incl_j = __shfl_sync(kFull, incl, j & 31u);
+          const uint32_t p = __shfl_sync(kFull, m_pbase, j & 31u) + item;
+          const uint32_t qc = __shfl_sync(kFull, m_qc, j & 31u);
           uint32_t s_query = 0xFFFFFFFFu - lane, s_key = 0;  // sample launch: this lane's sample (if any), handed over below
           if (item < total) {
-            const TileSeg sg = s_seg[sbase + j];
-            const uint32_t before = incl_j - sg.len;
-            const uint32_t p = sg.start + (item - before);
+            const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
             const TileQ q = s_q[sg.q];
             const TileTQ qq = s_tq[q.qi];
             const uint16_t* __restrict__ cl = cl0 + qq.clause_base;
@@ -823,6 +834,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
     // ---- stage B3: one warp per heavy pair, a window of f32 score slots ----------------------------------------------------
     {
       const uint32_t n_heavy = s_nheavy;
+      if (n_heavy) __syncthreads();  // the windows overlay the work list: every warp must be done with B2
       float* acc = s_acc + warp * kTile;
       for (; warp < n_win;) {  // (the warps without a window go straight to the barrier)
         uint32_t h = 0;
@@ -919,6 +931,9 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
             --n_e;
           }
         }
+        for (uint32_t g = 0; g < kTile / 128u; ++g)  // -0.0 = untouched (-0.0 + s == s)
+          *reinterpret_cast<float4*>(acc + g * 128u + lane * 4u) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
+        __syncwarp();
         float wmax = 0.0f;
         for (uint32_t c = 0; c < n_e; ++c) {  // clause order is the f32 summation order
           const uint32_t info = s_info[cl[c]];
@@ -938,7 +953,6 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
           for (uint32_t g = 0; g < kTile / 128u; ++g) {
             const uint32_t idx = g * 128u + lane * 4u;
             const float4 v = *reinterpret_cast<const float4*>(acc + idx);
-            *reinterpret_cast<float4*>(acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
             const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
             for (int c = 0; c < 4; ++c)
@@ -961,12 +975,9 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
         const float mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(wmax)));
         const bool cold = prune && (mx + ne) * 1.00001f < theta_f;
         if (cold && lane == 0) ++st_skip;
-        for (uint32_t g = 0; g < kTile / 128u; ++g) {
+        for (uint32_t g = 0; g < kTile / 128u && !cold; ++g) {
           const uint32_t idx = g * 128u + lane * 4u;
-          float4 v = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-          if (!cold) v = *reinterpret_cast<const float4*>(acc + idx);
-          *reinterpret_cast<float4*>(acc + idx) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-          if (cold) continue;
+          const float4 v = *reinterpret_cast<const float4*>(acc + idx);
           const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
@@ -994,7 +1005,7 @@ __global__ void __launch_bounds__(kTileThreads, 3) k_tile(const BatchParams P, c
     }
     __syncthreads();
   }
-  if (TP.counters) {
+  if constexpr (kCounters) {
     // warp-aggregated diagnostics
     unsigned long long v[7] = {st_pairs, st_skip, st_flat, st_heavy, st_ess, st_compl, st_push};
 #pragma unroll
