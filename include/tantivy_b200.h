@@ -175,6 +175,8 @@ typedef struct {
                                    essential postings applied, docs completed, docs at or above the threshold;
                                    [7] (always): dynamic shared memory bytes of a k_tile CTA of the last prepared group */
   uint64_t tile_ctas_per_sm;    /* k_tile CTAs an SM holds at once in the exact launches of the last prepared group (occupancy API) */
+  uint64_t tile_cycles[8];      /* cumulative, with TQ_TILE_COUNTERS=1: k_tile warp cycles (clock64) by stage: [0] cursor prologue,
+                                   [1] A (staging), [2] B1 (routing), [3] B2 (flat evaluation), [4] B3 (windows), [5] barrier waits */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */

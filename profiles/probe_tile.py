@@ -1,4 +1,4 @@
-"""Probe of the tile engine on a bench workload: per-kind kernel times, tile counters, parity of a query sample.
+"""Probe of the tile engine on a bench workload: per-kind kernel times, tile counters, k_tile's cycles by stage, parity of a query sample.
 usage: python profiles/probe_tile.py [workload] [nq] [steps] [check]   (env knobs: TQ_TILE*, see tq_ctx_create)"""
 import json
 import os
@@ -27,7 +27,18 @@ ctx = T.Context(0)
 shard.register(ctx)
 qbs = [bench.marshal(shard, b) for b in batches]
 keys = keys_ms = ("kernel_ms", "score_ms", "tile_ms", "theta_ms", "final_ms", "or_ms", "and_ms", "term_ms")
+STAGES = ("prologue", "A", "B1", "B2", "B3", "barrier")
+
+
+def stage_shares(cyc):
+    """k_tile's warp cycles by stage (tq_stats.tile_cycles, TQ_TILE_COUNTERS=1) as shares of their sum."""
+    tot = int(cyc[:len(STAGES)].sum())
+    return {s: round(int(c) / tot, 4) for s, c in zip(STAGES, cyc)} if tot else {}
+
+
 c0 = np.array(ctx.stats()["tile_counters"], dtype=np.int64)
+y0 = np.array(ctx.stats()["tile_cycles"], dtype=np.int64)
+y_first = None
 for i in range(steps + 2):
     t0 = time.perf_counter()
     bt = ctx.prepare(qbs[i % 2])
@@ -37,13 +48,21 @@ for i in range(steps + 2):
     t2 = time.perf_counter()
     st = ctx.stats()
     c1 = np.array(st["tile_counters"], dtype=np.int64)
+    y1 = np.array(st["tile_cycles"], dtype=np.int64)
+    if i == 2:
+        y_first = y0  # (the first two steps warm up: the summary below covers the rest)
     print(json.dumps({"step": i, "prepare_ms": round(1e3 * (t1 - t0), 2), "run_ms": round(1e3 * (t2 - t1), 2),
                       **{k: round(st[k], 3) for k in keys}, "launches": st["kernel_launches"], "units_tile": st["units_tile"],
                       "tile_postings": st["tile_postings"], "scratch_MB": st["tile_scratch_bytes"] >> 20, "fallback": st["tile_fallbacks"],
                       "groups": st["tile_groups"], "smem": int(c1[7]), "tile_ctas_per_sm": st["tile_ctas_per_sm"],
-                      "counters(pairs,skip,light,heavy,ess,compl,pass)": (c1 - c0)[:7].tolist()}), flush=True)
-    c0 = c1
+                      "counters(pairs,skip,light,heavy,ess,compl,pass)": (c1 - c0)[:7].tolist(),
+                      "stage_shares": stage_shares(y1 - y0)}), flush=True)
+    c0, y0 = c1, y1
     bt.close()
+if y_first is not None and (y0 - y_first).any():
+    d = y0 - y_first
+    print(json.dumps({"k_tile_stage_cycles(steps 2..)": dict(zip(STAGES, d[:len(STAGES)].tolist())), "stage_shares": stage_shares(d),
+                      "B1+B2": round(float(d[2] + d[3]) / float(d[:len(STAGES)].sum()), 4)}), flush=True)
 if os.environ.get("PROBE_THETA"):
     # how much better would the step be with (nearly) final thresholds from the start?  Run a batch up to its last phase, keep
     # its thresholds, then run the same batch again with those thresholds imported after the sample phase.

@@ -120,6 +120,7 @@ class Stats(C.Structure):
         ("tile_fallbacks", C.c_uint64),
         ("tile_counters", C.c_uint64 * 8),
         ("tile_ctas_per_sm", C.c_uint64),
+        ("tile_cycles", C.c_uint64 * 8),
     ]
 
 

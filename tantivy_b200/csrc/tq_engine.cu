@@ -168,7 +168,7 @@ struct tq_ctx {
   std::vector<tq_batch*> pool;
   tq_stats stats{};
   uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit;
-  unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics
+  unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 16, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
   uint32_t tile_ops = 7;  // bit per TQ_OP_*: which query shapes the tile engine takes
   uint32_t tile_seg_cap_hook = 0;
@@ -182,6 +182,15 @@ struct tq_ctx {
 };
 
 constexpr int kTileRounds = 4;  // launches of k_tile per run: the sample launch + three exact ones
+constexpr int kCounterWords = 24;  // tq_ctx::d_counters
+
+// The k_tile instances, indexed sample launch << 2 | counters << 1 | union-only (tile_kernel).
+using TileKernel = void (*)(const BatchParams, const TileParams, uint32_t);
+static const TileKernel kTileKernels[8] = {k_tile<false, false, false>, k_tile<false, false, true>, k_tile<false, true, false>, k_tile<false, true, true>,
+                                           k_tile<true, false, false>,  k_tile<true, false, true>,  k_tile<true, true, false>,  k_tile<true, true, true>};
+static TileKernel tile_kernel(bool sample, bool counters, bool union_only) {
+  return kTileKernels[(sample ? 4 : 0) + (counters ? 2 : 0) + (union_only ? 1 : 0)];
+}
 
 // Unit classes of the per-query kernels: the order of tq_batch::n_units / unit_base and of the batch's Unit array.
 enum UnitClass : int {
@@ -237,6 +246,7 @@ struct tq_batch {
     uint32_t n_chunks = 0;
     uint32_t unit_base[kTileRounds] = {0, 0, 0, 0}, n_units[kTileRounds] = {0, 0, 0, 0};
     size_t smem = 0;
+    bool union_only = false;  // the group's queries are all term queries and unions: the k_tile<*, *, true> instances run it
   };
   tq_ctx* ctx = nullptr;
   cudaStream_t stream = nullptr;
@@ -342,14 +352,14 @@ int tq_ctx_create(int device, tq_ctx** out) {
   if (err == cudaSuccess) err = cudaMalloc(&c->d_pos_descs, (size_t)c->pos_cap * sizeof(PosDesc));
   if (err == cudaSuccess) err = cudaMemset(c->d_pos_descs, 0, (size_t)c->pos_cap * sizeof(PosDesc));
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_phrase, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)phrase_smem_bytes(kPhraseMaxTerms));
-  if (err == cudaSuccess) err = cudaMalloc(&c->d_counters, 16 * sizeof(unsigned long long));
-  if (err == cudaSuccess) err = cudaMemset(c->d_counters, 0, 16 * sizeof(unsigned long long));
+  if (err == cudaSuccess) err = cudaMalloc(&c->d_counters, kCounterWords * sizeof(unsigned long long));
+  if (err == cudaSuccess) err = cudaMemset(c->d_counters, 0, kCounterWords * sizeof(unsigned long long));
   if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&c->build_stream, cudaStreamNonBlocking);
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kOrDynSmem);
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pipe_smem_bytes());
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)strip_smem_bytes(kMaxCached));
   // k_tile's occupancy is bound by shared memory: ask for the largest carveout so that the SM's full 228 KB is there to share
-  for (auto kern : {k_tile<false, false>, k_tile<false, true>, k_tile<true, false>, k_tile<true, true>}) {
+  for (auto kern : kTileKernels) {
     if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
   }
@@ -400,9 +410,9 @@ int tq_get_stats(tq_ctx* c, tq_stats* out) {
   *out = c->stats;
   out->lists_cached = c->list_cache.size();
   cudaSetDevice(c->device);
-  unsigned long long h[16];
+  unsigned long long h[kCounterWords];
   if (cudaMemcpy(h, c->d_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
-    for (int i = 0; i < 8; ++i) { out->or_windows[i] = h[i]; out->tile_counters[i] = h[8 + i]; }
+    for (int i = 0; i < 8; ++i) { out->or_windows[i] = h[i]; out->tile_counters[i] = h[8 + i]; out->tile_cycles[i] = h[16 + i]; }
   out->tile_counters[7] = c->tile_smem_last;
   out->tile_ctas_per_sm = c->tile_ctas_last;
   return TQ_OK;
@@ -861,6 +871,7 @@ struct GroupStage {
   std::vector<SChunk> chunks;
   uint32_t max_slots = 1, p_cap = 1024, max_big = 1, max_queries = 1, max_clause_words = 0, max_clauses = 1;
   size_t tix_words = 0;
+  bool union_only = true;  // every TQuery is a term query or a union (k_tile<*, *, true>)
 };
 
 // A (query, segment) of the per-query kernels, beside its QSeg: its unit class, the blocks / windows / tiles its units cover, and
@@ -1378,6 +1389,7 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         gs.queries.push_back(t2);
         kmax_g = std::max(kmax_g, pl.dq[tq.query].k);
         gs.max_clauses = std::max<uint32_t>(gs.max_clauses, tq.n_clauses);
+        if (tq.op == kTileOpAnd || tq.op == kTileOpBool || (tq.flags & 2u)) gs.union_only = false;
         // clause slots follow the permutation (the structure words of TQ_OP_BOOL queries do not)
         uint16_t* w = gs.clauses.data() + t2.clause_base;
         if (tq.op == kTileOpBool) map_bool_clauses(w, tq.n_clauses, [&](uint16_t s) { return new_of[s]; });
@@ -1544,7 +1556,9 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     c->tile_smem_last = run.smem;
     if (run.smem > 200u * 1024u) return fail(TQ_ERR_UNSUPPORTED, "tile group needs more shared memory than an SM has");
     int ctas = 0;
-    TQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k_tile<false, false>, kTileThreads, run.smem));
+    run.union_only = gs.union_only;
+    // (the exact instance the group runs without TQ_TILE_COUNTERS: the counters instances are built for 3 CTAs per SM)
+    TQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, tile_kernel(false, false, run.union_only), kTileThreads, run.smem));
     c->tile_ctas_last = (uint64_t)ctas;
   }
 
@@ -1688,8 +1702,7 @@ static int launch_tile_round(tq_batch* b, int r, uint64_t* launches) {
   const int sp = span_begin(b, SPAN_TILE);
   for (auto& g : b->groups) {
     if (!g.n_units[r]) continue;
-    const bool counters = g.params.counters != nullptr;
-    auto kern = r == 0 ? (counters ? k_tile<true, true> : k_tile<true, false>) : (counters ? k_tile<false, true> : k_tile<false, false>);
+    auto kern = tile_kernel(r == 0, g.params.counters != nullptr, g.union_only);
     kern<<<g.n_units[r], kTileThreads, g.smem, b->stream>>>(b->params, g.params, g.unit_base[r]);
     ++*launches;
   }

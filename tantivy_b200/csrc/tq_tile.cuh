@@ -99,9 +99,10 @@ struct TileParams {
   uint32_t* samples;       // [n_queries of the batch][sample_cap] score keys
   uint32_t* sample_count;  // [n_queries of the batch]
   uint32_t* flags;         // [0]: a tile held more pairs than p_cap (the batch is re-run on the per-query kernels)
-  unsigned long long* counters;  // [8] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
-                                 //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold
-                                 //     (null: the launch runs k_tile<*, false>)
+  unsigned long long* counters;  // [16] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
+                                 //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold;
+                                 //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage)
+                                 //     (null: the launch runs k_tile<*, false, *>)
   uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
   uint32_t sample_cap;
   uint32_t p_cap;      // pairs of one tile that fit in shared memory
@@ -273,15 +274,15 @@ struct TileTQ {
 // launch takes at most kSampleSeg of them)
 struct TileSeg { uint16_t q, clause; };
 
-// Union: the doc at tile offset `off`, met as posting p of essential clause c.  Exact score in the canonical order, or nothing when
-// the bounds show it cannot reach the threshold.  Returns true when `sum` is a complete score.
-__device__ __forceinline__ bool tile_eval_or(const TileView& V, const float* __restrict__ s_max, const uint16_t* __restrict__ cl, const TileQ& q,
-                                             uint32_t c, uint32_t p, uint32_t off, float theta_f, float& sum) {
+// Union: the doc at tile offset `off`, met as posting p of essential clause c (of n_e; n clauses, ne and shared_stripes as in TileQ).
+// Exact score in the canonical order, or nothing when the bounds show it cannot reach the threshold.  Returns true when `sum` is a
+// complete score.
+__device__ __forceinline__ bool tile_eval_or(const TileView& V, const float* __restrict__ s_max, const uint16_t* __restrict__ cl, uint32_t n_e,
+                                             uint32_t n, bool prune, float ne, uint32_t shared_stripes, uint32_t c, uint32_t p, uint32_t off,
+                                             float theta_f, float& sum) {
   bool f;
-  const uint32_t n_e = q.n_e(), n = q.n();
-  const bool prune = q.prune();
   sum = V.s_score[p];  // (-0.0 + s == s: SumCombiner starts from 0, score_combiner.rs:39-57)
-  if ((q.shared_stripes >> (off >> 5)) & 1u) {  // another essential clause lists a doc near this one: look the doc up
+  if ((shared_stripes >> (off >> 5)) & 1u) {  // another essential clause lists a doc near this one: look the doc up
     for (uint32_t c1 = 0; c1 < c; ++c1) {  // an earlier essential clause lists the doc: it is evaluated there
       tile_find(V, cl[c1], off, f);
       if (f) return false;
@@ -292,7 +293,7 @@ __device__ __forceinline__ bool tile_eval_or(const TileView& V, const float* __r
     }
   }
   // the non-essential suffix, densest last; stop as soon as what is left cannot lift the doc over the threshold
-  float rem = q.ne;
+  float rem = ne;
   for (uint32_t c2 = n_e; c2 < n; ++c2) {
     if (prune && (sum + rem) * 1.00001f < theta_f) return false;
     const uint32_t slot = cl[c2];
@@ -397,12 +398,28 @@ __host__ __device__ constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t ma
          (has_phrase ? (size_t)max_slots * 4 + 8 : 0);
 }
 
+// Stages of a tile as the cycle counters of k_tile<*, true, *> split a warp's time (TileParams::counters[8 + stage],
+// tq_stats.tile_cycles): the cursor prologue, A, B1, B2, B3, and the waits at the barriers between them.
+enum TileStage : int { kStPrologue, kStA, kStB1, kStB2, kStB3, kStBarrier, kTileStages };
+
 // One instantiation per launch kind, so that each compiles only what it runs: kSample = the sample launch (threshold samples
-// instead of candidates), kCounters = TQ_TILE_COUNTERS diagnostics.  The exact launches without counters do ~90 % of the
-// work; they must fit 64 registers so that four CTAs share an SM.
-template <bool kSample, bool kCounters>
+// instead of candidates), kCounters = TQ_TILE_COUNTERS diagnostics, kUnionOnly = every query of the group is a term query or a
+// union (no conjunction, no TQ_OP_BOOL, no phrase: the flat path broadcasts each work-list segment's query state from the lane
+// that reads the segment).  The exact launches without counters do ~90 % of the work; they must fit 64 registers so that four
+// CTAs share an SM.
+template <bool kSample, bool kCounters, bool kUnionOnly>
 __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_tile(const BatchParams P, const TileParams TP, uint32_t unit_base) {
   constexpr bool sample_mode = kSample;
+  // kCounters: each warp's clock64() time by stage (lane 0's view of it); mark(k) books the time since the previous mark to stage k
+  long long clk_last = kCounters ? clock64() : 0;
+  unsigned long long cyc[kTileStages] = {};
+  auto mark = [&](int k) {
+    if constexpr (kCounters) {
+      const long long now = clock64();
+      cyc[k] += (unsigned long long)(now - clk_last);
+      clk_last = now;
+    }
+  };
   extern __shared__ __align__(16) unsigned char s_dyn[];
   float* s_score = reinterpret_cast<float*>(s_dyn);                            // [p_cap]
   unsigned char* s_union = reinterpret_cast<unsigned char*>(s_score + TP.p_cap);
@@ -421,10 +438,10 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   uint16_t* s_heavy = s_off + TP.p_cap;                                        // [max_queries]
   uint16_t* s_cl = s_heavy + TP.max_queries;                                   // [cl_cap] this segment's clause slots
   // [max_slots] phrase groups only: index (into the pair arrays) of the slot's first pair staged for the current tile
-  uint32_t* s_ord0 = TP.has_phrase ? reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(s_cl + TP.cl_cap) + 3u) & ~(uintptr_t)3u) : nullptr;
+  uint32_t* s_ord0 = !kUnionOnly && TP.has_phrase ? reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(s_cl + TP.cl_cap) + 3u) & ~(uintptr_t)3u) : nullptr;
   __shared__ uint32_t s_total, s_nheavy, s_hpos, s_nflat, s_nseg, s_segpos, s_segvalid, s_ndefer;
   __shared__ uint32_t s_defer[kTileMaxQueries / 32u];  // queries that did not fit this round's work list
-  __shared__ unsigned long long s_stat[8];
+  __shared__ unsigned long long s_stat[8 + kTileStages];
   // stage A scratch, in the (then idle) segment list: the dense slots' ranges of this tile and each warp's prefix over its slots
   uint32_t* s_ba = reinterpret_cast<uint32_t*>(s_seg);                         // [kTileMaxBig] first pair of the slot in this tile
   uint32_t* s_bn = s_ba + kTileMaxBig;                                         // [kTileMaxBig] ... and how many
@@ -440,7 +457,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   // sparse slots: (first pair not staged yet, its doc or 0xFFFFFFFF once the list is exhausted), this CTA's share of the
   // launch's cursor scratch; slot s is always walked by the same thread, so no barrier guards it
   uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
-  if (kCounters && tid < 8) s_stat[tid] = 0ull;
+  if (kCounters && tid < 8 + kTileStages) s_stat[tid] = 0ull;
   if (tid < kTileMaxQueries / 32u) s_defer[tid] = 0u;
   // the segment's queries and their clause slots are read for every tile: keep them on chip (clause_base becomes an index into cl0)
   const bool cl_staged = G.n_clause_words <= TP.cl_cap;
@@ -485,18 +502,27 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       if (s < G.n_slots) cursor[s] = make_uint2(a[j], a[j] < df[j] ? __ldg(d[j] + a[j]) : 0xFFFFFFFFu);
     }
   }
+  mark(kStPrologue);
   __syncthreads();
+  mark(kStBarrier);
   unsigned long long st_pairs = 0, st_skip = 0, st_flat = 0, st_heavy = 0, st_ess = 0, st_compl = 0, st_push = 0;  // per-thread diagnostics
 
   for (uint32_t t = U.t0; t < U.t1; ++t) {
     const uint32_t lo = t * kTile, hi = lo + kTile;
+    // the thresholds of this thread's B1 queries (qi = tid, tid + kTileThreads): loaded now, they travel while the tile is staged.
+    // Thresholds only rise (atomicMax), so a value read before stage A still bounds the query's final k-th score from below
+    uint32_t th_pre0 = 0u, th_pre1 = 0u;
+    if (tid < G.n_queries) th_pre0 = *(volatile unsigned int*)&P.qstate[s_tq[tid].query].theta;
+    if (tid + kTileThreads < G.n_queries) th_pre1 = *(volatile unsigned int*)&P.qstate[s_tq[tid + kTileThreads].query].theta;
     if (tid < G.n_big) {  // three independent loads per dense slot: one round trip for the whole tile
       const uint32_t a = __ldg(G.tix + (size_t)t * G.n_big + tid), b = __ldg(G.tix + (size_t)(t + 1u) * G.n_big + tid);
       s_ba[tid] = __ldg(&slots[tid].pair_base) + a;
       s_bn[tid] = b - a;
     }
     if (tid == 0) { s_total = 0; s_nheavy = 0; s_hpos = 0; s_nflat = 0; s_nseg = 0; s_segpos = 0; s_segvalid = TP.seg_cap; s_ndefer = 0; }
+    mark(kStA);
     __syncthreads();
+    mark(kStBarrier);
     // ---- stage A: this tile's pairs of every slot -> shared memory --------------------------------------------------------
     if (warp < G.n_big) {
       // dense lists: warp w owns slots w, w+8, ... (<= 8 of them).  Their [tix[t], tix[t+1]) ranges are laid end to end and copied as
@@ -637,10 +663,13 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       s_mask[s] = mask;
       if (s_ord0) s_ord0[s] = sl.pair_base + cur;
     }
+    mark(kStA);
     __syncthreads();
+    mark(kStBarrier);
     if (s_total > TP.p_cap) {  // more pairs than the tile buffer holds: give the batch back to the per-query kernels
       if (tid == 0) atomicExch(TP.flags, 1u);
       __syncthreads();
+      mark(kStBarrier);
       continue;
     }
     // ---- stage B1: one thread per query -- bounds and routing ---------------------------------------------------------------
@@ -656,16 +685,16 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       }
       const TileTQ tq = s_tq[qi];
       const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
-      const uint32_t th_key = *(volatile unsigned int*)&P.qstate[tq.query].theta;
+      const uint32_t th_key = qi < kTileThreads ? th_pre0 : qi < 2u * kTileThreads ? th_pre1 : *(volatile unsigned int*)&P.qstate[tq.query].theta;
       const float theta_f = threshold_score(th_key);
       const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !sample_mode;
-      const uint32_t n = tq.n_clauses, op = tq.op_flags & 3u;
+      const uint32_t n = tq.n_clauses, op = kUnionOnly ? 0u : tq.op_flags & 3u;
       ++st_pairs;
       TileQ rec;
       rec.qi = (uint16_t)qi; rec.th_key = th_key; rec.n_op = (uint8_t)((op == kTileOpBool ? 0u : n) | (op << 6));
       uint32_t cnt = 0, n_segs = 0, rec_ne = 0;
       uint32_t b_d0 = 0, b_dn = 0;  // kTileOpBool: the driving words
-      if (op == kTileOpBool) {
+      if (!kUnionOnly && op == kTileOpBool) {
         const uint32_t ng = cl[0], ns = cl[2];
         uint32_t w = 4, best = 0xFFFFFFFFu;
         float bound = 0.0f;
@@ -686,7 +715,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
         for (uint32_t e = 0; e < b_dn; ++e) n_segs += (s_info[cl[b_d0 + e]] >> 16) ? 1u : 0u;
         rec.ne = __uint_as_float(b_d0 | (b_dn << 16));
         rec.shared_stripes = 0u;
-      } else if (op == kTileOpAnd) {
+      } else if (!kUnionOnly && op == kTileOpAnd) {
         float bound = 0.0f;
         uint32_t dmin = 0xFFFFFFFFu, drv = 0;
         for (uint32_t c = 0; c < n; ++c) {  // the clause with the fewest postings in this tile drives
@@ -743,10 +772,10 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
           const uint32_t qslot = atomicAdd(&s_nflat, 1u);
           s_q[qslot] = rec;
           uint32_t w = sb;
-          if (op == kTileOpBool) {
+          if (!kUnionOnly && op == kTileOpBool) {
             for (uint32_t e = 0; e < b_dn; ++e)
               if (s_info[cl[b_d0 + e]] >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)(b_d0 + e)};
-          } else if (op == kTileOpAnd) {
+          } else if (!kUnionOnly && op == kTileOpAnd) {
             s_seg[w] = TileSeg{(uint16_t)qslot, (uint16_t)rec_ne};
           } else {
             for (uint32_t c = 0; c < rec_ne; ++c)
@@ -758,7 +787,9 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       }
       if (heavy) s_heavy[atomicAdd(&s_nheavy, 1u)] = (uint16_t)qi;
     }
+    mark(kStB1);
     __syncthreads();
+    mark(kStBarrier);
     const bool more_rounds = s_ndefer != 0u;
     // ---- stage B2: the flat pairs' essential postings, one per thread --------------------------------------------------------
     {
@@ -770,9 +801,21 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
         if (sbase >= n_seg) break;
         // 32 segments, one per lane; their postings are dealt to the lanes 32 at a time (load-balanced expansion)
         uint32_t m_len = 0, m_qc = 0, m_start = 0;  // the lane's segment: postings [m_start, m_start + m_len), q | clause << 16
+        // kUnionOnly: the segment's query state, read once here and handed to the posting lanes with shuffles (instead of three
+        // dependent shared loads per posting): th_key, ne, shared_stripes, clause base | n << 16 | n_e << 22 | prune << 28, query
+        uint32_t m_th = 0, m_ne = 0, m_ss = 0, m_cb = 0, m_query = 0;
         if (sbase + lane < n_seg) {
           const TileSeg sg = s_seg[sbase + lane];
-          const uint32_t info = s_info[cl0[s_tq[s_q[sg.q].qi].clause_base + sg.clause]];
+          uint32_t info;
+          if constexpr (kUnionOnly) {
+            const TileQ q = s_q[sg.q];
+            const TileTQ qq = s_tq[q.qi];
+            info = s_info[cl0[qq.clause_base + sg.clause]];
+            m_th = q.th_key; m_ne = __float_as_uint(q.ne); m_ss = q.shared_stripes; m_query = qq.query;
+            m_cb = qq.clause_base | (q.n() << 16) | (q.n_e() << 22) | (q.prune() ? 1u << 28 : 0u);
+          } else {
+            info = s_info[cl0[s_tq[s_q[sg.q].qi].clause_base + sg.clause]];
+          }
           m_qc = sg.q | ((uint32_t)sg.clause << 16);
           m_start = info & 0xFFFFu;
           m_len = sample_mode ? min(info >> 16, kSampleSeg) : info >> 16;
@@ -789,27 +832,44 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
           const uint32_t starts = __reduce_or_sync(kFull, (m_len && rel < 32u) ? (1u << rel) : 0u);
           const uint32_t earlier = (uint32_t)__popc(__ballot_sync(kFull, m_len && excl < ibase));
           const uint32_t j = earlier - 1u + (uint32_t)__popc(starts & (0xFFFFFFFFu >> (31u - lane)));
-          const uint32_t p = __shfl_sync(kFull, m_pbase, j & 31u) + item;
-          const uint32_t qc = __shfl_sync(kFull, m_qc, j & 31u);
+          const uint32_t src = j & 31u;
+          const uint32_t p = __shfl_sync(kFull, m_pbase, src) + item;
+          const uint32_t qc = __shfl_sync(kFull, m_qc, src);
+          uint32_t b_th = 0, b_ne = 0, b_ss = 0, b_cb = 0, b_query = 0;
+          if constexpr (kUnionOnly) {
+            b_th = __shfl_sync(kFull, m_th, src);
+            b_ne = __shfl_sync(kFull, m_ne, src);
+            b_ss = __shfl_sync(kFull, m_ss, src);
+            b_cb = __shfl_sync(kFull, m_cb, src);
+            b_query = __shfl_sync(kFull, m_query, src);
+          }
           uint32_t s_query = 0xFFFFFFFFu - lane, s_key = 0;  // sample launch: this lane's sample (if any), handed over below
           if (item < total) {
-            const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
-            const TileQ q = s_q[sg.q];
-            const TileTQ qq = s_tq[q.qi];
-            const uint16_t* __restrict__ cl = cl0 + qq.clause_base;
             const uint32_t off = s_off[p];
             float sum;
             bool ok;
-            const bool io = (qq.op_flags & 32u) != 0;
-            if (q.op() == kTileOpBool) ok = tile_eval_bool(V, cl, __float_as_uint(q.ne) & 0xFFFFu, sg.clause, p, off, io, sum);
-            else if (q.op() == kTileOpAnd) ok = tile_eval_and(V, cl, q.n(), q.n_e(), p, off, io, sum);
-            else ok = tile_eval_or(V, s_max, cl, q, sg.clause, p, off, threshold_score(q.th_key), sum);
+            uint32_t query, th_key;
+            if constexpr (kUnionOnly) {
+              query = b_query; th_key = b_th;
+              ok = tile_eval_or(V, s_max, cl0 + (b_cb & 0xFFFFu), (b_cb >> 22) & 63u, (b_cb >> 16) & 63u, (b_cb >> 28) != 0u,
+                                __uint_as_float(b_ne), b_ss, qc >> 16, p, off, threshold_score(th_key), sum);
+            } else {
+              const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
+              const TileQ q = s_q[sg.q];
+              const TileTQ qq = s_tq[q.qi];
+              const uint16_t* __restrict__ cl = cl0 + qq.clause_base;
+              query = qq.query; th_key = q.th_key;
+              const bool io = (qq.op_flags & 32u) != 0;
+              if (q.op() == kTileOpBool) ok = tile_eval_bool(V, cl, __float_as_uint(q.ne) & 0xFFFFu, sg.clause, p, off, io, sum);
+              else if (q.op() == kTileOpAnd) ok = tile_eval_and(V, cl, q.n(), q.n_e(), p, off, io, sum);
+              else ok = tile_eval_or(V, s_max, cl, q.n_e(), q.n(), q.prune(), q.ne, q.shared_stripes, sg.clause, p, off, threshold_score(th_key), sum);
+            }
             if (ok) {
               ++st_compl;
               const uint32_t key = score_to_key(sum);
-              if (key >= q.th_key) ++st_push;
-              if (!sample_mode) tile_push(P, qq.query, sum, lo + off, G.segment_ord, q.th_key, G.alive);
-              else if (key >= q.th_key && key != 0u && (!G.alive || is_alive(G.alive, lo + off))) { s_query = qq.query; s_key = key; }  // (a deleted doc bounds nothing)
+              if (key >= th_key) ++st_push;
+              if (!sample_mode) tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive);
+              else if (key >= th_key && key != 0u && (!G.alive || is_alive(G.alive, lo + off))) { s_query = query; s_key = key; }  // (a deleted doc bounds nothing)
             }
           }
           if (sample_mode) {  // one atomic per query and warp step instead of one per sample (the counters are hot)
@@ -826,15 +886,18 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
         }
       }
     }
+    mark(kStB2);
     if (!more_rounds) break;
     __syncthreads();
     if (tid == 0) { s_nflat = 0; s_nseg = 0; s_segpos = 0; s_segvalid = TP.seg_cap; s_ndefer = 0; }
     __syncthreads();
+    mark(kStBarrier);
     }
     // ---- stage B3: one warp per heavy pair, a window of f32 score slots ----------------------------------------------------
     {
       const uint32_t n_heavy = s_nheavy;
       if (n_heavy) __syncthreads();  // the windows overlay the work list: every warp must be done with B2
+      mark(kStBarrier);
       float* acc = s_acc + warp * kTile;
       for (; warp < n_win;) {  // (the warps without a window go straight to the barrier)
         uint32_t h = 0;
@@ -850,7 +913,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
         const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !sample_mode;
         const uint32_t n = tq.n_clauses;
         if (lane == 0) ++st_heavy;
-        if ((tq.op_flags & 3u) == kTileOpBool) {  // lanes share the driving group's postings (as for conjunctions below)
+        if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpBool) {  // lanes share the driving group's postings (as for conjunctions below)
           const uint32_t ng = cl[0], ns = cl[2];
           uint32_t w = 4, best_tot = 0xFFFFFFFFu, d0 = 0, dn = 0;
           for (uint32_t g = 0; g < ng; ++g) {
@@ -889,7 +952,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
           __syncwarp();
           continue;
         }
-        if ((tq.op_flags & 3u) == kTileOpAnd) {  // lanes share the driving clause's postings; every lane looks its docs up in the others
+        if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpAnd) {  // lanes share the driving clause's postings; every lane looks its docs up in the others
           uint32_t dmin = 0xFFFFFFFFu, drv = 0;
           for (uint32_t c = 0; c < n; ++c) {
             const uint32_t len = s_info[cl[c]] >> 16;
@@ -1003,7 +1066,9 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
         __syncwarp();
       }
     }
+    mark(kStB3);
     __syncthreads();
+    mark(kStBarrier);
   }
   if constexpr (kCounters) {
     // warp-aggregated diagnostics
@@ -1015,8 +1080,10 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(kFull, x, o);
       if (lane == 0 && x) atomicAdd(&s_stat[i], x);
     }
+    if (lane == 0)
+      for (int k = 0; k < kTileStages; ++k) atomicAdd(&s_stat[8 + k], cyc[k]);
     __syncthreads();
-    if (tid < 7 && s_stat[tid]) atomicAdd(&TP.counters[tid], s_stat[tid]);
+    if (tid < 8 + kTileStages && tid != 7 && s_stat[tid]) atomicAdd(&TP.counters[tid], s_stat[tid]);
   }
 }
 
