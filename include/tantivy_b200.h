@@ -177,6 +177,8 @@ typedef struct {
   uint64_t tile_ctas_per_sm;    /* k_tile CTAs an SM holds at once in the exact launches of the last prepared group (occupancy API) */
   uint64_t tile_cycles[8];      /* cumulative, with TQ_TILE_COUNTERS=1: k_tile warp cycles (clock64) by stage: [0] cursor prologue,
                                    [1] A (staging), [2] B1 (routing), [3] B2 (flat evaluation), [4] B3 (windows), [5] barrier waits */
+  uint64_t tile_groups_union_only; /* of tile_groups: groups whose queries are all term queries and unions, which run the
+                                      union-only k_tile instances (k_tile<*, *, true>); the rest run the general instances */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */

@@ -1663,6 +1663,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
   b->stats.units_tile = pl.tile_units;
   b->stats.units_phrase = nu[UC_PHRASE];
   b->stats.tile_groups = b->groups.size();
+  for (auto& g : b->groups) b->stats.tile_groups_union_only += g.union_only ? 1u : 0u;
   b->stats.tile_postings = pl.tile_postings;
   for (auto& tg : pl.tgroups) b->stats.tile_list_bytes += tg.list_bytes;
   b->stats.tile_scratch_bytes = pl.tile_bytes;

@@ -399,6 +399,9 @@ def test_synth_union_pruning_is_exact(ctx, synth):
     g = ctx.search_batch(qb)
     c = oi.search_batch(qb, mode=0, n_threads=8)
     assert_same(g, c, qb.nq)
+    if ctx.engine == "tile":
+        st = ctx.stats()
+        assert st["tile_groups"] >= 1 and st["tile_groups_union_only"] == st["tile_groups"]
     # single-query batches use small units (many cold starts + threshold sharing between CTAs)
     for q in queries[:8]:
         qb1 = QueryBatch([q])
@@ -533,12 +536,23 @@ def test_tile_engine_is_what_runs(ctx, synth):
     st = ctx.stats()
     if ctx.engine == "tile":
         assert st["tile_groups"] == 1 and st["units_tile"] > 0 and st["tile_postings"] > 0 and st["tile_fallbacks"] == 0
+        assert st["tile_groups_union_only"] == 1  # unions alone: the union-only k_tile instance ran
         assert st["units_or"] == 0  # no per-query union kernel ran
     else:
         assert st["tile_groups"] == 0 and st["units_or"] > 0
 
 
-@pytest.mark.parametrize("hook", [dict(TQ_TILE_PCAP=64), dict(TQ_TILE_CAND_FLOOR=4), dict(TQ_TILE_SAMPLE_DIV=0, TQ_TILE_CAND_FLOOR=64)])
+# hooks that make a tile overflow its pair buffer or a query its candidate region (the run is repeated)
+TILE_OVERFLOW_HOOKS = [dict(TQ_TILE_PCAP=64), dict(TQ_TILE_CAND_FLOOR=4), dict(TQ_TILE_SAMPLE_DIV=0, TQ_TILE_CAND_FLOOR=64)]
+# hooks that send k_tile down each of its routes: a full work list (further routing rounds per tile; with 3 entries the wider unions
+# take the window path), window path only (2 or 8 window warps), flat path only, no sample launch, every list dense (bitmap lookups) /
+# every list sparse (binary searches), one CTA per launch, other launch cuts
+TILE_PATH_HOOKS = [dict(TQ_TILE_SEG_CAP=8), dict(TQ_TILE_SEG_CAP=3), dict(TQ_TILE_LIGHT_MAX=0), dict(TQ_TILE_LIGHT_MAX=0, TQ_TILE_WINDOWS=8),
+                   dict(TQ_TILE_LIGHT_MAX=100000), dict(TQ_TILE_SAMPLE_DIV=0), dict(TQ_TILE_BIG_MIN=1), dict(TQ_TILE_BIG_MIN=100000),
+                   dict(TQ_TILE_UNITS=1), dict(TQ_TILE_ROUND_DIV1=2, TQ_TILE_ROUND_DIV2=2)]
+
+
+@pytest.mark.parametrize("hook", TILE_OVERFLOW_HOOKS)
 def test_tile_overflow_is_repeated_on_the_per_query_kernels(synth, hook):
     """A tile with more pairs than its shared-memory buffer, or a query with more candidates than its region, never costs
     exactness: the run is repeated on the per-query kernels (tile_fallbacks == 1) and returns the oracle's rows."""
@@ -559,8 +573,7 @@ def test_tile_overflow_is_repeated_on_the_per_query_kernels(synth, hook):
         c.close()
 
 
-@pytest.mark.parametrize("hook", [dict(TQ_TILE_SEG_CAP=8), dict(TQ_TILE_SEG_CAP=3), dict(TQ_TILE_LIGHT_MAX=0), dict(TQ_TILE_LIGHT_MAX=0, TQ_TILE_WINDOWS=8), dict(TQ_TILE_LIGHT_MAX=100000), dict(TQ_TILE_SAMPLE_DIV=0),
-                                  dict(TQ_TILE_BIG_MIN=1), dict(TQ_TILE_BIG_MIN=100000), dict(TQ_TILE_UNITS=1), dict(TQ_TILE_ROUND_DIV1=2, TQ_TILE_ROUND_DIV2=2)])
+@pytest.mark.parametrize("hook", TILE_PATH_HOOKS)
 def test_tile_paths_agree(synth, hook):
     """Every route through k_tile gives the same rows: a full work list (further routing rounds per tile; with 3 entries the
     wider unions take the window path), window path only (2 or 8 window warps),
@@ -664,7 +677,10 @@ def test_bench_config_or5_top100_one_full_segment(ctx):
     qb = QueryBatch([ix.query(TQ_OP_OR, [ranks.index(r) for r in q], 100, segment_base=base) for q in qranks])
     g = ctx.search_batch(qb)
     assert_same(g, oi.search_batch(qb, mode=0, n_threads=32), qb.nq)
-    assert ctx.stats()["tile_fallbacks"] == 0
+    st = ctx.stats()
+    assert st["tile_fallbacks"] == 0
+    if ctx.engine == "tile":
+        assert st["tile_groups"] >= 1 and st["tile_groups_union_only"] == st["tile_groups"]
     ctx.segment_unregister(base, 0)
 
 
@@ -781,7 +797,10 @@ def _range_ctx(engine):
     return _ctx_with_env(TQ_TILE=1 if engine == "tile" else 0, TQ_TILE_TERMS=1)
 
 
-@pytest.mark.parametrize("cuts", [[0, 101_376, 202_752, 300_000], [0, 1, 77_777, 77_780, 262_144, 299_999, 300_000], [0, 0, 300_000]])
+DOC_RANGE_CUTS = [[0, 101_376, 202_752, 300_000], [0, 1, 77_777, 77_780, 262_144, 299_999, 300_000], [0, 0, 300_000]]
+
+
+@pytest.mark.parametrize("cuts", DOC_RANGE_CUTS)
 def test_doc_range_parts_merge_to_the_whole_segment(ctx, cuts):
     """tq_segment_set_doc_range: every part of a segment (one context each, as on several GPUs) returns the top-k / the Count of its
     docs; merged like segment fruits (merge_fruits) they are the rows of the whole segment.  Cuts inside tiles, inside bytes of the
