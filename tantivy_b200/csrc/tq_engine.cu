@@ -1389,7 +1389,7 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         gs.queries.push_back(t2);
         kmax_g = std::max(kmax_g, pl.dq[tq.query].k);
         gs.max_clauses = std::max<uint32_t>(gs.max_clauses, tq.n_clauses);
-        if (tq.op == kTileOpAnd || tq.op == kTileOpBool || (tq.flags & 2u)) gs.union_only = false;
+        if (tq.op == kTileOpAnd || tq.op == kTileOpBool) gs.union_only = false;
         // clause slots follow the permutation (the structure words of TQ_OP_BOOL queries do not)
         uint16_t* w = gs.clauses.data() + t2.clause_base;
         if (tq.op == kTileOpBool) map_bool_clauses(w, tq.n_clauses, [&](uint16_t s) { return new_of[s]; });

@@ -81,7 +81,7 @@ struct TQuery {  // one (query, segment): what Collector::collect_segment sees
   uint32_t clause_base;  // into TileParams::clauses: slot ordinals (local to the segment) in canonical summation order
   uint16_t n_clauses;
   uint8_t op;
-  uint8_t flags;  // bit 0: prunable (every weight finite and >= 0); bit 1: phrase (op = AND; `query` is the QSeg ordinal of the phrase);
+  uint8_t flags;  // bit 0: prunable (every weight finite and >= 0);
                   // bit 2: AND / BOOL groups in Intersection::score order, (s0 + s1) + (s2 + s3 + ...), not one after another
 };
 struct TUnit { uint32_t tseg, t0, t1, pad; };
@@ -114,15 +114,6 @@ struct TileParams {
   uint32_t light_max;  // (query, tile) pairs with at most this many essential postings are evaluated posting by posting (flat path);
                        // above it (and with more than one essential clause) a warp accumulates the query's window
   uint32_t n_win;      // warps of a CTA that own a window (2: heavy pairs are rare; 8 for groups with wide queries)
-  // phrase queries on the tile engine: conjunctions whose matches are handed to k_phrase_verify as records
-  //   [qseg, doc, (global slot, pair index) per term]  (pair index: into p_docs / p_scores / p_pos)
-  uint32_t has_phrase; // the group holds phrase queries (k_tile keeps every slot's first staged pair index on chip)
-  uint32_t ph_stride;  // words per record = 2 + 2 * (most terms of a phrase in the batch)
-  uint32_t ph_cap;     // records the buffer holds (more: flags[2], the batch is repeated on the per-query kernels)
-  uint32_t pad_ph;
-  uint32_t* p_pos;     // per pair of a slot with TSlot::pad & 1: sum of the term frequencies before it in its 128-doc block
-  uint32_t* ph_recs;
-  uint32_t* ph_count;
 };
 
 
@@ -137,7 +128,6 @@ __global__ void __launch_bounds__(kThreads, 4) k_score_lists(const BatchParams P
   float* out_scores = TP.p_scores + sl.pair_base;
   uint32_t* tix = nullptr;
   uint32_t n_big = 0, n_tiles = 0;
-  const bool want_pos = TP.p_pos != nullptr && (sl.pad & 1u);
   if (sl.big != kNoSlot) {
     const TSeg G = TP.segs[sl.tseg];
     tix = G.tix + sl.big;
@@ -170,15 +160,6 @@ __global__ void __launch_bounds__(kThreads, 4) k_score_lists(const BatchParams P
     // (fieldnorm bytes, block tables)
     __stcs(reinterpret_cast<uint4*>(out_docs + g0), make_uint4(doc[0], doc[1], doc[2], doc[3]));
     __stcs(reinterpret_cast<float4*>(out_scores + g0), make_float4(s[0], s[1], s[2], s[3]));
-    if (want_pos) {  // where the doc's positions start inside the block's share of the position stream (segment_postings.rs:232-254)
-      uint32_t tfv[4], pre[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) tfv[i] = g0 + i < L.doc_freq ? tf[i] : 0u;
-      const uint32_t sum4 = tfv[0] + tfv[1] + tfv[2] + tfv[3];
-      const uint32_t incl = warp_incl_scan(sum4, lane);
-      pre[0] = incl - sum4; pre[1] = pre[0] + tfv[0]; pre[2] = pre[1] + tfv[1]; pre[3] = pre[2] + tfv[2];
-      __stcs(reinterpret_cast<uint4*>(TP.p_pos + sl.pair_base + g0), make_uint4(pre[0], pre[1], pre[2], pre[3]));
-    }
     if (tix) {  // tile index of a dense list: tix[t] = first pair with doc >= t * kTile
       uint32_t pd = __shfl_up_sync(kFull, doc[3], 1);
       if (lane == 0) pd = prev_last;
@@ -198,45 +179,43 @@ __global__ void __launch_bounds__(kThreads, 4) k_score_lists(const BatchParams P
 }
 
 // ---- tile evaluation -----------------------------------------------------------------------------------------------------
-// What a tile keeps in shared memory per slot: info = start | len << 16 (pairs [start, start + len) of s_off / s_score, ascending
-// docs), the largest score, and for DENSE slots (the first n_big of a segment) a 1024-bit presence map with per-word ranks, so that
-// "does this list hold doc x, and where" is one bit test + one popcount instead of a binary search over hundreds of pairs.
+// What a tile keeps in shared memory per slot: info = start | len << 16 (pairs [start, start + len) of off / score, ascending
+// docs), the largest score (max), and for DENSE slots (the first n_big of a segment) a 1024-bit presence map (bits) with per-word
+// ranks (rank: pairs of the slot before word w), so that "does this list hold doc x, and where" is one bit test + one popcount
+// instead of a binary search over hundreds of pairs; for sparse slots a stripe mask (bit j set = the slot lists a doc of the tile's
+// j-th 32-doc stripe).  TileView holds every region of a CTA's dynamic shared memory (tile_smem_layout lists them).
+struct TileQ; struct TileSeg; struct TileStageA; struct TileTQ;
 struct TileView {
-  const uint16_t* s_off;
-  const float* s_score;
-  const uint32_t* s_info;
-  const uint32_t* s_bits;   // [max_big][32]
-  const uint16_t* s_rank;   // [max_big][32] pairs of the slot before word w
-  const uint32_t* s_mask;   // [max_slots] sparse slots: bit j set = the slot lists a doc of the tile's j-th 32-doc stripe
+  float* score; TileQ* q; TileSeg* seg; TileStageA* a; float* acc;  // (a: in the bytes of seg; acc: in those of q and seg)
+  uint32_t *info, *mask, *bits; float* max; TileTQ* tq; uint16_t *rank, *off, *heavy, *cl;
   uint32_t n_big;
 };
-
 __device__ __forceinline__ float tile_find(const TileView& V, uint32_t slot, uint32_t off, bool& found) {
-  const uint32_t info = V.s_info[slot];
+  const uint32_t info = V.info[slot];
   if (slot < V.n_big) {
-    const uint32_t w = V.s_bits[slot * 32u + (off >> 5)];
+    const uint32_t w = V.bits[slot * 32u + (off >> 5)];
     const uint32_t bit = 1u << (off & 31u);
     found = (w & bit) != 0u;
     if (!found) return 0.0f;
-    return V.s_score[(info & 0xFFFFu) + V.s_rank[slot * 32u + (off >> 5)] + __popc(w & (bit - 1u))];
+    return V.score[(info & 0xFFFFu) + V.rank[slot * 32u + (off >> 5)] + __popc(w & (bit - 1u))];
   }
   // sparse slot: most lookups miss -- one stripe bit answers them; the rest scans the few pairs of the slot
   found = false;
-  if (!((V.s_mask[slot] >> (off >> 5)) & 1u)) return 0.0f;
+  if (!((V.mask[slot] >> (off >> 5)) & 1u)) return 0.0f;
   uint32_t lo = info & 0xFFFFu;
   const uint32_t end = lo + (info >> 16);
   if (end - lo > 8u) {
     uint32_t hi = end;
     while (hi - lo > 4u) {
       const uint32_t m = (lo + hi) >> 1;
-      if (V.s_off[m] < off) lo = m + 1u; else hi = m;
+      if (V.off[m] < off) lo = m + 1u; else hi = m;
     }
   }
   for (; lo < end; ++lo) {
-    const uint32_t o = V.s_off[lo];
+    const uint32_t o = V.off[lo];
     if (o >= off) { found = o == off; break; }
   }
-  return found ? V.s_score[lo] : 0.0f;
+  return found ? V.score[lo] : 0.0f;
 }
 
 __device__ __forceinline__ void tile_push(const BatchParams& P, uint32_t query, float score, uint32_t doc, uint32_t segment_ord,
@@ -253,7 +232,7 @@ __device__ __forceinline__ void tile_push(const BatchParams& P, uint32_t query, 
 struct TileQ {
   uint16_t qi;           // the query: index into the CTA's copy of the segment's queries (batch ordinal, clause slots)
   uint8_t n_op;          // clauses [0:6) | op << 6
-  uint8_t ne_prune;      // essential prefix (unions) / driving clause (conjunctions) [0:6) | phrase << 6 | prune << 7
+  uint8_t ne_prune;      // essential prefix (unions) / driving clause (conjunctions) [0:6) | prune << 7
   uint32_t th_key;       // the query's threshold when the tile was entered
   float ne;              // bound of the non-essential suffix in this tile (unions); 0 for conjunctions
   uint32_t shared_stripes;  // unions: 32-doc stripes of the tile in which more than one essential clause lists a doc (a posting
@@ -268,20 +247,20 @@ struct TileTQ {
   uint32_t query;
   uint16_t clause_base;  // local to the segment
   uint8_t n_clauses;
-  uint8_t op_flags;      // op [0:2) | Intersection order << 5 | phrase << 6 | prunable << 7
+  uint8_t op_flags;      // op [0:2) | Intersection order << 5 | prunable << 7
 };
-// one essential clause of flat pair q: its postings in the tile are the slot's staged range (s_info of cl[clause]; the sample
+// one essential clause of flat pair q: its postings in the tile are the slot's staged range (info of cl[clause]; the sample
 // launch takes at most kSampleSeg of them)
 struct TileSeg { uint16_t q, clause; };
 
 // Union: the doc at tile offset `off`, met as posting p of essential clause c (of n_e; n clauses, ne and shared_stripes as in TileQ).
 // Exact score in the canonical order, or nothing when the bounds show it cannot reach the threshold.  Returns true when `sum` is a
 // complete score.
-__device__ __forceinline__ bool tile_eval_or(const TileView& V, const float* __restrict__ s_max, const uint16_t* __restrict__ cl, uint32_t n_e,
+__device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* __restrict__ cl, uint32_t n_e,
                                              uint32_t n, bool prune, float ne, uint32_t shared_stripes, uint32_t c, uint32_t p, uint32_t off,
                                              float theta_f, float& sum) {
   bool f;
-  sum = V.s_score[p];  // (-0.0 + s == s: SumCombiner starts from 0, score_combiner.rs:39-57)
+  sum = V.score[p];  // (-0.0 + s == s: SumCombiner starts from 0, score_combiner.rs:39-57)
   if ((shared_stripes >> (off >> 5)) & 1u) {  // another essential clause lists a doc near this one: look the doc up
     for (uint32_t c1 = 0; c1 < c; ++c1) {  // an earlier essential clause lists the doc: it is evaluated there
       tile_find(V, cl[c1], off, f);
@@ -297,7 +276,7 @@ __device__ __forceinline__ bool tile_eval_or(const TileView& V, const float* __r
   for (uint32_t c2 = n_e; c2 < n; ++c2) {
     if (prune && (sum + rem) * 1.00001f < theta_f) return false;
     const uint32_t slot = cl[c2];
-    rem -= s_max[slot];
+    rem -= V.max[slot];
     const float v = tile_find(V, slot, off, f);
     if (f) sum = __fadd_rn(sum, v);
   }
@@ -316,7 +295,7 @@ __device__ __forceinline__ bool tile_eval_and_t(const TileView& V, const uint16_
   float head = 0.0f;
   for (uint32_t c = 0; c < n; ++c) {
     float v;
-    if (c == drv) v = V.s_score[p];
+    if (c == drv) v = V.score[p];
     else {
       bool f;
       v = tile_find(V, cl[c], off, f);
@@ -356,7 +335,7 @@ __device__ __forceinline__ bool tile_eval_bool(const TileView& V, const uint16_t
     bool any = false;
     for (uint32_t e = 0; e < glen; ++e, ++w) {
       float v;
-      if (w == wi) { v = V.s_score[p]; f = true; } else v = tile_find(V, cl[w], off, f);
+      if (w == wi) { v = V.score[p]; f = true; } else v = tile_find(V, cl[w], off, f);
       if (f) { gs = any ? __fadd_rn(gs, v) : v; any = true; }
     }
     if (!any) return false;
@@ -369,7 +348,7 @@ __device__ __forceinline__ bool tile_eval_bool(const TileView& V, const uint16_t
   uint32_t cnt = 0;
   for (uint32_t e = 0; e < ns; ++e, ++w) {
     float v;
-    if (w == wi) { v = V.s_score[p]; f = true; } else v = tile_find(V, cl[w], off, f);
+    if (w == wi) { v = V.score[p]; f = true; } else v = tile_find(V, cl[w], off, f);
     if (f) { ss = cnt ? __fadd_rn(ss, v) : v; ++cnt; }
   }
   for (uint32_t e = 0; e < nn; ++e, ++w) {
@@ -381,97 +360,140 @@ __device__ __forceinline__ bool tile_eval_bool(const TileView& V, const uint16_t
   return true;
 }
 
-constexpr uint32_t kTileStageWords = 2u * kTileMaxBig + kTileWarps * 17u;
-// Shared memory of a k_tile CTA: the work list (TileQ records + segments), and in the same bytes the windows of the rare heavy
-// pairs (stage B3 starts after the last B2 of the tile) ...
-__host__ __device__ constexpr size_t tile_union_bytes(uint32_t max_queries, uint32_t seg_cap, uint32_t n_win) {
-  // (the segment list doubles as stage A's scratch: never smaller than kTileStageWords words)
-  const size_t seg_bytes = (size_t)seg_cap * sizeof(TileSeg) > kTileStageWords * 4u ? (size_t)seg_cap * sizeof(TileSeg) : kTileStageWords * 4u;
-  const size_t list_bytes = (size_t)max_queries * sizeof(TileQ) + seg_bytes, win_bytes = (size_t)n_win * kTile * 4;
-  return ((list_bytes > win_bytes ? list_bytes : win_bytes) + 15) & ~(size_t)15;
+// Stage A's scratch (in the then idle work-list segments): the dense slots' ranges of this tile and each warp's prefix over its slots
+struct TileStageA {
+  uint32_t ba[kTileMaxBig], bn[kTileMaxBig];  // first pair of the slot in this tile, and how many
+  uint32_t wpre[kTileWarps][9];
+  uint32_t wa[kTileWarps][8];
+};
+
+// Shared memory of a k_tile CTA: byte offsets of its regions, in this order (the sparse slots' cursors are not on chip:
+// TileParams::cursors).  f32 scores [p_cap] at 0; the work list: TileQ records [max_queries] (`list`) + TileSeg segments [seg_cap]
+// (`seg`, which stage A uses for its TileStageA scratch), and in the same bytes the [n_win][kTile] f32 windows of the rare heavy
+// pairs (stage B3 starts after the last B2 of the tile); per slot: pair range start | len << 16 (`info`), largest score in the tile
+// (`max`, >= 0) and sparse stripe mask [max_slots] each; presence maps [max_big][32]; TileTQ [max_queries]; u16 presence map ranks
+// [max_big][32], doc offsets [p_cap], heavy pairs [max_queries] and clause slots [cl_cap].
+struct TileSmem { uint32_t list, seg, info, max, mask, bits, tq, rank, off, heavy, cl, end; };
+__host__ __device__ constexpr TileSmem tile_smem_layout(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries,
+                                                        uint32_t seg_cap, uint32_t cl_cap, uint32_t n_win) {
+  const uint32_t seg_bytes = seg_cap * (uint32_t)sizeof(TileSeg) > (uint32_t)sizeof(TileStageA) ? seg_cap * (uint32_t)sizeof(TileSeg) : (uint32_t)sizeof(TileStageA);
+  const uint32_t list_bytes = max_queries * (uint32_t)sizeof(TileQ) + seg_bytes, win_bytes = n_win * kTile * 4u;
+  TileSmem L{};
+  L.list = p_cap * 4u;
+  L.seg = L.list + max_queries * (uint32_t)sizeof(TileQ);
+  L.info = L.list + (((list_bytes > win_bytes ? list_bytes : win_bytes) + 15u) & ~15u);
+  L.max = L.info + max_slots * 4u; L.mask = L.max + max_slots * 4u; L.bits = L.mask + max_slots * 4u;
+  L.tq = L.bits + max_big * 128u;
+  L.rank = L.tq + max_queries * (uint32_t)sizeof(TileTQ);
+  L.off = L.rank + max_big * 64u; L.heavy = L.off + p_cap * 2u; L.cl = L.heavy + max_queries * 2u;
+  L.end = L.cl + cl_cap * 2u + 64u;
+  return L;
 }
-// (the sparse slots' cursors are not on chip: TileParams::cursors)
 __host__ __device__ constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries, uint32_t seg_cap,
-                                                      uint32_t cl_cap, uint32_t n_win, uint32_t has_phrase = 0) {
-  return (size_t)p_cap * 4 + tile_union_bytes(max_queries, seg_cap, n_win) + (size_t)max_slots * 12 + (size_t)max_big * 128 +
-         (size_t)max_queries * sizeof(TileTQ) + (size_t)max_big * 64 + (size_t)p_cap * 2 + (size_t)max_queries * 2 + (size_t)cl_cap * 2 + 64 +
-         (has_phrase ? (size_t)max_slots * 4 + 8 : 0);
+                                                      uint32_t cl_cap, uint32_t n_win) {
+  return tile_smem_layout(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win).end;
 }
 
+__device__ __forceinline__ TileView tile_view(unsigned char* s_dyn, const TileParams& TP, uint32_t n_big) {
+  const TileSmem L = tile_smem_layout(TP.p_cap, TP.max_slots, TP.max_big, TP.max_queries, TP.seg_cap, TP.cl_cap, TP.n_win);
+  return TileView{reinterpret_cast<float*>(s_dyn),                reinterpret_cast<TileQ*>(s_dyn + L.list),
+                  reinterpret_cast<TileSeg*>(s_dyn + L.seg),       reinterpret_cast<TileStageA*>(s_dyn + L.seg),
+                  reinterpret_cast<float*>(s_dyn + L.list),        reinterpret_cast<uint32_t*>(s_dyn + L.info),
+                  reinterpret_cast<uint32_t*>(s_dyn + L.mask),     reinterpret_cast<uint32_t*>(s_dyn + L.bits),
+                  reinterpret_cast<float*>(s_dyn + L.max),         reinterpret_cast<TileTQ*>(s_dyn + L.tq),
+                  reinterpret_cast<uint16_t*>(s_dyn + L.rank),     reinterpret_cast<uint16_t*>(s_dyn + L.off),
+                  reinterpret_cast<uint16_t*>(s_dyn + L.heavy),    reinterpret_cast<uint16_t*>(s_dyn + L.cl),
+                  n_big};
+}
+
+// A CTA's counters of the current tile: pairs staged (A); heavy pairs (B1) and those a window took (B3); flat pairs (B1); work-list
+// segments claimed (B1), taken by a warp (B2) and written (the list filled up from `segvalid` on); whether queries were deferred
+// to another round of B1 + B2, and which.
+struct TileCtl { uint32_t total, nheavy, hpos, nflat, nseg, segpos, segvalid, ndefer, defer[kTileMaxQueries / 32u]; };
+// Per-thread diagnostics of k_tile<*, true, *> (TileParams::counters[0, 7)); the other instances compile them out.
+struct TileStats { unsigned long long pairs, skipped, flat, heavy, ess, completed, pushed; };
 // Stages of a tile as the cycle counters of k_tile<*, true, *> split a warp's time (TileParams::counters[8 + stage],
 // tq_stats.tile_cycles): the cursor prologue, A, B1, B2, B3, and the waits at the barriers between them.
 enum TileStage : int { kStPrologue, kStA, kStB1, kStB2, kStB3, kStBarrier, kTileStages };
 
-// One instantiation per launch kind, so that each compiles only what it runs: kSample = the sample launch (threshold samples
-// instead of candidates), kCounters = TQ_TILE_COUNTERS diagnostics, kUnionOnly = every query of the group is a term query or a
-// union (no conjunction, no TQ_OP_BOOL, no phrase: the flat path broadcasts each work-list segment's query state from the lane
-// that reads the segment).  The exact launches without counters do ~90 % of the work; they must fit 64 registers so that four
-// CTAs share an SM.
-template <bool kSample, bool kCounters, bool kUnionOnly>
-__global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_tile(const BatchParams P, const TileParams TP, uint32_t unit_base) {
-  constexpr bool sample_mode = kSample;
-  // kCounters: each warp's clock64() time by stage (lane 0's view of it); mark(k) books the time since the previous mark to stage k
-  long long clk_last = kCounters ? clock64() : 0;
-  unsigned long long cyc[kTileStages] = {};
-  auto mark = [&](int k) {
-    if constexpr (kCounters) {
-      const long long now = clock64();
-      cyc[k] += (unsigned long long)(now - clk_last);
-      clk_last = now;
+// ---- the decisions B1 (routing) and B3 (windows) share -------------------------------------------------------------------
+// TQ_OP_BOOL: the driving words [d0, d0 + dn) of cl -- the MUST group with the fewest postings in this tile (the first of equals),
+// or the SHOULD clauses when there is no MUST group -- and their postings (0: some MUST group has none).  `bound`: the sum of the
+// MUST and SHOULD clauses' tile maxima.
+__device__ __forceinline__ uint32_t tile_bool_drive(const TileView& V, const uint16_t* __restrict__ cl, uint32_t& d0, uint32_t& dn, float& bound) {
+  const uint32_t ng = cl[0], ns = cl[2];
+  uint32_t w = 4, best = 0xFFFFFFFFu;
+  bound = 0.0f;
+  for (uint32_t g = 0; g < ng; ++g) {
+    const uint32_t glen = cl[w];
+    uint32_t tot = 0;
+    for (uint32_t e = 0; e < glen; ++e) { const uint32_t slot = cl[w + 1u + e]; tot += V.info[slot] >> 16; bound += V.max[slot]; }
+    if (tot < best) { best = tot; d0 = w + 1u; dn = glen; }
+    w += 1u + glen;
+  }
+  uint32_t s_tot = 0;
+  for (uint32_t e = 0; e < ns; ++e) { const uint32_t slot = cl[w + e]; s_tot += V.info[slot] >> 16; bound += V.max[slot]; }
+  if (ng == 0u) { best = s_tot; d0 = w; dn = ns; }
+  return best;
+}
+
+// Conjunction: the driving clause `drv` -- the one with the fewest postings in this tile (the first of equals) -- and its postings.
+// `bound`: the sum of the clauses' tile maxima.
+__device__ __forceinline__ uint32_t tile_and_drive(const TileView& V, const uint16_t* __restrict__ cl, uint32_t n, uint32_t& drv, float& bound) {
+  uint32_t dmin = 0xFFFFFFFFu;
+  bound = 0.0f; drv = 0;
+  for (uint32_t c = 0; c < n; ++c) {
+    const uint32_t len = V.info[cl[c]] >> 16;
+    bound += V.max[cl[c]];
+    if (len < dmin) { dmin = len; drv = c; }
+  }
+  return dmin;
+}
+
+// Union (MaxScore): the essential prefix of clauses [0, n_e) shrinks while the tile maxima of the suffix it leaves add up to less
+// than the threshold; `ne` = the bound of that non-essential suffix.
+__device__ __forceinline__ uint32_t tile_essential(const TileView& V, const uint16_t* __restrict__ cl, uint32_t n_e, bool prune, float theta_f, float& ne) {
+  ne = 0.0f;
+  if (prune) {
+    while (n_e > 0) {
+      const float b = ne + V.max[cl[n_e - 1u]];
+      if (!(b * 1.00001f < theta_f)) break;  // (f32 sums of <= 32 terms differ by < 4e-6 relative between orders)
+      ne = b;
+      --n_e;
     }
-  };
-  extern __shared__ __align__(16) unsigned char s_dyn[];
-  float* s_score = reinterpret_cast<float*>(s_dyn);                            // [p_cap]
-  unsigned char* s_union = reinterpret_cast<unsigned char*>(s_score + TP.p_cap);
-  const size_t union_bytes = tile_union_bytes(TP.max_queries, TP.seg_cap, TP.n_win);
-  const uint32_t n_win = TP.n_win;
-  TileQ* s_q = reinterpret_cast<TileQ*>(s_union);                              // [max_queries] flat pairs of this tile (B1, B2)
-  TileSeg* s_seg = reinterpret_cast<TileSeg*>(s_q + TP.max_queries);           // [seg_cap]
-  float* s_acc = reinterpret_cast<float*>(s_union);                            // [n_win][kTile] windows of the heavy pairs (B3)
-  uint32_t* s_info = reinterpret_cast<uint32_t*>(s_union + union_bytes);       // [max_slots]
-  float* s_max = reinterpret_cast<float*>(s_info + TP.max_slots);              // [max_slots] largest score of the slot in this tile (>= 0)
-  uint32_t* s_mask = reinterpret_cast<uint32_t*>(s_max + TP.max_slots);        // [max_slots] stripe masks of the sparse slots
-  uint32_t* s_bits = s_mask + TP.max_slots;                                    // [max_big][32]
-  TileTQ* s_tq = reinterpret_cast<TileTQ*>(s_bits + TP.max_big * 32u);         // [max_queries] this segment's queries
-  uint16_t* s_rank = reinterpret_cast<uint16_t*>(s_tq + TP.max_queries);       // [max_big][32]
-  uint16_t* s_off = s_rank + TP.max_big * 32u;                                 // [p_cap]
-  uint16_t* s_heavy = s_off + TP.p_cap;                                        // [max_queries]
-  uint16_t* s_cl = s_heavy + TP.max_queries;                                   // [cl_cap] this segment's clause slots
-  // [max_slots] phrase groups only: index (into the pair arrays) of the slot's first pair staged for the current tile
-  uint32_t* s_ord0 = !kUnionOnly && TP.has_phrase ? reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(s_cl + TP.cl_cap) + 3u) & ~(uintptr_t)3u) : nullptr;
-  __shared__ uint32_t s_total, s_nheavy, s_hpos, s_nflat, s_nseg, s_segpos, s_segvalid, s_ndefer;
-  __shared__ uint32_t s_defer[kTileMaxQueries / 32u];  // queries that did not fit this round's work list
-  __shared__ unsigned long long s_stat[8 + kTileStages];
-  // stage A scratch, in the (then idle) segment list: the dense slots' ranges of this tile and each warp's prefix over its slots
-  uint32_t* s_ba = reinterpret_cast<uint32_t*>(s_seg);                         // [kTileMaxBig] first pair of the slot in this tile
-  uint32_t* s_bn = s_ba + kTileMaxBig;                                         // [kTileMaxBig] ... and how many
-  uint32_t (*s_wpre)[9] = reinterpret_cast<uint32_t (*)[9]>(s_bn + kTileMaxBig);
-  uint32_t (*s_wa)[8] = reinterpret_cast<uint32_t (*)[8]>(s_bn + kTileMaxBig + kTileWarps * 9u);
-  static_assert(2u * kTileMaxBig + kTileWarps * 17u <= kTileStageWords, "stage A scratch");
-  const TUnit U = TP.units[unit_base + blockIdx.x];
-  const TSeg G = TP.segs[U.tseg];
-  const TSlot* __restrict__ slots = TP.slots + G.slot_base;
-  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-  const float neg_zero = __uint_as_float(0x80000000u);
-  const TileView V{s_off, s_score, s_info, s_bits, s_rank, s_mask, G.n_big};
-  // sparse slots: (first pair not staged yet, its doc or 0xFFFFFFFF once the list is exhausted), this CTA's share of the
-  // launch's cursor scratch; slot s is always walked by the same thread, so no barrier guards it
-  uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
-  if (kCounters && tid < 8 + kTileStages) s_stat[tid] = 0ull;
-  if (tid < kTileMaxQueries / 32u) s_defer[tid] = 0u;
-  // the segment's queries and their clause slots are read for every tile: keep them on chip (clause_base becomes an index into cl0)
-  const bool cl_staged = G.n_clause_words <= TP.cl_cap;
-  const uint16_t* __restrict__ cl0 = cl_staged ? s_cl : TP.clauses + G.clause_base;
+  }
+  return n_e;
+}
+
+// Sample launch: the warp's best few keys (one per lane in `best`) that reach th_key become samples of the query, largest first.
+__device__ __forceinline__ void warp_push_samples(const TileParams& TP, uint32_t query, uint32_t best, uint32_t th_key, uint32_t lane) {
+  for (uint32_t r = 0; r < kSamplePerTile; ++r) {
+    const uint32_t mk = __reduce_max_sync(kFull, best);
+    if (mk == 0u || mk < th_key) break;
+    const unsigned who = __ballot_sync(kFull, best == mk);
+    if (lane == (uint32_t)__ffs(who) - 1u) {
+      const uint32_t idx = atomicAdd(&TP.sample_count[query], 1u);
+      if (idx < TP.sample_cap) TP.samples[(size_t)query * TP.sample_cap + idx] = mk;
+      best = 0;
+    }
+  }
+}
+
+// ---- the stages of a tile ------------------------------------------------------------------------------------------------
+// Prologue: the segment's queries and their clause slots are read for every tile -- keep them on chip (clause_base becomes an index
+// into the segment's clause words) -- and every sparse slot's cursor is positioned on its first pair at or after the unit's first
+// doc.  Four slots per thread at a time: the binary searches advance in lockstep, so their (dependent) loads overlap -- with
+// two-tile units this prologue is a tenth of the CTA's time.
+__device__ __forceinline__ void tile_prologue(const TileParams& TP, const TSeg& G, const TSlot* __restrict__ slots, const TileView& V,
+                                              bool cl_staged, uint2* cursor, uint32_t t0, uint32_t tid) {
   for (uint32_t i = tid; i < G.n_queries; i += kTileThreads) {
     const TQuery tq = TP.queries[G.query_base + i];
-    s_tq[i] = TileTQ{tq.query, (uint16_t)(tq.clause_base - G.clause_base), (uint8_t)tq.n_clauses, (uint8_t)((tq.op & 3u) | ((tq.flags & 4u) << 3) | ((tq.flags & 2u) << 5) | ((tq.flags & 1u) << 7))};
+    V.tq[i] = TileTQ{tq.query, (uint16_t)(tq.clause_base - G.clause_base), (uint8_t)tq.n_clauses, (uint8_t)((tq.op & 3u) | ((tq.flags & 4u) << 3) | ((tq.flags & 1u) << 7))};
   }
   if (cl_staged)
-    for (uint32_t i = tid; i < G.n_clause_words; i += kTileThreads) s_cl[i] = TP.clauses[G.clause_base + i];
-  // small slots: position the cursor on the first pair at or after the unit's first doc.  Four slots per thread at a time: the
-  // binary searches advance in lockstep, so their (dependent) loads overlap -- with two-tile units this prologue is a tenth of the CTA's time
+    for (uint32_t i = tid; i < G.n_clause_words; i += kTileThreads) V.cl[i] = TP.clauses[G.clause_base + i];
   for (uint32_t s0 = G.n_big + tid; s0 < G.n_slots; s0 += 4u * kTileThreads) {
-    const uint32_t lo0 = U.t0 * kTile;
+    const uint32_t lo0 = t0 * kTile;
     const uint32_t* d[4];
     uint32_t a[4], b[4], df[4];
 #pragma unroll
@@ -502,569 +524,546 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       if (s < G.n_slots) cursor[s] = make_uint2(a[j], a[j] < df[j] ? __ldg(d[j] + a[j]) : 0xFFFFFFFFu);
     }
   }
+}
+
+// Stage A, dense lists: warp w owns slots w, w+8, ... (<= 8 of them).  Their [tix[t], tix[t+1]) ranges (V.a->ba / bn) are laid end
+// to end and copied as ONE flat loop, so the loads of all the warp's slots are in flight together (one DRAM round trip per 128
+// pairs instead of three dependent ones per slot).
+__device__ __forceinline__ void tile_stage_dense(const TileParams& TP, const TSeg& G, const TileView& V, uint32_t& total, uint32_t lo,
+                                                 uint32_t warp, uint32_t lane) {
+  TileStageA& A = *V.a;
+  const uint32_t ne = (G.n_big - warp + kTileWarps - 1u) / kTileWarps;
+  uint32_t n_e = 0;
+  if (lane < ne) {
+    const uint32_t s = warp + lane * kTileWarps;
+    n_e = A.bn[s];
+    A.wa[warp][lane] = A.ba[s];
+  }
+  const uint32_t incl = warp_incl_scan(n_e, lane);
+  if (lane < 8u) A.wpre[warp][lane + 1u] = incl;
+  if (lane == 0) A.wpre[warp][0] = 0u;
+  const uint32_t total_w = __shfl_sync(kFull, incl, 7);
+  uint32_t base = 0;
+  if (lane == 0 && total_w) base = atomicAdd(&total, total_w);
+  base = __shfl_sync(kFull, base, 0);
+  for (uint32_t e = 0; e < ne; ++e) V.bits[(warp + e * kTileWarps) * 32u + lane] = 0u;
+  __syncwarp();
+  const bool fits = base + total_w <= TP.p_cap;
+  if (fits) {
+    for (uint32_t i0 = 0; i0 < total_w; i0 += 128u) {
+      uint32_t dd[4], ss[4];
+      float vv[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const uint32_t i = i0 + (uint32_t)u * 32u + lane;
+        dd[u] = 0xFFFFFFFFu;
+        if (i < total_w) {
+          uint32_t e = 0;
+          while (i >= A.wpre[warp][e + 1u]) ++e;
+          ss[u] = warp + e * kTileWarps;
+          const size_t g = (size_t)A.wa[warp][e] + (i - A.wpre[warp][e]);
+          dd[u] = __ldg(TP.p_docs + g);
+          vv[u] = __ldg(TP.p_scores + g);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const uint32_t i = i0 + (uint32_t)u * 32u + lane;
+        if (dd[u] != 0xFFFFFFFFu) {
+          const uint32_t off = dd[u] - lo;
+          V.off[base + i] = (uint16_t)off;
+          V.score[base + i] = vv[u];
+          atomicOr(&V.bits[ss[u] * 32u + (off >> 5)], 1u << (off & 31u));
+        }
+      }
+    }
+  }
+  __syncwarp();
+  for (uint32_t e = 0; e < ne; ++e) {
+    const uint32_t s = warp + e * kTileWarps;
+    const uint32_t b = base + A.wpre[warp][e], n = A.wpre[warp][e + 1u] - A.wpre[warp][e];
+    const uint32_t cnt = (uint32_t)__popc(V.bits[s * 32u + lane]);
+    V.rank[s * 32u + lane] = (uint16_t)(warp_incl_scan(cnt, lane) - cnt);
+    float mx = 0.0f;
+    if (fits)
+      for (uint32_t i = lane; i < n; i += 32) mx = fmaxf(mx, V.score[b + i]);
+    mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(mx)));  // mx >= 0
+    if (lane == 0) { V.info[s] = (b & 0xFFFFu) | (n << 16); V.max[s] = mx; }
+  }
+}
+
+// Stage A, sparse lists: one thread walks a slot's cursor (and fetches its next slot's cursor while it stages this one).
+__device__ __forceinline__ void tile_stage_sparse(const TileParams& TP, const TSeg& G, const TSlot* __restrict__ slots, const TileView& V,
+                                                  uint2* cursor, uint32_t& total, uint32_t lo, uint32_t tid) {
+  const uint32_t hi = lo + kTile;
+  uint2 next_cur = G.n_big + tid < G.n_slots ? cursor[G.n_big + tid] : make_uint2(0u, 0u);
+  for (uint32_t s = G.n_big + tid; s < G.n_slots; s += kTileThreads) {
+    const uint2 cs = next_cur;
+    if (s + kTileThreads < G.n_slots) next_cur = cursor[s + kTileThreads];  // (in flight while this slot is staged)
+    uint32_t nd = cs.y;
+    if (nd >= hi) {
+      V.info[s] = 0u; V.max[s] = 0.0f; V.mask[s] = 0u;
+      continue;
+    }
+    const TSlot sl = slots[s];
+    const uint32_t* __restrict__ d = TP.p_docs + sl.pair_base;
+    const float* __restrict__ sc = TP.p_scores + sl.pair_base;
+    const uint32_t cur = cs.x;
+    // the pair at the cursor belongs to this tile (nd < hi); fetch it and the next three, docs and scores, in ONE round trip
+    uint32_t d4[4];
+    float v4[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const bool in = cur + i < sl.doc_freq;
+      d4[i] = in ? __ldg(d + cur + i) : 0xFFFFFFFFu;
+      v4[i] = in ? __ldg(sc + cur + i) : 0.0f;
+    }
+    uint32_t n = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) n += d4[i] < hi ? 1u : 0u;  // ascending: the ones below hi are a prefix
+    if (n == 4u) {  // (rare for a sparse list) keep walking
+      for (;;) {
+        const uint32_t c = cur + n;
+        uint32_t e4[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) e4[i] = c + i < sl.doc_freq ? __ldg(d + c + i) : 0xFFFFFFFFu;
+        uint32_t k = 0;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) k += e4[i] < hi ? 1u : 0u;
+        n += k;
+        if (k < 4u) { nd = e4[k]; break; }
+      }
+    } else {
+      nd = d4[n];
+    }
+    cursor[s] = make_uint2(cur + n, nd);
+    if (nd < hi + kTile) {  // the next tile reads this list again: start its pairs on their way to L2 now
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(d + cur + n));
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(sc + cur + n));
+    }
+    const uint32_t base = atomicAdd(&total, n);
+    float mx = 0.0f;
+    uint32_t mask = 0;
+    if (base + n <= TP.p_cap) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if ((uint32_t)i < n) {
+          const uint32_t off = d4[i] - lo;
+          V.off[base + i] = (uint16_t)off;
+          V.score[base + i] = v4[i];
+          mask |= 1u << (off >> 5);
+          mx = fmaxf(mx, v4[i]);
+        }
+      }
+      for (uint32_t i = 4; i < n; ++i) {
+        const float v = __ldg(sc + cur + i);
+        const uint32_t off = __ldg(d + cur + i) - lo;
+        V.off[base + i] = (uint16_t)off;
+        V.score[base + i] = v;
+        mask |= 1u << (off >> 5);
+        mx = fmaxf(mx, v);
+      }
+    }
+    V.info[s] = (base & 0xFFFFu) | (n << 16);
+    V.max[s] = mx;
+    V.mask[s] = mask;
+  }
+}
+
+// Stage B1, one thread per query: bounds and routing of query qi in this tile.  Skipped: no doc of the tile can reach the query's
+// threshold;  flat: the essential postings become work-list segments that the CTA's threads share evenly (B2);  heavy: a warp
+// accumulates the query's window (B3; sample launches, and pairs with many postings).  A work list that fills up defers the
+// query to another round of B1 + B2 (the list is sized for the common case).  th_pre0 / th_pre1: the thresholds of queries tid and
+// tid + kTileThreads, loaded before stage A.
+template <bool kSample, bool kUnionOnly>
+__device__ __forceinline__ void tile_route(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C,
+                                           const uint16_t* __restrict__ cl0, uint32_t qi, uint32_t th_pre0, uint32_t th_pre1, TileStats& st) {
+  const TileTQ tq = V.tq[qi];
+  const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
+  const uint32_t th_key = qi < kTileThreads ? th_pre0 : qi < 2u * kTileThreads ? th_pre1 : (uint32_t)*(volatile unsigned int*)&P.qstate[tq.query].theta;
+  const float theta_f = threshold_score(th_key);
+  const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !kSample;
+  const uint32_t n = tq.n_clauses, op = kUnionOnly ? 0u : tq.op_flags & 3u;
+  ++st.pairs;
+  TileQ rec;
+  rec.qi = (uint16_t)qi; rec.th_key = th_key; rec.n_op = (uint8_t)((op == kTileOpBool ? 0u : n) | (op << 6));
+  uint32_t cnt = 0, n_segs = 0, rec_ne = 0;
+  uint32_t b_d0 = 0, b_dn = 0;  // kTileOpBool: the driving words
+  if (!kUnionOnly && op == kTileOpBool) {
+    float bound;
+    cnt = tile_bool_drive(V, cl, b_d0, b_dn, bound);
+    if (cnt == 0u || (prune && bound * 1.00001f < theta_f)) { ++st.skipped; return; }
+    for (uint32_t e = 0; e < b_dn; ++e) n_segs += (V.info[cl[b_d0 + e]] >> 16) ? 1u : 0u;
+    rec.ne = __uint_as_float(b_d0 | (b_dn << 16));
+    rec.shared_stripes = 0u;
+  } else if (!kUnionOnly && op == kTileOpAnd) {
+    float bound;
+    cnt = tile_and_drive(V, cl, n, rec_ne, bound);
+    if (cnt == 0u || (prune && bound * 1.00001f < theta_f)) { ++st.skipped; return; }
+    rec.ne = 0.0f; rec.shared_stripes = 0u;
+    n_segs = 1;
+  } else {
+    // sample launch: only the docs of the two heaviest clauses are scored (completely): the best docs of a union nearly
+    // always hold its rarest terms, and ANY real score is a valid sample
+    uint32_t n_e = n;
+    if (kSample) {  // ... extended by further clauses while the tile holds fewer than four of their postings
+      uint32_t have = 0;
+      n_e = 0;
+      while (n_e < n && (n_e < 2u || have < 4u)) { have += V.info[cl[n_e]] >> 16; ++n_e; }
+    }
+    float ne;
+    n_e = tile_essential(V, cl, n_e, prune, theta_f, ne);
+    if (n_e == 0) { ++st.skipped; return; }  // no doc of this tile can reach the threshold
+    uint32_t seen = 0, shared = 0;
+    for (uint32_t c = 0; c < n_e; ++c) {
+      const uint32_t slot = cl[c];
+      const uint32_t len = V.info[slot] >> 16;
+      cnt += len; n_segs += len ? 1u : 0u;
+      const uint32_t m = slot < G.n_big ? (len ? 0xFFFFFFFFu : 0u) : V.mask[slot];  // (dense lists: every stripe)
+      shared |= seen & m;
+      seen |= m;
+    }
+    if (cnt == 0) { ++st.skipped; return; }  // a doc without an essential posting stays below the threshold
+    rec_ne = n_e; rec.ne = ne; rec.shared_stripes = shared;
+  }
+  rec.ne_prune = (uint8_t)(rec_ne | (prune ? 128u : 0u));
+  // sample launch: ANY set of real scores is a valid sample -- at most kSampleSeg postings per driving clause, no window path
+  if (kSample && *(volatile unsigned int*)&TP.sample_count[tq.query] >= TP.sample_cap) return;
+  bool heavy = !kSample && cnt > TP.light_max && op != kTileOpAnd && op != kTileOpBool && rec_ne >= 2u;
+  if (n_segs > TP.seg_cap) heavy = true;  // (test hook sizes only)
+  if (!heavy) {
+    const uint32_t sb = atomicAdd(&C.nseg, n_segs);
+    if (sb + n_segs > TP.seg_cap) {  // the work list is full (entries from here on are not written): next round
+      atomicMin(&C.segvalid, sb);
+      atomicOr(&C.defer[qi >> 5], 1u << (qi & 31u));
+      C.ndefer = 1u;
+    } else {
+      const uint32_t qslot = atomicAdd(&C.nflat, 1u);
+      V.q[qslot] = rec;
+      uint32_t w = sb;
+      if (!kUnionOnly && op == kTileOpBool) {
+        for (uint32_t e = 0; e < b_dn; ++e)
+          if (V.info[cl[b_d0 + e]] >> 16) V.seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)(b_d0 + e)};
+      } else if (!kUnionOnly && op == kTileOpAnd) {
+        V.seg[w] = TileSeg{(uint16_t)qslot, (uint16_t)rec_ne};
+      } else {
+        for (uint32_t c = 0; c < rec_ne; ++c)
+          if (V.info[cl[c]] >> 16) V.seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)c};
+      }
+      ++st.flat;
+      st.ess += cnt;
+    }
+  }
+  if (heavy) V.heavy[atomicAdd(&C.nheavy, 1u)] = (uint16_t)qi;
+}
+
+// Stage B2: the flat pairs' essential postings, one per thread.  A warp takes 32 work-list segments at a time, one per lane, and
+// deals their postings to the lanes 32 at a time (load-balanced expansion).
+template <bool kSample, bool kUnionOnly>
+__device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C,
+                                          const uint16_t* __restrict__ cl0, uint32_t lo, uint32_t lane, TileStats& st) {
+  const uint32_t n_seg = min(C.nseg, C.segvalid);
+  for (;;) {
+    uint32_t sbase = 0;
+    if (lane == 0) sbase = atomicAdd(&C.segpos, 32u);
+    sbase = __shfl_sync(kFull, sbase, 0);
+    if (sbase >= n_seg) break;
+    uint32_t m_len = 0, m_qc = 0, m_start = 0;  // the lane's segment: postings [m_start, m_start + m_len), q | clause << 16
+    // kUnionOnly: the segment's query state, read once here and handed to the posting lanes with shuffles (instead of three
+    // dependent shared loads per posting): th_key, ne, shared_stripes, clause base | n << 16 | n_e << 22 | prune << 28, query
+    uint32_t m_th = 0, m_ne = 0, m_ss = 0, m_cb = 0, m_query = 0;
+    if (sbase + lane < n_seg) {
+      const TileSeg sg = V.seg[sbase + lane];
+      uint32_t info;
+      if constexpr (kUnionOnly) {
+        const TileQ q = V.q[sg.q];
+        const TileTQ qq = V.tq[q.qi];
+        info = V.info[cl0[qq.clause_base + sg.clause]];
+        m_th = q.th_key; m_ne = __float_as_uint(q.ne); m_ss = q.shared_stripes; m_query = qq.query;
+        m_cb = qq.clause_base | (q.n() << 16) | (q.n_e() << 22) | (q.prune() ? 1u << 28 : 0u);
+      } else {
+        info = V.info[cl0[V.tq[V.q[sg.q].qi].clause_base + sg.clause]];
+      }
+      m_qc = sg.q | ((uint32_t)sg.clause << 16);
+      m_start = info & 0xFFFFu;
+      m_len = kSample ? min(info >> 16, kSampleSeg) : info >> 16;
+    }
+    const uint32_t incl = warp_incl_scan(m_len, lane);
+    const uint32_t total = __shfl_sync(kFull, incl, 31);
+    const uint32_t excl = incl - m_len;
+    const uint32_t m_pbase = m_start - excl;  // (mod 2^32) the pair index of the chunk item ibase + lane is m_pbase + ibase + lane
+    for (uint32_t ibase = 0; ibase < total; ibase += 32u) {
+      const uint32_t item = ibase + lane;
+      // the segment of item `ibase + lane`: every listed segment holds a posting, so segment numbers grow by one at each
+      // start; (segments that start before this chunk) - 1 + (starts at or before the lane's item)
+      const uint32_t rel = excl - ibase;  // (wraps for segments that start before the chunk)
+      const uint32_t starts = __reduce_or_sync(kFull, (m_len && rel < 32u) ? (1u << rel) : 0u);
+      const uint32_t earlier = (uint32_t)__popc(__ballot_sync(kFull, m_len && excl < ibase));
+      const uint32_t j = earlier - 1u + (uint32_t)__popc(starts & (0xFFFFFFFFu >> (31u - lane)));
+      const uint32_t src = j & 31u;
+      const uint32_t p = __shfl_sync(kFull, m_pbase, src) + item;
+      const uint32_t qc = __shfl_sync(kFull, m_qc, src);
+      uint32_t b_th = 0, b_ne = 0, b_ss = 0, b_cb = 0, b_query = 0;
+      if constexpr (kUnionOnly) {
+        b_th = __shfl_sync(kFull, m_th, src);
+        b_ne = __shfl_sync(kFull, m_ne, src);
+        b_ss = __shfl_sync(kFull, m_ss, src);
+        b_cb = __shfl_sync(kFull, m_cb, src);
+        b_query = __shfl_sync(kFull, m_query, src);
+      }
+      uint32_t s_query = 0xFFFFFFFFu - lane, s_key = 0;  // sample launch: this lane's sample (if any), handed over below
+      if (item < total) {
+        const uint32_t off = V.off[p];
+        float sum;
+        bool ok;
+        uint32_t query, th_key;
+        if constexpr (kUnionOnly) {
+          query = b_query; th_key = b_th;
+          ok = tile_eval_or(V, cl0 + (b_cb & 0xFFFFu), (b_cb >> 22) & 63u, (b_cb >> 16) & 63u, (b_cb >> 28) != 0u,
+                            __uint_as_float(b_ne), b_ss, qc >> 16, p, off, threshold_score(th_key), sum);
+        } else {
+          const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
+          const TileQ q = V.q[sg.q];
+          const TileTQ qq = V.tq[q.qi];
+          const uint16_t* __restrict__ cl = cl0 + qq.clause_base;
+          query = qq.query; th_key = q.th_key;
+          const bool io = (qq.op_flags & 32u) != 0;
+          if (q.op() == kTileOpBool) ok = tile_eval_bool(V, cl, __float_as_uint(q.ne) & 0xFFFFu, sg.clause, p, off, io, sum);
+          else if (q.op() == kTileOpAnd) ok = tile_eval_and(V, cl, q.n(), q.n_e(), p, off, io, sum);
+          else ok = tile_eval_or(V, cl, q.n_e(), q.n(), q.prune(), q.ne, q.shared_stripes, sg.clause, p, off, threshold_score(th_key), sum);
+        }
+        if (ok) {
+          ++st.completed;
+          const uint32_t key = score_to_key(sum);
+          if (key >= th_key) ++st.pushed;
+          if (!kSample) tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive);
+          else if (key >= th_key && key != 0u && (!G.alive || is_alive(G.alive, lo + off))) { s_query = query; s_key = key; }  // (a deleted doc bounds nothing)
+        }
+      }
+      if (kSample) {  // one atomic per query and warp step instead of one per sample (the counters are hot)
+        const unsigned peers = __match_any_sync(kFull, s_query);
+        if (s_key) {
+          const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
+          uint32_t base = 0;
+          if (lane == leader) base = atomicAdd(&TP.sample_count[s_query], (uint32_t)__popc(peers));
+          base = __shfl_sync(peers, base, leader);
+          const uint32_t idx = base + (uint32_t)__popc(peers & lanemask_lt(lane));
+          if (idx < TP.sample_cap) TP.samples[(size_t)s_query * TP.sample_cap + idx] = s_key;
+        }
+      }
+    }
+  }
+}
+
+// Stage B3 of a conjunction or TQ_OP_BOOL query: the lanes share the postings of the driving words [d0, d0 + dn) of cl, and each
+// evaluates its docs with eval(word, posting, doc offset, sum).
+template <bool kSample, typename Eval>
+__device__ __forceinline__ void tile_heavy_driven(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, const uint16_t* __restrict__ cl,
+                                                  uint32_t d0, uint32_t dn, uint32_t query, uint32_t th_key, uint32_t lo, uint32_t lane, TileStats& st, Eval eval) {
+  uint32_t best = 0;
+  for (uint32_t w = d0; w < d0 + dn; ++w) {
+    const uint32_t info = V.info[cl[w]];
+    const uint32_t a = info & 0xFFFFu, e = a + (info >> 16);
+    for (uint32_t p = a + lane; p < e; p += 32) {
+      const uint32_t off = V.off[p];
+      float sum;
+      if (!eval(w, p, off, sum)) continue;
+      if (kSample) { if (!G.alive || is_alive(G.alive, lo + off)) best = max(best, score_to_key(sum)); }  // (a deleted doc bounds nothing)
+      else { ++st.completed; tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive); }
+    }
+    if (lane == 0) st.ess += e - a;
+  }
+  if (kSample) warp_push_samples(TP, query, best, th_key, lane);
+}
+
+// Stage B3: heavy pair qi, evaluated by one warp.  A union accumulates its essential clauses into the warp's window `acc` of f32
+// score slots, clause by clause (the f32 summation order), then completes each touched doc with the non-essential suffix.
+template <bool kSample, bool kUnionOnly>
+__device__ __forceinline__ void tile_heavy(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V,
+                                           const uint16_t* __restrict__ cl0, uint32_t qi, float* acc, uint32_t lo, uint32_t lane, TileStats& st) {
+  const TileTQ tq = V.tq[qi];
+  const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
+  uint32_t th_key = 0;
+  if (lane == 0) th_key = *(volatile unsigned int*)&P.qstate[tq.query].theta;
+  th_key = __shfl_sync(kFull, th_key, 0);  // one value for the whole warp (the query-wide threshold moves)
+  const float theta_f = threshold_score(th_key);
+  const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !kSample;
+  const uint32_t n = tq.n_clauses;
+  const bool io = (tq.op_flags & 32u) != 0;
+  if (lane == 0) ++st.heavy;
+  float bound, ne;  // (the bound B1 needs is not used here)
+  if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpBool) {
+    uint32_t d0 = 0, dn = 0;
+    tile_bool_drive(V, cl, d0, dn, bound);
+    return tile_heavy_driven<kSample>(P, TP, G, V, cl, d0, dn, tq.query, th_key, lo, lane, st,
+                                      [&](uint32_t w, uint32_t p, uint32_t off, float& sum) { return tile_eval_bool(V, cl, d0, w, p, off, io, sum); });
+  }
+  if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpAnd) {
+    uint32_t drv;
+    tile_and_drive(V, cl, n, drv, bound);
+    return tile_heavy_driven<kSample>(P, TP, G, V, cl, drv, 1u, tq.query, th_key, lo, lane, st,
+                                      [&](uint32_t w, uint32_t p, uint32_t off, float& sum) { return tile_eval_and(V, cl, n, w, p, off, io, sum); });
+  }
+  const uint32_t n_e = tile_essential(V, cl, n, prune, theta_f, ne);
+  for (uint32_t g = 0; g < kTile / 128u; ++g)  // -0.0 = untouched (-0.0 + s == s)
+    *reinterpret_cast<float4*>(acc + g * 128u + lane * 4u) = make_float4(-0.0f, -0.0f, -0.0f, -0.0f);
+  __syncwarp();
+  float wmax = 0.0f;
+  for (uint32_t c = 0; c < n_e; ++c) {  // clause order is the f32 summation order
+    const uint32_t info = V.info[cl[c]];
+    const uint32_t a = info & 0xFFFFu, e = a + (info >> 16);
+    for (uint32_t p = a + lane; p < e; p += 32) {
+      const uint32_t o = V.off[p];
+      const float v = __fadd_rn(acc[o], V.score[p]);
+      acc[o] = v;
+      wmax = fmaxf(wmax, v);
+    }
+    if (lane == 0) st.ess += e - a;
+    __syncwarp();
+  }
+  if (kSample) {
+    // the best partial maximum of every lane's slots; the top few of the warp are this (query, tile)'s samples
+    uint32_t best = 0;
+    for (uint32_t g = 0; g < kTile / 128u; ++g) {
+      const uint32_t idx = g * 128u + lane * 4u;
+      const float4 v = *reinterpret_cast<const float4*>(acc + idx);
+      const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (__float_as_uint(vv[c]) != 0x80000000u && (!G.alive || is_alive(G.alive, lo + idx + c))) best = max(best, score_to_key(vv[c]));  // a deleted doc's score bounds nothing
+    }
+    warp_push_samples(TP, tq.query, best, th_key, lane);
+    return;
+  }
+  // nothing of this window can reach the threshold when even its largest partial sum plus the bound cannot
+  const float mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(wmax)));
+  const bool cold = prune && (mx + ne) * 1.00001f < theta_f;
+  if (cold && lane == 0) ++st.skipped;
+  for (uint32_t g = 0; g < kTile / 128u && !cold; ++g) {
+    const uint32_t idx = g * 128u + lane * 4u;
+    const float4 v = *reinterpret_cast<const float4*>(acc + idx);
+    const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float sum = vv[c];
+      if (__float_as_uint(sum) == 0x80000000u) continue;  // untouched
+      const uint32_t off = idx + c;
+      float rem = ne;
+      bool dead = false;
+      for (uint32_t c2 = n_e; c2 < n; ++c2) {  // the non-essential suffix, with the same early exit as the flat path
+        if (prune && (sum + rem) * 1.00001f < theta_f) { dead = true; break; }
+        const uint32_t slot = cl[c2];
+        rem -= V.max[slot];
+        bool f;
+        const float x = tile_find(V, slot, off, f);
+        if (f) sum = __fadd_rn(sum, x);
+      }
+      if (dead) continue;
+      ++st.completed;
+      if (score_to_key(sum) >= th_key) ++st.pushed;
+      tile_push(P, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive);
+    }
+  }
+}
+
+// One instantiation per launch kind, so that each compiles only what it runs: kSample = the sample launch (threshold samples
+// instead of candidates), kCounters = TQ_TILE_COUNTERS diagnostics, kUnionOnly = every query of the group is a term query or a
+// union (no conjunction, no TQ_OP_BOOL: the flat path broadcasts each work-list segment's query state from the lane that reads
+// the segment).  The exact launches without counters do ~90 % of the work; they must fit 64 registers so that four CTAs share an SM.
+template <bool kSample, bool kCounters, bool kUnionOnly>
+__global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_tile(const BatchParams P, const TileParams TP, uint32_t unit_base) {
+  // kCounters: each warp's clock64() time by stage (lane 0's view of it); mark(k) books the time since the previous mark to stage k
+  long long clk_last = kCounters ? clock64() : 0;
+  unsigned long long cyc[kTileStages] = {};
+  auto mark = [&](int k) {
+    if constexpr (kCounters) {
+      const long long now = clock64();
+      cyc[k] += (unsigned long long)(now - clk_last);
+      clk_last = now;
+    }
+  };
+  extern __shared__ __align__(16) unsigned char s_dyn[];
+  __shared__ TileCtl C;
+  __shared__ unsigned long long s_stat[8 + kTileStages];
+  const TUnit U = TP.units[unit_base + blockIdx.x];
+  const TSeg G = TP.segs[U.tseg];
+  const TSlot* __restrict__ slots = TP.slots + G.slot_base;
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  const TileView V = tile_view(s_dyn, TP, G.n_big);
+  // sparse slots: (first pair not staged yet, its doc or 0xFFFFFFFF once the list is exhausted), this CTA's share of the
+  // launch's cursor scratch; slot s is always walked by the same thread, so no barrier guards it
+  uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
+  if (kCounters && tid < 8 + kTileStages) s_stat[tid] = 0ull;
+  if (tid < kTileMaxQueries / 32u) C.defer[tid] = 0u;
+  const bool cl_staged = G.n_clause_words <= TP.cl_cap;
+  const uint16_t* __restrict__ cl0 = cl_staged ? V.cl : TP.clauses + G.clause_base;
+  tile_prologue(TP, G, slots, V, cl_staged, cursor, U.t0, tid);
   mark(kStPrologue);
   __syncthreads();
   mark(kStBarrier);
-  unsigned long long st_pairs = 0, st_skip = 0, st_flat = 0, st_heavy = 0, st_ess = 0, st_compl = 0, st_push = 0;  // per-thread diagnostics
-
+  TileStats st{};
   for (uint32_t t = U.t0; t < U.t1; ++t) {
-    const uint32_t lo = t * kTile, hi = lo + kTile;
+    const uint32_t lo = t * kTile;
     // the thresholds of this thread's B1 queries (qi = tid, tid + kTileThreads): loaded now, they travel while the tile is staged.
     // Thresholds only rise (atomicMax), so a value read before stage A still bounds the query's final k-th score from below
     uint32_t th_pre0 = 0u, th_pre1 = 0u;
-    if (tid < G.n_queries) th_pre0 = *(volatile unsigned int*)&P.qstate[s_tq[tid].query].theta;
-    if (tid + kTileThreads < G.n_queries) th_pre1 = *(volatile unsigned int*)&P.qstate[s_tq[tid + kTileThreads].query].theta;
+    if (tid < G.n_queries) th_pre0 = *(volatile unsigned int*)&P.qstate[V.tq[tid].query].theta;
+    if (tid + kTileThreads < G.n_queries) th_pre1 = *(volatile unsigned int*)&P.qstate[V.tq[tid + kTileThreads].query].theta;
     if (tid < G.n_big) {  // three independent loads per dense slot: one round trip for the whole tile
       const uint32_t a = __ldg(G.tix + (size_t)t * G.n_big + tid), b = __ldg(G.tix + (size_t)(t + 1u) * G.n_big + tid);
-      s_ba[tid] = __ldg(&slots[tid].pair_base) + a;
-      s_bn[tid] = b - a;
+      V.a->ba[tid] = __ldg(&slots[tid].pair_base) + a;
+      V.a->bn[tid] = b - a;
     }
-    if (tid == 0) { s_total = 0; s_nheavy = 0; s_hpos = 0; s_nflat = 0; s_nseg = 0; s_segpos = 0; s_segvalid = TP.seg_cap; s_ndefer = 0; }
+    if (tid == 0) { C.total = 0; C.nheavy = 0; C.hpos = 0; C.nflat = 0; C.nseg = 0; C.segpos = 0; C.segvalid = TP.seg_cap; C.ndefer = 0; }
     mark(kStA);
     __syncthreads();
     mark(kStBarrier);
-    // ---- stage A: this tile's pairs of every slot -> shared memory --------------------------------------------------------
-    if (warp < G.n_big) {
-      // dense lists: warp w owns slots w, w+8, ... (<= 8 of them).  Their [tix[t], tix[t+1]) ranges are laid end to end and copied as
-      // ONE flat loop, so the loads of all the warp's slots are in flight together (one DRAM round trip per 128 pairs instead
-      // of three dependent ones per slot)
-      const uint32_t ne = (G.n_big - warp + kTileWarps - 1u) / kTileWarps;
-      uint32_t n_e = 0;
-      if (lane < ne) {
-        const uint32_t s = warp + lane * kTileWarps;
-        n_e = s_bn[s];
-        s_wa[warp][lane] = s_ba[s];
-      }
-      const uint32_t incl = warp_incl_scan(n_e, lane);
-      if (lane < 8u) s_wpre[warp][lane + 1u] = incl;
-      if (lane == 0) s_wpre[warp][0] = 0u;
-      const uint32_t total_w = __shfl_sync(kFull, incl, 7);
-      uint32_t base = 0;
-      if (lane == 0 && total_w) base = atomicAdd(&s_total, total_w);
-      base = __shfl_sync(kFull, base, 0);
-      for (uint32_t e = 0; e < ne; ++e) s_bits[(warp + e * kTileWarps) * 32u + lane] = 0u;
-      __syncwarp();
-      const bool fits = base + total_w <= TP.p_cap;
-      if (fits) {
-        for (uint32_t i0 = 0; i0 < total_w; i0 += 128u) {
-          uint32_t dd[4], ss[4];
-          float vv[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const uint32_t i = i0 + (uint32_t)u * 32u + lane;
-            dd[u] = 0xFFFFFFFFu;
-            if (i < total_w) {
-              uint32_t e = 0;
-              while (i >= s_wpre[warp][e + 1u]) ++e;
-              ss[u] = warp + e * kTileWarps;
-              const size_t g = (size_t)s_wa[warp][e] + (i - s_wpre[warp][e]);
-              dd[u] = __ldg(TP.p_docs + g);
-              vv[u] = __ldg(TP.p_scores + g);
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const uint32_t i = i0 + (uint32_t)u * 32u + lane;
-            if (dd[u] != 0xFFFFFFFFu) {
-              const uint32_t off = dd[u] - lo;
-              s_off[base + i] = (uint16_t)off;
-              s_score[base + i] = vv[u];
-              atomicOr(&s_bits[ss[u] * 32u + (off >> 5)], 1u << (off & 31u));
-            }
-          }
-        }
-      }
-      __syncwarp();
-      for (uint32_t e = 0; e < ne; ++e) {
-        const uint32_t s = warp + e * kTileWarps;
-        const uint32_t b = base + s_wpre[warp][e], n = s_wpre[warp][e + 1u] - s_wpre[warp][e];
-        const uint32_t cnt = (uint32_t)__popc(s_bits[s * 32u + lane]);
-        s_rank[s * 32u + lane] = (uint16_t)(warp_incl_scan(cnt, lane) - cnt);
-        float mx = 0.0f;
-        if (fits)
-          for (uint32_t i = lane; i < n; i += 32) mx = fmaxf(mx, s_score[b + i]);
-        mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(mx)));  // mx >= 0
-        if (lane == 0) {
-          s_info[s] = (b & 0xFFFFu) | (n << 16); s_max[s] = mx;
-          if (s_ord0) s_ord0[s] = s_wa[warp][e];
-        }
-      }
-    }
-    uint2 next_cur = G.n_big + tid < G.n_slots ? cursor[G.n_big + tid] : make_uint2(0u, 0u);
-    for (uint32_t s = G.n_big + tid; s < G.n_slots; s += kTileThreads) {  // sparse lists: one thread walks its cursor
-      const uint2 cs = next_cur;
-      if (s + kTileThreads < G.n_slots) next_cur = cursor[s + kTileThreads];  // (in flight while this slot is staged)
-      uint32_t nd = cs.y;
-      if (nd >= hi) {
-        s_info[s] = 0u; s_max[s] = 0.0f; s_mask[s] = 0u;
-        continue;
-      }
-      const TSlot sl = slots[s];
-      const uint32_t* __restrict__ d = TP.p_docs + sl.pair_base;
-      const float* __restrict__ sc = TP.p_scores + sl.pair_base;
-      const uint32_t cur = cs.x;
-      // the pair at the cursor belongs to this tile (nd < hi); fetch it and the next three, docs and scores, in ONE round trip
-      uint32_t d4[4];
-      float v4[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const bool in = cur + i < sl.doc_freq;
-        d4[i] = in ? __ldg(d + cur + i) : 0xFFFFFFFFu;
-        v4[i] = in ? __ldg(sc + cur + i) : 0.0f;
-      }
-      uint32_t n = 0;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) n += d4[i] < hi ? 1u : 0u;  // ascending: the ones below hi are a prefix
-      if (n == 4u) {  // (rare for a sparse list) keep walking
-        for (;;) {
-          const uint32_t c = cur + n;
-          uint32_t e4[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) e4[i] = c + i < sl.doc_freq ? __ldg(d + c + i) : 0xFFFFFFFFu;
-          uint32_t k = 0;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) k += e4[i] < hi ? 1u : 0u;
-          n += k;
-          if (k < 4u) { nd = e4[k]; break; }
-        }
-      } else {
-        nd = d4[n];
-      }
-      cursor[s] = make_uint2(cur + n, nd);
-      if (nd < hi + kTile) {  // the next tile reads this list again: start its pairs on their way to L2 now
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(d + cur + n));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(sc + cur + n));
-      }
-      const uint32_t base = atomicAdd(&s_total, n);
-      float mx = 0.0f;
-      uint32_t mask = 0;
-      if (base + n <= TP.p_cap) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if ((uint32_t)i < n) {
-            const uint32_t off = d4[i] - lo;
-            s_off[base + i] = (uint16_t)off;
-            s_score[base + i] = v4[i];
-            mask |= 1u << (off >> 5);
-            mx = fmaxf(mx, v4[i]);
-          }
-        }
-        for (uint32_t i = 4; i < n; ++i) {
-          const float v = __ldg(sc + cur + i);
-          const uint32_t off = __ldg(d + cur + i) - lo;
-          s_off[base + i] = (uint16_t)off;
-          s_score[base + i] = v;
-          mask |= 1u << (off >> 5);
-          mx = fmaxf(mx, v);
-        }
-      }
-      s_info[s] = (base & 0xFFFFu) | (n << 16);
-      s_max[s] = mx;
-      s_mask[s] = mask;
-      if (s_ord0) s_ord0[s] = sl.pair_base + cur;
-    }
+    // ---- stage A: this tile's pairs of every slot -> shared memory ----------------------------------------------------------
+    if (warp < G.n_big) tile_stage_dense(TP, G, V, C.total, lo, warp, lane);
+    tile_stage_sparse(TP, G, slots, V, cursor, C.total, lo, tid);
     mark(kStA);
     __syncthreads();
     mark(kStBarrier);
-    if (s_total > TP.p_cap) {  // more pairs than the tile buffer holds: give the batch back to the per-query kernels
+    if (C.total > TP.p_cap) {  // more pairs than the tile buffer holds: give the batch back to the per-query kernels
       if (tid == 0) atomicExch(TP.flags, 1u);
       __syncthreads();
       mark(kStBarrier);
       continue;
     }
-    // ---- stage B1: one thread per query -- bounds and routing ---------------------------------------------------------------
-    // skipped: no doc of the tile can reach the query's threshold;  flat: the essential postings become work items that the CTA's
-    // threads share evenly (B2);  heavy: a warp accumulates the query's window (B3; sample launches, and pairs with many postings).
-    // (a work list that fills up defers the remaining pairs to another round of B1 + B2: the list is sized for the common case)
+    // ---- stages B1 + B2, in rounds while queries are deferred -----------------------------------------------------------------
     for (uint32_t round = 0;; ++round) {
-    for (uint32_t qi = tid; qi < G.n_queries; qi += kTileThreads) {
-      if (round) {
-        const uint32_t bit = 1u << (qi & 31u);
-        if (!(s_defer[qi >> 5] & bit)) continue;
-        atomicAnd(&s_defer[qi >> 5], ~bit);
+      for (uint32_t qi = tid; qi < G.n_queries; qi += kTileThreads) {
+        if (round) {
+          const uint32_t bit = 1u << (qi & 31u);
+          if (!(C.defer[qi >> 5] & bit)) continue;
+          atomicAnd(&C.defer[qi >> 5], ~bit);
+        }
+        tile_route<kSample, kUnionOnly>(P, TP, G, V, C, cl0, qi, th_pre0, th_pre1, st);
       }
-      const TileTQ tq = s_tq[qi];
-      const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
-      const uint32_t th_key = qi < kTileThreads ? th_pre0 : qi < 2u * kTileThreads ? th_pre1 : *(volatile unsigned int*)&P.qstate[tq.query].theta;
-      const float theta_f = threshold_score(th_key);
-      const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !sample_mode;
-      const uint32_t n = tq.n_clauses, op = kUnionOnly ? 0u : tq.op_flags & 3u;
-      ++st_pairs;
-      TileQ rec;
-      rec.qi = (uint16_t)qi; rec.th_key = th_key; rec.n_op = (uint8_t)((op == kTileOpBool ? 0u : n) | (op << 6));
-      uint32_t cnt = 0, n_segs = 0, rec_ne = 0;
-      uint32_t b_d0 = 0, b_dn = 0;  // kTileOpBool: the driving words
-      if (!kUnionOnly && op == kTileOpBool) {
-        const uint32_t ng = cl[0], ns = cl[2];
-        uint32_t w = 4, best = 0xFFFFFFFFu;
-        float bound = 0.0f;
-        bool dead = false;
-        for (uint32_t g = 0; g < ng; ++g) {  // the MUST group with the fewest postings in this tile drives
-          const uint32_t glen = cl[w];
-          uint32_t tot = 0;
-          for (uint32_t e = 0; e < glen; ++e) { const uint32_t slot = cl[w + 1u + e]; tot += s_info[slot] >> 16; bound += s_max[slot]; }
-          if (tot == 0u) dead = true;
-          if (tot < best) { best = tot; b_d0 = w + 1u; b_dn = glen; }
-          w += 1u + glen;
-        }
-        uint32_t s_tot = 0;
-        for (uint32_t e = 0; e < ns; ++e) { const uint32_t slot = cl[w + e]; s_tot += s_info[slot] >> 16; bound += s_max[slot]; }
-        if (ng == 0u) { best = s_tot; b_d0 = w; b_dn = ns; }
-        if (dead || best == 0u || (prune && bound * 1.00001f < theta_f)) { ++st_skip; continue; }
-        cnt = best;
-        for (uint32_t e = 0; e < b_dn; ++e) n_segs += (s_info[cl[b_d0 + e]] >> 16) ? 1u : 0u;
-        rec.ne = __uint_as_float(b_d0 | (b_dn << 16));
-        rec.shared_stripes = 0u;
-      } else if (!kUnionOnly && op == kTileOpAnd) {
-        float bound = 0.0f;
-        uint32_t dmin = 0xFFFFFFFFu, drv = 0;
-        for (uint32_t c = 0; c < n; ++c) {  // the clause with the fewest postings in this tile drives
-          const uint32_t len = s_info[cl[c]] >> 16;
-          bound += s_max[cl[c]];
-          if (len < dmin) { dmin = len; drv = c; }
-        }
-        if (dmin == 0u || (prune && bound * 1.00001f < theta_f)) { ++st_skip; continue; }
-        rec_ne = drv; rec.ne = 0.0f; rec.shared_stripes = 0u;
-        cnt = dmin; n_segs = 1;
-      } else {
-        // sample launch: only the docs of the two heaviest clauses are scored (completely): the best docs of a union nearly
-        // always hold its rarest terms, and ANY real score is a valid sample
-        uint32_t n_e = n;
-        if (sample_mode) {  // ... extended by further clauses while the tile holds fewer than four of their postings
-          uint32_t have = 0;
-          n_e = 0;
-          while (n_e < n && (n_e < 2u || have < 4u)) { have += s_info[cl[n_e]] >> 16; ++n_e; }
-        }
-        float ne = 0.0f;
-        if (prune) {
-          while (n_e > 0) {
-            const float b = ne + s_max[cl[n_e - 1u]];
-            if (!(b * 1.00001f < theta_f)) break;  // (f32 sums of <= 32 terms differ by < 4e-6 relative between orders)
-            ne = b;
-            --n_e;
-          }
-        }
-        if (n_e == 0) { ++st_skip; continue; }  // no doc of this tile can reach the threshold
-        uint32_t seen = 0, shared = 0;
-        for (uint32_t c = 0; c < n_e; ++c) {
-          const uint32_t slot = cl[c];
-          const uint32_t len = s_info[slot] >> 16;
-          cnt += len; n_segs += len ? 1u : 0u;
-          const uint32_t m = slot < G.n_big ? (len ? 0xFFFFFFFFu : 0u) : s_mask[slot];  // (dense lists: every stripe)
-          shared |= seen & m;
-          seen |= m;
-        }
-        if (cnt == 0) { ++st_skip; continue; }  // a doc without an essential posting stays below the threshold
-        rec_ne = n_e; rec.ne = ne; rec.shared_stripes = shared;
-      }
-      rec.ne_prune = (uint8_t)(rec_ne | (prune ? 128u : 0u));
-      // sample launch: ANY set of real scores is a valid sample -- at most kSampleSeg postings per driving clause, no window path
-      if (sample_mode && *(volatile unsigned int*)&TP.sample_count[tq.query] >= TP.sample_cap) continue;
-      bool heavy = !sample_mode && cnt > TP.light_max && op != kTileOpAnd && op != kTileOpBool && rec_ne >= 2u;
-      if (n_segs > TP.seg_cap) heavy = true;  // (test hook sizes only)
-      if (!heavy) {
-        const uint32_t sb = atomicAdd(&s_nseg, n_segs);
-        if (sb + n_segs > TP.seg_cap) {  // the work list is full (entries from here on are not written): next round
-          atomicMin(&s_segvalid, sb);
-          atomicOr(&s_defer[qi >> 5], 1u << (qi & 31u));
-          s_ndefer = 1u;
-        } else {
-          const uint32_t qslot = atomicAdd(&s_nflat, 1u);
-          s_q[qslot] = rec;
-          uint32_t w = sb;
-          if (!kUnionOnly && op == kTileOpBool) {
-            for (uint32_t e = 0; e < b_dn; ++e)
-              if (s_info[cl[b_d0 + e]] >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)(b_d0 + e)};
-          } else if (!kUnionOnly && op == kTileOpAnd) {
-            s_seg[w] = TileSeg{(uint16_t)qslot, (uint16_t)rec_ne};
-          } else {
-            for (uint32_t c = 0; c < rec_ne; ++c)
-              if (s_info[cl[c]] >> 16) s_seg[w++] = TileSeg{(uint16_t)qslot, (uint16_t)c};
-          }
-          ++st_flat;
-          st_ess += cnt;
-        }
-      }
-      if (heavy) s_heavy[atomicAdd(&s_nheavy, 1u)] = (uint16_t)qi;
-    }
-    mark(kStB1);
-    __syncthreads();
-    mark(kStBarrier);
-    const bool more_rounds = s_ndefer != 0u;
-    // ---- stage B2: the flat pairs' essential postings, one per thread --------------------------------------------------------
-    {
-      const uint32_t n_seg = min(s_nseg, s_segvalid);
-      for (;;) {
-        uint32_t sbase = 0;
-        if (lane == 0) sbase = atomicAdd(&s_segpos, 32u);
-        sbase = __shfl_sync(kFull, sbase, 0);
-        if (sbase >= n_seg) break;
-        // 32 segments, one per lane; their postings are dealt to the lanes 32 at a time (load-balanced expansion)
-        uint32_t m_len = 0, m_qc = 0, m_start = 0;  // the lane's segment: postings [m_start, m_start + m_len), q | clause << 16
-        // kUnionOnly: the segment's query state, read once here and handed to the posting lanes with shuffles (instead of three
-        // dependent shared loads per posting): th_key, ne, shared_stripes, clause base | n << 16 | n_e << 22 | prune << 28, query
-        uint32_t m_th = 0, m_ne = 0, m_ss = 0, m_cb = 0, m_query = 0;
-        if (sbase + lane < n_seg) {
-          const TileSeg sg = s_seg[sbase + lane];
-          uint32_t info;
-          if constexpr (kUnionOnly) {
-            const TileQ q = s_q[sg.q];
-            const TileTQ qq = s_tq[q.qi];
-            info = s_info[cl0[qq.clause_base + sg.clause]];
-            m_th = q.th_key; m_ne = __float_as_uint(q.ne); m_ss = q.shared_stripes; m_query = qq.query;
-            m_cb = qq.clause_base | (q.n() << 16) | (q.n_e() << 22) | (q.prune() ? 1u << 28 : 0u);
-          } else {
-            info = s_info[cl0[s_tq[s_q[sg.q].qi].clause_base + sg.clause]];
-          }
-          m_qc = sg.q | ((uint32_t)sg.clause << 16);
-          m_start = info & 0xFFFFu;
-          m_len = sample_mode ? min(info >> 16, kSampleSeg) : info >> 16;
-        }
-        const uint32_t incl = warp_incl_scan(m_len, lane);
-        const uint32_t total = __shfl_sync(kFull, incl, 31);
-        const uint32_t excl = incl - m_len;
-        const uint32_t m_pbase = m_start - excl;  // (mod 2^32) the pair index of the chunk item ibase + lane is m_pbase + ibase + lane
-        for (uint32_t ibase = 0; ibase < total; ibase += 32u) {
-          const uint32_t item = ibase + lane;
-          // the segment of item `ibase + lane`: every listed segment holds a posting, so segment numbers grow by one at each
-          // start; (segments that start before this chunk) - 1 + (starts at or before the lane's item)
-          const uint32_t rel = excl - ibase;  // (wraps for segments that start before the chunk)
-          const uint32_t starts = __reduce_or_sync(kFull, (m_len && rel < 32u) ? (1u << rel) : 0u);
-          const uint32_t earlier = (uint32_t)__popc(__ballot_sync(kFull, m_len && excl < ibase));
-          const uint32_t j = earlier - 1u + (uint32_t)__popc(starts & (0xFFFFFFFFu >> (31u - lane)));
-          const uint32_t src = j & 31u;
-          const uint32_t p = __shfl_sync(kFull, m_pbase, src) + item;
-          const uint32_t qc = __shfl_sync(kFull, m_qc, src);
-          uint32_t b_th = 0, b_ne = 0, b_ss = 0, b_cb = 0, b_query = 0;
-          if constexpr (kUnionOnly) {
-            b_th = __shfl_sync(kFull, m_th, src);
-            b_ne = __shfl_sync(kFull, m_ne, src);
-            b_ss = __shfl_sync(kFull, m_ss, src);
-            b_cb = __shfl_sync(kFull, m_cb, src);
-            b_query = __shfl_sync(kFull, m_query, src);
-          }
-          uint32_t s_query = 0xFFFFFFFFu - lane, s_key = 0;  // sample launch: this lane's sample (if any), handed over below
-          if (item < total) {
-            const uint32_t off = s_off[p];
-            float sum;
-            bool ok;
-            uint32_t query, th_key;
-            if constexpr (kUnionOnly) {
-              query = b_query; th_key = b_th;
-              ok = tile_eval_or(V, s_max, cl0 + (b_cb & 0xFFFFu), (b_cb >> 22) & 63u, (b_cb >> 16) & 63u, (b_cb >> 28) != 0u,
-                                __uint_as_float(b_ne), b_ss, qc >> 16, p, off, threshold_score(th_key), sum);
-            } else {
-              const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
-              const TileQ q = s_q[sg.q];
-              const TileTQ qq = s_tq[q.qi];
-              const uint16_t* __restrict__ cl = cl0 + qq.clause_base;
-              query = qq.query; th_key = q.th_key;
-              const bool io = (qq.op_flags & 32u) != 0;
-              if (q.op() == kTileOpBool) ok = tile_eval_bool(V, cl, __float_as_uint(q.ne) & 0xFFFFu, sg.clause, p, off, io, sum);
-              else if (q.op() == kTileOpAnd) ok = tile_eval_and(V, cl, q.n(), q.n_e(), p, off, io, sum);
-              else ok = tile_eval_or(V, s_max, cl, q.n_e(), q.n(), q.prune(), q.ne, q.shared_stripes, sg.clause, p, off, threshold_score(th_key), sum);
-            }
-            if (ok) {
-              ++st_compl;
-              const uint32_t key = score_to_key(sum);
-              if (key >= th_key) ++st_push;
-              if (!sample_mode) tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive);
-              else if (key >= th_key && key != 0u && (!G.alive || is_alive(G.alive, lo + off))) { s_query = query; s_key = key; }  // (a deleted doc bounds nothing)
-            }
-          }
-          if (sample_mode) {  // one atomic per query and warp step instead of one per sample (the counters are hot)
-            const unsigned peers = __match_any_sync(kFull, s_query);
-            if (s_key) {
-              const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
-              uint32_t base = 0;
-              if (lane == leader) base = atomicAdd(&TP.sample_count[s_query], (uint32_t)__popc(peers));
-              base = __shfl_sync(peers, base, leader);
-              const uint32_t idx = base + (uint32_t)__popc(peers & lanemask_lt(lane));
-              if (idx < TP.sample_cap) TP.samples[(size_t)s_query * TP.sample_cap + idx] = s_key;
-            }
-          }
-        }
-      }
-    }
-    mark(kStB2);
-    if (!more_rounds) break;
-    __syncthreads();
-    if (tid == 0) { s_nflat = 0; s_nseg = 0; s_segpos = 0; s_segvalid = TP.seg_cap; s_ndefer = 0; }
-    __syncthreads();
-    mark(kStBarrier);
-    }
-    // ---- stage B3: one warp per heavy pair, a window of f32 score slots ----------------------------------------------------
-    {
-      const uint32_t n_heavy = s_nheavy;
-      if (n_heavy) __syncthreads();  // the windows overlay the work list: every warp must be done with B2
+      mark(kStB1);
+      __syncthreads();
       mark(kStBarrier);
-      float* acc = s_acc + warp * kTile;
-      for (; warp < n_win;) {  // (the warps without a window go straight to the barrier)
-        uint32_t h = 0;
-        if (lane == 0) h = atomicAdd(&s_hpos, 1u);
-        h = __shfl_sync(kFull, h, 0);
-        if (h >= n_heavy) break;
-        const TileTQ tq = s_tq[s_heavy[h]];
-        const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
-        uint32_t th_key = 0;
-        if (lane == 0) th_key = *(volatile unsigned int*)&P.qstate[tq.query].theta;
-        th_key = __shfl_sync(kFull, th_key, 0);  // one value for the whole warp (the query-wide threshold moves)
-        const float theta_f = threshold_score(th_key);
-        const bool prune = (tq.op_flags & 128u) && theta_f > 0.0f && !sample_mode;
-        const uint32_t n = tq.n_clauses;
-        if (lane == 0) ++st_heavy;
-        if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpBool) {  // lanes share the driving group's postings (as for conjunctions below)
-          const uint32_t ng = cl[0], ns = cl[2];
-          uint32_t w = 4, best_tot = 0xFFFFFFFFu, d0 = 0, dn = 0;
-          for (uint32_t g = 0; g < ng; ++g) {
-            const uint32_t glen = cl[w];
-            uint32_t tot = 0;
-            for (uint32_t e = 0; e < glen; ++e) tot += s_info[cl[w + 1u + e]] >> 16;
-            if (tot < best_tot) { best_tot = tot; d0 = w + 1u; dn = glen; }
-            w += 1u + glen;
-          }
-          if (ng == 0u) { d0 = w; dn = ns; }
-          uint32_t best = 0;
-          for (uint32_t e = 0; e < dn; ++e) {
-            const uint32_t info = s_info[cl[d0 + e]];
-            const uint32_t a = info & 0xFFFFu, en = a + (info >> 16);
-            for (uint32_t p = a + lane; p < en; p += 32) {
-              const uint32_t off = s_off[p];
-              float sum;
-              if (!tile_eval_bool(V, cl, d0, d0 + e, p, off, (tq.op_flags & 32u) != 0, sum)) continue;
-              if (sample_mode) { if (!G.alive || is_alive(G.alive, lo + off)) best = max(best, score_to_key(sum)); }
-              else { ++st_compl; tile_push(P, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive); }
-            }
-            if (lane == 0) st_ess += en - a;
-          }
-          if (sample_mode) {
-            for (uint32_t r = 0; r < kSamplePerTile; ++r) {
-              const uint32_t mk = __reduce_max_sync(kFull, best);
-              if (mk == 0u || mk < th_key) break;
-              const unsigned who = __ballot_sync(kFull, best == mk);
-              if (lane == (uint32_t)__ffs(who) - 1u) {
-                const uint32_t idx = atomicAdd(&TP.sample_count[tq.query], 1u);
-                if (idx < TP.sample_cap) TP.samples[(size_t)tq.query * TP.sample_cap + idx] = mk;
-                best = 0;
-              }
-            }
-          }
-          __syncwarp();
-          continue;
-        }
-        if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpAnd) {  // lanes share the driving clause's postings; every lane looks its docs up in the others
-          uint32_t dmin = 0xFFFFFFFFu, drv = 0;
-          for (uint32_t c = 0; c < n; ++c) {
-            const uint32_t len = s_info[cl[c]] >> 16;
-            if (len < dmin) { dmin = len; drv = c; }
-          }
-          const uint32_t info = s_info[cl[drv]];
-          const uint32_t a = info & 0xFFFFu, e = a + (info >> 16);
-          uint32_t best = 0;
-          for (uint32_t p = a + lane; p < e; p += 32) {
-            const uint32_t off = s_off[p];
-            float sum;
-            if (!tile_eval_and(V, cl, n, drv, p, off, (tq.op_flags & 32u) != 0, sum)) continue;
-            if (sample_mode) { if (!G.alive || is_alive(G.alive, lo + off)) best = max(best, score_to_key(sum)); }  // (a deleted doc bounds nothing)
-            else { ++st_compl; tile_push(P, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive); }
-          }
-          if (lane == 0) st_ess += e - a;
-          if (sample_mode) {
-            for (uint32_t r = 0; r < kSamplePerTile; ++r) {
-              const uint32_t mk = __reduce_max_sync(kFull, best);
-              if (mk == 0u || mk < th_key) break;
-              const unsigned who = __ballot_sync(kFull, best == mk);
-              if (lane == (uint32_t)__ffs(who) - 1u) {
-                const uint32_t idx = atomicAdd(&TP.sample_count[tq.query], 1u);
-                if (idx < TP.sample_cap) TP.samples[(size_t)tq.query * TP.sample_cap + idx] = mk;
-                best = 0;
-              }
-            }
-          }
-          __syncwarp();
-          continue;
-        }
-        uint32_t n_e = n;
-        float ne = 0.0f;
-        if (prune) {
-          while (n_e > 0) {
-            const float b = ne + s_max[cl[n_e - 1u]];
-            if (!(b * 1.00001f < theta_f)) break;
-            ne = b;
-            --n_e;
-          }
-        }
-        for (uint32_t g = 0; g < kTile / 128u; ++g)  // -0.0 = untouched (-0.0 + s == s)
-          *reinterpret_cast<float4*>(acc + g * 128u + lane * 4u) = make_float4(neg_zero, neg_zero, neg_zero, neg_zero);
-        __syncwarp();
-        float wmax = 0.0f;
-        for (uint32_t c = 0; c < n_e; ++c) {  // clause order is the f32 summation order
-          const uint32_t info = s_info[cl[c]];
-          const uint32_t a = info & 0xFFFFu, e = a + (info >> 16);
-          for (uint32_t p = a + lane; p < e; p += 32) {
-            const uint32_t o = s_off[p];
-            const float v = __fadd_rn(acc[o], s_score[p]);
-            acc[o] = v;
-            wmax = fmaxf(wmax, v);
-          }
-          if (lane == 0) st_ess += e - a;
-          __syncwarp();
-        }
-        if (sample_mode) {
-          // the best partial maximum of every lane's slots; the top few of the warp are this (query, tile)'s samples
-          uint32_t best = 0;
-          for (uint32_t g = 0; g < kTile / 128u; ++g) {
-            const uint32_t idx = g * 128u + lane * 4u;
-            const float4 v = *reinterpret_cast<const float4*>(acc + idx);
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-              if (__float_as_uint(vv[c]) != 0x80000000u && (!G.alive || is_alive(G.alive, lo + idx + c))) best = max(best, score_to_key(vv[c]));  // a deleted doc's score bounds nothing
-          }
-          for (uint32_t r = 0; r < kSamplePerTile; ++r) {
-            const uint32_t m = __reduce_max_sync(kFull, best);
-            if (m == 0u || m < th_key) break;
-            const unsigned who = __ballot_sync(kFull, best == m);
-            if (lane == (uint32_t)__ffs(who) - 1u) {
-              const uint32_t idx = atomicAdd(&TP.sample_count[tq.query], 1u);
-              if (idx < TP.sample_cap) TP.samples[(size_t)tq.query * TP.sample_cap + idx] = m;
-              best = 0;
-            }
-          }
-          __syncwarp();
-          continue;
-        }
-        // nothing of this window can reach the threshold when even its largest partial sum plus the bound cannot
-        const float mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(wmax)));
-        const bool cold = prune && (mx + ne) * 1.00001f < theta_f;
-        if (cold && lane == 0) ++st_skip;
-        for (uint32_t g = 0; g < kTile / 128u && !cold; ++g) {
-          const uint32_t idx = g * 128u + lane * 4u;
-          const float4 v = *reinterpret_cast<const float4*>(acc + idx);
-          const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            float sum = vv[c];
-            if (__float_as_uint(sum) == 0x80000000u) continue;  // untouched
-            const uint32_t off = idx + c;
-            float rem = ne;
-            bool dead = false;
-            for (uint32_t c2 = n_e; c2 < n; ++c2) {  // the non-essential suffix, with the same early exit as the flat path
-              if (prune && (sum + rem) * 1.00001f < theta_f) { dead = true; break; }
-              const uint32_t slot = cl[c2];
-              rem -= s_max[slot];
-              bool f;
-              const float x = tile_find(V, slot, off, f);
-              if (f) sum = __fadd_rn(sum, x);
-            }
-            if (dead) continue;
-            ++st_compl;
-            if (score_to_key(sum) >= th_key) ++st_push;
-            tile_push(P, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive);
-          }
-        }
-        __syncwarp();
-      }
+      const bool more_rounds = C.ndefer != 0u;
+      tile_flat<kSample, kUnionOnly>(P, TP, G, V, C, cl0, lo, lane, st);
+      mark(kStB2);
+      if (!more_rounds) break;
+      __syncthreads();
+      if (tid == 0) { C.nflat = 0; C.nseg = 0; C.segpos = 0; C.segvalid = TP.seg_cap; C.ndefer = 0; }
+      __syncthreads();
+      mark(kStBarrier);
+    }
+    // ---- stage B3: one warp per heavy pair, a window of f32 score slots ------------------------------------------------------
+    const uint32_t n_heavy = C.nheavy;
+    if (n_heavy) __syncthreads();  // the windows overlay the work list: every warp must be done with B2
+    mark(kStBarrier);
+    float* acc = V.acc + warp * kTile;
+    for (; warp < TP.n_win;) {  // (the warps without a window go straight to the barrier)
+      uint32_t h = 0;
+      if (lane == 0) h = atomicAdd(&C.hpos, 1u);
+      h = __shfl_sync(kFull, h, 0);
+      if (h >= n_heavy) break;
+      tile_heavy<kSample, kUnionOnly>(P, TP, G, V, cl0, V.heavy[h], acc, lo, lane, st);
+      __syncwarp();
     }
     mark(kStB3);
     __syncthreads();
@@ -1072,7 +1071,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   }
   if constexpr (kCounters) {
     // warp-aggregated diagnostics
-    unsigned long long v[7] = {st_pairs, st_skip, st_flat, st_heavy, st_ess, st_compl, st_push};
+    unsigned long long v[7] = {st.pairs, st.skipped, st.flat, st.heavy, st.ess, st.completed, st.pushed};
 #pragma unroll
     for (int i = 0; i < 7; ++i) {
       unsigned long long x = v[i];
