@@ -179,6 +179,9 @@ typedef struct {
                                    [1] A (staging), [2] B1 (routing), [3] B2 (flat evaluation), [4] B3 (windows), [5] barrier waits */
   uint64_t tile_groups_union_only; /* of tile_groups: groups whose queries are all term queries and unions, which run the
                                       union-only k_tile instances (k_tile<*, *, true>); the rest run the general instances */
+  uint64_t tile_b2_exits[4];    /* cumulative, with TQ_TILE_COUNTERS=1: union postings of the exact k_tile launches' flat evaluation
+                                   (stage B2) by how they ended: [0] dropped by the bound taken before the look-ups, [1] not the owner
+                                   (an earlier essential clause lists the doc), [2] dropped in the non-essential walk, [3] completed */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */

@@ -1,4 +1,5 @@
-"""Probe of the tile engine on a bench workload: per-kind kernel times, tile counters, k_tile's cycles by stage, parity of a query sample.
+"""Probe of the tile engine on a bench workload: per-kind kernel times, tile counters, how B2's union postings ended, k_tile's cycles
+by stage, parity of a query sample.
 usage: python profiles/probe_tile.py [workload] [nq] [steps] [check]   (env knobs: TQ_TILE*, see tq_ctx_create)"""
 import json
 import os
@@ -38,6 +39,7 @@ def stage_shares(cyc):
 
 c0 = np.array(ctx.stats()["tile_counters"], dtype=np.int64)
 y0 = np.array(ctx.stats()["tile_cycles"], dtype=np.int64)
+x0 = np.array(ctx.stats()["tile_b2_exits"], dtype=np.int64)
 y_first = None
 for i in range(steps + 2):
     t0 = time.perf_counter()
@@ -49,6 +51,7 @@ for i in range(steps + 2):
     st = ctx.stats()
     c1 = np.array(st["tile_counters"], dtype=np.int64)
     y1 = np.array(st["tile_cycles"], dtype=np.int64)
+    x1 = np.array(st["tile_b2_exits"], dtype=np.int64)
     if i == 2:
         y_first = y0  # (the first two steps warm up: the summary below covers the rest)
     print(json.dumps({"step": i, "prepare_ms": round(1e3 * (t1 - t0), 2), "run_ms": round(1e3 * (t2 - t1), 2),
@@ -56,8 +59,9 @@ for i in range(steps + 2):
                       "tile_postings": st["tile_postings"], "scratch_MB": st["tile_scratch_bytes"] >> 20, "fallback": st["tile_fallbacks"],
                       "groups": st["tile_groups"], "smem": int(c1[7]), "tile_ctas_per_sm": st["tile_ctas_per_sm"],
                       "counters(pairs,skip,light,heavy,ess,compl,pass)": (c1 - c0)[:7].tolist(),
+                      "b2_union_exits(bound,not_owner,walk,completed)": (x1 - x0).tolist(),
                       "stage_shares": stage_shares(y1 - y0)}), flush=True)
-    c0, y0 = c1, y1
+    c0, y0, x0 = c1, y1, x1
     bt.close()
 if y_first is not None and (y0 - y_first).any():
     d = y0 - y_first

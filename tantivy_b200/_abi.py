@@ -122,6 +122,7 @@ class Stats(C.Structure):
         ("tile_ctas_per_sm", C.c_uint64),
         ("tile_cycles", C.c_uint64 * 8),
         ("tile_groups_union_only", C.c_uint64),
+        ("tile_b2_exits", C.c_uint64 * 4),
     ]
 
 

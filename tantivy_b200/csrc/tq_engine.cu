@@ -168,7 +168,8 @@ struct tq_ctx {
   std::vector<tq_batch*> pool;
   tq_stats stats{};
   uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit;
-  unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage
+  unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
+                                             // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 16, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
   uint32_t tile_ops = 7;  // bit per TQ_OP_*: which query shapes the tile engine takes
   uint32_t tile_seg_cap_hook = 0;
@@ -182,7 +183,7 @@ struct tq_ctx {
 };
 
 constexpr int kTileRounds = 4;  // launches of k_tile per run: the sample launch + three exact ones
-constexpr int kCounterWords = 24;  // tq_ctx::d_counters
+constexpr int kCounterWords = 8 + kTileStatWords;  // tq_ctx::d_counters (k_tile adds to those from word 8 on)
 
 // The k_tile instances, indexed sample launch << 2 | counters << 1 | union-only (tile_kernel).
 using TileKernel = void (*)(const BatchParams, const TileParams, uint32_t);
@@ -411,8 +412,10 @@ int tq_get_stats(tq_ctx* c, tq_stats* out) {
   out->lists_cached = c->list_cache.size();
   cudaSetDevice(c->device);
   unsigned long long h[kCounterWords];
-  if (cudaMemcpy(h, c->d_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
+  if (cudaMemcpy(h, c->d_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
     for (int i = 0; i < 8; ++i) { out->or_windows[i] = h[i]; out->tile_counters[i] = h[8 + i]; out->tile_cycles[i] = h[16 + i]; }
+    for (int i = 0; i < kOrExits; ++i) out->tile_b2_exits[i] = h[24 + i];
+  }
   out->tile_counters[7] = c->tile_smem_last;
   out->tile_ctas_per_sm = c->tile_ctas_last;
   return TQ_OK;

@@ -101,7 +101,8 @@ struct TileParams {
   uint32_t* flags;         // [0]: a tile held more pairs than p_cap (the batch is re-run on the per-query kernels)
   unsigned long long* counters;  // [16] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
                                  //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold;
-                                 //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage)
+                                 //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage);
+                                 //     [16, 16 + kOrExits) B2's union postings by exit (TileOrExit)
                                  //     (null: the launch runs k_tile<*, false, *>)
   uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
   uint32_t sample_cap;
@@ -182,8 +183,9 @@ __global__ void __launch_bounds__(kThreads, 4) k_score_lists(const BatchParams P
 // What a tile keeps in shared memory per slot: info = start | len << 16 (pairs [start, start + len) of off / score, ascending
 // docs), the largest score (max), and for DENSE slots (the first n_big of a segment) a 1024-bit presence map (bits) with per-word
 // ranks (rank: pairs of the slot before word w), so that "does this list hold doc x, and where" is one bit test + one popcount
-// instead of a binary search over hundreds of pairs; for sparse slots a stripe mask (bit j set = the slot lists a doc of the tile's
-// j-th 32-doc stripe).  TileView holds every region of a CTA's dynamic shared memory (tile_smem_layout lists them).
+// instead of a binary search over hundreds of pairs; for every slot a stripe mask (bit j set = the slot lists a doc of the tile's
+// j-th 32-doc stripe; a dense slot's is the ballot of its non-zero presence words).  TileView holds every region of a CTA's dynamic
+// shared memory (tile_smem_layout lists them).
 struct TileQ; struct TileSeg; struct TileStageA; struct TileTQ;
 struct TileView {
   float* score; TileQ* q; TileSeg* seg; TileStageA* a; float* acc;  // (a: in the bytes of seg; acc: in those of q and seg)
@@ -253,18 +255,44 @@ struct TileTQ {
 // launch takes at most kSampleSeg of them)
 struct TileSeg { uint16_t q, clause; };
 
+// Union: what every clause after essential clause c can add to a doc of this tile -- the tile maxima of the essential clauses
+// (c, n_e) plus ne, the bound of the non-essential suffix.
+__device__ __forceinline__ float tile_or_tail(const TileView& V, const uint16_t* __restrict__ cl, uint32_t c, uint32_t n_e, float ne) {
+  float tail = ne;
+  for (uint32_t c2 = c + 1u; c2 < n_e; ++c2) tail += V.max[cl[c2]];
+  return tail;
+}
+
+// How tile_eval_or leaves a posting (k_tile<*, true, *> counts each: TileParams::counters[16 + exit], tq_stats.tile_b2_exits):
+// dropped by the bound taken before the look-ups, the doc belongs to an earlier essential clause, dropped in the non-essential
+// walk, complete score.  Only the counters instances record it (tile_eval_or<true, *>): the other instances keep the two-way exit,
+// whose branch structure the exit codes change (as the function's value they cost k_tile 5 % on or5_top100_100M_8seg, H100 80GB
+// HBM3 at 700 W).
+enum TileOrExit : uint32_t { kOrBound, kOrOwner, kOrWalk, kOrDone, kOrExits };
+
 // Union: the doc at tile offset `off`, met as posting p of essential clause c (of n_e; n clauses, ne and shared_stripes as in TileQ).
 // Exact score in the canonical order, or nothing when the bounds show it cannot reach the threshold.  Returns true when `sum` is a
-// complete score.
-__device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* __restrict__ cl, uint32_t n_e,
-                                             uint32_t n, bool prune, float ne, uint32_t shared_stripes, uint32_t c, uint32_t p, uint32_t off,
-                                             float theta_f, float& sum) {
+// complete score; kExit: `ex` says how the posting left.  kTail: `tail` = tile_or_tail(c) is given (else it is summed here, when
+// needed).
+template <bool kExit, bool kTail>
+__device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* __restrict__ cl, uint32_t n_e, uint32_t n, bool prune,
+                                             float ne, float tail, uint32_t shared_stripes, uint32_t c, uint32_t p, uint32_t off,
+                                             float theta_f, float& sum, uint32_t& ex) {
   bool f;
   sum = V.score[p];  // (-0.0 + s == s: SumCombiner starts from 0, score_combiner.rs:39-57)
   if ((shared_stripes >> (off >> 5)) & 1u) {  // another essential clause lists a doc near this one: look the doc up
+    // ... unless the bound says no: if an earlier clause lists the doc, it is dropped here anyway; if none does, its score is at
+    // most sum + tail (the f32 orders of the two sums differ by less than the margin, as in tile_essential)
+    if (prune && (sum + (kTail ? tail : tile_or_tail(V, cl, c, n_e, ne))) * 1.00001f < theta_f) {
+      if (kExit) ex = kOrBound;
+      return false;
+    }
     for (uint32_t c1 = 0; c1 < c; ++c1) {  // an earlier essential clause lists the doc: it is evaluated there
       tile_find(V, cl[c1], off, f);
-      if (f) return false;
+      if (f) {
+        if (kExit) ex = kOrOwner;
+        return false;
+      }
     }
     for (uint32_t c2 = c + 1u; c2 < n_e; ++c2) {
       const float v = tile_find(V, cl[c2], off, f);
@@ -274,12 +302,16 @@ __device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* 
   // the non-essential suffix, densest last; stop as soon as what is left cannot lift the doc over the threshold
   float rem = ne;
   for (uint32_t c2 = n_e; c2 < n; ++c2) {
-    if (prune && (sum + rem) * 1.00001f < theta_f) return false;
+    if (prune && (sum + rem) * 1.00001f < theta_f) {
+      if (kExit) ex = kOrWalk;
+      return false;
+    }
     const uint32_t slot = cl[c2];
     rem -= V.max[slot];
     const float v = tile_find(V, slot, off, f);
     if (f) sum = __fadd_rn(sum, v);
   }
+  if (kExit) ex = kOrDone;
   return true;
 }
 
@@ -371,7 +403,7 @@ struct TileStageA {
 // TileParams::cursors).  f32 scores [p_cap] at 0; the work list: TileQ records [max_queries] (`list`) + TileSeg segments [seg_cap]
 // (`seg`, which stage A uses for its TileStageA scratch), and in the same bytes the [n_win][kTile] f32 windows of the rare heavy
 // pairs (stage B3 starts after the last B2 of the tile); per slot: pair range start | len << 16 (`info`), largest score in the tile
-// (`max`, >= 0) and sparse stripe mask [max_slots] each; presence maps [max_big][32]; TileTQ [max_queries]; u16 presence map ranks
+// (`max`, >= 0) and stripe mask [max_slots] each; presence maps [max_big][32]; TileTQ [max_queries]; u16 presence map ranks
 // [max_big][32], doc offsets [p_cap], heavy pairs [max_queries] and clause slots [cl_cap].
 struct TileSmem { uint32_t list, seg, info, max, mask, bits, tq, rank, off, heavy, cl, end; };
 __host__ __device__ constexpr TileSmem tile_smem_layout(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries,
@@ -410,11 +442,14 @@ __device__ __forceinline__ TileView tile_view(unsigned char* s_dyn, const TilePa
 // segments claimed (B1), taken by a warp (B2) and written (the list filled up from `segvalid` on); whether queries were deferred
 // to another round of B1 + B2, and which.
 struct TileCtl { uint32_t total, nheavy, hpos, nflat, nseg, segpos, segvalid, ndefer, defer[kTileMaxQueries / 32u]; };
-// Per-thread diagnostics of k_tile<*, true, *> (TileParams::counters[0, 7)); the other instances compile them out.
-struct TileStats { unsigned long long pairs, skipped, flat, heavy, ess, completed, pushed; };
+// Per-thread diagnostics of k_tile<*, true, *> (TileParams::counters[0, 7), and or_exit: [16, 20)); the other instances compile
+// them out.  or_exit: the exact launches' B2 union postings by how tile_eval_or left them (TileOrExit; 32 bits: a thread's share of
+// one launch).
+struct TileStats { unsigned long long pairs, skipped, flat, heavy, ess, completed, pushed; uint32_t or_exit[kOrExits]; };
 // Stages of a tile as the cycle counters of k_tile<*, true, *> split a warp's time (TileParams::counters[8 + stage],
 // tq_stats.tile_cycles): the cursor prologue, A, B1, B2, B3, and the waits at the barriers between them.
 enum TileStage : int { kStPrologue, kStA, kStB1, kStB2, kStB3, kStBarrier, kTileStages };
+constexpr int kTileStatWords = 16 + kOrExits;  // TileParams::counters words k_tile<*, true, *> adds to
 
 // ---- the decisions B1 (routing) and B3 (windows) share -------------------------------------------------------------------
 // TQ_OP_BOOL: the driving words [d0, d0 + dn) of cl -- the MUST group with the fewest postings in this tile (the first of equals),
@@ -582,13 +617,15 @@ __device__ __forceinline__ void tile_stage_dense(const TileParams& TP, const TSe
   for (uint32_t e = 0; e < ne; ++e) {
     const uint32_t s = warp + e * kTileWarps;
     const uint32_t b = base + A.wpre[warp][e], n = A.wpre[warp][e + 1u] - A.wpre[warp][e];
-    const uint32_t cnt = (uint32_t)__popc(V.bits[s * 32u + lane]);
+    const uint32_t word = V.bits[s * 32u + lane];
+    const uint32_t cnt = (uint32_t)__popc(word);
     V.rank[s * 32u + lane] = (uint16_t)(warp_incl_scan(cnt, lane) - cnt);
+    const uint32_t mask = __ballot_sync(kFull, word != 0u);  // (presence word j = stripe j)
     float mx = 0.0f;
     if (fits)
       for (uint32_t i = lane; i < n; i += 32) mx = fmaxf(mx, V.score[b + i]);
     mx = __uint_as_float(__reduce_max_sync(kFull, __float_as_uint(mx)));  // mx >= 0
-    if (lane == 0) { V.info[s] = (b & 0xFFFFu) | (n << 16); V.max[s] = mx; }
+    if (lane == 0) { V.info[s] = (b & 0xFFFFu) | (n << 16); V.max[s] = mx; V.mask[s] = mask; }
   }
 }
 
@@ -676,7 +713,7 @@ __device__ __forceinline__ void tile_stage_sparse(const TileParams& TP, const TS
 // query to another round of B1 + B2 (the list is sized for the common case).  th_pre0 / th_pre1: the thresholds of queries tid and
 // tid + kTileThreads, loaded before stage A.
 template <bool kSample, bool kUnionOnly>
-__device__ __forceinline__ void tile_route(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C,
+__device__ __forceinline__ void tile_route(const BatchParams& P, const TileParams& TP, const TileView& V, TileCtl& C,
                                            const uint16_t* __restrict__ cl0, uint32_t qi, uint32_t th_pre0, uint32_t th_pre1, TileStats& st) {
   const TileTQ tq = V.tq[qi];
   const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
@@ -719,7 +756,7 @@ __device__ __forceinline__ void tile_route(const BatchParams& P, const TileParam
       const uint32_t slot = cl[c];
       const uint32_t len = V.info[slot] >> 16;
       cnt += len; n_segs += len ? 1u : 0u;
-      const uint32_t m = slot < G.n_big ? (len ? 0xFFFFFFFFu : 0u) : V.mask[slot];  // (dense lists: every stripe)
+      const uint32_t m = V.mask[slot];
       shared |= seen & m;
       seen |= m;
     }
@@ -759,7 +796,7 @@ __device__ __forceinline__ void tile_route(const BatchParams& P, const TileParam
 
 // Stage B2: the flat pairs' essential postings, one per thread.  A warp takes 32 work-list segments at a time, one per lane, and
 // deals their postings to the lanes 32 at a time (load-balanced expansion).
-template <bool kSample, bool kUnionOnly>
+template <bool kSample, bool kCounters, bool kUnionOnly>
 __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C,
                                           const uint16_t* __restrict__ cl0, uint32_t lo, uint32_t lane, TileStats& st) {
   const uint32_t n_seg = min(C.nseg, C.segvalid);
@@ -770,8 +807,9 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
     if (sbase >= n_seg) break;
     uint32_t m_len = 0, m_qc = 0, m_start = 0;  // the lane's segment: postings [m_start, m_start + m_len), q | clause << 16
     // kUnionOnly: the segment's query state, read once here and handed to the posting lanes with shuffles (instead of three
-    // dependent shared loads per posting): th_key, ne, shared_stripes, clause base | n << 16 | n_e << 22 | prune << 28, query
-    uint32_t m_th = 0, m_ne = 0, m_ss = 0, m_cb = 0, m_query = 0;
+    // dependent shared loads per posting): th_key, ne, the clause's tile_or_tail, shared_stripes, clause base | n << 16 |
+    // n_e << 22 | prune << 28, query
+    uint32_t m_th = 0, m_ne = 0, m_tail = 0, m_ss = 0, m_cb = 0, m_query = 0;
     if (sbase + lane < n_seg) {
       const TileSeg sg = V.seg[sbase + lane];
       uint32_t info;
@@ -780,6 +818,7 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
         const TileTQ qq = V.tq[q.qi];
         info = V.info[cl0[qq.clause_base + sg.clause]];
         m_th = q.th_key; m_ne = __float_as_uint(q.ne); m_ss = q.shared_stripes; m_query = qq.query;
+        m_tail = __float_as_uint(tile_or_tail(V, cl0 + qq.clause_base, sg.clause, q.n_e(), q.ne));
         m_cb = qq.clause_base | (q.n() << 16) | (q.n_e() << 22) | (q.prune() ? 1u << 28 : 0u);
       } else {
         info = V.info[cl0[V.tq[V.q[sg.q].qi].clause_base + sg.clause]];
@@ -803,10 +842,11 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
       const uint32_t src = j & 31u;
       const uint32_t p = __shfl_sync(kFull, m_pbase, src) + item;
       const uint32_t qc = __shfl_sync(kFull, m_qc, src);
-      uint32_t b_th = 0, b_ne = 0, b_ss = 0, b_cb = 0, b_query = 0;
+      uint32_t b_th = 0, b_ne = 0, b_tail = 0, b_ss = 0, b_cb = 0, b_query = 0;
       if constexpr (kUnionOnly) {
         b_th = __shfl_sync(kFull, m_th, src);
         b_ne = __shfl_sync(kFull, m_ne, src);
+        b_tail = __shfl_sync(kFull, m_tail, src);
         b_ss = __shfl_sync(kFull, m_ss, src);
         b_cb = __shfl_sync(kFull, m_cb, src);
         b_query = __shfl_sync(kFull, m_query, src);
@@ -817,10 +857,11 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
         float sum;
         bool ok;
         uint32_t query, th_key;
+        uint32_t ex = kOrExits;  // (a union's posting: how tile_eval_or left it)
         if constexpr (kUnionOnly) {
           query = b_query; th_key = b_th;
-          ok = tile_eval_or(V, cl0 + (b_cb & 0xFFFFu), (b_cb >> 22) & 63u, (b_cb >> 16) & 63u, (b_cb >> 28) != 0u,
-                            __uint_as_float(b_ne), b_ss, qc >> 16, p, off, threshold_score(th_key), sum);
+          ok = tile_eval_or<kCounters && !kSample, true>(V, cl0 + (b_cb & 0xFFFFu), (b_cb >> 22) & 63u, (b_cb >> 16) & 63u, (b_cb >> 28) != 0u,
+                                                         __uint_as_float(b_ne), __uint_as_float(b_tail), b_ss, qc >> 16, p, off, threshold_score(th_key), sum, ex);
         } else {
           const TileSeg sg{(uint16_t)qc, (uint16_t)(qc >> 16)};
           const TileQ q = V.q[sg.q];
@@ -830,8 +871,9 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
           const bool io = (qq.op_flags & 32u) != 0;
           if (q.op() == kTileOpBool) ok = tile_eval_bool(V, cl, __float_as_uint(q.ne) & 0xFFFFu, sg.clause, p, off, io, sum);
           else if (q.op() == kTileOpAnd) ok = tile_eval_and(V, cl, q.n(), q.n_e(), p, off, io, sum);
-          else ok = tile_eval_or(V, cl, q.n_e(), q.n(), q.prune(), q.ne, q.shared_stripes, sg.clause, p, off, threshold_score(th_key), sum);
+          else ok = tile_eval_or<kCounters && !kSample, false>(V, cl, q.n_e(), q.n(), q.prune(), q.ne, 0.0f, q.shared_stripes, sg.clause, p, off, threshold_score(th_key), sum, ex);
         }
+        if (kCounters && !kSample) { st.or_exit[0] += ex == kOrBound; st.or_exit[1] += ex == kOrOwner; st.or_exit[2] += ex == kOrWalk; st.or_exit[3] += ex == kOrDone; }
         if (ok) {
           ++st.completed;
           const uint32_t key = score_to_key(sum);
@@ -984,7 +1026,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   };
   extern __shared__ __align__(16) unsigned char s_dyn[];
   __shared__ TileCtl C;
-  __shared__ unsigned long long s_stat[8 + kTileStages];
+  __shared__ unsigned long long s_stat[kTileStatWords];
   const TUnit U = TP.units[unit_base + blockIdx.x];
   const TSeg G = TP.segs[U.tseg];
   const TSlot* __restrict__ slots = TP.slots + G.slot_base;
@@ -993,7 +1035,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   // sparse slots: (first pair not staged yet, its doc or 0xFFFFFFFF once the list is exhausted), this CTA's share of the
   // launch's cursor scratch; slot s is always walked by the same thread, so no barrier guards it
   uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
-  if (kCounters && tid < 8 + kTileStages) s_stat[tid] = 0ull;
+  if (kCounters && tid < kTileStatWords) s_stat[tid] = 0ull;
   if (tid < kTileMaxQueries / 32u) C.defer[tid] = 0u;
   const bool cl_staged = G.n_clause_words <= TP.cl_cap;
   const uint16_t* __restrict__ cl0 = cl_staged ? V.cl : TP.clauses + G.clause_base;
@@ -1038,13 +1080,13 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
           if (!(C.defer[qi >> 5] & bit)) continue;
           atomicAnd(&C.defer[qi >> 5], ~bit);
         }
-        tile_route<kSample, kUnionOnly>(P, TP, G, V, C, cl0, qi, th_pre0, th_pre1, st);
+        tile_route<kSample, kUnionOnly>(P, TP, V, C, cl0, qi, th_pre0, th_pre1, st);
       }
       mark(kStB1);
       __syncthreads();
       mark(kStBarrier);
       const bool more_rounds = C.ndefer != 0u;
-      tile_flat<kSample, kUnionOnly>(P, TP, G, V, C, cl0, lo, lane, st);
+      tile_flat<kSample, kCounters, kUnionOnly>(P, TP, G, V, C, cl0, lo, lane, st);
       mark(kStB2);
       if (!more_rounds) break;
       __syncthreads();
@@ -1070,19 +1112,20 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
     mark(kStBarrier);
   }
   if constexpr (kCounters) {
-    // warp-aggregated diagnostics
-    unsigned long long v[7] = {st.pairs, st.skipped, st.flat, st.heavy, st.ess, st.completed, st.pushed};
+    // warp-aggregated diagnostics (s_stat / TileParams::counters: the 7 of TileStats, 8 + the stages, 16 + the union exits)
+    unsigned long long v[7 + kOrExits] = {st.pairs, st.skipped, st.flat, st.heavy, st.ess, st.completed, st.pushed,
+                                          st.or_exit[0], st.or_exit[1], st.or_exit[2], st.or_exit[3]};
 #pragma unroll
-    for (int i = 0; i < 7; ++i) {
+    for (int i = 0; i < 7 + kOrExits; ++i) {
       unsigned long long x = v[i];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(kFull, x, o);
-      if (lane == 0 && x) atomicAdd(&s_stat[i], x);
+      if (lane == 0 && x) atomicAdd(&s_stat[i < 7 ? i : 16 + (i - 7)], x);
     }
     if (lane == 0)
       for (int k = 0; k < kTileStages; ++k) atomicAdd(&s_stat[8 + k], cyc[k]);
     __syncthreads();
-    if (tid < 8 + kTileStages && tid != 7 && s_stat[tid]) atomicAdd(&TP.counters[tid], s_stat[tid]);
+    if (tid < kTileStatWords && tid != 7 && s_stat[tid]) atomicAdd(&TP.counters[tid], s_stat[tid]);
   }
 }
 

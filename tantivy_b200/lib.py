@@ -306,7 +306,7 @@ class Context:
     def stats(self):
         s = Stats()
         _check(LIB.tq_get_stats(self.h, C.byref(s)), self.h)
-        return {name: (list(getattr(s, name)) if name in ("or_windows", "tile_counters", "tile_cycles") else getattr(s, name)) for name, _ in Stats._fields_}
+        return {name: (list(getattr(s, name)) if name in ("or_windows", "tile_counters", "tile_cycles", "tile_b2_exits") else getattr(s, name)) for name, _ in Stats._fields_}
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
         """All arguments are raw device addresses (int), e.g. torch tensors' data_ptr()."""
