@@ -160,7 +160,7 @@ typedef struct {
    * ones), [3] cold windows (essential clauses only), [5] bytes of packed postings + fieldnorms actually read
    * (SURVEY.md §8d: the roofline figure of a pruned kernel).  Only k_or_strip counts here; the other slots stay 0. */
   uint64_t or_windows[8];
-  uint64_t units_or_strip; /* of units_or: CTAs of the barrier-free strip kernel (k_or_strip); the rest ran k_or_pipe (<= 8 clauses) or k_or */
+  uint64_t units_or_strip; /* of units_or: CTAs of the barrier-free strip kernel (k_or_strip); the rest ran k_or */
   /* shared-decode tile engine (k_score_lists + k_tile, csrc/tq_tile.cuh) */
   float score_ms, tile_ms, theta_ms;  /* device time of k_score_lists / all k_tile launches / the k_theta passes of the batch */
   float phrase_ms;                    /* device time of k_phrase */

@@ -195,7 +195,7 @@ static TileKernel tile_kernel(bool sample, bool counters, bool union_only) {
 
 // Unit classes of the per-query kernels: the order of tq_batch::n_units / unit_base and of the batch's Unit array.
 enum UnitClass : int {
-  UC_TERM = TQ_OP_TERM, UC_AND = TQ_OP_AND, UC_OR_WINDOW = TQ_OP_OR,  // k_term, k_and, k_or / k_or_pipe
+  UC_TERM = TQ_OP_TERM, UC_AND = TQ_OP_AND, UC_OR_WINDOW = TQ_OP_OR,  // k_term, k_and, k_or
   UC_STRIP, UC_STRIP_ROUND1, UC_STRIP_ROUND2, UC_STRIP_ROUND3,        // k_or_strip: main launch (last phase), threshold rounds (phases 0..2)
   UC_PHRASE, UC_CLASSES                                               // k_phrase
 };
@@ -275,7 +275,6 @@ struct tq_batch {
   uint32_t phrase_ct = 2;                 // most terms of a phrase in the batch (k_phrase's candidate stride)
   const PhraseAux* phrase_aux = nullptr;  // device: per clause of the batch's phrase queries (parallel to qlists)
   uint32_t strip_cached_max = 0;
-  uint32_t or_max_lists = 0;  // most clauses of any window-kernel union in the batch
   size_t qinit_off = 0;
   int next_phase = 0;  // of the current run (0: none started)
   size_t qstate_off = 0, cands_off = 0, res_off = 0, res_bytes = 0, n_cands = 0;
@@ -357,7 +356,6 @@ int tq_ctx_create(int device, tq_ctx** out) {
   if (err == cudaSuccess) err = cudaMemset(c->d_counters, 0, kCounterWords * sizeof(unsigned long long));
   if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&c->build_stream, cudaStreamNonBlocking);
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kOrDynSmem);
-  if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_pipe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pipe_smem_bytes());
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)strip_smem_bytes(kMaxCached));
   // k_tile's occupancy is bound by shared memory: ask for the largest carveout so that the SM's full 228 KB is there to share
   for (auto kern : kTileKernels) {
@@ -903,8 +901,8 @@ struct BatchPlan {
   std::vector<SegWork> work;    // parallel to qsegs
   std::vector<PhraseAux> qaux;  // parallel to qlists once a phrase query shows up
   std::vector<Unit> units[UC_CLASSES];
-  uint32_t n_qsegs_op[4] = {0, 0, 0, 0};  // (query, segment) pairs of k_term, k_and + k_phrase, the window kernels, k_or_strip
-  uint32_t strip_cached_max = 0, or_max_lists = 0, phrase_ct = 2;
+  uint32_t n_qsegs_op[4] = {0, 0, 0, 0};  // (query, segment) pairs of k_term, k_and + k_phrase, k_or, k_or_strip
+  uint32_t strip_cached_max = 0, phrase_ct = 2;
   // tile engine
   std::vector<TileGroupBuild> tgroups;
   std::vector<GroupStage> gstage;  // parallel to tgroups
@@ -1258,7 +1256,6 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
         cls = UC_STRIP;
       }
     }
-    if (cls == UC_OR_WINDOW) pl.or_max_lists = std::max<uint32_t>(pl.or_max_lists, (uint32_t)here.size());
     for (auto& h : here) pl.qlists.push_back(h.second);
     qs.n_lists = (uint32_t)here.size();
     const uint32_t lead_total = here[0].first / 128u + ((here[0].first % 128u) ? 1u : 0u);
@@ -1523,7 +1520,6 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
   b->qinit_off = o_qinit;
   b->phrase_aux = st.on_device<const PhraseAux>(o_qaux);
   b->strip_cached_max = pl.strip_cached_max;
-  b->or_max_lists = pl.or_max_lists;
   b->phrase_ct = std::min<uint32_t>(pl.phrase_ct, kPhraseMaxTerms);
   for (size_t gi = 0; gi < pl.gstage.size(); ++gi) {
     const GroupStage& gs = pl.gstage[gi];
@@ -1757,12 +1753,8 @@ static int run_phase(tq_batch* b, int phase) {
     }
     if (b->n_units[UC_OR_WINDOW]) {
       const int sp = span_begin(b, SPAN_OR);
-      // window unions: the TMA/mbarrier pipeline when every union has few enough clauses for its tables, else the plain kernel
-      if (b->or_max_lists <= kPipeMaxLists)
-        k_or_pipe<<<b->n_units[UC_OR_WINDOW], kPipeThreads, pipe_smem_bytes(), b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);
-      else
-        k_or<<<b->n_units[UC_OR_WINDOW], kThreads, kOrDynSmem, b->stream>>>(P, b->unit_base[UC_OR_WINDOW]);
-      ++launches;
+      // window unions: every union the strip kernel does not take
+      k_or<<<b->n_units[UC_OR_WINDOW], kThreads, kOrDynSmem, b->stream>>>(P, b->unit_base[UC_OR_WINDOW]); ++launches;
       span_end(b, sp);
     }
     if (tiles) {  // K1 + K2 once for every distinct list of the batch

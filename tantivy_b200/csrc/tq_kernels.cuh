@@ -613,12 +613,8 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
 //    16-byte block records gives position and record, the packed vectors follow (2 dependent loads);
 //  * thinner clauses keep their current block DECODED AND SCORED in shared memory (docs + scores); a window only
 //    looks at it when the block's next unread doc falls inside the window, so a block is decoded once per strip.
-// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or_pipe, or
-// k_or for more than kPipeMaxLists clauses.
-#ifndef TQ_KWIN
-#define TQ_KWIN 1024
-#endif
-constexpr uint32_t kWin = TQ_KWIN;  // docs per window (multiple of 512)
+// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or.
+constexpr uint32_t kWin = 1024;  // docs per window (multiple of 512)
 constexpr uint32_t kWBuf = 256;
 constexpr uint32_t kMaxCached = 6;
 constexpr uint32_t kStripWarps = 4;
@@ -1042,268 +1038,6 @@ __global__ void __launch_bounds__(kStripThreads) k_or_strip(const BatchParams P,
       c.pad = 0;
       P.cands[Q.cand_base + base + i] = c;
     }
-  }
-}
-
-// ---- union, pipelined form: TMA bulk copies + mbarrier ring ------------------------------------------------------
-// ncu showed k_or latency bound (about one block per warp in flight, IPC ~1 per SM).  Here a PRODUCER warp walks the
-// block tables of all clauses, one doc-id window after the other, and streams every packed block the window needs
-// into a shared-memory ring with cp.async.bulk (TMA), many blocks and several windows ahead of the 8 CONSUMER warps,
-// which only ever touch shared memory: wait on the slot's mbarrier, pull their vectors, decode, score, add in clause
-// order (named barrier among the consumers between clauses), harvest.  Bytes in flight per SM go from a few hundred
-// to tens of KB.  The window's fieldnorm bytes arrive the same way.
-constexpr uint32_t kPipeSlots = 24;         // ring slots of 1 KB (a block is at most 63 vectors = 1008 B)
-constexpr uint32_t kPipeSlotBytes = 1024 + 16;
-constexpr uint32_t kPipeThreads = kThreads + 32;  // 8 consumer warps + 1 producer warp
-constexpr uint32_t kPipeMaxLists = 8;
-constexpr uint32_t kPipeBatch = 16;          // blocks decoded in parallel before the ordered add (<= kPipeSlots - 8)
-
-struct PipeWindow {  // written by the producer, read by the consumers
-  uint32_t lo, hi, any, pad;
-  uint32_t first[kPipeMaxLists];  // ring item number of the clause's first block in this window
-  uint32_t cnt[kPipeMaxLists];    // how many blocks of the clause overlap the window
-};
-struct PipeShared {
-  unsigned long long full[kPipeSlots], empty[kPipeSlots];
-  unsigned long long win_full[2], win_empty[2];
-  uint2 desc[kPipeSlots];  // .x meta (0xFFFFFFFF: VInt tail, no bytes), .y last doc of the previous block, low bit of block index in... see below
-  uint32_t blk[kPipeSlots]; // block ordinal (needed for the tail pseudo block)
-  PipeWindow win[2];
-  uint32_t npass;           // consumers: pass count of the harvest
-};
-__host__ __device__ constexpr size_t pipe_smem_bytes() {
-  return kTileDocs * sizeof(float) + 2 * kTileDocs + kPipeSlots * kPipeSlotBytes;
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  return ok != 0;
-}
-// A wait that can never hang the device: a protocol error traps after ~2^26 polls instead of spinning for ever.
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 22)) __trap();
-  }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void pipe_consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-__global__ void __launch_bounds__(kPipeThreads, 2) k_or_pipe(const BatchParams P, uint32_t unit_base) {
-  extern __shared__ __align__(16) unsigned char s_raw[];
-  float* s_acc = reinterpret_cast<float*>(s_raw);                                  // [kTileDocs]
-  uint8_t* s_fn = s_raw + kTileDocs * sizeof(float);                               // [2][kTileDocs]
-  unsigned char* s_ring = s_fn + 2 * kTileDocs;                                    // [kPipeSlots][kPipeSlotBytes]
-  __shared__ CtaTopK s_top;
-  __shared__ PipeShared ps;
-  __shared__ ListDesc s_list[kPipeMaxLists];
-  __shared__ QList s_ql[kPipeMaxLists];
-  const Unit U = P.units[unit_base + blockIdx.x];
-  const QSeg S = P.qsegs[U.qseg];
-  const DQuery Q = P.queries[S.query];
-  QState* qs = P.qstate + S.query;
-  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const bool staged_fn = (S.flags & 1u) && S.fieldnorm != nullptr;
-  const float neg_zero = __uint_as_float(0x80000000u);
-  if (threadIdx.x < S.n_lists) {
-    s_ql[threadIdx.x] = P.qlists[S.lists_base + threadIdx.x];
-    s_list[threadIdx.x] = P.lists[s_ql[threadIdx.x].list_id];
-  }
-  if (threadIdx.x == 0) {
-    for (uint32_t i = 0; i < kPipeSlots; ++i) { mbar_init(&ps.full[i], 1); mbar_init(&ps.empty[i], 1); }
-    for (uint32_t i = 0; i < 2; ++i) { mbar_init(&ps.win_full[i], 1); mbar_init(&ps.win_empty[i], kWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    s_top.count = 0; s_top.theta = (unsigned long long)qs->theta << 32;
-    ps.npass = 0;
-  }
-  for (uint32_t i = threadIdx.x; i < kTileDocs; i += kPipeThreads) s_acc[i] = neg_zero;
-  __syncthreads();
-  const uint32_t n_windows = U.end - U.begin;
-
-  if (warp == kWarps) {
-    // =========================== producer ======================================================================
-    __shared__ uint32_t p_cur[kPipeMaxLists], p_cnt[kPipeMaxLists];  // per clause: first block of the window, block count
-    if (lane < kPipeMaxLists) p_cur[lane] = 0;
-    __syncwarp();
-    uint32_t n_item = 0;  // ring item counter
-    for (uint32_t wi = 0; wi < n_windows; ++wi) {
-      const uint32_t tile = U.begin + wi;
-      const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
-      const uint32_t buf = wi & 1u;
-      if (wi >= 2) mbar_wait(&ps.win_empty[buf], ((wi >> 1) - 1u) & 1u);  // the consumers are done with this buffer's previous window
-      // where every clause stands in this window
-      uint32_t total = 0;
-      for (uint32_t t = 0; t < S.n_lists; ++t) {
-        const ListDesc& L = s_list[t];
-        uint32_t first;
-        const uint32_t cnt = window_blocks(L.last_doc, L.n_total, p_cur[t], lo, hi, lane, first);
-        __syncwarp();
-        if (lane == 0) { p_cur[t] = first; p_cnt[t] = cnt; }
-        total += cnt;
-      }
-      __syncwarp();
-      if (lane == 0) {
-        PipeWindow& w = ps.win[buf];
-        w.lo = lo; w.hi = hi; w.any = total;
-        uint32_t n = n_item;
-        for (uint32_t t = 0; t < kPipeMaxLists; ++t) {
-          const uint32_t c = t < S.n_lists ? p_cnt[t] : 0u;
-          w.first[t] = n; w.cnt[t] = c; n += c;
-        }
-        if (staged_fn && total) {
-          mbar_arrive_expect_tx(&ps.win_full[buf], kTileDocs);
-          bulk_g2s(s_fn + buf * kTileDocs, S.fieldnorm + lo, kTileDocs, &ps.win_full[buf]);
-        } else {
-          mbar_arrive(&ps.win_full[buf]);
-        }
-      }
-      __syncwarp();
-      for (uint32_t t = 0; t < S.n_lists; ++t) {
-        const ListDesc& L = s_list[t];
-        const uint32_t cnt = p_cnt[t], blo = p_cur[t];
-        // 16 blocks per step, one lane per block.  A slot frees up only when the consumers have added a whole BATCH,
-        // and that batch may contain blocks of this very step, so a lane must never make another lane wait: every
-        // lane polls its slot once per turn and issues the moment it is free.
-        for (uint32_t base = 0; base < cnt; base += 16) {
-          const uint32_t i = base + lane;
-          bool pending = lane < 16 && i < cnt;
-          const uint32_t b = blo + i;
-          const uint32_t n = n_item + i;
-          const uint32_t slot = n % kPipeSlots, round = n / kPipeSlots;
-          uint32_t turns = 0;
-          while (__ballot_sync(kFull, pending)) {
-            if (pending && mbar_try_wait(&ps.empty[slot], (round & 1u) ^ 1u)) {  // free (true at once in the first round)
-              pending = false;
-              ps.blk[slot] = b;
-              if (b >= L.n_blocks) {  // VInt tail: already decoded in global memory, nothing to copy
-                ps.desc[slot] = make_uint2(0xFFFFFFFFu, 0u);
-                mbar_arrive(&ps.full[slot]);
-              } else {
-                const uint4 rec = __ldg(L.tab4 + b);
-                ps.desc[slot] = make_uint2(rec.z, rec.w == 0xFFFFFFFFu ? 0u : rec.w);
-                const uint32_t bytes = 16u * ((rec.z & 31u) + (L.has_freq ? ((rec.z >> 8) & 63u) : 0u));
-                if (bytes) {
-                  mbar_arrive_expect_tx(&ps.full[slot], bytes);
-                  bulk_g2s(s_ring + slot * kPipeSlotBytes, L.blocks + rec.y, bytes, &ps.full[slot]);
-                } else {
-                  mbar_arrive(&ps.full[slot]);
-                }
-              }
-            }
-            if (++turns > (1u << 24)) __trap();  // protocol error: fail loudly instead of hanging the device
-          }
-        }
-        n_item += cnt;
-      }
-    }
-  } else {
-    // =========================== consumers =====================================================================
-    const TopK T{s_top.keys, &s_top.count, &s_top.theta, &s_top.scratch, 1u, (unsigned)kThreads};
-    unsigned int theta_g_seen = 0;
-    for (uint32_t wi = 0; wi < n_windows; ++wi) {
-      const uint32_t buf = wi & 1u;
-      mbar_wait(&ps.win_full[buf], (wi >> 1) & 1u);
-      const PipeWindow& w = ps.win[buf];
-      const uint32_t lo = w.lo, hi = w.hi;
-      const bool any = w.any != 0;
-      if (threadIdx.x == 0) {
-        const unsigned long long g = (unsigned long long)theta_g_seen << 32;
-        if (g > s_top.theta) s_top.theta = g;
-        theta_g_seen = *(volatile unsigned int*)&qs->theta;
-      }
-      if (any) {
-        const uint8_t* fn_tile = s_fn + buf * kTileDocs;
-        // The window's blocks are taken in batches of kPipeBatch (clause order).  Phase 1, no ordering needed: the
-        // warps decode and SCORE the batch's blocks in parallel and park (slot, score) pairs in the block's own ring
-        // slot.  Phase 2, ordered: clause by clause the pairs are added to the score slots (a few instructions per
-        // posting), with a consumer barrier between clauses.  Only the cheap phase is serialised by the clause order.
-        const uint32_t n0 = w.first[0];
-        const uint32_t total = w.any;
-        for (uint32_t done = 0; done < total; done += kPipeBatch) {
-          const uint32_t nb = min(total - done, kPipeBatch);
-          for (uint32_t j = done + warp; j < done + nb; j += kWarps) {
-            uint32_t t = 0;
-            while (t + 1 < S.n_lists && j >= w.first[t + 1] - n0) ++t;  // clause of item j (first[] is non-decreasing)
-            const ListDesc& L = s_list[t];
-            const Scorer scr = make_scorer(P, s_ql[t]);
-            const uint32_t n = n0 + j;
-            const uint32_t slot = n % kPipeSlots, round = n / kPipeSlots;
-            mbar_wait(&ps.full[slot], round & 1u);
-            const uint2 d = ps.desc[slot];
-            const uint32_t b = ps.blk[slot];
-            unsigned char* sbase = s_ring + slot * kPipeSlotBytes;
-            BlockFetch f;
-            f.meta = d.x; f.prev = d.y;
-            if (d.x != 0xFFFFFFFFu) {
-              const uint32_t db = d.x & 31u, tb = (d.x >> 8) & 63u;
-              const uint4* v = reinterpret_cast<const uint4*>(sbase);
-              const uint32_t wd = (lane * db) >> 5;
-              f.dlo = v[wd]; f.dhi = v[wd + 1];
-              if (L.has_freq) { const uint32_t wt = db + ((lane * tb) >> 5); f.tlo = v[wt]; f.thi = v[wt + 1]; }
-            }
-            uint32_t doc[4], tf[4];
-            fetch_decode(L, b, f, lane, doc, tf);
-            __syncwarp();  // every lane has its vectors: the slot's bytes can be overwritten by the pairs
-            uint16_t* pslot = reinterpret_cast<uint16_t*>(sbase);
-            float* pscore = reinterpret_cast<float*>(sbase + 256);
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              uint16_t s16 = 0xFFFFu;
-              float sc = 0.0f;
-              if (doc[k4] >= lo && doc[k4] < hi) {
-                const uint32_t slot_d = doc[k4] - lo;
-                const uint32_t id = staged_fn ? (uint32_t)fn_tile[slot_d] : (L.fieldnorm ? (uint32_t)__ldg(L.fieldnorm + doc[k4]) : 1u);
-                sc = bm25_score_id(scr, id, tf[k4]);
-                s16 = (uint16_t)slot_d;
-              }
-              pslot[lane * 4 + k4] = s16;
-              pscore[lane * 4 + k4] = sc;
-            }
-          }
-          pipe_consumer_sync();  // all pairs of the batch are parked
-          for (uint32_t t = 0; t < S.n_lists; ++t) {
-            if (w.cnt[t] == 0) continue;
-            const uint32_t c_lo = w.first[t] - n0, c_hi = c_lo + w.cnt[t];
-            const uint32_t j_lo = max(c_lo, done), j_hi = min(c_hi, done + nb);
-            if (j_lo >= j_hi) continue;  // clause not in this batch (uniform across the consumers)
-            for (uint32_t j = j_lo + ((warp + kWarps - (j_lo & (kWarps - 1))) & (kWarps - 1)); j < j_hi; j += kWarps) {
-              // j % kWarps == warp: the warp that parked the pairs also adds them and then frees the slot
-              const uint32_t n = n0 + j;
-              const uint32_t slot = n % kPipeSlots;
-              const unsigned char* sbase = s_ring + slot * kPipeSlotBytes;
-              const ushort4 s4 = reinterpret_cast<const ushort4*>(sbase)[lane];
-              const float4 v4 = reinterpret_cast<const float4*>(sbase + 256)[lane];
-              if (s4.x != 0xFFFFu) s_acc[s4.x] = __fadd_rn(s_acc[s4.x], v4.x);
-              if (s4.y != 0xFFFFu) s_acc[s4.y] = __fadd_rn(s_acc[s4.y], v4.y);
-              if (s4.z != 0xFFFFu) s_acc[s4.z] = __fadd_rn(s_acc[s4.z], v4.z);
-              if (s4.w != 0xFFFFu) s_acc[s4.w] = __fadd_rn(s_acc[s4.w], v4.w);
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&ps.empty[slot]);
-            }
-            pipe_consumer_sync();  // clause order is the f32 summation order
-          }
-        }
-        or_harvest(T, s_acc, S, lo, Q.k, &qs->theta, &ps.npass, lane);
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ps.win_empty[buf]);  // this warp no longer reads the window's table or fieldnorms
-    }
-    topk_flush(T, Q, qs, P.cands, S.segment_ord);
   }
 }
 

@@ -33,7 +33,7 @@ def _ctx_with_env(**env):
 
 
 # every test runs on both union engines: "tile" = the shared-decode tile engine (k_score_lists + k_tile, the default),
-# "legacy" = the per-query kernels (k_or_strip / k_or_pipe / k_or) that the tile engine falls back to
+# "legacy" = the per-query kernels (k_or_strip / k_or) that the tile engine falls back to
 @pytest.fixture(scope="module", params=["tile", "legacy"])
 def ctx(request):
     # (TQ_TILE_TERMS=1: single-term batches stay on the tile engine here; the default rule has a test of its own)
@@ -376,7 +376,7 @@ def test_synth_mixed_batch(ctx, synth):
         # unions above are strip unions
         w = st["or_windows"]
         assert w[1] + w[2] + w[3] > 0 and w[5] > 0 and [w[i] for i in (0, 4, 6, 7)] == [0, 0, 0, 0]
-        # with k > 128 the unions take k_or_pipe; neither it nor the compactions of the term and AND CTAs count there
+        # with k > 128 the unions take k_or; neither it nor the compactions of the term and AND CTAs count there
         queries = [ix.query(TQ_OP_TERM, [0], 10, segment_base=base), ix.query(TQ_OP_AND, [0, 1], 10, segment_base=base),
                    ix.query(TQ_OP_OR, [0, 1], 256, segment_base=base), ix.query(TQ_OP_OR, [0, 1, 2, 3, 4, 5], 1000, segment_base=base)]
         qb = QueryBatch(queries)
