@@ -126,7 +126,9 @@ typedef struct {
   uint32_t flags;
   float threshold;
   /* TQ_OP_PHRASE only (NULL / 0 otherwise): term_pos[i] belongs to term_segs[i]; term_offset[t] = position of clause t
-   * inside the phrase (PhraseQuery::new_with_offset, phrase_query.rs); weight[0] / avg_fieldnorm[0] (or the first
+   * inside the phrase (PhraseQuery::new_with_offset, phrase_query.rs).  The clauses may come in any order: like PhraseQuery,
+   * the library orders them by offset (stable: clauses with equal offsets keep their order), which decides the phrase
+   * count of a sloppy two-term phrase whose terms have equal doc_freq in a segment.  weight[0] / avg_fieldnorm[0] (or the first
    * tf_cache table) describe the phrase's single Bm25Weight, the other entries are ignored; slop (PhraseQuery::set_slop) may be non-zero
    * for two-term phrases. */
   const tq_term_pos* term_pos;

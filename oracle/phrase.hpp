@@ -146,8 +146,11 @@ struct PhraseScorer {
   FieldNormReader fieldnorm_reader;
   Bm25Weight similarity_weight;
 
-  // term_postings: (offset in the phrase, term); PhraseScorer::new_with_offset
+  // term_postings: (offset in the phrase, term) in any order; PhraseScorer::new_with_offset.  PhraseQuery first puts its terms
+  // in offset order (phrase_query.rs:48-53, stable), so the size_hint sort below breaks ties by offset: which term is `left`
+  // of a sloppy two-term count depends on it
   void init(std::vector<std::pair<uint32_t, PhraseTerm>> term_postings) {
+    std::stable_sort(term_postings.begin(), term_postings.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
     uint32_t max_offset = 0;
     for (auto& tp : term_postings) max_offset = std::max(max_offset, tp.first);
     for (auto& tp : term_postings) { tp.second.offset = max_offset - tp.first; terms.push_back(std::move(tp.second)); }

@@ -1162,10 +1162,13 @@ int plan_segments(tq_ctx* c, BatchPlan& pl, const tq_query& q, int op, const uin
     auto by_doc_freq = [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.first < b.first; };
     if (is_phrase) {
       // PhraseScorer keeps its terms by ascending size_hint (intersection.rs:40-52); every clause carries
-      // (max_offset - its offset), the shift that lines the terms' positions up (phrase_scorer.rs:349-398)
+      // (max_offset - its offset), the shift that lines the terms' positions up (phrase_scorer.rs:349-398).
+      // PhraseQuery has put the terms in offset order first (phrase_query.rs:48-53), so equal doc_freqs keep that order:
+      // it decides which term is `left` of a sloppy two-term count (phrase_count_slop2)
       uint32_t max_offset = 0;
       for (uint32_t t = 0; t < q.n_terms; ++t) max_offset = std::max(max_offset, q.term_offset[t]);
       for (size_t a = 0; a < sp.here.size(); ++a) sp.here[a].range_len = max_offset - q.term_offset[sp.term_idx[a]];  // (range_len is free here)
+      std::stable_sort(sp.here.begin(), sp.here.end(), [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.range_len > b.range_len; });
       std::stable_sort(sp.here.begin(), sp.here.end(), by_doc_freq);
     }
     if (op == TQ_OP_AND)  // leader = rarest, then ascending doc_freq; stable (block_wand_intersection.rs:27)

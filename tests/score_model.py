@@ -1,6 +1,7 @@
 """A plain numpy model of the reference's BM25 scorers and collectors, independent of `oracle/` and of the product library.
 
-Inputs are the raw posting lists, doc lengths, alive bits and the query dict of `tantivy_b200._abi.QueryBatch`.  The query's
+Inputs are the raw posting lists, doc lengths, alive bits, the terms' positions (phrase queries) and the query dict of
+`tantivy_b200._abi.QueryBatch`.  The query's
 Bm25Weight.weight and average fieldnorm (or explicit tf cache) are taken as given; everything else is computed in np.float32 with
 the reference's operation order (paths relative to the reference tree, quickwit-oss/tantivy @ 70f0b03).  numpy's f32 + - * / round
 to nearest like the reference's f32 code, so the model is bit-exact where the order is.  Every score is computed again in float64
@@ -8,8 +9,8 @@ and checked against a rounding bound: a formula slip that the oracle and the mod
 """
 import numpy as np
 
-from tantivy_b200._abi import (TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT, TQ_OCCUR_SHOULD, TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_TERM,
-                               TQ_TERM_IGNORE_FREQ)
+from tantivy_b200._abi import (TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT, TQ_OCCUR_SHOULD, TQ_OP_AND, TQ_OP_BOOL, TQ_OP_OR, TQ_OP_PHRASE,
+                               TQ_OP_TERM, TQ_TERM_IGNORE_FREQ)
 from tests.helpers import _FN_TABLE, fieldnorm_ids
 
 f32, f64 = np.float32, np.float64
@@ -20,15 +21,17 @@ EPS = 2.0 ** -23
 class Segment:
     """One segment of one field: posting lists [(docs, tfs or None)], per-doc token counts (None: a field without
     fieldnorms, constant fieldnorm 1, term_weight.rs:218), alive bits (np.packbits little-endian, None: no deletes),
-    basic=True for a field indexed without freqs (IndexRecordOption::Basic)."""
+    basic=True for a field indexed without freqs (IndexRecordOption::Basic), positions (phrase queries) = for every list index
+    {doc: ascending positions of the term in the doc}."""
 
-    def __init__(self, segment_ord, lists, lengths, alive=None, basic=False, max_doc=None):
+    def __init__(self, segment_ord, lists, lengths, alive=None, basic=False, max_doc=None, positions=None):
         self.segment_ord = segment_ord
         self.lists = [(np.asarray(d, np.uint32), None if t is None else np.asarray(t, np.uint32)) for d, t in lists]
         self.max_doc = len(lengths) if lengths is not None else max_doc
         self.fn_ids = fieldnorm_ids(lengths) if lengths is not None else np.ones(self.max_doc, np.uint8)
         self.alive = None if alive is None else np.unpackbits(np.asarray(alive, np.uint8), bitorder="little")[:self.max_doc].astype(bool)
         self.basic = basic
+        self.positions = positions
 
 
 def tf_cache(avg, dtype=f32):
@@ -121,6 +124,8 @@ def _intersect(parts, max_doc, intersection_order):
 def _segment_matches(seg, q, terms, intersection_order=None):
     """complex_scorer / the specialised scorers for one segment: a _Dense of the matching docs (before deletes), or None."""
     op = q["op"]
+    if op == TQ_OP_PHRASE:
+        return _phrase_matches(seg, q, terms)
     present = {ts[0] for ts in q["term_segs"] if ts[1] == seg.segment_ord and ts[3] > 0}
     n = len(q["weights"])
     scorer = {c: _Term(seg, q, c, terms[c]) for c in range(n) if c in present}
@@ -174,6 +179,70 @@ def _segment_matches(seg, q, terms, intersection_order=None):
     for t in must_not:  # Exclude (exclude.rs)
         ok[t.docs] = False
     out.has = ok
+    return out
+
+
+def slop_matches(left, right, slop):
+    """intersection_count_with_slop as documented (phrase_scorer.rs:138-186): walking both ascending lists, a left position within
+    `slop` of the right one is a match -- unless a later left position is still not beyond the right one, which is the better
+    match -- and then both sides move on; otherwise the side with the smaller position moves on.  Not symmetric: a right
+    position may precede its left one by up to `slop`.  Returns the matched right positions (their count is the phrase count)."""
+    out, i, j = [], 0, 0
+    while i < len(left) and j < len(right):
+        if abs(int(left[i]) - int(right[j])) <= slop:
+            while i + 1 < len(left) and left[i + 1] <= right[j]:
+                i += 1
+            out.append(right[j])
+            i, j = i + 1, j + 1
+        elif left[i] < right[j]:
+            i += 1
+        else:
+            j += 1
+    return out
+
+
+def _phrase_matches(seg, q, terms):
+    """PhraseWeight::scorer over one segment (phrase_query.rs:48-53, phrase_weight.rs, phrase_scorer.rs:349-589): the clauses in
+    offset order (stable), each clause's positions shifted by max_offset - its offset; docs that hold every clause; phrase count =
+    size of the intersection of the shifted sets, or with slop (two terms) slop_matches(left, right) where left is the first clause
+    after a stable sort by this segment's doc_freq (the Intersection's order, intersection.rs:89).  Score = weight[0] *
+    tf_factor(fieldnorm_id, count) with row 0 of tf_cache (or avg_fieldnorm[0]): ONE Bm25Weight for the whole phrase."""
+    n = len(q["weights"])
+    present = {ts[0] for ts in q["term_segs"] if ts[1] == seg.segment_ord and ts[3] > 0}
+    if len(present) < n:  # a clause without postings here: no match
+        return None
+    offsets = [int(o) for o in q["term_offset"]]
+    order = sorted(range(n), key=lambda c: offsets[c])
+    max_off = max(offsets)
+    slop = int(q.get("slop", 0))
+    if slop:
+        assert n == 2, "sloppy phrases of three and more terms are not modelled"
+        order = sorted(order, key=lambda c: len(seg.lists[terms[c]][0]))
+    docs = seg.lists[terms[order[0]]][0]
+    for c in order[1:]:
+        docs = np.intersect1d(docs, seg.lists[terms[c]][0])
+    cnt = np.zeros(seg.max_doc, np.int64)
+    for d in docs.tolist():
+        shifted = [[p + max_off - offsets[c] for p in seg.positions[terms[c]][d]] for c in order]
+        if slop:
+            cnt[d] = len(slop_matches(shifted[0], shifted[1], slop))
+        else:
+            cnt[d] = len(set.intersection(*[set(s) for s in shifted]))
+    out = _Dense(seg.max_doc)
+    out.has = cnt > 0
+    cache = q.get("tf_cache")
+    if cache is not None:
+        c32 = np.asarray(cache, f32).reshape(-1, 256)[0]
+        c64 = c32.astype(f64)
+    else:
+        c32, c64 = tf_cache(q["avg_fieldnorm"][0]), tf_cache(q["avg_fieldnorm"][0], f64)
+    w = f32(q["weights"][0])
+    t32, t64 = cnt.astype(f32), cnt.astype(f64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        out.s32 = np.where(out.has, w * (t32 / (t32 + c32[seg.fn_ids])), f32(0))
+        out.s64 = np.where(out.has, f64(w) * (t64 / (t64 + c64[seg.fn_ids])), 0.0)
+    out.mag = np.abs(out.s64)
+    out.n = out.has.astype(np.int32)
     return out
 
 

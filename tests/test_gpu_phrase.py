@@ -9,6 +9,7 @@ pytestmark = pytest.mark.gpu
 import tantivy_b200 as T  # noqa: E402
 from oracle import tq_oracle as O  # noqa: E402
 from tantivy_b200._abi import TQ_OP_PHRASE, TQ_RECORD_FREQS_POSITIONS, QueryBatch  # noqa: E402
+from tests import score_model as M  # noqa: E402
 from tests.helpers import OracleSegment, f32, hits  # noqa: E402
 from tests.test_phrase_goldens import build  # noqa: E402
 
@@ -24,29 +25,55 @@ _next = [7000]
 
 
 class PosSegment:
-    """One segment of `texts`: posting lists with term frequencies, the matching `.pos` bytes, per-term ranges."""
+    """One segment: posting lists with term frequencies, the matching `.pos` bytes, per-term ranges.  Built from `texts`, or
+    with PosSegment.from_positions from explicit positions."""
 
     def __init__(self, texts, writer_cls=T.FieldWriter):
+        postings, lengths = build(texts)
+        self._build({t: {d: ps for d, ps in pl} for t, pl in postings.items()}, np.maximum(np.array(lengths), 1), None, writer_cls)
+
+    @classmethod
+    def from_positions(cls, positions, lengths, alive=None, writer_cls=T.FieldWriter):
+        """positions = {term: {doc: ascending positions}}, lengths = every doc's token count (its fieldnorm), alive = the
+        segment's alive bitset (np.packbits, little-endian) or None."""
+        s = cls.__new__(cls)
+        s._build(positions, np.asarray(lengths), alive, writer_cls)
+        return s
+
+    def _build(self, positions, lengths, alive, writer_cls):
         _next[0] += 1
         self.ord = _next[0]
-        postings, lengths = build(texts)
-        self.vocab = sorted(postings)
+        self.vocab = sorted(positions)
+        self.positions = positions
+        self.alive = alive
         lists, pos, self.pos_range = [], [], {}
         cursor = 0
         for t in self.vocab:
-            pl = postings[t]
-            lists.append((np.array([d for d, _ in pl], dtype=np.uint32), np.array([len(ps) for _, ps in pl], dtype=np.uint32)))
+            docs = sorted(positions[t])
+            lists.append((np.array(docs, dtype=np.uint32), np.array([len(positions[t][d]) for d in docs], dtype=np.uint32)))
             deltas = []
-            for _, ps in pl:
+            for d in docs:
+                ps = positions[t][d]
                 deltas += [ps[0]] + [b - a for a, b in zip(ps, ps[1:])]
             data = bytes(O.positions_serialize(deltas))
             self.pos_range[t] = (cursor, cursor + len(data))
             cursor += len(data)
             pos.append(data)
         self.pos_bytes = np.frombuffer(b"".join(pos), dtype=np.uint8)
-        self.seg = OracleSegment(lists, np.maximum(np.array(lengths), 1), record_option=TQ_RECORD_FREQS_POSITIONS, segment_ord=self.ord, writer_cls=writer_cls)
-        self.n_docs = len(texts)
+        self.lengths = lengths
+        self.seg = OracleSegment(lists, lengths, record_option=TQ_RECORD_FREQS_POSITIONS, segment_ord=self.ord, writer_cls=writer_cls, alive=alive)
+        self.n_docs = len(lengths)
         self.tokens = self.seg.total_num_tokens
+
+    def model(self, vocab):
+        """The same segment for tests/score_model.py, one posting list per term of `vocab` (empty where it is absent)."""
+        lists, pos = [], []
+        for t in vocab:
+            p = self.positions.get(t, {})
+            docs = sorted(p)
+            lists.append((np.array(docs, dtype=np.uint32), np.array([len(p[d]) for d in docs], dtype=np.uint32)))
+            pos.append(p)
+        return M.Segment(self.ord, lists, self.lengths, alive=self.alive, positions=pos)
 
     def register(self, target):
         self.seg.register(target)

@@ -291,3 +291,94 @@ def test_random_boolean_shapes_cover_the_generator():
     assert {b for s in shapes for b in s["boosts"]} == set(BOOL_BOOSTS)
     assert {s["k"] for s in shapes} == set(BOOL_KS)
     assert any(f for s in shapes for f in s["flags"])
+
+
+# ---- phrase queries ------------------------------------------------------------------------------------------------------
+def _phrase_segs(*texts_per_seg):
+    from tests.test_gpu_phrase import PosSegment
+    return [PosSegment(t, writer_cls=O.FieldWriter) for t in texts_per_seg]
+
+
+def _phrase_rows(segs, phrase, k=10, offsets=None, **extra):
+    """(model rows, oracle rows) of one phrase query over `segs`; offsets[c] = the phrase offset of clause c."""
+    from tests.test_gpu_phrase import phrase_query
+    q, _, _, _ = phrase_query(segs, phrase, k, offsets=offsets)
+    q.update(extra)
+    vocab = sorted({t for s in segs for t in s.vocab} | set(phrase))
+    want = M.search([s.model(vocab) for s in segs], q, [vocab.index(t) for t in phrase])
+    ix = O.OracleIndex()
+    for s in segs:
+        s.register(ix)
+    return want, hits(ix.search_batch(QueryBatch([q]), mode=0))
+
+
+def test_phrase_model_reproduces_the_reference_phrase_tests():
+    """phrase_query/mod.rs:41-91,163-169 (as tests/test_phrase_goldens.py states them): doc sets and the two pinned scores."""
+    texts = ["b b b d c g c", "a b b d c g c", "a b a b c", "c a b a d ga a", "a b c"]
+    segs = _phrase_segs(texts)
+    for phrase, docs in ((["a", "b"], [1, 2, 3, 4]), (["a", "b", "c"], [2, 4]), (["b", "b"], [0, 1]), (["g", "a"], [])):
+        want, got = _phrase_rows(segs, phrase)
+        assert sorted(d for _, _, d in want) == docs and got == want, phrase
+    want, got = _phrase_rows(_phrase_segs(["a b b d c g c", "a b a b c"]), ["a", "b"])
+    assert sorted(d for _, _, d in want) == [0, 1] and got == want
+    want, got = _phrase_rows(_phrase_segs(["a b c", "a b c a b"]), ["a", "b"])
+    by_doc = {d: s for s, _, d in want}
+    assert _near(by_doc[0], 0.40618482) and _near(by_doc[1], 0.46844664) and got == want
+
+
+def test_phrase_model_slop_doc_sets():
+    """The doc sets test_two_term_phrases_with_slop asserts on the device."""
+    segs = _phrase_segs(["a b c d", "a c b", "b a", "a x x b", "a x x x b", "b x a x b a", "a a a b b b", "c c", "b"])
+    docs = {}
+    for slop in (1, 2, 3):
+        want, got = _phrase_rows(segs, ["a", "b"], slop=slop)
+        assert got == want, slop
+        docs[slop] = sorted(d for _, _, d in want)
+    assert docs[1] == [0, 1, 5, 6] and docs[2] == [0, 1, 2, 3, 5, 6] and {3, 4} <= set(docs[3])
+
+
+@pytest.mark.parametrize("left,right,slop,expected", [
+    # phrase_scorer.rs test_slop: the matched right positions
+    ([1], [2], 1, [2]), ([1], [3], 1, []), ([1], [3], 2, [3]), ([], [2], 100000, []), ([5, 7, 11], [1, 5, 10, 12], 1, [5, 10]),
+    ([1, 5, 6, 9, 10, 12], [6, 8, 9, 12], 1, [6, 8, 9, 12]), ([1, 5, 6, 9, 10, 12], [6, 8, 9, 12], 10, [6, 8, 9, 12]),
+    ([1, 3, 5], [2, 4, 6], 1, [2, 4, 6]),
+    # test_merge_slop
+    ([1, 2], [1], 1, [1]), ([3], [4], 2, [4]), ([1, 5, 6, 9, 10, 12], [6, 8, 9, 12], 10, [6, 8, 9, 12]),
+])
+def test_phrase_model_slop_matches_the_reference_cases(left, right, slop, expected):
+    assert M.slop_matches(left, right, slop) == expected
+
+
+def test_phrase_clauses_are_taken_in_offset_order():
+    """One doc "a a b b", the phrase a@0 b@1 with slop 1, clauses passed as (b, offset 1), (a, offset 0).  Both terms have doc_freq
+    1, so the offset order decides `left`: shifted a = [1, 2], b = [2, 3]; left = a counts 1 (left = b would count 2).  The oracle
+    agrees with the model in both clause orders."""
+    segs = _phrase_segs(["a a b b"])
+    one, got = _phrase_rows(segs, ["a", "b"], offsets=[0, 1], slop=1)
+    assert got == one
+    swapped, got = _phrase_rows(segs, ["b", "a"], offsets=[1, 0], slop=1)
+    assert swapped == one and got == one
+    assert len(one) == 1 and one == _phrase_rows(segs, ["a", "b"])[0]  # the score of phrase count 1: "a b" without slop
+
+
+def test_random_phrases_match_the_oracle():
+    """Random texts in three segments (one with deletes): phrases of 2 to 8 terms, gaps / repeated / out-of-order offsets, slop,
+    thresholds: model == oracle, and the model is not vacuous."""
+    rng = np.random.default_rng(808)
+    vocab = ["w0", "w1", "w2", "w3", "w4"]
+    p = [0.4, 0.25, 0.15, 0.12, 0.08]
+    texts = [[" ".join(rng.choice(vocab, size=int(rng.integers(2, 40)), p=p)) for _ in range(n)] for n in (300, 500, 200)]
+    segs = _phrase_segs(*texts)
+    alive = np.packbits(rng.random(segs[1].n_docs) > 0.3, bitorder="little")
+    from tests.test_gpu_phrase import PosSegment
+    segs[1] = PosSegment.from_positions(segs[1].positions, segs[1].lengths, alive=alive, writer_cls=O.FieldWriter)
+    n_hits = 0
+    cases = [(["w0", "w1"], None, 0), (["w1", "w0"], [1, 0], 2), (["w0", "w2", "w1"], [0, 2, 5], 0), (["w0", "w1", "w0"], [3, 4, 5], 0),
+             (["w0", "w1", "w1"], [0, 1, 1], 0), (["w0", "w1", "w2"], [2, 0, 1], 0), (["w0", "w0"], [0, 0], 1), (["w0"] * 8, None, 0),
+             (["w0", "w1", "w0", "w0", "w2", "w0"], None, 0), (["w3", "w4"], [1, 0], 1), (["w3", "w4"], [1, 0], 3)]
+    for phrase, offsets, slop in cases:
+        for extra in ({}, {"threshold": 1.0}):
+            want, got = _phrase_rows(segs, phrase, k=50, offsets=offsets, slop=slop, **extra)
+            assert got == want, (phrase, offsets, slop, extra)
+            n_hits += len(want)
+    assert n_hits > 200
