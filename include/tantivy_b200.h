@@ -183,7 +183,8 @@ typedef struct {
                                       union-only k_tile instances (k_tile<*, *, true>); the rest run the general instances */
   uint64_t tile_b2_exits[4];    /* cumulative, with TQ_TILE_COUNTERS=1: union postings of the exact k_tile launches' flat evaluation
                                    (stage B2) by how they ended: [0] dropped by the bound taken before the look-ups, [1] not the owner
-                                   (an earlier essential clause lists the doc), [2] dropped in the non-essential walk, [3] completed */
+                                   (completed the walk, but an earlier essential clause lists the doc), [2] dropped in the
+                                   non-essential walk, [3] completed */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */

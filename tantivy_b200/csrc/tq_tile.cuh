@@ -264,10 +264,10 @@ __device__ __forceinline__ float tile_or_tail(const TileView& V, const uint16_t*
 }
 
 // How tile_eval_or leaves a posting (k_tile<*, true, *> counts each: TileParams::counters[16 + exit], tq_stats.tile_b2_exits):
-// dropped by the bound taken before the look-ups, the doc belongs to an earlier essential clause, dropped in the non-essential
-// walk, complete score.  Only the counters instances record it (tile_eval_or<true, *>): the other instances keep the two-way exit,
-// whose branch structure the exit codes change (as the function's value they cost k_tile 5 % on or5_top100_100M_8seg, H100 80GB
-// HBM3 at 700 W).
+// dropped by the bound taken before the look-ups, complete score but the doc belongs to an earlier essential clause (asked after
+// the walk), dropped in the non-essential walk, complete score.  Only the counters instances record it (tile_eval_or<true, *>):
+// the other instances keep the two-way exit, whose branch structure the exit codes change (as the function's value they cost
+// k_tile 5 % on or5_top100_100M_8seg, H100 80GB HBM3 at 700 W).
 enum TileOrExit : uint32_t { kOrBound, kOrOwner, kOrWalk, kOrDone, kOrExits };
 
 // Union: the doc at tile offset `off`, met as posting p of essential clause c (of n_e; n clauses, ne and shared_stripes as in TileQ).
@@ -280,19 +280,13 @@ __device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* 
                                              float theta_f, float& sum, uint32_t& ex) {
   bool f;
   sum = V.score[p];  // (-0.0 + s == s: SumCombiner starts from 0, score_combiner.rs:39-57)
-  if ((shared_stripes >> (off >> 5)) & 1u) {  // another essential clause lists a doc near this one: look the doc up
-    // ... unless the bound says no: if an earlier clause lists the doc, it is dropped here anyway; if none does, its score is at
+  const bool shared = (shared_stripes >> (off >> 5)) & 1u;
+  if (shared) {  // another essential clause lists a doc near this one: look the doc up
+    // ... unless the bound says no: if an earlier clause lists the doc, it is dropped anyway; if none does, its score is at
     // most sum + tail (the f32 orders of the two sums differ by less than the margin, as in tile_essential)
     if (prune && (sum + (kTail ? tail : tile_or_tail(V, cl, c, n_e, ne))) * 1.00001f < theta_f) {
       if (kExit) ex = kOrBound;
       return false;
-    }
-    for (uint32_t c1 = 0; c1 < c; ++c1) {  // an earlier essential clause lists the doc: it is evaluated there
-      tile_find(V, cl[c1], off, f);
-      if (f) {
-        if (kExit) ex = kOrOwner;
-        return false;
-      }
     }
     for (uint32_t c2 = c + 1u; c2 < n_e; ++c2) {
       const float v = tile_find(V, cl[c2], off, f);
@@ -311,6 +305,17 @@ __device__ __forceinline__ bool tile_eval_or(const TileView& V, const uint16_t* 
     const float v = tile_find(V, slot, off, f);
     if (f) sum = __fadd_rn(sum, v);
   }
+  // the doc is evaluated by the first essential clause that lists it.  Asked last: whether an earlier clause lists the doc does
+  // not change the sum above, and most postings of a shared stripe leave in the walk, so only the few that get here look up the
+  // earlier clauses (outside a shared stripe no other essential clause lists the doc)
+  if (shared)
+    for (uint32_t c1 = 0; c1 < c; ++c1) {
+      tile_find(V, cl[c1], off, f);
+      if (f) {
+        if (kExit) ex = kOrOwner;
+        return false;
+      }
+    }
   if (kExit) ex = kOrDone;
   return true;
 }
