@@ -167,7 +167,7 @@ struct tq_ctx {
   DevBuf build_dev;
   std::vector<tq_batch*> pool;
   tq_stats stats{};
-  uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit;
+  uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit, strip_windows_per_unit;
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 16, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
@@ -323,6 +323,8 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->term_blocks_per_unit = env_u32("TQ_TERM_BLOCKS_PER_UNIT", 512);
   c->and_blocks_per_unit = env_u32("TQ_AND_BLOCKS_PER_UNIT", 128);
   c->or_tiles_per_unit = env_u32("TQ_OR_TILES_PER_UNIT", 16);
+  // test hook: smallest k_or_strip unit, in kWin-doc windows (1 or 7: warps with no window or one, unit and strip edges in small segments)
+  c->strip_windows_per_unit = std::max<uint32_t>(1u, env_u32("TQ_STRIP_WINDOWS_PER_UNIT", kStripWarps * 64u));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -1303,7 +1305,7 @@ int cut_units(const tq_ctx* c, BatchPlan& pl) {
     const SegWork& w = pl.work[s];
     const uint32_t total = w.total;
     const uint32_t min_per = w.cls == UC_TERM ? c->term_blocks_per_unit
-                             : ((w.cls == UC_AND || w.cls == UC_PHRASE) ? c->and_blocks_per_unit : (w.cls == UC_STRIP ? kStripWarps * 64u : c->or_tiles_per_unit));
+                             : ((w.cls == UC_AND || w.cls == UC_PHRASE) ? c->and_blocks_per_unit : (w.cls == UC_STRIP ? c->strip_windows_per_unit : c->or_tiles_per_unit));
     const uint32_t n_same = pl.n_qsegs_op[w.cls == UC_PHRASE ? UC_AND : w.cls];
     const uint32_t want_units = std::max<uint32_t>(1u, (target_units + n_same - 1) / n_same);
     const uint32_t per = std::max<uint32_t>(min_per, (total + want_units - 1) / want_units);

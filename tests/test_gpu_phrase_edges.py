@@ -250,7 +250,9 @@ def _battery_is_not_vacuous(b):
     assert sum(len(w) for w in b.want) > 5000
 
 
-ROUTES = {"side_stream": {}, "one_stream": dict(TQ_PHRASE_SIDE_STREAM=0), "no_tile": dict(TQ_TILE=0), "repeated": dict(TQ_TILE_PCAP=64)}
+ROUTES = {"side_stream": {}, "one_stream": dict(TQ_PHRASE_SIDE_STREAM=0), "no_tile": dict(TQ_TILE=0), "repeated": dict(TQ_TILE_PCAP=64),
+          # k_phrase cut into one unit per leader block, and one unit per (query, segment) pair (the unit size of a full batch)
+          "small_units": dict(TQ_TILE=0, TQ_AND_BLOCKS_PER_UNIT=1, TQ_TARGET_UNITS=1 << 24), "one_unit": dict(TQ_TARGET_UNITS=1)}
 
 
 @pytest.mark.parametrize("route", list(ROUTES))
@@ -263,7 +265,7 @@ def test_phrase_battery_on_every_route(battery, route):
         assert st["units_phrase"] > 0
         if route in ("side_stream", "one_stream"):
             assert st["tile_groups"] >= 1 and st["tile_fallbacks"] == 0
-        if route == "no_tile":
+        if route in ("no_tile", "small_units"):
             assert st["tile_groups"] == 0
         if route == "repeated":
             assert st["tile_fallbacks"] == 1
