@@ -12,7 +12,10 @@
  * (rayon threads call collect_segment concurrently, src/core/executor.rs:60-100).
  *
  * Doc ids are bit-exact w.r.t. the reference CPU path; scores are f32 computed with the
- * reference's operation order (src/query/bm25.rs:158-175).
+ * reference's operation order (src/query/bm25.rs:158-175).  A zero score comes back as +0.0, also
+ * where the reference's is -0.0 (a weight of -0.0, or a negative one whose product underflows):
+ * the reference compares scores with partial_cmp, which ties the two zeros and orders them by
+ * DocAddress (sort_by_score.rs:99-107), and so do the score keys here.
  */
 #ifndef TANTIVY_B200_H
 #define TANTIVY_B200_H

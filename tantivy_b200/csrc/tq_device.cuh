@@ -109,8 +109,10 @@ struct BatchParams {
 };
 
 // ---- small helpers ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t score_to_key(float f) {  // order preserving for every float
-  const uint32_t u = __float_as_uint(f);
+// Order preserving for every float, with -0.0 and +0.0 on ONE key (the reference compares scores with partial_cmp, which ties
+// them, and orders the tie by DocAddress: sort_by_score.rs:99-107); key_to_score gives that key back as +0.0.
+__device__ __forceinline__ uint32_t score_to_key(float f) {
+  const uint32_t u = __float_as_uint(__fadd_rn(f, 0.0f));  // (-0.0 + +0.0 = +0.0; every other float is itself)
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }
 __device__ __forceinline__ float key_to_score(uint32_t k) {
@@ -241,9 +243,12 @@ __device__ __noinline__ float bm25_factor_large_tf(const float* __restrict__ cac
   const float t = __uint2float_rn(tf);
   return __fdiv_rn(t, __fadd_rn(t, __ldg(cache + id)));
 }
+// A weight of -0.0, or a negative one whose product underflows, scores -0.0.  The score accumulators use -0.0 as "no posting
+// here", so the score is taken as +0.0, which the reference ties with -0.0 anyway (partial_cmp).
+__device__ __forceinline__ float bm25_term_score(float weight, float fac) { return __fadd_rn(__fmul_rn(weight, fac), 0.0f); }
 __device__ __forceinline__ float bm25_score_id(const Scorer& sc, uint32_t id, uint32_t tf) {
   const float fac = tf < kTfRows ? __ldg(sc.tf_table + (tf << 8) + id) : bm25_factor_large_tf(sc.cache, id, tf);
-  return __fmul_rn(sc.weight, fac);
+  return bm25_term_score(sc.weight, fac);
 }
 __device__ __forceinline__ float bm25_score(const Scorer& sc, const uint8_t* __restrict__ fieldnorm, uint32_t doc, uint32_t tf) {
   const uint32_t id = fieldnorm ? (uint32_t)__ldg(fieldnorm + doc) : 1u;  // constant fieldnorm 1 -> id 1

@@ -294,9 +294,10 @@ struct tq_batch {
 
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
-// host twin of score_to_key (tq_device.cuh): order-preserving u32 image of a float
+// host twin of score_to_key (tq_device.cuh): order-preserving u32 image of a float, -0.0 and +0.0 on one key
 static uint32_t host_score_key(float f) {
   uint32_t u;
+  f += 0.0f;
   memcpy(&u, &f, 4);
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }

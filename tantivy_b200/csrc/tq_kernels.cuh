@@ -929,7 +929,7 @@ __global__ void __launch_bounds__(kStripThreads) k_or_strip(const BatchParams P,
             for (int i = 0; i < 4; ++i) a[i] = W.acc[slot[i]];
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-              const float nv = __fadd_rn(a[i], __fmul_rn(sc.weight, fac[i]));
+              const float nv = __fadd_rn(a[i], bm25_term_score(sc.weight, fac[i]));
               W.acc[slot[i]] = nv;
               wmax = in[i] ? fmaxf(wmax, nv) : wmax;
             }

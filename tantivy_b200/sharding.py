@@ -86,8 +86,8 @@ def merge_rows_host(scores, segs, docs, counts, k):
 
 def score_keys(scores):
     """Order-preserving u32 image of f32 scores, as int64 (host twin of score_to_key in csrc/tq_device.cuh):
-    the unit in which shards exchange thresholds; 0 = no bound."""
-    u = np.asarray(scores, dtype=np.float32).view(np.uint32).astype(np.int64)
+    the unit in which shards exchange thresholds; 0 = no bound.  -0.0 and +0.0 share one key (partial_cmp ties them)."""
+    u = (np.asarray(scores, dtype=np.float32) + np.float32(0)).view(np.uint32).astype(np.int64)
     return np.where(u >> 31, u ^ 0xFFFFFFFF, u ^ 0x80000000)
 
 
@@ -222,7 +222,25 @@ class CrossGpuMerger:
         self.rows_g = torch.zeros((self.world, self.pitch), dtype=i32, device=device)
         self.rows_o = torch.zeros((self.pitch,), dtype=i32, device=device)
         self.rows_h = None  # pinned host copy of the merged rows (fetch_host)
+        self.device = device
+        self._ks = {}  # id(QueryBatch) -> (the QueryBatch, each query's own k on the device): the merged counts are clamped to it
         self._streams = {}
+
+    def _check(self, batch):
+        """The packed rows are read at stride self.k, and tq_batch_results_pack_dev writes them at the batch's largest k: a batch of
+        another shape would be misread without any error."""
+        qb = batch.qb
+        if qb.nq != self.nq or qb.kmax != self.k:
+            raise ValueError(f"CrossGpuMerger(nq={self.nq}, k={self.k}) cannot merge a batch of nq={qb.nq}, k_max={qb.kmax}")
+        if id(qb) not in self._ks:  # (one copy per QueryBatch, made before any of its work is queued)
+            self._ks[id(qb)] = (qb, self.torch.tensor(qb.q["k"][:self.nq].astype(np.int32), device=self.device))
+
+    def _merge(self, batch, h):
+        """k_merge of the gathered rows on stream `h` keeps up to self.k rows per query (the batch's largest k); a query with a
+        smaller k keeps its own k, as TopDocs over all the segments would."""
+        self.ctx.merge_topk_packed_dev(h, self.world, self.nq, self.k, self.k, self.rows_g.data_ptr(), self.pitch, self.rows_o.data_ptr())
+        counts = self.rows_o[3 * self.nq * self.k:self.words]
+        self.torch.minimum(counts, self._ks[id(batch.qb)][1], out=counts)
 
     def _stream(self, batch):
         h = batch.stream()
@@ -232,6 +250,7 @@ class CrossGpuMerger:
 
     def run(self, batch):
         """All phases of a prepared batch with the exact threshold exchange in between."""
+        self._check(batch)
         ext, _ = self._stream(batch)
         n = batch.phases()
         with self.torch.cuda.stream(ext):  # NCCL orders itself behind / in front of the kernels of this stream
@@ -245,11 +264,12 @@ class CrossGpuMerger:
     def __call__(self, batch):
         """batch: a finished tantivy_b200.Batch of this rank.  Returns (scores, segment ords, docs, counts) device tensors of
         the merged rows (every rank holds them); they are complete once the batch's stream is (torch.cuda.synchronize())."""
+        self._check(batch)
         ext, h = self._stream(batch)
         batch.results_pack_dev(self.rows_l.data_ptr())  # waits for the run; the copies are on the batch's stream
         with self.torch.cuda.stream(ext):
             self.dist.all_gather_into_tensor(self.rows_g, self.rows_l)
-            self.ctx.merge_topk_packed_dev(h, self.world, self.nq, self.k, self.k, self.rows_g.data_ptr(), self.pitch, self.rows_o.data_ptr())
+            self._merge(batch, h)
             self.rows_o[self.words:].zero_()
         return self._views()
 
@@ -263,11 +283,12 @@ class CrossGpuMerger:
         returns at once -- the caller may queue the NEXT batch's run (on its own stream, with a merger of its own) before it waits
         for this one in complete().  The run's overflow flags travel with the rows (4 words per rank; their maximum lands behind
         the merged rows), so every rank takes the same decision in complete()."""
+        self._check(batch)
         ext, h = self._stream(batch)
         batch.results_pack_dev_async(self.rows_l.data_ptr())
         with self.torch.cuda.stream(ext):
             self.dist.all_gather_into_tensor(self.rows_g, self.rows_l)
-            self.ctx.merge_topk_packed_dev(h, self.world, self.nq, self.k, self.k, self.rows_g.data_ptr(), self.pitch, self.rows_o.data_ptr())
+            self._merge(batch, h)
             self.torch.amax(self.rows_g[:, self.words:], dim=0, out=self.rows_o[self.words:])
 
     def complete(self, batch, rows_to_host=True):

@@ -254,11 +254,20 @@ def _check_rounding(d, sel):
     assert len(bad) == 0, f"f32 score off its f64 value beyond rounding: {d.s32[sel][bad[:4]]} vs {d.s64[sel][bad[:4]]}"
 
 
-def search(segments, q, terms, intersection_order=None):
+def merge_fruits(lists, k):
+    """merge_fruits (sort_key_top_collector.rs:76-95): the rows [(score, segment_ord, doc)] of several lists in one, by score desc
+    (partial_cmp: -0.0 and +0.0 are equal, sort_by_score.rs:99-107), then segment asc, doc asc; the first k."""
+    rows = sorted((r for rows in lists for r in rows), key=lambda r: (-r[0], r[1], r[2]))
+    return [(float(s), int(so), int(doc)) for s, so, doc in rows[:k]]
+
+
+def search(segments, q, terms, intersection_order=None, doc_ranges=None):
     """TopDocs over the segments: rows [(score, segment_ord, doc)] sorted by score desc, segment asc, doc asc (merge_fruits,
     top_score_collector.rs:591-600), deleted docs skipped, with a threshold only scores strictly above it (weight.rs:47-60).
     terms[c] = the posting list (index into Segment.lists) of clause c; q["term_segs"] says in which segments it has postings.
-    intersection_order forces one summation order for every intersection (None: the reference's rule)."""
+    intersection_order forces one summation order for every intersection (None: the reference's rule).
+    doc_ranges = {segment_ord: (lo, hi)}: only docs [lo, hi) of that segment exist (the others count as deleted), e.g. the part of
+    a segment one shard holds; `segments` itself may be any subset of the index's (a shard's), with the weights of the whole index."""
     rows = []
     thr = q.get("threshold")
     has_thr = thr is not None and thr == thr  # (a NaN threshold is no threshold)
@@ -269,13 +278,16 @@ def search(segments, q, terms, intersection_order=None):
         sel = d.has.copy()
         if seg.alive is not None:
             sel &= seg.alive
+        if doc_ranges is not None and seg.segment_ord in doc_ranges:
+            lo, hi = doc_ranges[seg.segment_ord]
+            sel[:lo] = False
+            sel[hi:] = False
         _check_rounding(d, sel)
         if has_thr:
             sel &= d.s32 > f32(thr)
         docs = np.nonzero(sel)[0]
         rows += [(f32(s), seg.segment_ord, int(doc)) for s, doc in zip(d.s32[docs], docs)]
-    rows.sort(key=lambda r: (-r[0], r[1], r[2]))
-    return [(float(s), so, doc) for s, so, doc in rows[:q["k"]]]
+    return merge_fruits([rows], q["k"])
 
 
 def count(segments, q, terms):

@@ -382,3 +382,47 @@ def test_random_phrases_match_the_oracle():
             assert got == want, (phrase, offsets, slop, extra)
             n_hits += len(want)
     assert n_hits > 200
+
+
+# ---- merge_fruits: the cross-segment and cross-shard merge ----------------------------------------------------------------
+def test_merge_fruits_of_segments_and_doc_range_parts_is_the_whole_search():
+    """The rows of each segment alone, and of doc-range parts of the segments (docs outside a part count as deleted), merged by
+    merge_fruits are the rows of one search over every segment: for terms, AND, OR and boolean shapes, k from 1 to 1000."""
+    rng = np.random.default_rng(77)
+    osegs, msegs = _random_pairs(rng, 3, 6, deletes=True, max_doc_range=(2000, 6000))
+    queries, terms = [], []
+    for op, c in [(TQ_OP_TERM, [1]), (TQ_OP_AND, [0, 2]), (TQ_OP_OR, [0, 1, 2, 3, 4, 5]), (TQ_OP_OR, [3, 4])]:
+        for k in (1, 10, 1000):
+            queries.append(make_query(op, osegs, c, k))
+            terms.append(c)
+    for c, occ, grp, msm in BOOL_SHAPES[:6]:
+        queries.append(bool_query(make_query(TQ_OP_OR, osegs, c, 100), occ, grp, msm))
+        terms.append(c)
+    n_rows = 0
+    for q, t in zip(queries, terms):
+        want = M.search(msegs, q, t)
+        n_rows += len(want)
+        assert M.merge_fruits([M.search([s], q, t) for s in msegs], q["k"]) == want
+        parts = []
+        for s in msegs:
+            cuts = [0, 1, s.max_doc // 3, s.max_doc // 3, s.max_doc - 7, s.max_doc]
+            parts += [M.search([s], q, t, doc_ranges={s.segment_ord: (lo, hi)}) for lo, hi in zip(cuts[:-1], cuts[1:])]
+        assert M.merge_fruits(parts, q["k"]) == want
+        assert M.merge_fruits(parts[::-1], q["k"]) == want  # (the order of the lists does not matter)
+    assert n_rows > 2000
+
+
+def test_signed_zero_scores_tie_and_are_ordered_by_doc():
+    """An OR of a +0.0-weight clause and a -0.0-weight clause: every score is +-0.0, and -0.0 == +0.0 as under partial_cmp, so the
+    rows come in (segment, doc) order whichever zero a doc has -- the -0.0 clause's lower docs first.  merge_fruits agrees."""
+    lists = [(np.arange(10, 20), np.ones(10)), (np.arange(0, 10), np.ones(10))]
+    o0, m0 = _pair(lists, np.full(20, 5), segment_ord=0)
+    o1, m1 = _pair(lists, np.full(20, 5), segment_ord=1)
+    q = make_query(TQ_OP_OR, [o0, o1], [0, 1], 100)
+    q["weights"] = [0.0, -0.0]
+    rows = M.search([m0, m1], q, [0, 1])
+    assert [(so, d) for _, so, d in rows] == [(so, d) for so in (0, 1) for d in range(20)]
+    signs = {d: np.signbit(s) for s, so, d in rows if so == 0}
+    assert all(signs[d] for d in range(10)) and not any(signs[d] for d in range(10, 20))  # (both zeros are there)
+    assert M.merge_fruits([M.search([m1], q, [0, 1]), M.search([m0], q, [0, 1])], 100) == rows
+    assert M.merge_fruits([[(0.0, 3, 5)], [(-0.0, 3, 4)], [(-0.0, 2, 9)], [(1e-45, 9, 9)]], 3) == [(1e-45, 9, 9), (-0.0, 2, 9), (-0.0, 3, 4)]
