@@ -211,6 +211,8 @@ int tq_segment_register(tq_ctx*, uint32_t segment_ord, uint32_t field, uint32_t 
 /* The `.pos` sub-file of a registered (segment, field) with record_option TQ_RECORD_FREQS_POSITIONS (copied to HBM):
  * what SegmentReader::inverted_index hands to PositionReader (src/positions/reader.rs:43-55).  Needed by TQ_OP_PHRASE. */
 int tq_segment_register_positions(tq_ctx*, uint32_t segment_ord, uint32_t field, const uint8_t* pos_body, size_t pos_len);
+/* Frees a (segment, field) and its cached tables; their ids are reused.  Returns TQ_ERR_INVALID_ARGUMENT while a prepared batch
+ * that names the segment has not been destroyed (tq_batch_destroy), since that batch still reads the segment's memory. */
 int tq_segment_unregister(tq_ctx*, uint32_t segment_ord, uint32_t field);
 /* Restricts what THIS context evaluates of a registered (segment, field) to the docs [doc_lo, doc_hi): the intra-segment split of
  * SURVEY.md §8(e) -- one huge segment registered on several contexts / GPUs, each with its own doc range (the posting lists are

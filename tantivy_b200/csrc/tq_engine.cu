@@ -101,6 +101,20 @@ struct ListKeyHash {
     return (size_t)(h ^ (h >> 29));
   }
 };
+// A position table is read together with its term's postings (k_phrase), so its key holds both offsets exactly: two terms whose
+// (postings_start, positions_start) pairs differ never share a table.
+struct PosKey {
+  uint32_t segment_ord, field;
+  uint64_t postings_start, positions_start;
+  bool operator==(const PosKey& o) const {
+    return segment_ord == o.segment_ord && field == o.field && postings_start == o.postings_start && positions_start == o.positions_start;
+  }
+};
+struct PosKeyHash {
+  size_t operator()(const PosKey& k) const {
+    return ListKeyHash{}(ListKey{k.segment_ord, k.field, k.postings_start}) ^ (size_t)(k.positions_start * 0xFF51AFD7ED558CCDull);
+  }
+};
 
 // Bump allocator over big cudaMalloc chunks for the per-term block tables (immutable, never freed
 // individually; dropped with the context).
@@ -160,8 +174,9 @@ struct tq_ctx {
   std::vector<uint32_t> free_ids;  // list ids of unregistered segments (and of rolled-back builds), reused first
   PosDesc* d_pos_descs = nullptr;  // position tables (phrase queries), same life cycle as the block tables
   uint32_t pos_cap = 0, n_pos = 0;
-  std::unordered_map<ListKey, uint32_t, ListKeyHash> pos_cache;  // (segment, field, positions_start) -> pos id
+  std::unordered_map<PosKey, uint32_t, PosKeyHash> pos_cache;  // (segment, field, postings_start, positions_start) -> pos id
   std::vector<uint32_t> free_pos_ids;
+  std::map<std::pair<uint32_t, uint32_t>, uint32_t> seg_users;  // (segment, field) -> prepared batches not yet destroyed that name it
   cudaStream_t build_stream = nullptr;
   PinBuf build_pin;
   DevBuf build_dev;
@@ -281,6 +296,7 @@ struct tq_batch {
   struct { size_t scores, segs, docs, counts; } res_at{};  // the result columns inside the res_bytes at res_off (and in res_pin)
   tq_stats stats{};
   bool ran = false;
+  std::vector<std::pair<uint32_t, uint32_t>> held;  // the (segment, field)s its queries name, counted in tq_ctx::seg_users until destroyed
 };
 
 #define TQ_CUDA(expr)                                                                         \
@@ -543,6 +559,7 @@ int tq_segment_unregister(tq_ctx* c, uint32_t segment_ord, uint32_t field) {
   std::lock_guard<std::mutex> g(c->mu);
   auto it = c->segments.find({segment_ord, field});
   if (it == c->segments.end()) return fail(TQ_ERR_NOT_FOUND, "segment/field not registered");
+  if (c->seg_users.count({segment_ord, field})) return fail(TQ_ERR_INVALID_ARGUMENT, "a prepared batch still uses the segment");
   cudaDeviceSynchronize();
   cudaFree(it->second.d_idx); cudaFree(it->second.d_fieldnorm); cudaFree(it->second.d_alive);
   cudaFree(it->second.d_pos); cudaFree(it->second.d_pos_pool);
@@ -651,7 +668,7 @@ int flush_builds(tq_ctx* c, std::vector<PendingBuild>& pending, uint64_t* built)
   return TQ_OK;
 }
 
-struct PendingPos { PosJob job; ListKey key; };
+struct PendingPos { PosJob job; PosKey key; };
 
 void rollback_pos(tq_ctx* c, std::vector<PendingPos>& pending) {
   for (auto& pp : pending) {
@@ -675,7 +692,7 @@ int get_pos(tq_ctx* c, const tq_term_seg& ts, const tq_term_pos& tp, std::vector
   if (!seg.d_pos) return fail(TQ_ERR_INVALID_ARGUMENT, "phrase query on a segment without registered positions (tq_segment_register_positions)");
   if (tp.positions_end < tp.positions_start || tp.positions_end > seg.pos_len) return fail(TQ_ERR_INVALID_ARGUMENT, "positions range outside the `.pos` body");
   if (tp.positions_end - tp.positions_start > 0xFFFFFFFFull) return fail(TQ_ERR_UNSUPPORTED, "position stream larger than 4 GiB");
-  const ListKey key{ts.segment_ord, ts.field, tp.positions_start ^ (ts.postings_start << 1) ^ (1ull << 62)};
+  const PosKey key{ts.segment_ord, ts.field, ts.postings_start, tp.positions_start};
   auto it = c->pos_cache.find(key);
   if (it != c->pos_cache.end()) { *pos_id = it->second; return TQ_OK; }
   if (c->free_pos_ids.empty() && c->n_pos >= c->pos_cap) return fail(TQ_ERR_OOM, "position table cache full (TQ_MAX_POS_LISTS)");
@@ -1611,6 +1628,19 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
 
 }  // namespace
 
+// A prepared batch holds list ids and alive pointers of the segments its queries name: tq_segment_unregister refuses those
+// segments until the batch is destroyed.  ctx->mu held.
+static void hold_segments(tq_ctx* c, tq_batch* b, const tq_query* queries, size_t nq) {
+  for (size_t qi = 0; qi < nq; ++qi)
+    for (uint32_t i = 0; i < queries[qi].n_term_segs; ++i) {
+      const std::pair<uint32_t, uint32_t> key{queries[qi].term_segs[i].segment_ord, queries[qi].term_segs[i].field};
+      if (b->held.empty() || b->held.back() != key) b->held.push_back(key);
+    }
+  std::sort(b->held.begin(), b->held.end());
+  b->held.erase(std::unique(b->held.begin(), b->held.end()), b->held.end());
+  for (const auto& key : b->held) ++c->seg_users[key];
+}
+
 // repeat (finalize_run): 0 = a caller's batch.  1 = the repeat of an overflowed run: TERM / AND / OR / phrase queries take the
 // per-query kernels; TQ_OP_BOOL queries stay on the tile engine with candidate regions as large as their postings and the largest
 // tile buffer.  2 = as 1, but every TQ_OP_BOOL query in a tile group of its own.
@@ -1650,6 +1680,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
     if (rc == TQ_OK) rc = flush_builds(c, pl.pending, &pl.built);
     if (rc == TQ_OK) rc = flush_pos_builds(c, pl.pending_pos);
     if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);
   }
   int rc = stage_tile_groups(c, pl);
   if (rc == TQ_OK && !pl.tgroups.empty()) b->owned.assign(queries, nq);  // the queries are kept: an overflowing run is repeated (finalize_run)
@@ -1686,6 +1717,11 @@ void tq_batch_destroy(tq_batch* b) {
   b->next_phase = 0;
   b->ran = false;
   std::lock_guard<std::mutex> g(b->ctx->mu);
+  for (const auto& key : b->held) {
+    auto it = b->ctx->seg_users.find(key);
+    if (--it->second == 0) b->ctx->seg_users.erase(it);
+  }
+  b->held.clear();
   b->ctx->pool.push_back(b);  // buffers are recycled by the next batch
 }
 
