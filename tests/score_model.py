@@ -290,11 +290,65 @@ def search(segments, q, terms, intersection_order=None, doc_ranges=None):
     return merge_fruits([rows], q["k"])
 
 
-def count(segments, q, terms):
-    """Count collector: alive docs that match (count_collector.rs)."""
+def count(segments, q, terms, doc_ranges=None):
+    """Count collector: alive docs that match (count_collector.rs); doc_ranges as in search."""
     total = 0
     for seg in segments:
         d = _segment_matches(seg, q, terms)
-        if d is not None:
-            total += int((d.has & seg.alive).sum()) if seg.alive is not None else int(d.has.sum())
+        if d is None:
+            continue
+        sel = d.has & seg.alive if seg.alive is not None else d.has.copy()
+        if doc_ranges is not None and seg.segment_ord in doc_ranges:
+            lo, hi = doc_ranges[seg.segment_ord]
+            sel[:lo] = False
+            sel[hi:] = False
+        total += int(sel.sum())
     return total
+
+
+class Compacted:
+    """A segment of any max_doc (up to 2^31 - 2) on a compacted doc space, for search and count.  A score depends only on a doc's
+    postings, fieldnorm id and alive bit, and the order of rows only on the order of doc ids, so the model is exact over the sorted
+    union of the docs that occur in the segment's lists (and positions), mapped onto 0..n-1: `docs[i]` is the real id of doc i.
+    fn_ids = the segment's fieldnorm id per doc (uint8, None: no fieldnorms), alive = its packed alive bitset (None: no deletes);
+    neither is expanded to max_doc.  Weights and average fieldnorms stay those of the real index: queries carry them."""
+
+    def __init__(self, segment_ord, lists, max_doc, fn_ids=None, alive=None, basic=False, positions=None):
+        parts = [np.asarray(d, np.uint32) for d, _ in lists]
+        if positions is not None:
+            parts += [np.fromiter(p, np.uint32, len(p)) for p in positions]
+        self.docs = np.unique(np.concatenate(parts)) if parts else np.zeros(0, np.uint32)
+        assert len(self.docs) == 0 or int(self.docs[-1]) < max_doc
+        self.max_doc = max_doc
+        mapped = [(np.searchsorted(self.docs, np.asarray(d, np.uint32)), t) for d, t in lists]
+        lengths = None if fn_ids is None else _FN_TABLE[np.asarray(fn_ids)[self.docs]]
+        bits = None
+        if alive is not None:
+            a = np.asarray(alive, np.uint8)
+            bits = np.packbits((a[self.docs >> 3] >> (self.docs & 7)) & 1, bitorder="little")
+        pos = None
+        if positions is not None:
+            pos = [{int(np.searchsorted(self.docs, d)): ps for d, ps in p.items()} for p in positions]
+        self.seg = Segment(segment_ord, mapped, lengths, alive=bits, basic=basic, max_doc=len(self.docs), positions=pos)
+
+    def doc_range(self, lo, hi):
+        """[lo, hi) of real doc ids on the compacted space."""
+        return int(np.searchsorted(self.docs, lo)), int(np.searchsorted(self.docs, hi))
+
+
+def _compacted_ranges(csegs, doc_ranges):
+    if doc_ranges is None:
+        return None
+    by = {c.seg.segment_ord: c for c in csegs}
+    return {so: by[so].doc_range(lo, hi) for so, (lo, hi) in doc_ranges.items() if so in by}
+
+
+def search_compacted(csegs, q, terms, intersection_order=None, doc_ranges=None):
+    """search over Compacted segments: rows with real doc ids; doc_ranges in real doc ids."""
+    rows = search([c.seg for c in csegs], q, terms, intersection_order, _compacted_ranges(csegs, doc_ranges))
+    docs = {c.seg.segment_ord: c.docs for c in csegs}
+    return [(s, g, int(docs[g][d])) for s, g, d in rows]
+
+
+def count_compacted(csegs, q, terms, doc_ranges=None):
+    return count([c.seg for c in csegs], q, terms, _compacted_ranges(csegs, doc_ranges))
