@@ -113,9 +113,14 @@ typedef struct {
  *                    (FreqReadingOption::SkipFreq, block_segment_postings.rs:97-140,343-360).
  * flags/threshold  = TQ_QUERY_HAS_THRESHOLD: only docs with score > threshold are collected -- the initial
  *                    `threshold` argument of Weight::for_each_pruning (src/query/weight.rs:123-132); a caller that
- *                    already holds k hits (another shard, an earlier page) passes its k-th score to prune more. */
+ *                    already holds k hits (another shard, an earlier page) passes its k-th score to prune more.
+ *                    TQ_QUERY_COUNT_HITS (TERM / AND / OR / BOOL): the batch also counts the query's matching ALIVE docs -- the
+ *                    `Count` half of searcher.search(&query, &(Count, TopDocs::with_limit(k)))  (collector/mod.rs:322-365);
+ *                    tq_batch_fetch_hits returns it.  The count ignores k and every threshold (they prune the rows only);
+ *                    with TQ_OP_PHRASE the flag fails at prepare with TQ_ERR_INVALID_ARGUMENT. */
 #define TQ_TERM_IGNORE_FREQ 1u
 #define TQ_QUERY_HAS_THRESHOLD 1u
+#define TQ_QUERY_COUNT_HITS 2u
 typedef struct {
   int32_t op;
   uint32_t n_terms;
@@ -188,6 +193,8 @@ typedef struct {
                                    (stage B2) by how they ended: [0] dropped by the bound taken before the look-ups, [1] not the owner
                                    (completed the walk, but an earlier essential clause lists the doc), [2] dropped in the
                                    non-essential walk, [3] completed */
+  float count_hits_ms;          /* device time of the launches that count TQ_QUERY_COUNT_HITS queries (k_count_tiles, k_count, k_count_bool) */
+  uint64_t units_count_hits;    /* CTAs of those launches */
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */
@@ -267,6 +274,11 @@ int tq_batch_topkeys_export_dev(tq_batch*, uint32_t* keys_dev, uint32_t k_stride
 int tq_batch_thresholds_from_keys_dev(tq_batch*, const uint32_t* gathered_keys_dev, uint32_t n_shards, uint32_t k_stride);
 int tq_batch_fetch(tq_batch*, uint32_t out_stride, float* out_scores, uint32_t* out_segment_ord,
                    uint32_t* out_doc, uint32_t* out_count);
+/* The Count half of (Count, TopDocs): out_hits[q] (nq entries) = tq_count_batch's answer for query q on this context (alive
+ * docs, doc ranges applied) when q carries TQ_QUERY_COUNT_HITS, else 0.  Call it after a finished run (tq_batch_run or the last
+ * phase); like tq_batch_fetch it resolves an overflowed run first.  Every run counts from zero.  The tile engine counts from the
+ * postings the run has already decoded; queries on the per-query kernels are counted by the Count kernels in the same run. */
+int tq_batch_fetch_hits(tq_batch*, uint64_t* out_hits);
 /* Device pointers of the result rows of a finished run: row stride = k_max of the batch. */
 int tq_batch_results_dev(tq_batch*, const float** scores_dev, const uint32_t** segment_ord_dev,
                          const uint32_t** doc_dev, const uint32_t** count_dev, uint32_t* stride);

@@ -16,6 +16,7 @@ TQ_MAX_K = 1024
 TQ_MAX_TERMS = 32
 TQ_TERM_IGNORE_FREQ = 1
 TQ_QUERY_HAS_THRESHOLD = 1
+TQ_QUERY_COUNT_HITS = 2
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -123,6 +124,8 @@ class Stats(C.Structure):
         ("tile_cycles", C.c_uint64 * 8),
         ("tile_groups_union_only", C.c_uint64),
         ("tile_b2_exits", C.c_uint64 * 4),
+        ("count_hits_ms", C.c_float),
+        ("units_count_hits", C.c_uint64),
     ]
 
 
@@ -141,6 +144,7 @@ class QueryBatch:
       (term_idx, segment_ord, field, doc_freq, postings_start, postings_end),
       tf_cache (optional [n_terms,256]), term_flags (optional [n_terms] bytes, TQ_TERM_IGNORE_FREQ),
       threshold (optional float: only docs scoring above it are collected),
+      count_hits (optional bool: the batch also counts the query's matching alive docs, Batch.fetch_hits),
       phrase queries (op TQ_OP_PHRASE): term_pos = list of (positions_start, positions_end) parallel to term_segs,
       term_offset = [n_terms] offsets in the phrase, slop (optional, must be 0 on the device path);
       boolean queries (op TQ_OP_BOOL): term_occur = [n_terms] TQ_OCCUR_*, term_group = optional [n_terms] group ids of the MUST
@@ -193,6 +197,8 @@ class QueryBatch:
             if q.get("threshold") is not None:
                 row["flags"] = TQ_QUERY_HAS_THRESHOLD
                 row["threshold"] = q["threshold"]
+            if q.get("count_hits"):
+                row["flags"] |= TQ_QUERY_COUNT_HITS
             tpos = q.get("term_pos")
             if tpos is not None:
                 tp = np.zeros(max(len(tpos), 1), dtype=TERM_POS_DTYPE)

@@ -263,6 +263,10 @@ struct tq_batch {
     uint32_t unit_base[kTileRounds] = {0, 0, 0, 0}, n_units[kTileRounds] = {0, 0, 0, 0};
     size_t smem = 0;
     bool union_only = false;  // the group's queries are all term queries and unions: the k_tile<*, *, true> instances run it
+    CountTileParams count{};  // k_count_tiles: the group's TQ_QUERY_COUNT_HITS queries
+    uint32_t n_count_units = 0;
+    size_t count_smem = 0;
+    std::vector<uint32_t> count_queries;  // batch ordinals of those queries (recounted by the Count kernels if count.overflow is set)
   };
   tq_ctx* ctx = nullptr;
   cudaStream_t stream = nullptr;
@@ -296,6 +300,15 @@ struct tq_batch {
   struct { size_t scores, segs, docs, counts; } res_at{};  // the result columns inside the res_bytes at res_off (and in res_pin)
   tq_stats stats{};
   bool ran = false;
+  // TQ_QUERY_COUNT_HITS: per-query hit counters (u64 [nq]) and the groups' overflow words (u32 [groups]) in `scratch` at hits_off,
+  // zeroed by phase 0; the Count kernels of the queries on the per-query kernels; hits_host = their doc_freq shortcuts
+  bool count_hits = false;
+  size_t hits_off = 0, hits_bytes = 0;
+  CountParams count_p{};
+  CountBoolParams count_bool_p{};
+  uint32_t n_count_units = 0, n_count_bool_units = 0;
+  std::vector<uint64_t> hits_host;
+  PinBuf hits_pin;
   std::vector<std::pair<uint32_t, uint32_t>> held;  // the (segment, field)s its queries name, counted in tq_ctx::seg_users until destroyed
 };
 
@@ -393,7 +406,7 @@ void tq_batch_destroy_real(tq_batch* b) {
   if (b->side) { cudaStreamSynchronize(b->side); cudaStreamDestroy(b->side); }
   if (b->ev_side0) cudaEventDestroy(b->ev_side0);
   if (b->ev_side1) cudaEventDestroy(b->ev_side1);
-  b->pin.release(); b->dev.release(); b->scratch.release(); b->res_pin.release(); b->tile_dev.release();
+  b->pin.release(); b->dev.release(); b->scratch.release(); b->res_pin.release(); b->tile_dev.release(); b->hits_pin.release();
   if (b->flags_pin) cudaFreeHost(b->flags_pin);
   if (b->ev_start) cudaEventDestroy(b->ev_start);
   if (b->ev_k0) cudaEventDestroy(b->ev_k0);
@@ -741,7 +754,7 @@ int flush_pos_builds(tq_ctx* c, std::vector<PendingPos>& pending) {
 
 // ---- batches ---------------------------------------------------------------------------------------
 // Kernel time by kind: CUDA events recorded on the batch's stream around every launch (group of launches) of that kind.
-enum SpanKind { SPAN_TERM = 0, SPAN_AND, SPAN_OR, SPAN_FINAL, SPAN_SCORE, SPAN_TILE, SPAN_THETA, SPAN_PHRASE, SPAN_KINDS };
+enum SpanKind { SPAN_TERM = 0, SPAN_AND, SPAN_OR, SPAN_FINAL, SPAN_SCORE, SPAN_TILE, SPAN_THETA, SPAN_PHRASE, SPAN_COUNT, SPAN_KINDS };
 
 static int span_begin(tq_batch* b, int kind, cudaStream_t on = nullptr) {
   if (b->n_spans == b->spans.size()) {
@@ -773,6 +786,7 @@ static void collect_times(tq_batch* b) {
   b->stats.tile_ms = by_kind[SPAN_TILE];
   b->stats.theta_ms = by_kind[SPAN_THETA];
   b->stats.phrase_ms = by_kind[SPAN_PHRASE];
+  b->stats.count_hits_ms = by_kind[SPAN_COUNT];
 }
 
 // The run's kernel times into its stats, and its stats into the context's (tq_get_stats).
@@ -889,6 +903,8 @@ struct GroupStage {
   std::vector<TQuery> queries;
   std::vector<uint16_t> clauses;
   std::vector<TUnit> units[kTileRounds];
+  std::vector<TUnit> count_units;     // k_count_tiles: every tile of the segments that hold a TQ_QUERY_COUNT_HITS query
+  std::vector<uint32_t> count_queries;  // batch ordinals of those queries
   std::vector<SChunk> chunks;
   uint32_t max_slots = 1, p_cap = 1024, max_big = 1, max_queries = 1, max_clause_words = 0, max_clauses = 1;
   size_t tix_words = 0;
@@ -898,6 +914,17 @@ struct GroupStage {
 // A (query, segment) of the per-query kernels, beside its QSeg: its unit class, the blocks / windows / tiles its units cover, and
 // whether it is a strip pair with a threshold sample pass (MaxScore can then skip its dense clauses).
 struct SegWork { UnitClass cls; uint32_t total; bool sample; };
+
+// The Count collector's work for a set of queries: (query, segment) pairs of k_count (term / AND / OR: their list ids) and of
+// k_count_bool (TQ_OP_BOOL: structure words with list ids), one unit per 8 tiles of 8192 docs.
+struct CountPlan {
+  std::vector<uint32_t> list_ids;
+  std::vector<CountSeg> segs;
+  std::vector<Unit> units;
+  std::vector<uint32_t> bool_words;
+  std::vector<CountBoolSeg> bool_segs;
+  std::vector<Unit> bool_units;
+};
 
 // The plan of one batch: what the stages of batch_prepare_impl hand on to each other.
 struct BatchPlan {
@@ -928,6 +955,11 @@ struct BatchPlan {
   std::vector<GroupStage> gstage;  // parallel to tgroups
   uint64_t tile_pairs_total = 0, pair_cursor = 0, tile_postings = 0, tile_units = 0;
   size_t tix_total_words = 0, tile_bytes = 0;
+  // TQ_QUERY_COUNT_HITS (not in a repeat: the hits of the original run stand): the queries on the per-query kernels are counted
+  // by k_count / k_count_bool (count), the doc_freq shortcuts go to hits_host; the tile groups' queries by k_count_tiles
+  bool count_hits = false;
+  CountPlan count;
+  std::vector<uint64_t> hits_host;
   // totals
   uint64_t built = 0, alg_bytes = 0, postings = 0, op_bytes[3] = {0, 0, 0};
   uint32_t kmax = 1;
@@ -1044,8 +1076,8 @@ bool tile_fits(const tq_ctx* c, const TileGroupBuild& g, const SegPlan* plans, s
   return true;
 }
 
-// Adds the query to the group; returns the number of new pair elements it brought.
-uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, const SegPlan* plans, size_t n_plans) {
+// Adds the query to the group (count: k_count_tiles counts its hits); returns the number of new pair elements it brought.
+uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, bool count, const SegPlan* plans, size_t n_plans) {
   const uint64_t pairs_before = g.pairs;
   for (size_t pi = 0; pi < n_plans; ++pi) {
     const SegPlan& sp = plans[pi];
@@ -1065,7 +1097,7 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, const SegPlan* pl
     tq.clause_base = (uint32_t)sb.clauses.size();
     tq.n_clauses = (uint16_t)(op == TQ_OP_BOOL ? sp.bool_words.size() : sp.here.size());
     tq.op = (uint8_t)(op == TQ_OP_BOOL ? kTileOpBool : op);
-    tq.flags = (sp.prunable ? 1u : 0u) | (sp.intersection_order ? 4u : 0u);
+    tq.flags = (sp.prunable ? 1u : 0u) | (sp.intersection_order ? 4u : 0u) | (count ? kTileQueryCount : 0u);
     uint16_t slot_of_here[TQ_MAX_TERMS];
     size_t hi_idx = 0;
     for (auto& h : sp.here) {
@@ -1234,7 +1266,7 @@ bool route_to_tile(const tq_ctx* c, BatchPlan& pl, size_t qi, int op, uint64_t q
   }
   const uint64_t tile_pair_budget = (uint64_t)c->tile_scratch_mb * (1u << 20) / 8u;
   if (!fits || pl.tile_pairs_total + q_postings + 128ull * pl.n_plans * q.n_terms > tile_pair_budget) return false;
-  pl.tile_pairs_total += tile_admit(tg.back(), (uint32_t)qi, op, plans, pl.n_plans);
+  pl.tile_pairs_total += tile_admit(tg.back(), (uint32_t)qi, op, pl.count_hits && (q.flags & TQ_QUERY_COUNT_HITS), plans, pl.n_plans);
   // every doc at or above the running threshold is handed over: the sample launch and the k_theta passes keep that
   // near k; a query that still overflows has the run repeated (flags[1], finalize_run).  A query hands each doc over at
   // most once (every tile once per run, a doc once per (query, tile): by its first posting in the driving clauses), so
@@ -1291,11 +1323,73 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
   }
 }
 
+// The Count work of query qi (Count collector, count_collector.rs; Weight::count, term_weight.rs:179-219): its (query, segment)
+// pairs go to cp; a term on a segment without deletes is answered from its doc_freq, added to *host_add (term_weight.rs:179-190).
+// ctx->mu held.
+int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBuild>& pending, std::vector<const tq_term_seg*>& order,
+               CountPlan& cp, uint64_t* host_add) {
+  if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
+  if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_BOOL) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
+  if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
+  if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
+  if (q.op == TQ_OP_BOOL && (!q.term_occur || !q.weight)) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_BOOL needs term_occur and weights");
+  return for_each_segment(q, order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
+    if (q.op == TQ_OP_BOOL) {  // mixed shapes: the structure of this segment, with list ids in place of the clause indices
+      uint32_t tix_[TQ_MAX_TERMS], dfs_[TQ_MAX_TERMS], ids_[TQ_MAX_TERMS];
+      float ws_[TQ_MAX_TERMS];
+      const Segment* seg = nullptr;
+      for (size_t a = 0; a < n_here; ++a) {
+        int rc = get_list(c, *ts[a], false, pending, &ids_[a], &seg);
+        if (rc != TQ_OK) return rc;
+        tix_[a] = ts[a]->term_idx; dfs_[a] = ts[a]->doc_freq; ws_[a] = q.weight[ts[a]->term_idx];
+      }
+      std::vector<uint16_t> words;
+      bool io_unused;  // (a count adds no scores)
+      const int st = bool_structure(q, tix_, dfs_, ws_, n_here, 0u, words, &io_unused);
+      if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
+      if (st == 0) return TQ_OK;
+      CountBoolSeg bs{};
+      bs.query = qi; bs.words_base = (uint32_t)cp.bool_words.size(); bs.max_doc = seg->max_doc; bs.alive = seg->d_alive;
+      cp.bool_words.insert(cp.bool_words.end(), words.begin(), words.end());
+      map_bool_clauses(cp.bool_words.data() + bs.words_base, words.size(), [&](uint32_t a) { return ids_[a]; });
+      const uint32_t tiles = (bs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
+      for (uint32_t t0 = 0; t0 < tiles; t0 += per) cp.bool_units.push_back(Unit{(uint32_t)cp.bool_segs.size(), t0, std::min(tiles, t0 + per), 0});
+      cp.bool_segs.push_back(bs);
+      return TQ_OK;
+    }
+    if (q.op == TQ_OP_AND && n_here < q.n_terms) return TQ_OK;  // a clause without postings: empty intersection
+    CountSeg cs{};
+    cs.query = qi; cs.lists_base = (uint32_t)cp.list_ids.size(); cs.n_lists = (uint32_t)n_here; cs.op = (uint32_t)q.op;
+    const Segment* seg = nullptr;
+    uint64_t df_single = 0;
+    for (size_t a = 0; a < n_here; ++a) {
+      uint32_t id;
+      int rc = get_list(c, *ts[a], false, pending, &id, &seg);
+      if (rc != TQ_OK) return rc;
+      cp.list_ids.push_back(id);
+      df_single = ts[a]->doc_freq;
+    }
+    cs.max_doc = seg->max_doc;
+    cs.alive = seg->d_alive;
+    if (n_here == 1 && !seg->d_alive) {  // TermWeight::count without deletes: the term's doc_freq (term_weight.rs:179-190)
+      *host_add += df_single;
+      cp.list_ids.resize(cs.lists_base);
+    } else {
+      const uint32_t tiles = (cs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
+      for (uint32_t t0 = 0; t0 < tiles; t0 += per) cp.units.push_back(Unit{(uint32_t)cp.segs.size(), t0, std::min(tiles, t0 + per), 0});
+      cp.segs.push_back(cs);
+    }
+    return TQ_OK;
+  });
+}
+
 // Validates query qi and plans it: into a tile group, or onto the per-query kernels.  ctx->mu held.
 int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi) {
   const tq_query& q = pl.queries[qi];
   int rc = validate_query(c, q);
   if (rc != TQ_OK) return rc;
+  const bool count = pl.count_hits && (q.flags & TQ_QUERY_COUNT_HITS);
+  if (count && q.op == TQ_OP_PHRASE) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_QUERY_COUNT_HITS: Count of a phrase query is not on the device path");
   // effective shape: an AND / OR of one clause is that clause (boolean_weight.rs:57-68, block_wand_union.rs:154-157)
   const int op = q.op == TQ_OP_PHRASE ? TQ_OP_PHRASE : (q.op == TQ_OP_BOOL ? TQ_OP_BOOL : (q.n_terms == 1 ? TQ_OP_TERM : q.op));
   pl.kmax = std::max(pl.kmax, q.k);
@@ -1311,7 +1405,8 @@ int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi) {
   if (route_to_tile(c, pl, qi, op, q_postings)) return TQ_OK;
   if (op == TQ_OP_BOOL && pl.n_plans) return fail(TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL query does not fit the tile engine's buffers (split the batch / raise TQ_TILE_SCRATCH_MB)");
   append_qsegs(c, pl, qi, op);
-  return TQ_OK;
+  // its hits: the Count kernels, in the same run (the per-query kernels leave no decoded lists behind)
+  return count ? plan_count(c, q, (uint32_t)qi, pl.pending, pl.order, pl.count, &pl.hits_host[qi]) : TQ_OK;
 }
 
 // Work units. A unit is one CTA's share of a (query, segment). With few (query, segment) pairs in the
@@ -1368,6 +1463,9 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
     double dens_max = 0;
     uint64_t tiles_total = 0;
     uint32_t kmax_g = 1;
+    uint64_t group_tiles = 0;
+    for (auto& sb : tg.segs) group_tiles += sb.t_hi - sb.t_lo;
+    const uint32_t count_per = (uint32_t)std::max<uint64_t>(8u, (group_tiles + 1023u) / 1024u);
     for (auto& sb : tg.segs) {
       // dense lists first (they get a tile index and whole warps), then the rest; clause ordinals follow the permutation
       std::vector<uint32_t> perm(sb.slots.size());
@@ -1418,6 +1516,16 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         if (tq.op == kTileOpBool) map_bool_clauses(w, tq.n_clauses, [&](uint16_t s) { return new_of[s]; });
         else for (uint32_t e = 0; e < tq.n_clauses; ++e) w[e] = (uint16_t)new_of[w[e]];
       }
+      bool count_seg = false;
+      for (auto& tq : sb.queries) {
+        if (!(tq.flags & kTileQueryCount)) continue;
+        count_seg = true;
+        gs.count_queries.push_back(tq.query);
+      }
+      if (count_seg) {  // k_count_tiles skips nothing: every tile of the doc range, about 1024 CTAs per group over all its segments
+        for (uint32_t t0 = sb.t_lo; t0 < sb.t_hi; t0 += count_per)
+          gs.count_units.push_back(TUnit{(uint32_t)gs.segs.size(), t0, std::min(sb.t_hi, t0 + count_per), 0});
+      }
       gs.max_slots = std::max(gs.max_slots, G.n_slots);
       gs.max_big = std::max(gs.max_big, G.n_big);
       gs.max_queries = std::max(gs.max_queries, G.n_queries);
@@ -1425,8 +1533,10 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
       tiles_total += sb.t_hi - sb.t_lo;
       gs.segs.push_back(G);
     }
+    std::sort(gs.count_queries.begin(), gs.count_queries.end());
+    gs.count_queries.erase(std::unique(gs.count_queries.begin(), gs.count_queries.end()), gs.count_queries.end());
     pl.tix_total_words += gs.tix_words;
-    gs.p_cap = (uint32_t)std::min<double>(kTileMaxPairs, std::max(1024.0, dens_max * kTile * 1.25 + 192.0));
+    gs.p_cap =(uint32_t)std::min<double>(kTileMaxPairs, std::max(1024.0, dens_max * kTile * 1.25 + 192.0));
     gs.p_cap = (gs.p_cap + 63u) & ~63u;
     if (c->tile_pcap_hook) gs.p_cap = c->tile_pcap_hook;  // (test hook: overflowing tiles)
     if (pl.repeat) gs.p_cap = kTileMaxPairs;  // the repeat of an overflowed run: the largest tile buffer there is
@@ -1490,21 +1600,27 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
   const size_t o_qlists = st.add(pl.qlists), o_qsegs = st.add(pl.qsegs), o_qaux = st.add(pl.qaux), o_units = st.add(units);
   const size_t o_queries = st.add(pl.dq);
   const size_t o_qinit = st.add(nullptr, nq1 * sizeof(QState));  // per-run initial state (threshold keys), filled below
-  struct GroupOff { size_t slots, segs, queries, clauses, units, chunks; };
+  struct GroupOff { size_t slots, segs, queries, clauses, units, chunks, count_units; };
   std::vector<GroupOff> goff(pl.gstage.size());
   std::vector<std::vector<TUnit>> gunits(pl.gstage.size());
   b->groups.resize(pl.gstage.size());
   for (size_t gi = 0; gi < pl.gstage.size(); ++gi) {
     const GroupStage& gs = pl.gstage[gi];
     gunits[gi] = concat_units(gs.units, b->groups[gi].unit_base, b->groups[gi].n_units);
-    goff[gi] = GroupOff{st.add(gs.slots), st.add(gs.segs), st.add(gs.queries), st.add(gs.clauses), st.add(gunits[gi]), st.add(gs.chunks)};
+    goff[gi] = GroupOff{st.add(gs.slots), st.add(gs.segs), st.add(gs.queries), st.add(gs.clauses), st.add(gunits[gi]), st.add(gs.chunks),
+                        gs.count_units.empty() ? 0 : st.add(gs.count_units)};
   }
+  // the Count kernels of the TQ_QUERY_COUNT_HITS queries on the per-query kernels
+  const CountPlan& cp = pl.count;
+  size_t o_cnt_ids = 0, o_cnt_segs = 0, o_cnt_units = 0, o_cntb_words = 0, o_cntb_segs = 0, o_cntb_units = 0;
+  if (!cp.units.empty()) { o_cnt_ids = st.add(cp.list_ids); o_cnt_segs = st.add(cp.segs); o_cnt_units = st.add(cp.units); }
+  if (!cp.bool_units.empty()) { o_cntb_words = st.add(cp.bool_words); o_cntb_segs = st.add(cp.bool_segs); o_cntb_units = st.add(cp.bool_units); }
   b->desc_bytes = st.bytes;
   TQ_CUDA(st.reserve(b->pin, b->dev));
 
   // ---- tile scratch: pair arrays | tile indexes | samples | sample counts | flags + counters --------------------------------
   uint32_t sample_cap = 0;
-  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0, to_cursors = 0;
+  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0, to_cursors = 0, to_count_cursors = 0;
   if (!pl.gstage.empty()) {
     uint64_t sample_units_tiles = 0;
     for (auto& gs : pl.gstage) for (auto& u : gs.units[0]) sample_units_tiles += u.t1 - u.t0;
@@ -1520,6 +1636,9 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     for (auto& gs : pl.gstage)
       for (auto& u : gs.units) cursors = std::max<size_t>(cursors, u.size() * gs.max_slots);
     to_cursors = so2; so2 = align256(so2 + cursors * sizeof(uint2));
+    size_t count_cursors = 0;  // k_count_tiles' own cursors (its launches run next to k_tile's, one group after another)
+    for (auto& gs : pl.gstage) count_cursors = std::max<size_t>(count_cursors, gs.count_units.size() * gs.max_slots);
+    to_count_cursors = so2; so2 = align256(so2 + count_cursors * sizeof(uint2));
     pl.tile_bytes = so2;
     TQ_CUDA(b->tile_dev.ensure(pl.tile_bytes));
   }
@@ -1582,9 +1701,12 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     // (the exact instance the group runs without TQ_TILE_COUNTERS: the counters instances are built for 3 CTAs per SM)
     TQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, tile_kernel(false, false, run.union_only), kTileThreads, run.smem));
     c->tile_ctas_last = (uint64_t)ctas;
+    run.n_count_units = (uint32_t)gs.count_units.size();
+    run.count_queries = gs.count_queries;
+    run.count_smem = count_tiles_smem_bytes(TP.max_slots, TP.max_big, TP.max_queries);
   }
 
-  // ---- scratch: qstate | candidates | results ------------------------------------------------------
+  // ---- scratch: qstate | candidates | results | hits + the groups' count overflow words ---------------------------------
   b->kmax = pl.kmax;
   b->n_cands = pl.n_cands;
   size_t so = 0;
@@ -1595,7 +1717,33 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
   b->res_at = {0, col, 2 * col, 3 * col};
   b->res_bytes = b->res_at.counts + align256(nq1 * 4);
   so += b->res_bytes;
+  b->count_hits = pl.count_hits;
+  b->hits_off = so;
+  b->hits_bytes = pl.count_hits ? nq1 * 8 + b->groups.size() * 4 : 0;
+  so = align256(so + b->hits_bytes);
   TQ_CUDA(b->scratch.ensure(so));
+  if (pl.count_hits) {
+    TQ_CUDA(b->hits_pin.ensure(b->hits_bytes));
+    b->hits_host = pl.hits_host;
+    unsigned long long* hits = reinterpret_cast<unsigned long long*>(b->scratch.p + b->hits_off);
+    uint32_t* ovf = reinterpret_cast<uint32_t*>(hits + nq1);
+    for (size_t gi = 0; gi < b->groups.size(); ++gi) {
+      tq_batch::TileGroup& run = b->groups[gi];
+      run.count = CountTileParams{run.n_count_units ? st.on_device<const TUnit>(goff[gi].count_units) : nullptr,
+                                  reinterpret_cast<uint2*>(b->tile_dev.p + to_count_cursors), hits, ovf + gi};
+    }
+    b->n_count_units = (uint32_t)cp.units.size();
+    b->n_count_bool_units = (uint32_t)cp.bool_units.size();
+    if (b->n_count_units)
+      b->count_p = CountParams{c->d_lists, st.on_device<const uint32_t>(o_cnt_ids), st.on_device<const CountSeg>(o_cnt_segs),
+                               st.on_device<const Unit>(o_cnt_units), hits};
+    if (b->n_count_bool_units)
+      b->count_bool_p = CountBoolParams{c->d_lists, st.on_device<const uint32_t>(o_cntb_words), st.on_device<const CountBoolSeg>(o_cntb_segs),
+                                        st.on_device<const Unit>(o_cntb_units), hits};
+  } else {
+    b->hits_host.clear();
+    b->n_count_units = b->n_count_bool_units = 0;
+  }
   TQ_CUDA(b->res_pin.ensure(b->res_bytes));
 
   BatchParams& P = b->params;
@@ -1663,6 +1811,8 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
   BatchPlan pl{queries, nq, repeat};
   pl.dq.resize(nq);
   pl.q_cands.assign(nq, 0);
+  for (size_t qi = 0; qi < nq && !repeat && !pl.count_hits; ++qi) pl.count_hits = (queries[qi].flags & TQ_QUERY_COUNT_HITS) != 0;
+  if (pl.count_hits) pl.hits_host.assign(nq, 0);
   // Single-term queries ride along on the tile engine when the batch has multi-term queries whose decoded lists they share
   // (mixed workload: 32.6 K q/s against 28.6 K with them on k_term); a batch of nothing but single-term queries has nothing to
   // share and streams its lists through k_term (configs[0]: 1.39 M q/s against 0.49 M).  TQ_TILE_TERMS: 0 never, 1 always, 2 this rule.
@@ -1703,6 +1853,8 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
   b->stats.tile_postings = pl.tile_postings;
   for (auto& tg : pl.tgroups) b->stats.tile_list_bytes += tg.list_bytes;
   b->stats.tile_scratch_bytes = pl.tile_bytes;
+  b->stats.units_count_hits = (uint64_t)b->n_count_units + b->n_count_bool_units;
+  for (auto& g : b->groups) b->stats.units_count_hits += g.n_count_units;
   guard.ok = true;
   *out = b;
   return TQ_OK;
@@ -1765,6 +1917,7 @@ static int run_phase(tq_batch* b, int phase) {
     if (b->side_pending) { TQ_CUDA(cudaStreamWaitEvent(b->stream, b->ev_side1, 0)); b->side_pending = false; }  // (a run that was abandoned)
     TQ_CUDA(cudaMemcpyAsync(P.qstate, b->dev.p + b->qinit_off, std::max<size_t>(b->nq, 1) * sizeof(QState), cudaMemcpyDeviceToDevice, b->stream));
     if (tiles) TQ_CUDA(cudaMemsetAsync(b->tile_dev.p + b->tile_zero_off, 0, b->tile_zero_bytes, b->stream));
+    if (b->count_hits) TQ_CUDA(cudaMemsetAsync(b->scratch.p + b->hits_off, 0, b->hits_bytes, b->stream));  // every run counts from zero
     TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
     if (b->n_units[UC_TERM]) {
       const int sp = span_begin(b, SPAN_TERM);
@@ -1805,6 +1958,28 @@ static int run_phase(tq_batch* b, int phase) {
         if (g.n_chunks) { k_score_lists<<<g.n_chunks, kThreads, 0, b->stream>>>(P, g.params, 0u); ++launches; }
       span_end(b, sp);
       TQ_CUDA(cudaGetLastError());
+    }
+    if (b->count_hits) {
+      // TQ_QUERY_COUNT_HITS: k_count_tiles reads the scored pairs and tile indexes, which nothing writes after k_score_lists, and
+      // adds to counters of its own -- it runs on the second stream next to the k_tile launches (as k_phrase does); the Count
+      // kernels of the queries on the per-query kernels go with it
+      const bool aside = tiles;
+      cudaStream_t on = aside ? b->side : b->stream;
+      if (aside) {
+        TQ_CUDA(cudaEventRecord(b->ev_side0, b->stream));
+        TQ_CUDA(cudaStreamWaitEvent(b->side, b->ev_side0, 0));
+      }
+      const int sp = span_begin(b, SPAN_COUNT, on);
+      for (auto& g : b->groups)
+        if (g.n_count_units) { k_count_tiles<<<g.n_count_units, kTileThreads, g.count_smem, on>>>(g.params, g.count); ++launches; }
+      if (b->n_count_bool_units) { k_count_bool<<<b->n_count_bool_units, kThreads, 0, on>>>(b->count_bool_p); ++launches; }
+      if (b->n_count_units) { k_count<<<b->n_count_units, kThreads, 0, on>>>(b->count_p); ++launches; }
+      span_end(b, sp, on);
+      TQ_CUDA(cudaGetLastError());
+      if (aside) {
+        TQ_CUDA(cudaEventRecord(b->ev_side1, b->side));
+        b->side_pending = true;
+      }
     }
     b->stats.kernel_launches = 0;
   }
@@ -2022,6 +2197,32 @@ int tq_batch_fetch(tq_batch* b, uint32_t out_stride, float* out_scores, uint32_t
   return TQ_OK;
 }
 
+int tq_batch_fetch_hits(tq_batch* b, uint64_t* out_hits) {
+  if (!b || !b->ran) return fail(TQ_ERR_INVALID_ARGUMENT, "batch has not run");
+  if (!out_hits && b->nq) return fail(TQ_ERR_INVALID_ARGUMENT, "null output");
+  TQ_CUDA(cudaSetDevice(b->ctx->device));
+  { const int rc = finalize_run(b); if (rc != TQ_OK) return rc; }  // (a repeat after a tile overflow does not count: these hits stand)
+  for (uint32_t q = 0; q < b->nq; ++q) out_hits[q] = 0;
+  if (!b->count_hits) return TQ_OK;
+  TQ_CUDA(cudaMemcpyAsync(b->hits_pin.p, b->scratch.p + b->hits_off, b->hits_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  const uint64_t* hits = reinterpret_cast<const uint64_t*>(b->hits_pin.p);
+  const uint32_t* ovf = reinterpret_cast<const uint32_t*>(hits + std::max<uint32_t>(b->nq, 1));
+  for (uint32_t q = 0; q < b->nq; ++q) out_hits[q] = hits[q] + b->hits_host[q];
+  // a group whose tile held more sparse offsets than k_count_tiles keeps: its queries are counted again by the Count kernels
+  for (size_t gi = 0; gi < b->groups.size(); ++gi) {
+    const std::vector<uint32_t>& qs = b->groups[gi].count_queries;
+    if (!ovf[gi] || qs.empty()) continue;
+    std::vector<tq_query> sub(qs.size());
+    std::vector<uint64_t> counts(qs.size());
+    for (size_t i = 0; i < qs.size(); ++i) sub[i] = b->owned.q[qs[i]];
+    const int rc = tq_count_batch(b->ctx, sub.data(), sub.size(), counts.data());
+    if (rc != TQ_OK) return rc;
+    for (size_t i = 0; i < qs.size(); ++i) out_hits[qs[i]] = counts[i];
+  }
+  return TQ_OK;
+}
+
 int tq_search_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint32_t out_stride, float* out_scores, uint32_t* out_segment_ord,
                     uint32_t* out_doc, uint32_t* out_count) {
   tq_batch* b = nullptr;
@@ -2106,12 +2307,7 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
   tq_batch* b = acquire_batch(c);
   if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
   struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
-  std::vector<uint32_t> list_ids;
-  std::vector<CountSeg> segs;
-  std::vector<Unit> units;
-  std::vector<uint32_t> bool_words;  // TQ_OP_BOOL (query, segment) pairs: their structure words with list ids
-  std::vector<CountBoolSeg> bool_segs;
-  std::vector<Unit> bool_units;
+  CountPlan cp;
   {
     std::lock_guard<std::mutex> g(c->mu);
     std::vector<PendingBuild> pending;
@@ -2119,71 +2315,18 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
     uint64_t built = 0;
     std::vector<const tq_term_seg*> order;
     for (size_t qi = 0; qi < nq; ++qi) {
-      const tq_query& q = queries[qi];
-      if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
-      if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_BOOL) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
-      if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
-      if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
-      if (q.op == TQ_OP_BOOL && (!q.term_occur || !q.weight)) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_BOOL needs term_occur and weights");
-      const int rc = for_each_segment(q, order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
-        if (q.op == TQ_OP_BOOL) {  // mixed shapes: the structure of this segment, with list ids in place of the clause indices
-          uint32_t tix_[TQ_MAX_TERMS], dfs_[TQ_MAX_TERMS], ids_[TQ_MAX_TERMS];
-          float ws_[TQ_MAX_TERMS];
-          const Segment* seg = nullptr;
-          for (size_t a = 0; a < n_here; ++a) {
-            int rc = get_list(c, *ts[a], false, pending, &ids_[a], &seg);
-            if (rc != TQ_OK) return rc;
-            tix_[a] = ts[a]->term_idx; dfs_[a] = ts[a]->doc_freq; ws_[a] = q.weight[ts[a]->term_idx];
-          }
-          std::vector<uint16_t> words;
-          bool io_unused;  // (a count adds no scores)
-          const int st = bool_structure(q, tix_, dfs_, ws_, n_here, 0u, words, &io_unused);
-          if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
-          if (st == 0) return TQ_OK;
-          CountBoolSeg bs{};
-          bs.query = (uint32_t)qi; bs.words_base = (uint32_t)bool_words.size(); bs.max_doc = seg->max_doc; bs.alive = seg->d_alive;
-          bool_words.insert(bool_words.end(), words.begin(), words.end());
-          map_bool_clauses(bool_words.data() + bs.words_base, words.size(), [&](uint32_t a) { return ids_[a]; });
-          const uint32_t tiles = (bs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-          for (uint32_t t0 = 0; t0 < tiles; t0 += per) bool_units.push_back(Unit{(uint32_t)bool_segs.size(), t0, std::min(tiles, t0 + per), 0});
-          bool_segs.push_back(bs);
-          return TQ_OK;
-        }
-        if (q.op == TQ_OP_AND && n_here < q.n_terms) return TQ_OK;  // a clause without postings: empty intersection
-        CountSeg cs{};
-        cs.query = (uint32_t)qi; cs.lists_base = (uint32_t)list_ids.size(); cs.n_lists = (uint32_t)n_here; cs.op = (uint32_t)q.op;
-        const Segment* seg = nullptr;
-        uint64_t df_single = 0;
-        for (size_t a = 0; a < n_here; ++a) {
-          uint32_t id;
-          int rc = get_list(c, *ts[a], false, pending, &id, &seg);
-          if (rc != TQ_OK) return rc;
-          list_ids.push_back(id);
-          df_single = ts[a]->doc_freq;
-        }
-        cs.max_doc = seg->max_doc;
-        cs.alive = seg->d_alive;
-        if (n_here == 1 && !seg->d_alive) {  // TermWeight::count without deletes: the term's doc_freq (term_weight.rs:179-190)
-          out_counts[qi] += df_single;
-          list_ids.resize(cs.lists_base);
-        } else {
-          const uint32_t tiles = (cs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-          for (uint32_t t0 = 0; t0 < tiles; t0 += per) units.push_back(Unit{(uint32_t)segs.size(), t0, std::min(tiles, t0 + per), 0});
-          segs.push_back(cs);
-        }
-        return TQ_OK;
-      });
+      const int rc = plan_count(c, queries[qi], (uint32_t)qi, pending, order, cp, &out_counts[qi]);
       if (rc != TQ_OK) return rc;
     }
     int rc = flush_builds(c, pending, &built);
     if (rc != TQ_OK) return rc;
   }
-  if (!bool_units.empty()) {  // mixed boolean shapes: their own kernel, counts added to out_counts
-    const int rc = count_on_device(b, bool_words, bool_segs, bool_units, nq, out_counts, k_count_bool);
+  if (!cp.bool_units.empty()) {  // mixed boolean shapes: their own kernel, counts added to out_counts
+    const int rc = count_on_device(b, cp.bool_words, cp.bool_segs, cp.bool_units, nq, out_counts, k_count_bool);
     if (rc != TQ_OK) return rc;
   }
-  if (units.empty()) return TQ_OK;
-  return count_on_device(b, list_ids, segs, units, nq, out_counts, k_count);
+  if (cp.units.empty()) return TQ_OK;
+  return count_on_device(b, cp.list_ids, cp.segs, cp.units, nq, out_counts, k_count);
 }
 
 // ---- codec-level access ---------------------------------------------------------------------------

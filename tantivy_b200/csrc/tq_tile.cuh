@@ -1134,6 +1134,182 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   }
 }
 
+// ---- Count next to TopDocs -------------------------------------------------------------------------------------------------
+// k_count_tiles: the Count half of (Count, TopDocs) (collector/mod.rs:322-365) for the group's queries that carry
+// TQ_QUERY_COUNT_HITS (TQuery::flags & kTileQueryCount), taken from the pairs k_score_lists has already written -- no list is
+// decoded again.  A CTA walks a range of tiles of one segment; unlike k_tile it skips nothing, so its units cover every tile of the
+// segment's doc range.  Per tile it builds each slot's presence in shared memory: a dense slot (the first n_big) as a 1024-bit map,
+// one bit per pair of its tile-index range (what tile_stage_dense stages, without the scores: no pair buffer, no capacity); a
+// sparse slot as the doc offsets of its few pairs, walked with a cursor as tile_stage_sparse does (the cursors are this kernel's
+// own: k_tile's are in use by the launches next to it).  Then a warp per flagged query evaluates the tile as 32 stripe words, one
+// per lane: a term query or a union ORs its clause words, a conjunction ANDs them, TQ_OP_BOOL ANDs its MUST groups (each the OR of
+// its clauses), keeps the docs that at least `need` SHOULD words list (a bit-sliced counter per lane: <= 32 clauses fit six words)
+// and clears the MUST_NOT words.  And-ed with the alive words (tq_segment_set_doc_range has cleared the docs outside the range in
+// them), popcount, a warp sum; one 64-bit add per (query, CTA).  A tile whose sparse offsets exceed kCountSparseCap sets the
+// group's overflow word: its flagged queries are then recounted by k_count / k_count_bool (tq_batch_fetch_hits).
+constexpr uint8_t kTileQueryCount = 8;      // TQuery::flags bit 3: count the query's hits (k_tile does not read it)
+constexpr uint32_t kCountSparseCap = 8192;  // doc offsets of the sparse slots of one tile held in shared memory
+
+struct CountTileParams {
+  const TUnit* units;            // this group's count units
+  uint2* cursors;                // [CTAs][max_slots] sparse slots' cursors: (first pair not walked yet, its doc)
+  unsigned long long* hits;      // [queries of the batch]
+  uint32_t* overflow;            // this group's word: a tile held more sparse offsets than kCountSparseCap
+};
+
+// Shared memory of a k_count_tiles CTA: presence maps [max_big][32] | sparse slots' start | len << 16 [max_slots] |
+// per-query hit counts [max_queries] | sparse doc offsets (u16) [kCountSparseCap]
+__host__ __device__ constexpr size_t count_tiles_smem_bytes(uint32_t max_slots, uint32_t max_big, uint32_t max_queries) {
+  return (size_t)max_big * 128u + (size_t)max_slots * 4u + (size_t)max_queries * 4u + kCountSparseCap * 2u;
+}
+static_assert(count_tiles_smem_bytes(kTileMaxSlots, kTileMaxBig, kTileMaxQueries) <= 48u * 1024u,
+              "k_count_tiles launches without raising its dynamic shared memory limit");
+
+// Lane `lane`'s stripe word of `slot` in this tile: bit i = the slot lists doc lo + 32 * lane + i.
+__device__ __forceinline__ uint32_t count_word(const uint32_t* bits, const uint32_t* info, const uint16_t* off, uint32_t n_big, uint32_t slot,
+                                               uint32_t lane) {
+  if (slot < n_big) return bits[slot * 32u + lane];
+  const uint32_t in = info[slot];
+  uint32_t w = 0;
+  for (uint32_t i = in & 0xFFFFu, e = i + (in >> 16); i < e; ++i) {
+    const uint32_t o = off[i];
+    if ((o >> 5) == lane) w |= 1u << (o & 31u);
+  }
+  return w;
+}
+
+__global__ void __launch_bounds__(kTileThreads) k_count_tiles(const TileParams TP, const CountTileParams CP) {
+  extern __shared__ __align__(16) unsigned char s_dyn[];
+  __shared__ uint32_t s_total;
+  const TUnit U = CP.units[blockIdx.x];
+  const TSeg G = TP.segs[U.tseg];
+  const TSlot* __restrict__ slots = TP.slots + G.slot_base;
+  uint32_t* bits = reinterpret_cast<uint32_t*>(s_dyn);
+  uint32_t* info = bits + TP.max_big * 32u;
+  uint32_t* cnt = info + TP.max_slots;
+  uint16_t* off = reinterpret_cast<uint16_t*>(cnt + TP.max_queries);
+  uint2* cursor = CP.cursors + (size_t)blockIdx.x * TP.max_slots;
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  for (uint32_t i = tid; i < G.n_queries; i += kTileThreads) cnt[i] = 0u;
+  {  // every sparse slot's cursor on its first pair at or after the unit's first doc
+    const uint32_t lo0 = U.t0 * kTile;
+    for (uint32_t s = G.n_big + tid; s < G.n_slots; s += kTileThreads) {
+      const TSlot sl = slots[s];
+      const uint32_t* __restrict__ d = TP.p_docs + sl.pair_base;
+      uint32_t a = 0, b = sl.doc_freq;
+      while (a < b) {
+        const uint32_t m = (a + b) >> 1;
+        if (__ldg(d + m) < lo0) a = m + 1u; else b = m;
+      }
+      cursor[s] = make_uint2(a, a < sl.doc_freq ? __ldg(d + a) : 0xFFFFFFFFu);
+    }
+  }
+  for (uint32_t t = U.t0; t < U.t1; ++t) {
+    const uint32_t lo = t * kTile, hi = lo + kTile;
+    if (tid == 0) s_total = 0u;
+    for (uint32_t i = tid; i < G.n_big * 32u; i += kTileThreads) bits[i] = 0u;
+    __syncthreads();
+    // dense slots: warp w takes slots w, w + 8, ..., 128 pairs per step
+    for (uint32_t s = warp; s < G.n_big; s += kTileWarps) {
+      const uint32_t a = __ldg(G.tix + (size_t)t * G.n_big + s), e = __ldg(G.tix + (size_t)(t + 1u) * G.n_big + s);
+      const uint32_t* __restrict__ d = TP.p_docs + __ldg(&slots[s].pair_base);
+      for (uint32_t i0 = a; i0 < e; i0 += 128u) {
+        uint32_t dv[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const uint32_t i = i0 + (uint32_t)u * 32u + lane;
+          dv[u] = i < e ? __ldg(d + i) : 0xFFFFFFFFu;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (dv[u] != 0xFFFFFFFFu) {
+            const uint32_t o = dv[u] - lo;
+            atomicOr(&bits[s * 32u + (o >> 5)], 1u << (o & 31u));
+          }
+      }
+    }
+    // sparse slots: a thread walks a slot's cursor through the tile
+    for (uint32_t s = G.n_big + tid; s < G.n_slots; s += kTileThreads) {
+      const uint2 cs = cursor[s];
+      if (cs.y >= hi) { info[s] = 0u; continue; }
+      const TSlot sl = slots[s];
+      const uint32_t* __restrict__ d = TP.p_docs + sl.pair_base;
+      uint32_t n = 1, nd;
+      for (;;) {
+        const uint32_t c = cs.x + n;
+        nd = c < sl.doc_freq ? __ldg(d + c) : 0xFFFFFFFFu;
+        if (nd >= hi) break;
+        ++n;
+      }
+      cursor[s] = make_uint2(cs.x + n, nd);
+      const uint32_t base = atomicAdd(&s_total, n);
+      if (base + n <= kCountSparseCap) {
+        off[base] = (uint16_t)(cs.y - lo);
+        for (uint32_t i = 1; i < n; ++i) off[base + i] = (uint16_t)(__ldg(d + cs.x + i) - lo);
+      }
+      info[s] = (base & 0xFFFFu) | (n << 16);
+    }
+    __syncthreads();
+    if (s_total > kCountSparseCap) {  // the group's flagged queries are recounted without this kernel: nothing more to do here
+      if (tid == 0) atomicOr(CP.overflow, 1u);
+      return;
+    }
+    // lane j's alive word covers docs lo + 32 j .. + 31 (little-endian 64-bit words read as 32-bit halves); no list holds a doc
+    // at or beyond max_doc, so those words are never needed
+    uint32_t live = 0xFFFFFFFFu;
+    if (G.alive) live = lo + lane * 32u < G.max_doc ? __ldg(reinterpret_cast<const uint32_t*>(G.alive) + (lo >> 5) + lane) : 0u;
+    for (uint32_t qi = warp; qi < G.n_queries; qi += kTileWarps) {
+      const TQuery tq = TP.queries[G.query_base + qi];
+      if (!(tq.flags & kTileQueryCount)) continue;
+      const uint16_t* __restrict__ cl = TP.clauses + tq.clause_base;
+      uint32_t m;
+      if (tq.op == kTileOpBool) {
+        const uint32_t ng = cl[0], need = cl[1], ns = cl[2], nn = cl[3];
+        uint32_t w = 4;
+        m = 0xFFFFFFFFu;
+        for (uint32_t g = 0; g < ng; ++g) {
+          const uint32_t glen = cl[w++];
+          uint32_t gm = 0;
+          for (uint32_t e = 0; e < glen; ++e, ++w) gm |= count_word(bits, info, off, G.n_big, cl[w], lane);
+          m &= gm;
+        }
+        if (need && __any_sync(kFull, m)) {
+          uint32_t sc[6] = {0, 0, 0, 0, 0, 0};  // bit-sliced per-doc count of the SHOULD clauses that list the doc
+          for (uint32_t e = 0; e < ns; ++e) {
+            uint32_t carry = count_word(bits, info, off, G.n_big, cl[w + e], lane);
+#pragma unroll
+            for (int b = 0; b < 6; ++b) {
+              const uint32_t c2 = sc[b] & carry;
+              sc[b] ^= carry;
+              carry = c2;
+            }
+          }
+          uint32_t gt = 0, eq = 0xFFFFFFFFu;  // count > need so far / count == need so far, from the top bit down
+#pragma unroll
+          for (int b = 5; b >= 0; --b) {
+            if ((need >> b) & 1u) eq &= sc[b];
+            else { gt |= eq & sc[b]; eq &= ~sc[b]; }
+          }
+          m &= gt | eq;
+        }
+        w += ns;
+        for (uint32_t e = 0; e < nn; ++e) m &= ~count_word(bits, info, off, G.n_big, cl[w + e], lane);
+      } else if (tq.op == kTileOpAnd) {
+        m = 0xFFFFFFFFu;
+        for (uint32_t c = 0; c < tq.n_clauses && __any_sync(kFull, m); ++c) m &= count_word(bits, info, off, G.n_big, cl[c], lane);
+      } else {
+        m = 0;
+        for (uint32_t c = 0; c < tq.n_clauses; ++c) m |= count_word(bits, info, off, G.n_big, cl[c], lane);
+      }
+      const uint32_t n = __reduce_add_sync(kFull, (uint32_t)__popc(m & live));
+      if (lane == 0) cnt[qi] += n;
+    }
+    __syncthreads();
+  }
+  for (uint32_t i = tid; i < G.n_queries; i += kTileThreads)
+    if (cnt[i]) atomicAdd(CP.hits + TP.queries[G.query_base + i].query, (unsigned long long)cnt[i]);
+}
+
 // ---- thresholds from score keys -------------------------------------------------------------------------------------------
 // k-th largest of n u32 keys (4-pass radix select), block-wide; returns 0 when n < k.  `need_out`: how many keys equal to the
 // result are needed on top of the strictly larger ones to make k.

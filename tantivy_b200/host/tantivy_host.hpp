@@ -420,6 +420,41 @@ class Searcher {
     return (size_t)n;
   }
 
+  // searcher.search(&query, &(Count, TopDocs::with_limit(k)))  (the tuple collector, collector/mod.rs:322-365): both halves from
+  // ONE device batch -- the count is taken from the postings the top-k search decodes anyway (TQ_QUERY_COUNT_HITS).
+  std::pair<size_t, std::vector<std::pair<Score, DocAddress>>> search(const Query& query, const std::pair<Count, TopDocs>& collectors) const {
+    const TopDocs& collector = collectors.second;
+    const size_t k = collector.limit() + collector.offset();
+    if (k > TQ_MAX_K) throw TantivyError(TantivyError::InvalidArgument, "limit + offset exceeds TQ_MAX_K");
+    Plan p = plan(query, (uint32_t)k);
+    if (p.matches_nothing) return {0, {}};
+    tq_query q;
+    std::memset(&q, 0, sizeof(q));
+    q.op = p.op; q.n_terms = (uint32_t)p.weight.size(); q.k = (uint32_t)k; q.n_term_segs = (uint32_t)p.term_segs.size();
+    q.term_segs = p.term_segs.data(); q.weight = p.weight.data(); q.avg_fieldnorm = p.avg.data(); q.term_flags = p.flags.data();
+    q.flags = TQ_QUERY_COUNT_HITS;
+    tq_ctx* ctx = device_->ensure(segments_);
+    tq_batch* b = nullptr;
+    auto check = [&](int rc, const char* what) {
+      if (rc == TQ_OK) return;
+      const std::string msg = std::string(what) + ": " + tq_last_error(ctx);
+      if (b) tq_batch_destroy(b);
+      throw TantivyError(TantivyError::SystemError, msg);
+    };
+    std::vector<float> sc(k);
+    std::vector<uint32_t> sg(k), dc(k);
+    uint32_t cnt = 0;
+    uint64_t n_hits = 0;
+    check(tq_batch_prepare(ctx, &q, 1, &b), "tq_batch_prepare");
+    check(tq_batch_run(b), "tq_batch_run");
+    check(tq_batch_fetch(b, (uint32_t)k, sc.data(), sg.data(), dc.data(), &cnt), "tq_batch_fetch");
+    check(tq_batch_fetch_hits(b, &n_hits), "tq_batch_fetch_hits");
+    tq_batch_destroy(b);
+    std::vector<std::pair<Score, DocAddress>> rows;
+    for (size_t r = collector.offset(); r < cnt; ++r) rows.emplace_back(sc[r], DocAddress(sg[r], dc[r]));
+    return {(size_t)n_hits, std::move(rows)};
+  }
+
   // Many queries in one device batch (throughput; single queries are launch-latency bound).
   std::vector<std::vector<std::pair<Score, DocAddress>>> search_batch(const std::vector<const Query*>& queries, const TopDocs& collector) const {
     const size_t k = collector.limit() + collector.offset();

@@ -44,6 +44,7 @@ def _load():
     lib.tq_batch_topkeys_export_dev.argtypes = [vp, vp, C.c_uint32]
     lib.tq_batch_thresholds_from_keys_dev.argtypes = [vp, vp, C.c_uint32, C.c_uint32]
     lib.tq_batch_fetch.argtypes = [vp, C.c_uint32, f32p, u32p, u32p, u32p]
+    lib.tq_batch_fetch_hits.argtypes = [vp, u64p]
     lib.tq_batch_results_dev.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_uint32)]
     lib.tq_batch_results_copy_dev.argtypes = [vp, vp, vp, vp, vp]
     lib.tq_batch_destroy.argtypes = [vp]
@@ -413,6 +414,13 @@ class Batch:
         stride, scores, segs, docs, counts = out or self.qb.alloc_out()
         _check(LIB.tq_batch_fetch(self.h, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p), ptr(counts, u32p)), self.ctx.h)
         return scores, segs, docs, counts
+
+    def fetch_hits(self):
+        """The Count half of (Count, TopDocs): uint64 [nq], the matching alive docs of every query run with count_hits=True
+        (0 for the others).  After a finished run, like fetch."""
+        out = np.zeros(max(self.qb.nq, 1), dtype=np.uint64)
+        _check(LIB.tq_batch_fetch_hits(self.h, ptr(out, u64p)), self.ctx.h)
+        return out[:self.qb.nq]
 
     def results_dev(self):
         s, g, d, c = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
