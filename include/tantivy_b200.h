@@ -121,6 +121,13 @@ typedef struct {
 #define TQ_TERM_IGNORE_FREQ 1u
 #define TQ_QUERY_HAS_THRESHOLD 1u
 #define TQ_QUERY_COUNT_HITS 2u
+/* TQ_QUERY_FILTER: FilterCollector::new(field, predicate, inner) (src/collector/filter_collector_wrapper.rs:160-199) around the
+ * query's TopDocs and Count: only docs that are alive, inside this context's doc range AND set in the bitset registered for
+ * (filter_id, segment) with tq_filter_register reach the collectors (collector/mod.rs:186-221 drops the deleted docs first).
+ * Scores are the unfiltered query's.  Every segment the query names must have a bitset for filter_id, else prepare (and
+ * tq_count_batch) fail with TQ_ERR_NOT_FOUND: a missing filter never reads as "all docs" or "no docs".  filter_id is read only
+ * with this flag.  TQ_OP_PHRASE takes it for TopDocs. */
+#define TQ_QUERY_FILTER 4u
 typedef struct {
   int32_t op;
   uint32_t n_terms;
@@ -147,6 +154,7 @@ typedef struct {
    * MUST clause is a group of its own; ignored for the other Occurs). */
   const uint8_t* term_occur;
   const uint8_t* term_group;
+  uint32_t filter_id; /* TQ_QUERY_FILTER only: the doc filter of tq_filter_register */
 } tq_query;
 
 /* Counters of the last finished batch (per ctx). */
@@ -229,6 +237,21 @@ int tq_segment_unregister(tq_ctx*, uint32_t segment_ord, uint32_t field);
  * narrowed.  Docs outside the range behave like deleted docs (Count included); the tile engine skips their tiles altogether. */
 int tq_segment_set_doc_range(tq_ctx*, uint32_t segment_ord, uint32_t field, uint32_t doc_lo, uint32_t doc_hi);
 
+/* Per-query doc filters (FilterCollector, src/collector/filter_collector_wrapper.rs:160-199; TQ_QUERY_FILTER).  The caller
+ * evaluates its predicate over the segment's fast-field column once -- a doc without a value is rejected, a multi-valued doc is
+ * accepted if any value passes (:160-169) -- into `bits` in the `.del` layout (little-endian 64-bit words, bit set = keep) and
+ * reuses the filter across queries.  One bitset per (filter_id, segment_ord), copied; it applies to every field registered under
+ * that ordinal (a doc filter belongs to the segment, not to a field).  At least one field of the ordinal must be registered
+ * (else TQ_ERR_NOT_FOUND) and len * 8 >= max_doc (else TQ_ERR_INVALID_ARGUMENT); bits at or beyond max_doc are ignored.
+ * Registering a (filter, segment) again replaces its bitset.  The context keeps alive AND doc range AND filter per (filter,
+ * segment, field) on the device, built when a query first uses it, and the 1024-doc tiles it leaves non-empty: the tile engine
+ * visits only those.  tq_filter_register of a filter, and tq_filter_unregister, return TQ_ERR_INVALID_ARGUMENT while a prepared
+ * batch that names the filter has not been destroyed (tq_batch_destroy).  Unregistering the last field of a segment ordinal
+ * drops the ordinal's filter bitsets: a reused ordinal never inherits an old filter. */
+int tq_filter_register(tq_ctx*, uint32_t filter_id, uint32_t segment_ord, const uint8_t* bits, size_t len);
+/* Frees every bitset of the filter; TQ_ERR_NOT_FOUND if none is registered. */
+int tq_filter_unregister(tq_ctx*, uint32_t filter_id);
+
 /* ---- search -------------------------------------------------------------------------- */
 /* The whole hot path for a batch of queries, host buffers in / host buffers out:
  * block decode -> AND/OR/term -> BM25 -> per-segment top-k -> merge_fruits.
@@ -242,7 +265,8 @@ int tq_search_batch(tq_ctx*, const tq_query* queries, size_t nq, uint32_t out_st
 /* The Count collector for term / AND / OR / mixed boolean (TQ_OP_BOOL) queries (src/collector/count_collector.rs;
  * Weight::count, term_weight.rs:179-219): out_counts[q] = number of ALIVE docs matching query q over all its segments.
  * k and thresholds of the queries are ignored (TQ_OP_BOOL reads the weights: they order the clauses).  A term query on a
- * segment without deletes is answered from doc_freq, as the reference does. */
+ * segment without deletes is answered from doc_freq, as the reference does -- unless it carries TQ_QUERY_FILTER (Count inside
+ * FilterCollector): then only the docs its filter keeps are counted, over the 8192-doc tiles the filter leaves non-empty. */
 int tq_count_batch(tq_ctx*, const tq_query* queries, size_t nq, uint64_t* out_counts);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
@@ -335,6 +359,11 @@ int tq_multi_segment_register_split(tq_multi*, uint32_t segment_ord, uint32_t fi
 int tq_multi_search_batch(tq_multi*, const tq_query* queries, size_t nq, uint32_t out_stride,
                           float* out_scores, uint32_t* out_segment_ord, uint32_t* out_doc,
                           uint32_t* out_count);
+/* tq_filter_register on every device that holds a field of segment_ord (all of them for a split segment: each device's doc range
+ * does the rest); TQ_ERR_NOT_FOUND if none does.  Refused on all devices if a prepared batch on any of them names the filter. */
+int tq_multi_filter_register(tq_multi*, uint32_t filter_id, uint32_t segment_ord, const uint8_t* bits, size_t len);
+/* tq_filter_unregister on every device that has the filter; TQ_ERR_NOT_FOUND if none has it. */
+int tq_multi_filter_unregister(tq_multi*, uint32_t filter_id);
 
 /* ---- codec-level access (parity tests and the decode micro-benchmark) ----------------- */
 /* Decodes one whole posting list on the device (BlockSegmentPostings::open + advance loop,

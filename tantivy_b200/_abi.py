@@ -17,6 +17,7 @@ TQ_MAX_TERMS = 32
 TQ_TERM_IGNORE_FREQ = 1
 TQ_QUERY_HAS_THRESHOLD = 1
 TQ_QUERY_COUNT_HITS = 2
+TQ_QUERY_FILTER = 4
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -71,16 +72,20 @@ class Query(C.Structure):
         ("min_should_match", C.c_uint32),
         ("term_occur", u8p),
         ("term_group", u8p),
+        ("filter_id", C.c_uint32),
     ]
 
 
-QUERY_DTYPE = np.dtype(
+_QUERY_FIELDS = np.dtype(
     [("op", "<i4"), ("n_terms", "<u4"), ("k", "<u4"), ("n_term_segs", "<u4"),
      ("term_segs", "<u8"), ("weight", "<u8"), ("avg_fieldnorm", "<u8"), ("tf_cache", "<u8"), ("term_flags", "<u8"),
      ("flags", "<u4"), ("threshold", "<f4"), ("term_pos", "<u8"), ("term_offset", "<u8"), ("slop", "<u4"), ("min_should_match", "<u4"),
-     ("term_occur", "<u8"), ("term_group", "<u8")]
+     ("term_occur", "<u8"), ("term_group", "<u8"), ("filter_id", "<u4")]
 )
-assert QUERY_DTYPE.itemsize == C.sizeof(Query) == 104
+# (the C struct ends in 4 bytes of padding: it is 8-byte aligned)
+QUERY_DTYPE = np.dtype({"names": list(_QUERY_FIELDS.names), "formats": [_QUERY_FIELDS.fields[n][0] for n in _QUERY_FIELDS.names],
+                        "offsets": [_QUERY_FIELDS.fields[n][1] for n in _QUERY_FIELDS.names], "itemsize": C.sizeof(Query)})
+assert QUERY_DTYPE.itemsize == C.sizeof(Query) == 112
 
 
 class Stats(C.Structure):
@@ -148,7 +153,9 @@ class QueryBatch:
       phrase queries (op TQ_OP_PHRASE): term_pos = list of (positions_start, positions_end) parallel to term_segs,
       term_offset = [n_terms] offsets in the phrase, slop (optional, must be 0 on the device path);
       boolean queries (op TQ_OP_BOOL): term_occur = [n_terms] TQ_OCCUR_*, term_group = optional [n_terms] group ids of the MUST
-      clauses, min_should_match (optional).
+      clauses, min_should_match (optional);
+      filter (optional int id of a doc filter registered with Context.filter_register: FilterCollector around the query's
+      TopDocs and Count; sets TQ_QUERY_FILTER).
     Built with numpy so that a batch of thousands of queries marshals in milliseconds.
     """
 
@@ -199,6 +206,12 @@ class QueryBatch:
                 row["threshold"] = q["threshold"]
             if q.get("count_hits"):
                 row["flags"] |= TQ_QUERY_COUNT_HITS
+            filt = q.get("filter")
+            if filt is not None:
+                if isinstance(filt, (bool, np.bool_)) or not isinstance(filt, (int, np.integer)) or not 0 <= int(filt) < 1 << 32:
+                    raise ValueError(f"query {i}: filter must be a filter id in 0 .. 2**32 - 1, got {filt!r}")
+                row["flags"] |= TQ_QUERY_FILTER
+                row["filter_id"] = int(filt)
             tpos = q.get("term_pos")
             if tpos is not None:
                 tp = np.zeros(max(len(tpos), 1), dtype=TERM_POS_DTYPE)

@@ -15,6 +15,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -156,6 +157,20 @@ struct Segment {
   size_t pos_pool_cap = 0;        // (the first 8 bytes of the pool are the cursor)
 };
 
+// A run of tiles [t0, t1) that a filtered query visits.
+struct TileRun { uint32_t t0, t1; };
+
+// What a filtered query (TQ_QUERY_FILTER) reads of one (filter, segment, field): alive AND doc range AND filter on the device
+// (k_filter_combine, padded like the alive copy: k_count and the BOOL path read whole 32-bit words), and the tiles it leaves
+// non-empty, from the host bits and the doc range: runs of 1024-doc tiles of the tile engine (gaps of up to kRunGap empty tiles
+// merged, since every unit pays a cursor prologue) and of the Count kernels' 8192-doc tiles.  Built at first use, rebuilt by
+// tq_segment_set_doc_range, dropped with the segment or the filter.
+struct FilterView {
+  uint8_t* d_bits = nullptr;
+  std::vector<TileRun> runs, count_runs;
+};
+constexpr uint32_t kRunGap = 4;
+
 uint32_t env_u32(const char* name, uint32_t def) {
   const char* v = getenv(name);
   if (!v || !*v) return def;
@@ -177,6 +192,9 @@ struct tq_ctx {
   std::unordered_map<PosKey, uint32_t, PosKeyHash> pos_cache;  // (segment, field, postings_start, positions_start) -> pos id
   std::vector<uint32_t> free_pos_ids;
   std::map<std::pair<uint32_t, uint32_t>, uint32_t> seg_users;  // (segment, field) -> prepared batches not yet destroyed that name it
+  std::map<std::pair<uint32_t, uint32_t>, std::vector<uint8_t>> filters;  // (filter_id, segment_ord) -> the caller's bits, ceil(max_doc / 8) bytes
+  std::map<std::tuple<uint32_t, uint32_t, uint32_t>, FilterView> filter_views;  // (filter_id, segment_ord, field)
+  std::map<uint32_t, uint32_t> filter_users;  // filter_id -> prepared batches not yet destroyed that name it
   cudaStream_t build_stream = nullptr;
   PinBuf build_pin;
   DevBuf build_dev;
@@ -310,6 +328,7 @@ struct tq_batch {
   std::vector<uint64_t> hits_host;
   PinBuf hits_pin;
   std::vector<std::pair<uint32_t, uint32_t>> held;  // the (segment, field)s its queries name, counted in tq_ctx::seg_users until destroyed
+  std::vector<uint32_t> held_filters;               // the filters its queries name, counted in tq_ctx::filter_users until destroyed
 };
 
 #define TQ_CUDA(expr)                                                                         \
@@ -329,6 +348,87 @@ static uint32_t host_score_key(float f) {
   f += 0.0f;
   memcpy(&u, &f, 4);
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
+}
+
+// ---- per-query doc filters (TQ_QUERY_FILTER) -----------------------------------------------------------------------------------
+// Is any bit of docs [a, b) set?
+static bool any_bit(const uint8_t* bits, uint64_t a, uint64_t b) {
+  for (; a < b && (a & 7u); ++a) if ((bits[a >> 3] >> (a & 7u)) & 1u) return true;
+  for (; a + 64 <= b; a += 64) { uint64_t w; memcpy(&w, bits + (a >> 3), 8); if (w) return true; }
+  for (; a + 8 <= b; a += 8) if (bits[a >> 3]) return true;
+  for (; a < b; ++a) if ((bits[a >> 3] >> (a & 7u)) & 1u) return true;
+  return false;
+}
+
+// The `tile`-doc tiles of the docs [lo, hi) that hold a set bit, as runs; runs at most `gap` empty tiles apart are merged.
+static std::vector<TileRun> tile_runs(const uint8_t* bits, uint32_t lo, uint32_t hi, uint32_t tile, uint32_t gap) {
+  std::vector<TileRun> runs;
+  if (lo >= hi) return runs;
+  const uint32_t t_lo = lo / tile, t_hi = (uint32_t)(((uint64_t)hi + tile - 1) / tile);
+  for (uint32_t t = t_lo; t < t_hi; ++t) {
+    const uint64_t a = std::max<uint64_t>(lo, (uint64_t)t * tile), b = std::min<uint64_t>(hi, (uint64_t)(t + 1) * tile);
+    if (!any_bit(bits, a, b)) continue;
+    if (!runs.empty() && t - runs.back().t1 <= gap) runs.back().t1 = t + 1;
+    else runs.push_back(TileRun{t, t + 1});
+  }
+  return runs;
+}
+
+// (Re)builds the view of one (filter, segment, field) from the filter's host bits, the segment's alive bitset and its doc range.
+// ctx->mu held; nothing on the device reads the view meanwhile (a first build, or tq_segment_set_doc_range after its device sync).
+static int build_view(tq_ctx* c, const Segment& s, const std::vector<uint8_t>& bits, FilterView& v) {
+  const size_t nbytes = ((size_t)s.max_doc + 7) / 8, padded = ((nbytes + 7) & ~(size_t)7) + 8;
+  const uint32_t n_words = (uint32_t)(((uint64_t)s.max_doc + 31) / 32);
+  if (!v.d_bits) TQ_CUDA(cudaMalloc(&v.d_bits, padded));
+  TQ_CUDA(c->build_dev.ensure(padded));
+  TQ_CUDA(cudaMemsetAsync(c->build_dev.p, 0, padded, c->build_stream));
+  if (nbytes) TQ_CUDA(cudaMemcpyAsync(c->build_dev.p, bits.data(), std::min(nbytes, bits.size()), cudaMemcpyHostToDevice, c->build_stream));
+  TQ_CUDA(cudaMemsetAsync(v.d_bits, 0, padded, c->build_stream));
+  if (n_words)
+    k_filter_combine<<<(n_words + 255) / 256, 256, 0, c->build_stream>>>(reinterpret_cast<const uint32_t*>(s.d_alive), reinterpret_cast<const uint32_t*>(c->build_dev.p),
+                                                                         n_words, s.doc_lo, s.doc_hi, reinterpret_cast<uint32_t*>(v.d_bits));
+  TQ_CUDA(cudaGetLastError());
+  TQ_CUDA(cudaStreamSynchronize(c->build_stream));
+  v.runs = tile_runs(bits.data(), s.doc_lo, s.doc_hi, kTile, kRunGap);
+  v.count_runs = tile_runs(bits.data(), s.doc_lo, s.doc_hi, kTileDocs, 0);
+  return TQ_OK;
+}
+
+// Every segment a filtered query names has a bitset for its filter.  ctx->mu held.
+static int check_filter(const tq_ctx* c, const tq_query& q) {
+  if (!(q.flags & TQ_QUERY_FILTER)) return TQ_OK;
+  for (uint32_t i = 0; i < q.n_term_segs; ++i)
+    if (!c->filters.count({q.filter_id, q.term_segs[i].segment_ord}))
+      return fail(TQ_ERR_NOT_FOUND, "a filtered query names a segment without a bitset for its filter (tq_filter_register)");
+  return TQ_OK;
+}
+
+// The docs query q may collect in segment s: its alive bitset, or for a filtered query the (filter, segment, field) view, built at
+// first use.  *view: null for an unfiltered query.  ctx->mu held.
+static int query_alive(tq_ctx* c, const tq_query& q, const Segment& s, const uint8_t** alive, const FilterView** view) {
+  *view = nullptr;
+  *alive = s.d_alive;
+  if (!(q.flags & TQ_QUERY_FILTER)) return TQ_OK;
+  auto fit = c->filters.find({q.filter_id, s.segment_ord});
+  if (fit == c->filters.end()) return fail(TQ_ERR_NOT_FOUND, "a filtered query names a segment without a bitset for its filter (tq_filter_register)");
+  const auto key = std::make_tuple(q.filter_id, s.segment_ord, s.field);
+  auto it = c->filter_views.find(key);
+  if (it == c->filter_views.end()) {
+    FilterView v;
+    const int rc = build_view(c, s, fit->second, v);
+    if (rc != TQ_OK) { cudaFree(v.d_bits); return rc; }
+    it = c->filter_views.emplace(key, std::move(v)).first;
+  }
+  *view = &it->second;
+  *alive = it->second.d_bits;
+  return TQ_OK;
+}
+
+// Frees the views whose (filter_id, segment_ord, field) satisfies pred.  ctx->mu held, the device idle.
+template <class Pred>
+static void drop_views(tq_ctx* c, Pred pred) {
+  for (auto it = c->filter_views.begin(); it != c->filter_views.end();)
+    if (pred(it->first)) { cudaFree(it->second.d_bits); it = c->filter_views.erase(it); } else ++it;
 }
 
 extern "C" {
@@ -427,6 +527,7 @@ void tq_ctx_destroy(tq_ctx* c) {
     cudaFree(kv.second.d_pos); cudaFree(kv.second.d_pos_pool);
     kv.second.arena.release();
   }
+  for (auto& kv : c->filter_views) cudaFree(kv.second.d_bits);
   cudaFree(c->d_pos_descs);
   c->build_pin.release(); c->build_dev.release();
   if (c->build_stream) cudaStreamDestroy(c->build_stream);
@@ -563,6 +664,11 @@ int tq_segment_set_doc_range(tq_ctx* c, uint32_t segment_ord, uint32_t field, ui
   if (e == cudaSuccess) e = clear_bits(doc_hi, s.doc_hi);
   if (e != cudaSuccess) return fail(TQ_ERR_CUDA, std::string("doc range: ") + cudaGetErrorString(e));
   s.doc_lo = doc_lo; s.doc_hi = doc_hi;
+  for (auto& kv : c->filter_views)  // the segment's filter views follow the new range (in place: prepared batches keep their pointers)
+    if (std::get<1>(kv.first) == segment_ord && std::get<2>(kv.first) == field) {
+      const int rc = build_view(c, s, c->filters.at({std::get<0>(kv.first), segment_ord}), kv.second);
+      if (rc != TQ_OK) return rc;
+    }
   return TQ_OK;
 }
 
@@ -582,6 +688,46 @@ int tq_segment_unregister(tq_ctx* c, uint32_t segment_ord, uint32_t field) {
   c->segments.erase(it);
   for (auto li = c->list_cache.begin(); li != c->list_cache.end();)
     if (li->first.segment_ord == segment_ord && li->first.field == field) { c->free_ids.push_back(li->second); li = c->list_cache.erase(li); } else ++li;  // ... and their ids are reused
+  drop_views(c, [&](const std::tuple<uint32_t, uint32_t, uint32_t>& k) { return std::get<1>(k) == segment_ord && std::get<2>(k) == field; });
+  auto rest = c->segments.lower_bound({segment_ord, 0u});
+  if (rest == c->segments.end() || rest->first.first != segment_ord)  // the ordinal's last field: its filters go too (a reused ordinal starts clean)
+    for (auto fi = c->filters.begin(); fi != c->filters.end();)
+      if (fi->first.second == segment_ord) fi = c->filters.erase(fi); else ++fi;
+  return TQ_OK;
+}
+
+int tq_filter_register(tq_ctx* c, uint32_t filter_id, uint32_t segment_ord, const uint8_t* bits, size_t len) {
+  if (!c || (!bits && len)) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  std::lock_guard<std::mutex> g(c->mu);
+  uint32_t max_doc = 0;
+  bool any = false;
+  for (auto it = c->segments.lower_bound({segment_ord, 0u}); it != c->segments.end() && it->first.first == segment_ord; ++it) {
+    any = true;
+    max_doc = std::max(max_doc, it->second.max_doc);
+  }
+  if (!any) return fail(TQ_ERR_NOT_FOUND, "no field of the segment ordinal is registered");
+  if (len * 8 < max_doc) return fail(TQ_ERR_INVALID_ARGUMENT, "filter bitset shorter than max_doc");
+  if (c->filter_users.count(filter_id)) return fail(TQ_ERR_INVALID_ARGUMENT, "a prepared batch still uses the filter");
+  const size_t nbytes = ((size_t)max_doc + 7) / 8;
+  std::vector<uint8_t> copy(bits, bits + nbytes);
+  if (max_doc & 7u) copy.back() &= (uint8_t)((1u << (max_doc & 7u)) - 1u);  // bits at and beyond max_doc are ignored
+  cudaDeviceSynchronize();
+  drop_views(c, [&](const std::tuple<uint32_t, uint32_t, uint32_t>& k) { return std::get<0>(k) == filter_id && std::get<1>(k) == segment_ord; });
+  c->filters[{filter_id, segment_ord}] = std::move(copy);
+  return TQ_OK;
+}
+
+int tq_filter_unregister(tq_ctx* c, uint32_t filter_id) {
+  if (!c) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  std::lock_guard<std::mutex> g(c->mu);
+  if (c->filter_users.count(filter_id)) return fail(TQ_ERR_INVALID_ARGUMENT, "a prepared batch still uses the filter");
+  auto first = c->filters.lower_bound({filter_id, 0u});
+  if (first == c->filters.end() || first->first.first != filter_id) return fail(TQ_ERR_NOT_FOUND, "filter not registered");
+  cudaDeviceSynchronize();
+  drop_views(c, [&](const std::tuple<uint32_t, uint32_t, uint32_t>& k) { return std::get<0>(k) == filter_id; });
+  while (first != c->filters.end() && first->first.first == filter_id) first = c->filters.erase(first);
   return TQ_OK;
 }
 
@@ -863,6 +1009,8 @@ struct SegPlan {
   std::vector<uint16_t> bool_words;  // TQ_OP_BOOL: [n_groups, need_should, n_should, n_not, (len, clauses..) per group, shoulds.., nots..],
                                      // clauses as indices into `here` (tile_admit turns them into slots)
   const uint8_t* fn0 = nullptr;
+  const uint8_t* alive = nullptr;      // the docs the query may collect here: the segment's alive bitset, or its filter view's
+  const FilterView* view = nullptr;    // TQ_QUERY_FILTER: the view (its non-empty tiles)
   uint32_t no_freq = 0;  // bit a: the a-th clause in arrival order does not read freqs (Basic field or TQ_TERM_IGNORE_FREQ)
   // AND / BOOL: the MUST scorers add up as Intersection::score does, (s0 + s1) + (s2 + s3 + ...), instead of one after another
   // as in block_wand_intersection (oracle/query.hpp, for_each_intersection, says when the reference takes which)
@@ -875,6 +1023,7 @@ struct TileGroupBuild {
     uint32_t segment_ord = 0, max_doc = 0;
     uint32_t t_lo = 0, t_hi = 0;  // tiles that overlap the segment's doc range (tq_segment_set_doc_range)
     const uint8_t* alive = nullptr;
+    const FilterView* view = nullptr;  // the group's filter (one per group): its launches visit only the view's tile runs
     std::vector<TSlot> slots;  // (TSlot::pad chains the slots of one list: several weights / tables of a list are rare)
     std::vector<TQuery> queries;
     std::vector<uint16_t> clauses;
@@ -952,6 +1101,7 @@ struct BatchPlan {
   uint32_t strip_cached_max = 0, phrase_ct = 2;
   // tile engine
   std::vector<TileGroupBuild> tgroups;
+  std::unordered_map<uint64_t, size_t> open_group;  // filter key (0: none, 1 << 32 | filter_id) -> the group that takes its next queries
   std::vector<GroupStage> gstage;  // parallel to tgroups
   uint64_t tile_pairs_total = 0, pair_cursor = 0, tile_postings = 0, tile_units = 0;
   size_t tix_total_words = 0, tile_bytes = 0;
@@ -1087,7 +1237,8 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, bool count, const
       g.segs.emplace_back();
       g.segs.back().segment_ord = sp.segment_ord;
       g.segs.back().max_doc = sp.seg->max_doc;
-      g.segs.back().alive = sp.seg->d_alive;
+      g.segs.back().alive = sp.alive;
+      g.segs.back().view = sp.view;
       g.segs.back().t_lo = sp.seg->doc_lo / kTile;
       g.segs.back().t_hi = (uint32_t)(((uint64_t)sp.seg->doc_hi + kTile - 1) / kTile);
     }
@@ -1211,6 +1362,9 @@ int plan_segments(tq_ctx* c, BatchPlan& pl, const tq_query& q, int op, const uin
       pl.postings += t.doc_freq;
       *q_postings += t.doc_freq;
     }
+    const int frc = query_alive(c, q, *sp.seg, &sp.alive, &sp.view);
+    if (frc != TQ_OK) return frc;
+    if (sp.view && sp.view->runs.empty()) { --pl.n_plans; return TQ_OK; }  // the filter keeps no doc of this segment's range
     auto by_doc_freq = [](const SegPlan::Clause& a, const SegPlan::Clause& b) { return a.first < b.first; };
     if (is_phrase) {
       // PhraseScorer keeps its terms by ascending size_hint (intersection.rs:40-52); every clause carries
@@ -1254,19 +1408,26 @@ bool route_to_tile(const tq_ctx* c, BatchPlan& pl, size_t qi, int op, uint64_t q
                                  : c->tile != 0 && (((c->tile_ops >> op) & 1u) || op == TQ_OP_BOOL) && (op != TQ_OP_TERM || pl.terms_on_tile);
   if (!to_tile || !pl.n_plans) return false;
   std::vector<TileGroupBuild>& tg = pl.tgroups;
-  if (tg.empty() || (pl.repeat == 2 && !tg.back().segs.empty())) tg.emplace_back();
+  // a group holds the queries of one filter (or of none): its segments' alive words are that filter's views
+  const uint64_t fkey = (q.flags & TQ_QUERY_FILTER) ? (1ull << 32 | q.filter_id) : 0ull;
+  auto open = pl.open_group.find(fkey);
+  if (open == pl.open_group.end() || (pl.repeat == 2 && !tg[open->second].segs.empty())) {
+    tg.emplace_back();
+    open = pl.open_group.insert_or_assign(fkey, tg.size() - 1).first;
+  }
   // wide unions: every query brings its clause words, work-list entries and (mostly distinct) lists into the CTA's shared
   // memory; smaller groups keep two CTAs per SM (configs[4]: 1.64 s -> 1.05 s per 512 20-term queries on 500M docs)
   const uint32_t max_q = q.n_terms > 8 ? std::min(c->tile_max_queries, c->tile_wide_queries) : c->tile_max_queries;
   const SegPlan* plans = pl.plans.data();
-  bool fits = tile_fits(c, tg.back(), plans, pl.n_plans, max_q, false) || tile_fits(c, tg.back(), plans, pl.n_plans, max_q, true);
-  if (!fits && !tg.back().segs.empty() && tile_fits(c, TileGroupBuild{}, plans, pl.n_plans, max_q, false)) {  // the current group is full: open the next one
+  bool fits = tile_fits(c, tg[open->second], plans, pl.n_plans, max_q, false) || tile_fits(c, tg[open->second], plans, pl.n_plans, max_q, true);
+  if (!fits && !tg[open->second].segs.empty() && tile_fits(c, TileGroupBuild{}, plans, pl.n_plans, max_q, false)) {  // the current group is full: open the next one
     tg.emplace_back();
+    open->second = tg.size() - 1;
     fits = true;
   }
   const uint64_t tile_pair_budget = (uint64_t)c->tile_scratch_mb * (1u << 20) / 8u;
   if (!fits || pl.tile_pairs_total + q_postings + 128ull * pl.n_plans * q.n_terms > tile_pair_budget) return false;
-  pl.tile_pairs_total += tile_admit(tg.back(), (uint32_t)qi, op, pl.count_hits && (q.flags & TQ_QUERY_COUNT_HITS), plans, pl.n_plans);
+  pl.tile_pairs_total += tile_admit(tg[open->second], (uint32_t)qi, op, pl.count_hits && (q.flags & TQ_QUERY_COUNT_HITS), plans, pl.n_plans);
   // every doc at or above the running threshold is handed over: the sample launch and the k_theta passes keep that
   // near k; a query that still overflows has the run repeated (flags[1], finalize_run).  A query hands each doc over at
   // most once (every tile once per run, a doc once per (query, tile): by its first posting in the driving clauses), so
@@ -1289,7 +1450,7 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
     qs.lists_base = (uint32_t)pl.qlists.size();
     qs.segment_ord = sp.segment_ord;
     qs.max_doc = sp.seg->max_doc;
-    qs.alive = sp.seg->d_alive;
+    qs.alive = sp.alive;
     qs.fieldnorm = sp.uniform_fn ? sp.fn0 : nullptr;
     const bool prunable = sp.prunable && op != TQ_OP_TERM;
     qs.flags = (sp.uniform_fn ? 1u : 0u) | (prunable ? 2u : 0u) | (sp.intersection_order ? 4u : 0u);
@@ -1333,6 +1494,18 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
   if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
   if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
   if (q.op == TQ_OP_BOOL && (!q.term_occur || !q.weight)) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_BOOL needs term_occur and weights");
+  const int frc = check_filter(c, q);
+  if (frc != TQ_OK) return frc;
+  // units of 8 tiles of 8192 docs over the segment; a filtered query's only over the tiles its filter view leaves non-empty
+  auto cut = [](std::vector<Unit>& units, uint32_t seg_idx, uint32_t max_doc, const FilterView* view) {
+    const uint32_t tiles = (max_doc + kTileDocs - 1) / kTileDocs, per = 8;
+    if (!view) {
+      for (uint32_t t0 = 0; t0 < tiles; t0 += per) units.push_back(Unit{seg_idx, t0, std::min(tiles, t0 + per), 0});
+      return;
+    }
+    for (const TileRun& r : view->count_runs)
+      for (uint32_t t0 = r.t0; t0 < r.t1; t0 += per) units.push_back(Unit{seg_idx, t0, std::min(r.t1, t0 + per), 0});
+  };
   return for_each_segment(q, order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
     if (q.op == TQ_OP_BOOL) {  // mixed shapes: the structure of this segment, with list ids in place of the clause indices
       uint32_t tix_[TQ_MAX_TERMS], dfs_[TQ_MAX_TERMS], ids_[TQ_MAX_TERMS];
@@ -1349,11 +1522,13 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
       if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
       if (st == 0) return TQ_OK;
       CountBoolSeg bs{};
-      bs.query = qi; bs.words_base = (uint32_t)cp.bool_words.size(); bs.max_doc = seg->max_doc; bs.alive = seg->d_alive;
+      const FilterView* view = nullptr;
+      const int arc = query_alive(c, q, *seg, &bs.alive, &view);
+      if (arc != TQ_OK) return arc;
+      bs.query = qi; bs.words_base = (uint32_t)cp.bool_words.size(); bs.max_doc = seg->max_doc;
       cp.bool_words.insert(cp.bool_words.end(), words.begin(), words.end());
       map_bool_clauses(cp.bool_words.data() + bs.words_base, words.size(), [&](uint32_t a) { return ids_[a]; });
-      const uint32_t tiles = (bs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-      for (uint32_t t0 = 0; t0 < tiles; t0 += per) cp.bool_units.push_back(Unit{(uint32_t)cp.bool_segs.size(), t0, std::min(tiles, t0 + per), 0});
+      cut(cp.bool_units, (uint32_t)cp.bool_segs.size(), bs.max_doc, view);
       cp.bool_segs.push_back(bs);
       return TQ_OK;
     }
@@ -1370,13 +1545,14 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
       df_single = ts[a]->doc_freq;
     }
     cs.max_doc = seg->max_doc;
-    cs.alive = seg->d_alive;
-    if (n_here == 1 && !seg->d_alive) {  // TermWeight::count without deletes: the term's doc_freq (term_weight.rs:179-190)
+    const FilterView* view = nullptr;
+    const int arc = query_alive(c, q, *seg, &cs.alive, &view);
+    if (arc != TQ_OK) return arc;
+    if (n_here == 1 && !cs.alive) {  // TermWeight::count without deletes (nor a filter): the term's doc_freq (term_weight.rs:179-190)
       *host_add += df_single;
       cp.list_ids.resize(cs.lists_base);
     } else {
-      const uint32_t tiles = (cs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-      for (uint32_t t0 = 0; t0 < tiles; t0 += per) cp.units.push_back(Unit{(uint32_t)cp.segs.size(), t0, std::min(tiles, t0 + per), 0});
+      cut(cp.units, (uint32_t)cp.segs.size(), cs.max_doc, view);
       cp.segs.push_back(cs);
     }
     return TQ_OK;
@@ -1387,6 +1563,7 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
 int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi) {
   const tq_query& q = pl.queries[qi];
   int rc = validate_query(c, q);
+  if (rc == TQ_OK) rc = check_filter(c, q);
   if (rc != TQ_OK) return rc;
   const bool count = pl.count_hits && (q.flags & TQ_QUERY_COUNT_HITS);
   if (count && q.op == TQ_OP_PHRASE) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_QUERY_COUNT_HITS: Count of a phrase query is not on the device path");
@@ -1453,6 +1630,36 @@ int cut_units(const tq_ctx* c, BatchPlan& pl) {
   return TQ_OK;
 }
 
+// The tiles a group's launches visit in one of its segments: its whole doc range, or the runs its filter view leaves non-empty.
+std::vector<TileRun> seg_runs(const TileGroupBuild::SegB& sb) {
+  if (sb.view) return sb.view->runs;
+  if (sb.t_hi > sb.t_lo) return {TileRun{sb.t_lo, sb.t_hi}};
+  return {};
+}
+uint64_t run_tiles(const std::vector<TileRun>& runs) {
+  uint64_t n = 0;
+  for (const TileRun& r : runs) n += r.t1 - r.t0;
+  return n;
+}
+// Units of at most `per` tiles over the tiles [v0, v1) of `runs` taken one after another; no unit spans two runs.
+void push_run_units(std::vector<TUnit>& out, uint32_t si, const std::vector<TileRun>& runs, uint64_t v0, uint64_t v1, uint32_t per) {
+  uint64_t base = 0;
+  for (const TileRun& r : runs) {
+    const uint64_t len = r.t1 - r.t0, lo = std::max(v0, base), hi = std::min(v1, base + len);
+    for (uint64_t a = lo; a < hi; a += per) out.push_back(TUnit{si, (uint32_t)(r.t0 + (a - base)), (uint32_t)(r.t0 + (std::min(hi, a + per) - base)), 0});
+    base += len;
+    if (base >= v1) break;
+  }
+}
+// Tile v of `runs` taken one after another (v < run_tiles(runs)), with the end of its run.
+TileRun run_tile(const std::vector<TileRun>& runs, uint64_t v) {
+  for (const TileRun& r : runs) {
+    if (v < r.t1 - r.t0) return TileRun{(uint32_t)(r.t0 + v), r.t1};
+    v -= r.t1 - r.t0;
+  }
+  return TileRun{runs.back().t1 - 1, runs.back().t1};
+}
+
 // Tile groups: slot order, pair bases, score chunks, tile ranges of the launches.
 int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
   pl.gstage.resize(pl.tgroups.size());
@@ -1464,7 +1671,12 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
     uint64_t tiles_total = 0;
     uint32_t kmax_g = 1;
     uint64_t group_tiles = 0;
-    for (auto& sb : tg.segs) group_tiles += sb.t_hi - sb.t_lo;
+    // the launches cover only these tiles; tiles_total and the sample spread count them alone, so a sparse filter still gets its samples
+    std::vector<std::vector<TileRun>> runs(tg.segs.size());
+    for (size_t si = 0; si < tg.segs.size(); ++si) {
+      runs[si] = seg_runs(tg.segs[si]);
+      group_tiles += run_tiles(runs[si]);
+    }
     const uint32_t count_per = (uint32_t)std::max<uint64_t>(8u, (group_tiles + 1023u) / 1024u);
     for (auto& sb : tg.segs) {
       // dense lists first (they get a tile index and whole warps), then the rest; clause ordinals follow the permutation
@@ -1522,15 +1734,14 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         count_seg = true;
         gs.count_queries.push_back(tq.query);
       }
-      if (count_seg) {  // k_count_tiles skips nothing: every tile of the doc range, about 1024 CTAs per group over all its segments
-        for (uint32_t t0 = sb.t_lo; t0 < sb.t_hi; t0 += count_per)
-          gs.count_units.push_back(TUnit{(uint32_t)gs.segs.size(), t0, std::min(sb.t_hi, t0 + count_per), 0});
-      }
+      const std::vector<TileRun>& sruns = runs[gs.segs.size()];  // (G is this group's segment gs.segs.size(), i.e. sb)
+      if (count_seg)  // k_count_tiles: every tile the launches visit, about 1024 CTAs per group over all its segments
+        push_run_units(gs.count_units, (uint32_t)gs.segs.size(), sruns, 0, run_tiles(sruns), count_per);
       gs.max_slots = std::max(gs.max_slots, G.n_slots);
       gs.max_big = std::max(gs.max_big, G.n_big);
       gs.max_queries = std::max(gs.max_queries, G.n_queries);
       dens_max = std::max(dens_max, sb.dens);
-      tiles_total += sb.t_hi - sb.t_lo;
+      tiles_total += run_tiles(sruns);
       gs.segs.push_back(G);
     }
     std::sort(gs.count_queries.begin(), gs.count_queries.end());
@@ -1546,7 +1757,9 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
     // enough sampled tiles for k_max samples to exist: each (query, tile) contributes at most kSamplePerTile
     const uint64_t want_sample_tiles = std::min<uint64_t>(tiles_total / 2, std::max<uint64_t>(tiles_total / sample_div, (uint64_t)kmax_g / 2u + 8u));
     for (uint32_t si = 0; si < gs.segs.size(); ++si) {
-      const uint32_t tl = tg.segs[si].t_lo, nt = tg.segs[si].t_hi - tl;  // (the whole segment unless a doc range was set)
+      // the segment's tiles taken one after another: its doc range (the whole segment unless one was set), or a filter's runs
+      const std::vector<TileRun>& sruns = runs[si];
+      const uint32_t nt = (uint32_t)run_tiles(sruns);
       if (nt == 0) continue;
       if (c->tile_sample_div > 1 && nt >= 8 && tiles_total) {
         // short runs of tiles spread over the segment, one CTA each (a sample launch has few tiles: it needs them all in flight)
@@ -1556,7 +1769,8 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         for (uint32_t r = 0; r < runs; ++r) {
           const uint32_t start = (uint32_t)(((uint64_t)(2 * r + 1) * nt) / (2 * runs));
           const uint32_t t0 = std::min(start, nt - 1), t1 = std::min(nt, t0 + len);
-          gs.units[0].push_back(TUnit{si, tl + t0, tl + t1, 0});
+          const TileRun at = run_tile(sruns, t0);  // (a sample run ends with its tile run)
+          gs.units[0].push_back(TUnit{si, at.t0, std::min(at.t1, at.t0 + (t1 - t0)), 0});
         }
       }
       const uint32_t cut1 = nt >= 16 ? nt / std::max(2u, c->tile_round_div1) : 0, cut2 = nt >= 16 ? std::max(cut1, nt / std::max(2u, c->tile_round_div2)) : 0;
@@ -1567,7 +1781,7 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
         // this launch's share of the target, by its share of all tiles; at least 8 tiles per unit (cursor start-up)
         const uint64_t round_tiles_all = std::max<uint64_t>(1, (uint64_t)tiles_total * span / nt);
         const uint32_t per = (uint32_t)std::max<uint64_t>(tiles_total >= 16ull * target ? 8 : 2, (round_tiles_all + target - 1) / target);
-        for (uint32_t t0 = cuts[r]; t0 < cuts[r + 1]; t0 += per) gs.units[1 + r].push_back(TUnit{si, tl + t0, tl + std::min(cuts[r + 1], t0 + per), 0});
+        push_run_units(gs.units[1 + r], si, sruns, cuts[r], cuts[r + 1], per);
       }
     }
     for (int r = 0; r < kTileRounds; ++r) pl.tile_units += gs.units[r].size();
@@ -1776,6 +1990,16 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
 
 }  // namespace
 
+// ... and the filter views of the filters its queries name: tq_filter_register / tq_filter_unregister refuse those filters until
+// the batch is destroyed.  ctx->mu held.
+static void hold_filters(tq_ctx* c, tq_batch* b, const tq_query* queries, size_t nq) {
+  for (size_t qi = 0; qi < nq; ++qi)
+    if (queries[qi].flags & TQ_QUERY_FILTER) b->held_filters.push_back(queries[qi].filter_id);
+  std::sort(b->held_filters.begin(), b->held_filters.end());
+  b->held_filters.erase(std::unique(b->held_filters.begin(), b->held_filters.end()), b->held_filters.end());
+  for (uint32_t f : b->held_filters) ++c->filter_users[f];
+}
+
 // A prepared batch holds list ids and alive pointers of the segments its queries name: tq_segment_unregister refuses those
 // segments until the batch is destroyed.  ctx->mu held.
 static void hold_segments(tq_ctx* c, tq_batch* b, const tq_query* queries, size_t nq) {
@@ -1787,6 +2011,7 @@ static void hold_segments(tq_ctx* c, tq_batch* b, const tq_query* queries, size_
   std::sort(b->held.begin(), b->held.end());
   b->held.erase(std::unique(b->held.begin(), b->held.end()), b->held.end());
   for (const auto& key : b->held) ++c->seg_users[key];
+  hold_filters(c, b, queries, nq);
 }
 
 // repeat (finalize_run): 0 = a caller's batch.  1 = the repeat of an overflowed run: TERM / AND / OR / phrase queries take the
@@ -1874,6 +2099,11 @@ void tq_batch_destroy(tq_batch* b) {
     if (--it->second == 0) b->ctx->seg_users.erase(it);
   }
   b->held.clear();
+  for (uint32_t f : b->held_filters) {
+    auto it = b->ctx->filter_users.find(f);
+    if (--it->second == 0) b->ctx->filter_users.erase(it);
+  }
+  b->held_filters.clear();
   b->ctx->pool.push_back(b);  // buffers are recycled by the next batch
 }
 
@@ -2320,6 +2550,7 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
     }
     int rc = flush_builds(c, pending, &built);
     if (rc != TQ_OK) return rc;
+    hold_filters(c, b, queries, nq);  // (their views stay until the counts are in: the guard's tq_batch_destroy lets go)
   }
   if (!cp.bool_units.empty()) {  // mixed boolean shapes: their own kernel, counts added to out_counts
     const int rc = count_on_device(b, cp.bool_words, cp.bool_segs, cp.bool_units, nq, out_counts, k_count_bool);
@@ -2643,6 +2874,44 @@ int tq_multi_search_batch(tq_multi* m, const tq_query* queries, size_t nq, uint3
       out_doc[q * out_stride + i] = all[i].d;
     }
   }
+  return TQ_OK;
+}
+
+int tq_multi_filter_register(tq_multi* m, uint32_t filter_id, uint32_t segment_ord, const uint8_t* bits, size_t len) {
+  if (!m) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(m->mu);
+  std::vector<int> devs;  // every device that holds a field of the ordinal
+  for (auto it = m->owner.lower_bound({segment_ord, 0u}); it != m->owner.end() && it->first.first == segment_ord; ++it)
+    devs.insert(devs.end(), it->second.begin(), it->second.end());
+  std::sort(devs.begin(), devs.end());
+  devs.erase(std::unique(devs.begin(), devs.end()), devs.end());
+  if (devs.empty()) { m->err = g_err = "no field of the segment ordinal is registered"; return TQ_ERR_NOT_FOUND; }
+  for (tq_ctx* c : m->ctxs) {  // all or nothing: refused if a prepared batch on any device names the filter
+    std::lock_guard<std::mutex> gc(c->mu);
+    if (c->filter_users.count(filter_id)) { m->err = g_err = "a prepared batch still uses the filter"; return TQ_ERR_INVALID_ARGUMENT; }
+  }
+  for (int d : devs) {
+    const int rc = tq_filter_register(m->ctxs[d], filter_id, segment_ord, bits, len);
+    if (rc != TQ_OK) { m->err = g_err; return rc; }
+  }
+  return TQ_OK;
+}
+
+int tq_multi_filter_unregister(tq_multi* m, uint32_t filter_id) {
+  if (!m) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(m->mu);
+  for (tq_ctx* c : m->ctxs) {
+    std::lock_guard<std::mutex> gc(c->mu);
+    if (c->filter_users.count(filter_id)) { m->err = g_err = "a prepared batch still uses the filter"; return TQ_ERR_INVALID_ARGUMENT; }
+  }
+  bool any = false;
+  for (tq_ctx* c : m->ctxs) {
+    const int rc = tq_filter_unregister(c, filter_id);
+    if (rc == TQ_ERR_NOT_FOUND) continue;
+    if (rc != TQ_OK) { m->err = g_err; return rc; }
+    any = true;
+  }
+  if (!any) { m->err = g_err = "filter not registered"; return TQ_ERR_NOT_FOUND; }
   return TQ_OK;
 }
 

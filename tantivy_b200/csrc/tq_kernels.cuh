@@ -1244,6 +1244,21 @@ __global__ void __launch_bounds__(kThreads) k_count_bool(const CountBoolParams P
   }
 }
 
+// The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
+// words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
+// collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.
+__global__ void k_filter_combine(const uint32_t* __restrict__ alive, const uint32_t* __restrict__ filter, uint32_t n_words,
+                                 uint32_t doc_lo, uint32_t doc_hi, uint32_t* __restrict__ out) {
+  const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= n_words) return;
+  const uint32_t lo = w * 32u, a = max(doc_lo, lo), b = min(doc_hi, lo + 32u);
+  uint32_t m = 0;
+  if (a < b) m = (b - lo == 32u ? 0xFFFFFFFFu : (1u << (b - lo)) - 1u) & ~((1u << (a - lo)) - 1u);
+  uint32_t v = filter[w] & m;
+  if (alive) v &= alive[w];
+  out[w] = v;
+}
+
 // The exact k-th largest score key among a query's candidates so far (4-pass radix select) becomes a lower bound of
 // its threshold: run between the sampled windows and the main launch of k_or_strip.
 __global__ void __launch_bounds__(kThreads) k_theta(const BatchParams P) {

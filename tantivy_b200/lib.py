@@ -32,6 +32,10 @@ def _load():
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
     lib.tq_segment_set_doc_range.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    lib.tq_filter_register.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
+    lib.tq_filter_unregister.argtypes = [vp, C.c_uint32]
+    lib.tq_multi_filter_register.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
+    lib.tq_multi_filter_unregister.argtypes = [vp, C.c_uint32]
     lib.tq_search_batch.argtypes = [vp, C.POINTER(Query), sz, C.c_uint32, f32p, u32p, u32p, u32p]
     lib.tq_batch_prepare.argtypes = [vp, C.POINTER(Query), sz, C.POINTER(vp)]
     lib.tq_count_batch.argtypes = [vp, C.POINTER(Query), sz, u64p]
@@ -274,6 +278,16 @@ class Context:
         """This context evaluates only the docs [doc_lo, doc_hi) of the segment (intra-segment split over GPUs)."""
         _check(LIB.tq_segment_set_doc_range(self.h, segment_ord, field, doc_lo, doc_hi), self.h)
 
+    def filter_register(self, filter_id, segment_ord, bits):
+        """The doc filter `filter_id` of one segment (every field registered under the ordinal): `bits` in the `.del` layout,
+        bit d & 7 of byte d >> 3 set = keep doc d (np.packbits(mask, bitorder="little")).  Queries with filter=filter_id collect
+        only the alive docs it keeps (FilterCollector)."""
+        b = np.ascontiguousarray(bits, dtype=np.uint8)
+        _check(LIB.tq_filter_register(self.h, filter_id, segment_ord, ptr(b, u8p), b.size), self.h)
+
+    def filter_unregister(self, filter_id):
+        _check(LIB.tq_filter_unregister(self.h, filter_id), self.h)
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -352,6 +366,18 @@ class MultiContext:
         al = None if alive is None else np.ascontiguousarray(alive, dtype=np.uint8)
         rc = LIB.tq_multi_segment_register_split(self.h, segment_ord, field, max_doc, record_option, ptr(idx_body, u8p), idx_body.size,
                                                  ptr(fn, u8p), 0 if fn is None else fn.size, ptr(al, u8p), 0 if al is None else al.size)
+        if rc != 0:
+            raise TqError(f"tantivy_b200 error {rc}: {LIB.tq_multi_last_error(self.h).decode(errors='replace')}")
+
+    def filter_register(self, filter_id, segment_ord, bits):
+        """Context.filter_register on every device that holds the segment (all of them for a split segment)."""
+        b = np.ascontiguousarray(bits, dtype=np.uint8)
+        rc = LIB.tq_multi_filter_register(self.h, filter_id, segment_ord, ptr(b, u8p), b.size)
+        if rc != 0:
+            raise TqError(f"tantivy_b200 error {rc}: {LIB.tq_multi_last_error(self.h).decode(errors='replace')}")
+
+    def filter_unregister(self, filter_id):
+        rc = LIB.tq_multi_filter_unregister(self.h, filter_id)
         if rc != 0:
             raise TqError(f"tantivy_b200 error {rc}: {LIB.tq_multi_last_error(self.h).decode(errors='replace')}")
 

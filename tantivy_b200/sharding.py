@@ -141,6 +141,12 @@ class ShardedIndex:
             if self.ix.record_option == 2:
                 target.register_positions(g, 0, self.ix.positions(i))
 
+    def register_filter(self, target, filter_id, bits_per_local_segment):
+        """The doc filter `filter_id` on this rank's segments: bits_per_local_segment[i] = the `.del`-layout bitset of local
+        segment i over its whole doc space (a split segment's doc range does the rest on the device)."""
+        for i, g in enumerate(self.global_ords):
+            target.filter_register(filter_id, g, bits_per_local_segment[i])
+
     def marshal(self, queries):
         """queries: iterable of (op code, [term ordinals], k) -> QueryBatch restricted to this rank's segments.
         op 3 = phrase (terms in phrase order): ONE Bm25Weight::for_terms weight from the GLOBAL statistics."""
