@@ -200,7 +200,7 @@ struct tq_ctx {
   DevBuf build_dev;
   std::vector<tq_batch*> pool;
   tq_stats stats{};
-  uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit, strip_windows_per_unit;
+  uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit, strip_windows_per_unit, count_hits_tiles_per_unit;
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 16, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
@@ -455,6 +455,8 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->or_tiles_per_unit = env_u32("TQ_OR_TILES_PER_UNIT", 16);
   // test hook: smallest k_or_strip unit, in kWin-doc windows (1 or 7: warps with no window or one, unit and strip edges in small segments)
   c->strip_windows_per_unit = std::max<uint32_t>(1u, env_u32("TQ_STRIP_WINDOWS_PER_UNIT", kStripWarps * 64u));
+  // test hook: smallest k_count_tiles unit, in tiles (1: every tile edge is a unit edge, where the sparse cursors are searched)
+  c->count_hits_tiles_per_unit = std::max<uint32_t>(1u, env_u32("TQ_COUNT_HITS_TILES_PER_UNIT", 8));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -1677,7 +1679,7 @@ int stage_tile_groups(const tq_ctx* c, BatchPlan& pl) {
       runs[si] = seg_runs(tg.segs[si]);
       group_tiles += run_tiles(runs[si]);
     }
-    const uint32_t count_per = (uint32_t)std::max<uint64_t>(8u, (group_tiles + 1023u) / 1024u);
+    const uint32_t count_per = (uint32_t)std::max<uint64_t>(c->count_hits_tiles_per_unit, (group_tiles + 1023u) / 1024u);
     for (auto& sb : tg.segs) {
       // dense lists first (they get a tile index and whole warps), then the rest; clause ordinals follow the permutation
       std::vector<uint32_t> perm(sb.slots.size());

@@ -397,32 +397,3 @@ def test_bool_doc_range_parts_merge_to_the_whole_segment(ctx, cuts):
         assert (m[1][q, :n] == want[1][q, :n]).all() and (m[2][q, :n] == want[2][q, :n]).all()
         assert (m[0][q, :n].view(np.uint32) == want[0][q, :n].view(np.uint32)).all()
 
-
-# ---- k_count_bool ---------------------------------------------------------------------------------------------------------
-def test_count_bool_32_should_clauses_at_tile_edges(ctx):
-    """Count with 32 SHOULD clauses and minimum_should_match 0..33 (plus MUST / MUST_NOT variants) on segments whose max_doc is
-    not a multiple of 32, with matches on both sides of every 8192-doc tile edge of k_count_bool."""
-    rng = np.random.default_rng(61)
-    segs = []
-    for max_doc in (3 * 8192 + 77, 8192 + 1, 40_001):
-        edges = [e + d for e in range(8192, max_doc, 8192) for d in (-2, -1, 0, 1) if e + d < max_doc] + [0, max_doc - 1]
-        lists = []
-        for t in range(32):
-            p = 0.02 + 0.6 * t / 32
-            docs = np.nonzero(rng.random(max_doc) < p)[0]
-            docs = np.union1d(docs, [e for e in edges if rng.random() < 0.8]).astype(np.uint32)
-            lists.append((docs, rng.integers(1, 4, size=len(docs)).astype(np.uint32)))
-        alive = np.packbits(rng.random(max_doc) > 0.1, bitorder="little")
-        segs.append(OracleSegment(lists, rng.integers(1, 80, size=max_doc), segment_ord=fresh_ord(), writer_cls=T.FieldWriter, alive=alive))
-    oi = both(ctx, segs)
-    qs = []
-    for msm in (0, 1, 2, 5, 16, 24, 31, 32, 33):
-        qs.append(bool_query(make_query(TQ_OP_OR, segs, list(range(32)), 1), [TQ_OCCUR_SHOULD] * 32, msm=msm))
-        qs.append(bool_query(make_query(TQ_OP_OR, segs, list(range(32)), 1), [TQ_OCCUR_SHOULD] * 30 + [TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT],
-                             msm=min(msm, 31)))
-    qb = QueryBatch(qs)
-    g, c = ctx.count_batch(qb), oi.count_batch(qb)
-    assert (g == c).all(), (g, c)
-    assert g[0] > 0 and g[2 * 4] > 0 and g[-2] == 0  # msm 0 and 16 match; msm 33 of 32 cannot
-    for s in segs:
-        ctx.segment_unregister(s.segment_ord, 0)
