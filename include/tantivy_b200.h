@@ -218,7 +218,11 @@ int tq_get_stats(tq_ctx*, tq_stats* out);
  * fieldnorm   = the field's sub-file of `.fieldnorm` (max_doc bytes); NULL => constant
  *               fieldnorm 1 (term_weight.rs:218).
  * alive_bitset= `.del` payload without its 4-byte max_value header: little-endian 64-bit
- *               words, bit set = alive (common/src/bitset.rs:362-407); NULL => no deletes. */
+ *               words, bit set = alive (common/src/bitset.rs:362-407); NULL => no deletes.
+ * Every field of one segment ordinal is registered with the same max_doc and the same `.del` bits, as the fields of one
+ * tantivy segment share them; a query may name several fields of an ordinal (a clause each), which are then scored together.
+ * A query whose clauses name fields of one ordinal that differ in max_doc or doc range (tq_segment_set_doc_range) is refused
+ * with TQ_ERR_INVALID_ARGUMENT. */
 int tq_segment_register(tq_ctx*, uint32_t segment_ord, uint32_t field, uint32_t max_doc,
                         int record_option, const uint8_t* idx_body, size_t idx_len,
                         const uint8_t* fieldnorm, size_t fieldnorm_len,
@@ -340,7 +344,10 @@ int tq_merge_topk_packed_dev(tq_ctx*, void* cuda_stream, uint32_t n_lists, uint3
  * device, every (segment, field) lives on one of them (device_index -1 = the least loaded), tq_multi_search_batch runs
  * the devices' shares concurrently (one host thread per device), exchanges the exact k-th best score keys between the
  * phases -- every device prunes like a single device holding all segments -- and merges the rows on the host
- * (merge_fruits, sort_key_top_collector.rs:54-95).  Same arguments and result layout as tq_search_batch. */
+ * (merge_fruits, sort_key_top_collector.rs:54-95).  Same arguments and result layout as tq_search_batch.
+ * Every field of a segment ordinal lives on the same device(s), so that a query's clauses on the ordinal are scored together:
+ * a further field of an ordinal goes where the first one went, whole or split.  Registering it with another device_index, with
+ * another max_doc, or whole after split (or split after whole) fails with TQ_ERR_INVALID_ARGUMENT. */
 typedef struct tq_multi tq_multi;
 int tq_multi_create(const int* devices, int n_devices, tq_multi** out);
 void tq_multi_destroy(tq_multi*);

@@ -1032,14 +1032,25 @@ struct TileGroupBuild {
     double dens = 0;  // sum of doc_freq / max_doc over the slots: expected pairs per doc
   };
   std::vector<SegB> segs;
-  std::unordered_map<uint32_t, uint32_t> seg_of;  // segment_ord -> index in segs
-  std::vector<uint32_t> slot_head;                 // list id -> first slot of that list in its segment (kNoSlot: none); a list lives in one segment
-  uint32_t find_slot(const SegB& sb, const QList& ql) const {
-    if (ql.list_id >= slot_head.size()) return kNoSlot;
-    for (uint32_t s = slot_head[ql.list_id]; s != kNoSlot; s = sb.slots[s].pad) {
-      const TSlot& sl = sb.slots[s];
-      if (memcmp(&sl.weight, &ql.weight, 4) == 0 && sl.cache_idx == ql.cache_idx) return s;
+  // (segment_ord, field of the plan's alive words) -> index in segs: fields of one ordinal may differ in doc range, alive copy
+  // and filter view, so each field a query's plan takes them from has its own entry
+  std::unordered_map<uint64_t, uint32_t> seg_of;
+  static uint64_t seg_key(const SegPlan& sp) { return (uint64_t)sp.segment_ord << 32 | sp.seg->field; }
+  // list id -> first slot of that list in its home entry slot_home[list id] (kNoSlot: in no entry).  A list lives in one
+  // (segment, field), but a query whose clauses span fields brings it into the entry of another field too: there it is looked up
+  // among the entry's slots.
+  std::vector<uint32_t> slot_head, slot_home;
+  uint32_t find_slot(uint32_t si, const QList& ql) const {
+    if (ql.list_id >= slot_head.size() || slot_head[ql.list_id] == kNoSlot) return kNoSlot;
+    const SegB& sb = segs[si];
+    auto same = [&](const TSlot& sl) { return memcmp(&sl.weight, &ql.weight, 4) == 0 && sl.cache_idx == ql.cache_idx; };
+    if (slot_home[ql.list_id] != si) {
+      for (uint32_t s = 0; s < sb.slots.size(); ++s)
+        if (sb.slots[s].list_id == ql.list_id && same(sb.slots[s])) return s;
+      return kNoSlot;
     }
+    for (uint32_t s = slot_head[ql.list_id]; s != kNoSlot; s = sb.slots[s].pad)
+      if (same(sb.slots[s])) return s;
     return kNoSlot;
   }
   uint64_t pairs = 0;                              // elements of the pair arrays (doc_freq rounded up to 128 per slot)
@@ -1212,13 +1223,13 @@ int bool_structure(const tq_query& q, const uint32_t* term_idx, const uint32_t* 
 bool tile_fits(const tq_ctx* c, const TileGroupBuild& g, const SegPlan* plans, size_t n_plans, uint32_t max_queries, bool exact) {
   for (size_t pi = 0; pi < n_plans; ++pi) {
     const SegPlan& sp = plans[pi];
-    auto it = g.seg_of.find(sp.segment_ord);
+    auto it = g.seg_of.find(TileGroupBuild::seg_key(sp));
     const TileGroupBuild::SegB* sb = it == g.seg_of.end() ? nullptr : &g.segs[it->second];
     if (sb && sb->queries.size() + 1 > max_queries) return false;
     size_t n_slots = sb ? sb->slots.size() : 0;
     double dens = sb ? sb->dens : 0.0;
     for (auto& h : sp.here) {
-      if (exact && sb && g.find_slot(*sb, h.second) != kNoSlot) continue;
+      if (exact && sb && g.find_slot(it->second, h.second) != kNoSlot) continue;
       ++n_slots;
       dens += (double)h.first / std::max(1u, sp.seg->max_doc);
     }
@@ -1233,9 +1244,9 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, bool count, const
   const uint64_t pairs_before = g.pairs;
   for (size_t pi = 0; pi < n_plans; ++pi) {
     const SegPlan& sp = plans[pi];
-    auto it = g.seg_of.find(sp.segment_ord);
+    auto it = g.seg_of.find(TileGroupBuild::seg_key(sp));
     if (it == g.seg_of.end()) {
-      it = g.seg_of.emplace(sp.segment_ord, (uint32_t)g.segs.size()).first;
+      it = g.seg_of.emplace(TileGroupBuild::seg_key(sp), (uint32_t)g.segs.size()).first;
       g.segs.emplace_back();
       g.segs.back().segment_ord = sp.segment_ord;
       g.segs.back().max_doc = sp.seg->max_doc;
@@ -1254,15 +1265,22 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, bool count, const
     uint16_t slot_of_here[TQ_MAX_TERMS];
     size_t hi_idx = 0;
     for (auto& h : sp.here) {
-      uint32_t slot = g.find_slot(sb, h.second);
+      uint32_t slot = g.find_slot(it->second, h.second);
       if (slot == kNoSlot) {
         slot = (uint32_t)sb.slots.size();
         TSlot sl{};
         sl.list_id = h.second.list_id; sl.weight = h.second.weight; sl.cache_idx = h.second.cache_idx; sl.doc_freq = h.first;
         sl.big = kNoSlot;
-        if (h.second.list_id >= g.slot_head.size()) g.slot_head.resize((size_t)h.second.list_id + 1024, kNoSlot);
-        sl.pad = g.slot_head[h.second.list_id];  // chain
-        g.slot_head[h.second.list_id] = slot;
+        sl.pad = kNoSlot;
+        if (h.second.list_id >= g.slot_head.size()) {
+          g.slot_head.resize((size_t)h.second.list_id + 1024, kNoSlot);
+          g.slot_home.resize((size_t)h.second.list_id + 1024, kNoSlot);
+        }
+        if (g.slot_head[h.second.list_id] == kNoSlot) g.slot_home[h.second.list_id] = it->second;
+        if (g.slot_home[h.second.list_id] == it->second) {  // chain (in the home entry)
+          sl.pad = g.slot_head[h.second.list_id];
+          g.slot_head[h.second.list_id] = slot;
+        }
         sb.slots.push_back(sl);
         sb.dens += (double)h.first / std::max(1u, sp.seg->max_doc);
         g.pairs += ((uint64_t)h.first + 127) / 128 * 128;
@@ -1279,6 +1297,13 @@ uint64_t tile_admit(TileGroupBuild& g, uint32_t query, int op, bool count, const
     sb.queries.push_back(tq);
   }
   return g.pairs - pairs_before;
+}
+
+// The fields of one segment ordinal that a query's clauses name must hold the same docs: a (query, segment) collects from one
+// field's alive words (doc range included) and covers one max_doc.
+bool same_docs(const Segment& a, const Segment& b) { return a.max_doc == b.max_doc && a.doc_lo == b.doc_lo && a.doc_hi == b.doc_hi; }
+int fail_fields() {
+  return fail(TQ_ERR_INVALID_ARGUMENT, "the clauses of a query name fields of one segment that differ in max_doc or doc range");
 }
 
 // tq_stats' bytes_term / bytes_and / bytes_or class of a query shape: phrases count as AND, mixed boolean queries as OR.
@@ -1345,8 +1370,10 @@ int plan_segments(tq_ctx* c, BatchPlan& pl, const tq_query& q, int op, const uin
       const tq_term_seg& t = *ts[a];
       uint32_t id;
       const bool ignore_freq = q.term_flags && (q.term_flags[t.term_idx] & TQ_TERM_IGNORE_FREQ);
+      const Segment* prev = sp.seg;
       int rc = get_list(c, t, ignore_freq, pl.pending, &id, &sp.seg);
       if (rc != TQ_OK) return rc;
+      if (a > 0 && !same_docs(*prev, *sp.seg)) return fail_fields();
       if (ignore_freq || sp.seg->record_option == TQ_RECORD_BASIC) sp.no_freq |= 1u << a;
       if (a == 0) sp.fn0 = sp.seg->d_fieldnorm; else sp.uniform_fn &= (sp.seg->d_fieldnorm == sp.fn0);
       const uint32_t tw = is_phrase ? 0 : t.term_idx;
@@ -1514,8 +1541,10 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
       float ws_[TQ_MAX_TERMS];
       const Segment* seg = nullptr;
       for (size_t a = 0; a < n_here; ++a) {
+        const Segment* prev = seg;
         int rc = get_list(c, *ts[a], false, pending, &ids_[a], &seg);
         if (rc != TQ_OK) return rc;
+        if (a > 0 && !same_docs(*prev, *seg)) return fail_fields();
         tix_[a] = ts[a]->term_idx; dfs_[a] = ts[a]->doc_freq; ws_[a] = q.weight[ts[a]->term_idx];
       }
       std::vector<uint16_t> words;
@@ -1541,8 +1570,10 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBui
     uint64_t df_single = 0;
     for (size_t a = 0; a < n_here; ++a) {
       uint32_t id;
+      const Segment* prev = seg;
       int rc = get_list(c, *ts[a], false, pending, &id, &seg);
       if (rc != TQ_OK) return rc;
+      if (a > 0 && !same_docs(*prev, *seg)) return fail_fields();
       cp.list_ids.push_back(id);
       df_single = ts[a]->doc_freq;
     }
@@ -2685,6 +2716,8 @@ struct tq_multi {
   std::vector<tq_ctx*> ctxs;
   std::map<std::pair<uint32_t, uint32_t>, std::vector<int>> owner;  // (segment_ord, field) -> indices into ctxs (several: the segment is split by doc range)
   std::vector<uint64_t> load;                           // bytes registered per device
+  struct Placement { uint32_t max_doc; bool split; std::vector<int> devices; };
+  std::map<uint32_t, Placement> placed;  // segment_ord -> where its fields live: every field of an ordinal on the same devices
   std::mutex mu;
   std::string err;
 };
@@ -2737,7 +2770,16 @@ int tq_multi_segment_register(tq_multi* m, int device_index, uint32_t segment_or
   if (!m) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
   std::lock_guard<std::mutex> g(m->mu);
   if (device_index >= (int)m->ctxs.size()) { m->err = "device_index"; return TQ_ERR_INVALID_ARGUMENT; }
-  if (device_index < 0) {  // least loaded device: segments shard naturally (SURVEY.md §8e)
+  // a query's clauses on one ordinal are scored on one device: a further field of an ordinal goes where its first one went
+  auto pit = m->placed.find(segment_ord);
+  if (pit != m->placed.end()) {
+    const char* why = pit->second.split ? "the ordinal's other fields are split over the devices (tq_multi_segment_register_split)"
+                    : pit->second.max_doc != max_doc ? "max_doc differs from the ordinal's other fields"
+                    : device_index >= 0 && device_index != pit->second.devices[0] ? "device_index differs from the device of the ordinal's other fields"
+                    : nullptr;
+    if (why) { m->err = g_err = why; return TQ_ERR_INVALID_ARGUMENT; }
+    device_index = pit->second.devices[0];
+  } else if (device_index < 0) {  // least loaded device: segments shard naturally (SURVEY.md §8e)
     device_index = 0;
     for (size_t i = 1; i < m->load.size(); ++i) if (m->load[i] < m->load[device_index]) device_index = (int)i;
   }
@@ -2745,6 +2787,7 @@ int tq_multi_segment_register(tq_multi* m, int device_index, uint32_t segment_or
                                      alive_bitset, alive_len);
   if (rc != TQ_OK) { m->err = g_err; return rc; }
   m->owner[{segment_ord, field}] = std::vector<int>{device_index};
+  m->placed.emplace(segment_ord, tq_multi::Placement{max_doc, false, {device_index}});
   m->load[device_index] += idx_len + fieldnorm_len;
   return TQ_OK;
 }
@@ -2756,6 +2799,11 @@ int tq_multi_segment_register_split(tq_multi* m, uint32_t segment_ord, uint32_t 
                                     const uint8_t* alive_bitset, size_t alive_len) {
   if (!m) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
   std::lock_guard<std::mutex> g(m->mu);
+  auto pit = m->placed.find(segment_ord);
+  if (pit != m->placed.end() && (!pit->second.split || pit->second.max_doc != max_doc)) {
+    m->err = g_err = !pit->second.split ? "the ordinal's other fields are registered whole (tq_multi_segment_register)" : "max_doc differs from the ordinal's other fields";
+    return TQ_ERR_INVALID_ARGUMENT;
+  }
   const uint32_t nd = (uint32_t)m->ctxs.size();
   const uint32_t per = (uint32_t)((((uint64_t)max_doc + nd - 1) / nd + kTile - 1) / kTile * kTile);
   std::vector<int> owners;
@@ -2774,6 +2822,7 @@ int tq_multi_segment_register_split(tq_multi* m, uint32_t segment_ord, uint32_t 
     m->load[d] += idx_len + fieldnorm_len;
   }
   m->owner[{segment_ord, field}] = owners;
+  m->placed.emplace(segment_ord, tq_multi::Placement{max_doc, true, owners});
   return TQ_OK;
 }
 

@@ -32,6 +32,25 @@ class Segment:
         self.alive = None if alive is None else np.unpackbits(np.asarray(alive, np.uint8), bitorder="little")[:self.max_doc].astype(bool)
         self.basic = basic
         self.positions = positions
+        self.fields = None  # (multi_field: field id -> that field's Segment)
+
+    @classmethod
+    def multi_field(cls, segment_ord, fields, max_doc, alive=None):
+        """One segment ordinal with several fields: fields = {field id: dict(lists=, lengths= (None: no fieldnorms), basic=,
+        positions=)}.  Every field shares max_doc and the alive bits, as the fields of one tantivy segment do; a clause reads the
+        field its term_segs entry names (lists, fieldnorm ids and record option of that field)."""
+        per = {f: cls(segment_ord, d["lists"], d.get("lengths"), alive=alive, basic=d.get("basic", False), max_doc=max_doc,
+                      positions=d.get("positions")) for f, d in fields.items()}
+        assert all(s.max_doc == max_doc for s in per.values())
+        seg = per[min(per)]
+        out = cls.__new__(cls)
+        out.__dict__.update(seg.__dict__)
+        out.fields = per
+        return out
+
+    def field(self, f):
+        """The Segment of field f (a single-field segment is every field's: its callers name field 0 or none)."""
+        return self if self.fields is None else self.fields[f]
 
 
 def tf_cache(avg, dtype=f32):
@@ -124,11 +143,11 @@ def _intersect(parts, max_doc, intersection_order):
 def _segment_matches(seg, q, terms, intersection_order=None):
     """complex_scorer / the specialised scorers for one segment: a _Dense of the matching docs (before deletes), or None."""
     op = q["op"]
+    field_of = {ts[0]: ts[2] for ts in q["term_segs"] if ts[1] == seg.segment_ord and ts[3] > 0}  # present clause -> its field
     if op == TQ_OP_PHRASE:
-        return _phrase_matches(seg, q, terms)
-    present = {ts[0] for ts in q["term_segs"] if ts[1] == seg.segment_ord and ts[3] > 0}
+        return _phrase_matches(seg.field(field_of[0]) if 0 in field_of else seg, q, terms)
     n = len(q["weights"])
-    scorer = {c: _Term(seg, q, c, terms[c]) for c in range(n) if c in present}
+    scorer = {c: _Term(seg.field(field_of[c]), q, c, terms[c]) for c in range(n) if c in field_of}  # (in clause order)
     if op == TQ_OP_TERM or (op in (TQ_OP_AND, TQ_OP_OR) and n == 1):
         return _union(list(scorer.values()), seg.max_doc) if scorer else None
     if op == TQ_OP_OR:

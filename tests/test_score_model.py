@@ -426,3 +426,48 @@ def test_signed_zero_scores_tie_and_are_ordered_by_doc():
     assert all(signs[d] for d in range(10)) and not any(signs[d] for d in range(10, 20))  # (both zeros are there)
     assert M.merge_fruits([M.search([m1], q, [0, 1]), M.search([m0], q, [0, 1])], 100) == rows
     assert M.merge_fruits([[(0.0, 3, 5)], [(-0.0, 3, 4)], [(-0.0, 2, 9)], [(1e-45, 9, 9)]], 3) == [(1e-45, 9, 9), (-0.0, 2, 9), (-0.0, 3, 4)]
+
+
+# ---- multi-field segments ----------------------------------------------------------------------------------------------
+def test_one_field_multi_field_segment_is_the_single_field_model():
+    """A segment written as a one-field multi-field segment gives the rows and counts of the plain Segment, bit for bit."""
+    rng = np.random.default_rng(77)
+    osegs, msegs = _random_pairs(rng, 3, 6, deletes=True)
+    wrapped = [M.Segment.multi_field(m.segment_ord, {0: dict(lists=m.lists, lengths=l, basic=m.basic)}, m.max_doc, alive=o.alive)
+               for o, m, l in zip(osegs, msegs, [o.fieldnorms for o in osegs])]
+    queries, terms = [], []
+    for op, c in [(TQ_OP_TERM, [1]), (TQ_OP_AND, [0, 1, 2, 3, 4]), (TQ_OP_OR, [0, 1, 2, 3, 4, 5])]:
+        for k in (1, 10, 1000):
+            queries.append(make_query(op, osegs, c, k))
+            terms.append(c)
+    for c, occ, grp, msm in BOOL_SHAPES:
+        queries.append(bool_query(make_query(TQ_OP_OR, osegs, c, 1000), occ, grp, msm))
+        terms.append(c)
+    for q, t in zip(queries, terms):
+        a, b = M.search(msegs, q, t), M.search(wrapped, q, t)
+        assert [(np.float32(s).view(np.uint32), g, d) for s, g, d in a] == [(np.float32(s).view(np.uint32), g, d) for s, g, d in b]
+        assert M.count(msegs, q, t) == M.count(wrapped, q, t)
+
+
+@pytest.fixture(scope="module")
+def multi_field_index():
+    from tests.multi_field import Index
+    return Index(sizes=(30_000, 7_001, 5_000))
+
+
+def test_multi_field_model_is_the_oracle(multi_field_index):
+    """Clauses over several fields of one segment ordinal (each field its own lists, fieldnorms and record option, one alive
+    bitset): the model's rows and counts equal the oracle's, which looks up every clause's (segment, field)."""
+    from tests.multi_field import battery
+    ix = multi_field_index
+    oi = ix.register(O.OracleIndex())
+    qts = battery(ix, phrase=False)
+    assert max(len(q["weights"]) for q, _ in qts) == 32
+    res = oi.search_batch(QueryBatch([q for q, _ in qts]), mode=0)
+    for i, (q, t) in enumerate(qts):
+        assert hits(res, i) == M.search(ix.models(), q, t), (i, q["op"], t)
+    counts = oi.count_batch(QueryBatch([q for q, _ in qts]))
+    assert list(counts) == [M.count(ix.models(), q, t) for q, t in qts]
+    # the fields do sum on one doc: some OR row holds clauses of two fields
+    q, t = next(x for x in qts if x[0]["op"] == TQ_OP_OR and x[0]["k"] == 1024)
+    assert len({ts[2] for ts in q["term_segs"]}) >= 2
