@@ -201,7 +201,7 @@ typedef struct {
                                    (stage B2) by how they ended: [0] dropped by the bound taken before the look-ups, [1] not the owner
                                    (completed the walk, but an earlier essential clause lists the doc), [2] dropped in the
                                    non-essential walk, [3] completed */
-  float count_hits_ms;          /* device time of the launches that count TQ_QUERY_COUNT_HITS queries (k_count_tiles, k_count, k_count_bool) */
+  float count_hits_ms;          /* device time of the launches that count TQ_QUERY_COUNT_HITS queries (k_count_tiles, k_count) */
   uint64_t units_count_hits;    /* CTAs of those launches */
 } tq_stats;
 

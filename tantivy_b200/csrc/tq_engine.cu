@@ -161,9 +161,9 @@ struct Segment {
 struct TileRun { uint32_t t0, t1; };
 
 // What a filtered query (TQ_QUERY_FILTER) reads of one (filter, segment, field): alive AND doc range AND filter on the device
-// (k_filter_combine, padded like the alive copy: k_count and the BOOL path read whole 32-bit words), and the tiles it leaves
+// (k_filter_combine, padded like the alive copy: k_count reads whole 32-bit words), and the tiles it leaves
 // non-empty, from the host bits and the doc range: runs of 1024-doc tiles of the tile engine (gaps of up to kRunGap empty tiles
-// merged, since every unit pays a cursor prologue) and of the Count kernels' 8192-doc tiles.  Built at first use, rebuilt by
+// merged, since every unit pays a cursor prologue) and of k_count's 8192-doc tiles.  Built at first use, rebuilt by
 // tq_segment_set_doc_range, dropped with the segment or the filter.
 struct FilterView {
   uint8_t* d_bits = nullptr;
@@ -284,7 +284,7 @@ struct tq_batch {
     CountTileParams count{};  // k_count_tiles: the group's TQ_QUERY_COUNT_HITS queries
     uint32_t n_count_units = 0;
     size_t count_smem = 0;
-    std::vector<uint32_t> count_queries;  // batch ordinals of those queries (recounted by the Count kernels if count.overflow is set)
+    std::vector<uint32_t> count_queries;  // batch ordinals of those queries (recounted by k_count if count.overflow is set)
   };
   tq_ctx* ctx = nullptr;
   cudaStream_t stream = nullptr;
@@ -319,12 +319,12 @@ struct tq_batch {
   tq_stats stats{};
   bool ran = false;
   // TQ_QUERY_COUNT_HITS: per-query hit counters (u64 [nq]) and the groups' overflow words (u32 [groups]) in `scratch` at hits_off,
-  // zeroed by phase 0; the Count kernels of the queries on the per-query kernels; hits_host = their doc_freq shortcuts
+  // zeroed by phase 0; k_count for the queries on the per-query kernels; hits_host = their doc_freq shortcuts
   bool count_hits = false;
   size_t hits_off = 0, hits_bytes = 0;
   CountParams count_p{};
-  CountBoolParams count_bool_p{};
-  uint32_t n_count_units = 0, n_count_bool_units = 0;
+  uint32_t n_count_units = 0;
+  bool count_mixed = false;  // k_count<true>: some pair has SHOULD or MUST_NOT clauses
   std::vector<uint64_t> hits_host;
   PinBuf hits_pin;
   std::vector<std::pair<uint32_t, uint32_t>> held;  // the (segment, field)s its queries name, counted in tq_ctx::seg_users until destroyed
@@ -959,20 +959,19 @@ static cudaError_t copy_rows(const tq_batch* src, cudaStream_t stream, float* sc
   return e;
 }
 
-// One Count kernel over (query, segment) pairs: stages their clause words (list ids, or BOOL structure words with list ids), the
-// pairs, the units and zeroed per-query counters, runs `kernel` and adds the counts to out_counts.
-template <class Params, class Seg>
-static int count_on_device(tq_batch* b, const std::vector<uint32_t>& words, const std::vector<Seg>& segs, const std::vector<Unit>& units,
-                           size_t nq, uint64_t* out_counts, void (*kernel)(Params)) {
+// k_count over (query, segment) pairs: stages their structure words, the pairs, the units and zeroed per-query counters, runs the
+// kernel and adds the counts to out_counts.
+static int count_on_device(tq_batch* b, const std::vector<uint32_t>& words, const std::vector<CountSeg>& segs, const std::vector<Unit>& units,
+                           bool mixed, size_t nq, uint64_t* out_counts) {
   const std::vector<unsigned long long> zeros(nq, 0);
   Staging st;
   const size_t o_w = st.add(words), o_s = st.add(segs), o_u = st.add(units), o_c = st.add(zeros);
   TQ_CUDA(st.reserve(b->pin, b->dev));
   st.copy();
-  const Params P{b->ctx->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const Seg>(o_s), st.on_device<const Unit>(o_u),
-                 st.on_device<unsigned long long>(o_c)};
+  const CountParams P{b->ctx->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                      st.on_device<unsigned long long>(o_c)};
   TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
-  kernel<<<(unsigned)units.size(), kThreads, 0, b->stream>>>(P);
+  (mixed ? k_count<true> : k_count<false>)<<<(unsigned)units.size(), kThreads, 0, b->stream>>>(P);
   TQ_CUDA(cudaGetLastError());
   TQ_CUDA(cudaMemcpyAsync(b->pin.p + o_c, b->dev.p + o_c, nq * 8, cudaMemcpyDeviceToHost, b->stream));
   TQ_CUDA(cudaStreamSynchronize(b->stream));
@@ -1077,15 +1076,13 @@ struct GroupStage {
 // whether it is a strip pair with a threshold sample pass (MaxScore can then skip its dense clauses).
 struct SegWork { UnitClass cls; uint32_t total; bool sample; };
 
-// The Count collector's work for a set of queries: (query, segment) pairs of k_count (term / AND / OR: their list ids) and of
-// k_count_bool (TQ_OP_BOOL: structure words with list ids), one unit per 8 tiles of 8192 docs.
+// The Count collector's work for a set of queries: the (query, segment) pairs of k_count with their structure words (list ids in
+// place of the clause indices), one unit per 8 tiles of 8192 docs.
 struct CountPlan {
-  std::vector<uint32_t> list_ids;
+  std::vector<uint32_t> words;
   std::vector<CountSeg> segs;
   std::vector<Unit> units;
-  std::vector<uint32_t> bool_words;
-  std::vector<CountBoolSeg> bool_segs;
-  std::vector<Unit> bool_units;
+  bool mixed = false;  // some pair has SHOULD or MUST_NOT clauses: k_count<true>
 };
 
 // The plan of one batch: what the stages of batch_prepare_impl hand on to each other.
@@ -1119,7 +1116,7 @@ struct BatchPlan {
   uint64_t tile_pairs_total = 0, pair_cursor = 0, tile_postings = 0, tile_units = 0;
   size_t tix_total_words = 0, tile_bytes = 0;
   // TQ_QUERY_COUNT_HITS (not in a repeat: the hits of the original run stand): the queries on the per-query kernels are counted
-  // by k_count / k_count_bool (count), the doc_freq shortcuts go to hits_host; the tile groups' queries by k_count_tiles
+  // by k_count (count), the doc_freq shortcuts go to hits_host; the tile groups' queries by k_count_tiles
   bool count_hits = false;
   CountPlan count;
   std::vector<uint64_t> hits_host;
@@ -1130,6 +1127,7 @@ struct BatchPlan {
 };
 
 // Calls f(lists, n) per segment on the query's (clause, segment) lists with postings, by (segment, clause); stops at the first error.
+// A clause names a segment once, so n <= n_terms.
 template <class F>
 int for_each_segment(const tq_query& q, std::vector<const tq_term_seg*>& order, F&& f) {
   order.clear();
@@ -1141,7 +1139,8 @@ int for_each_segment(const tq_query& q, std::vector<const tq_term_seg*>& order, 
     return a->segment_ord != b->segment_ord ? a->segment_ord < b->segment_ord : a->term_idx < b->term_idx;
   });
   for (size_t i = 0, j; i < order.size(); i = j) {
-    for (j = i + 1; j < order.size() && order[j]->segment_ord == order[i]->segment_ord; ++j) {}
+    for (j = i + 1; j < order.size() && order[j]->segment_ord == order[i]->segment_ord; ++j)
+      if (order[j]->term_idx == order[j - 1]->term_idx) return fail(TQ_ERR_INVALID_ARGUMENT, "duplicate (term_idx, segment_ord)");
     const int rc = f(order.data() + i, j - i);
     if (rc != TQ_OK) return rc;
   }
@@ -1309,13 +1308,20 @@ int fail_fields() {
 // tq_stats' bytes_term / bytes_and / bytes_or class of a query shape: phrases count as AND, mixed boolean queries as OR.
 int bytes_class(int op) { return op == TQ_OP_PHRASE ? TQ_OP_AND : (op == TQ_OP_BOOL ? TQ_OP_OR : op); }
 
+// The shape of a query for search (phrase_ok) and for Count, which has no phrase path.
+int check_shape(const tq_query& q, bool phrase_ok) {
+  if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
+  if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_BOOL && !(phrase_ok && q.op == TQ_OP_PHRASE))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "op");
+  if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
+  return TQ_OK;
+}
+
 int validate_query(const tq_ctx* c, const tq_query& q) {
   if (q.k == 0 || q.k > TQ_MAX_K) return fail(TQ_ERR_INVALID_ARGUMENT, "k must be in 1..TQ_MAX_K");
-  if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
-  const bool is_bool = q.op == TQ_OP_BOOL;
-  if (is_bool && (c->tile == 0 || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
-  if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_PHRASE && !is_bool) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
-  if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
+  const int rc = check_shape(q, true);
+  if (rc != TQ_OK) return rc;
+  if (q.op == TQ_OP_BOOL && (c->tile == 0 || !q.term_occur)) return fail(!q.term_occur ? TQ_ERR_INVALID_ARGUMENT : TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL needs term_occur and the tile engine (TQ_TILE=1)");
   if (!q.weight || (!q.avg_fieldnorm && !q.tf_cache) || (!q.term_segs && q.n_term_segs)) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
   if (q.op == TQ_OP_PHRASE) {
     if (q.n_terms < 2 || q.n_terms > TQ_MAX_PHRASE_TERMS) return fail(TQ_ERR_UNSUPPORTED, "a phrase takes 2..TQ_MAX_PHRASE_TERMS terms on the device path");
@@ -1356,8 +1362,6 @@ int plan_segments(tq_ctx* c, BatchPlan& pl, const tq_query& q, int op, const uin
   const bool is_phrase = op == TQ_OP_PHRASE;
   pl.n_plans = 0;
   return for_each_segment(q, pl.order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
-    for (size_t a = 1; a < n_here; ++a)
-      if (ts[a]->term_idx == ts[a - 1]->term_idx) return fail(TQ_ERR_INVALID_ARGUMENT, "duplicate (term_idx, segment_ord)");
     if ((op == TQ_OP_AND || is_phrase) && n_here != q.n_terms) return TQ_OK;  // a clause is absent: empty intersection
     if (pl.n_plans == pl.plans.size()) pl.plans.emplace_back();
     SegPlan& sp = pl.plans[pl.n_plans++];
@@ -1518,76 +1522,61 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
 // ctx->mu held.
 int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<PendingBuild>& pending, std::vector<const tq_term_seg*>& order,
                CountPlan& cp, uint64_t* host_add) {
-  if (q.n_terms == 0 || q.n_terms > TQ_MAX_TERMS) return fail(TQ_ERR_INVALID_ARGUMENT, "n_terms must be in 1..TQ_MAX_TERMS");
-  if (q.op != TQ_OP_TERM && q.op != TQ_OP_AND && q.op != TQ_OP_OR && q.op != TQ_OP_BOOL) return fail(TQ_ERR_INVALID_ARGUMENT, "op");
-  if (q.op == TQ_OP_TERM && q.n_terms != 1) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_TERM takes one term");
+  int rc = check_shape(q, false);
+  if (rc != TQ_OK) return rc;
   if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
   if (q.op == TQ_OP_BOOL && (!q.term_occur || !q.weight)) return fail(TQ_ERR_INVALID_ARGUMENT, "TQ_OP_BOOL needs term_occur and weights");
-  const int frc = check_filter(c, q);
-  if (frc != TQ_OK) return frc;
-  // units of 8 tiles of 8192 docs over the segment; a filtered query's only over the tiles its filter view leaves non-empty
-  auto cut = [](std::vector<Unit>& units, uint32_t seg_idx, uint32_t max_doc, const FilterView* view) {
-    const uint32_t tiles = (max_doc + kTileDocs - 1) / kTileDocs, per = 8;
-    if (!view) {
-      for (uint32_t t0 = 0; t0 < tiles; t0 += per) units.push_back(Unit{seg_idx, t0, std::min(tiles, t0 + per), 0});
-      return;
-    }
-    for (const TileRun& r : view->count_runs)
-      for (uint32_t t0 = r.t0; t0 < r.t1; t0 += per) units.push_back(Unit{seg_idx, t0, std::min(r.t1, t0 + per), 0});
-  };
+  rc = check_filter(c, q);
+  if (rc != TQ_OK) return rc;
+  std::vector<uint16_t> words;
   return for_each_segment(q, order, [&](const tq_term_seg* const* ts, size_t n_here) -> int {
-    if (q.op == TQ_OP_BOOL) {  // mixed shapes: the structure of this segment, with list ids in place of the clause indices
-      uint32_t tix_[TQ_MAX_TERMS], dfs_[TQ_MAX_TERMS], ids_[TQ_MAX_TERMS];
-      float ws_[TQ_MAX_TERMS];
-      const Segment* seg = nullptr;
-      for (size_t a = 0; a < n_here; ++a) {
-        const Segment* prev = seg;
-        int rc = get_list(c, *ts[a], false, pending, &ids_[a], &seg);
-        if (rc != TQ_OK) return rc;
-        if (a > 0 && !same_docs(*prev, *seg)) return fail_fields();
-        tix_[a] = ts[a]->term_idx; dfs_[a] = ts[a]->doc_freq; ws_[a] = q.weight[ts[a]->term_idx];
-      }
-      std::vector<uint16_t> words;
+    if (q.op == TQ_OP_AND && n_here < q.n_terms) return TQ_OK;  // a clause without postings: empty intersection
+    uint32_t ids[TQ_MAX_TERMS];
+    const Segment* seg = nullptr;
+    for (size_t a = 0; a < n_here; ++a) {
+      const Segment* prev = seg;
+      const int lrc = get_list(c, *ts[a], false, pending, &ids[a], &seg);
+      if (lrc != TQ_OK) return lrc;
+      if (a > 0 && !same_docs(*prev, *seg)) return fail_fields();
+    }
+    // the structure words of this segment, clauses as indices into ts: a term or an OR is one MUST group of its clauses, an AND
+    // one group per clause
+    if (q.op == TQ_OP_BOOL) {
+      uint32_t tix[TQ_MAX_TERMS], dfs[TQ_MAX_TERMS];
+      float ws[TQ_MAX_TERMS];
+      for (size_t a = 0; a < n_here; ++a) { tix[a] = ts[a]->term_idx; dfs[a] = ts[a]->doc_freq; ws[a] = q.weight[ts[a]->term_idx]; }
       bool io_unused;  // (a count adds no scores)
-      const int st = bool_structure(q, tix_, dfs_, ws_, n_here, 0u, words, &io_unused);
+      const int st = bool_structure(q, tix, dfs, ws, n_here, 0u, words, &io_unused);
       if (st < 0) return fail(TQ_ERR_INVALID_ARGUMENT, "term_occur");
       if (st == 0) return TQ_OK;
-      CountBoolSeg bs{};
-      const FilterView* view = nullptr;
-      const int arc = query_alive(c, q, *seg, &bs.alive, &view);
-      if (arc != TQ_OK) return arc;
-      bs.query = qi; bs.words_base = (uint32_t)cp.bool_words.size(); bs.max_doc = seg->max_doc;
-      cp.bool_words.insert(cp.bool_words.end(), words.begin(), words.end());
-      map_bool_clauses(cp.bool_words.data() + bs.words_base, words.size(), [&](uint32_t a) { return ids_[a]; });
-      cut(cp.bool_units, (uint32_t)cp.bool_segs.size(), bs.max_doc, view);
-      cp.bool_segs.push_back(bs);
-      return TQ_OK;
+    } else if (q.op == TQ_OP_AND) {
+      words.assign({(uint16_t)n_here, 0, 0, 0});
+      for (size_t a = 0; a < n_here; ++a) words.insert(words.end(), {1, (uint16_t)a});
+    } else {
+      words.assign({1, 0, 0, 0, (uint16_t)n_here});
+      for (size_t a = 0; a < n_here; ++a) words.push_back((uint16_t)a);
     }
-    if (q.op == TQ_OP_AND && n_here < q.n_terms) return TQ_OK;  // a clause without postings: empty intersection
     CountSeg cs{};
-    cs.query = qi; cs.lists_base = (uint32_t)cp.list_ids.size(); cs.n_lists = (uint32_t)n_here; cs.op = (uint32_t)q.op;
-    const Segment* seg = nullptr;
-    uint64_t df_single = 0;
-    for (size_t a = 0; a < n_here; ++a) {
-      uint32_t id;
-      const Segment* prev = seg;
-      int rc = get_list(c, *ts[a], false, pending, &id, &seg);
-      if (rc != TQ_OK) return rc;
-      if (a > 0 && !same_docs(*prev, *seg)) return fail_fields();
-      cp.list_ids.push_back(id);
-      df_single = ts[a]->doc_freq;
-    }
-    cs.max_doc = seg->max_doc;
     const FilterView* view = nullptr;
     const int arc = query_alive(c, q, *seg, &cs.alive, &view);
     if (arc != TQ_OK) return arc;
-    if (n_here == 1 && !cs.alive) {  // TermWeight::count without deletes (nor a filter): the term's doc_freq (term_weight.rs:179-190)
-      *host_add += df_single;
-      cp.list_ids.resize(cs.lists_base);
-    } else {
-      cut(cp.units, (uint32_t)cp.segs.size(), cs.max_doc, view);
-      cp.segs.push_back(cs);
+    if (q.op != TQ_OP_BOOL && n_here == 1 && !cs.alive) {  // TermWeight::count without deletes (nor a filter): the term's doc_freq (term_weight.rs:179-190)
+      *host_add += ts[0]->doc_freq;
+      return TQ_OK;
     }
+    cp.mixed = cp.mixed || words[1] != 0 || words[3] != 0;  // need, n_not
+    cs.query = qi; cs.words_base = (uint32_t)cp.words.size(); cs.max_doc = seg->max_doc;
+    cp.words.insert(cp.words.end(), words.begin(), words.end());
+    map_bool_clauses(cp.words.data() + cs.words_base, words.size(), [&](uint32_t a) { return ids[a]; });
+    // units of 8 tiles of 8192 docs over the segment; a filtered query's only over the tiles its filter view leaves non-empty
+    const uint32_t seg_idx = (uint32_t)cp.segs.size(), tiles = (cs.max_doc + kTileDocs - 1) / kTileDocs, per = 8;
+    if (!view) {
+      for (uint32_t t0 = 0; t0 < tiles; t0 += per) cp.units.push_back(Unit{seg_idx, t0, std::min(tiles, t0 + per), 0});
+    } else {
+      for (const TileRun& r : view->count_runs)
+        for (uint32_t t0 = r.t0; t0 < r.t1; t0 += per) cp.units.push_back(Unit{seg_idx, t0, std::min(r.t1, t0 + per), 0});
+    }
+    cp.segs.push_back(cs);
     return TQ_OK;
   });
 }
@@ -1615,7 +1604,7 @@ int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi) {
   if (route_to_tile(c, pl, qi, op, q_postings)) return TQ_OK;
   if (op == TQ_OP_BOOL && pl.n_plans) return fail(TQ_ERR_UNSUPPORTED, "TQ_OP_BOOL query does not fit the tile engine's buffers (split the batch / raise TQ_TILE_SCRATCH_MB)");
   append_qsegs(c, pl, qi, op);
-  // its hits: the Count kernels, in the same run (the per-query kernels leave no decoded lists behind)
+  // its hits: k_count, in the same run (the per-query kernels leave no decoded lists behind)
   return count ? plan_count(c, q, (uint32_t)qi, pl.pending, pl.order, pl.count, &pl.hits_host[qi]) : TQ_OK;
 }
 
@@ -1857,11 +1846,10 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     goff[gi] = GroupOff{st.add(gs.slots), st.add(gs.segs), st.add(gs.queries), st.add(gs.clauses), st.add(gunits[gi]), st.add(gs.chunks),
                         gs.count_units.empty() ? 0 : st.add(gs.count_units)};
   }
-  // the Count kernels of the TQ_QUERY_COUNT_HITS queries on the per-query kernels
+  // k_count for the TQ_QUERY_COUNT_HITS queries on the per-query kernels
   const CountPlan& cp = pl.count;
-  size_t o_cnt_ids = 0, o_cnt_segs = 0, o_cnt_units = 0, o_cntb_words = 0, o_cntb_segs = 0, o_cntb_units = 0;
-  if (!cp.units.empty()) { o_cnt_ids = st.add(cp.list_ids); o_cnt_segs = st.add(cp.segs); o_cnt_units = st.add(cp.units); }
-  if (!cp.bool_units.empty()) { o_cntb_words = st.add(cp.bool_words); o_cntb_segs = st.add(cp.bool_segs); o_cntb_units = st.add(cp.bool_units); }
+  size_t o_cnt_words = 0, o_cnt_segs = 0, o_cnt_units = 0;
+  if (!cp.units.empty()) { o_cnt_words = st.add(cp.words); o_cnt_segs = st.add(cp.segs); o_cnt_units = st.add(cp.units); }
   b->desc_bytes = st.bytes;
   TQ_CUDA(st.reserve(b->pin, b->dev));
 
@@ -1980,16 +1968,13 @@ int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
                                   reinterpret_cast<uint2*>(b->tile_dev.p + to_count_cursors), hits, ovf + gi};
     }
     b->n_count_units = (uint32_t)cp.units.size();
-    b->n_count_bool_units = (uint32_t)cp.bool_units.size();
+    b->count_mixed = cp.mixed;
     if (b->n_count_units)
-      b->count_p = CountParams{c->d_lists, st.on_device<const uint32_t>(o_cnt_ids), st.on_device<const CountSeg>(o_cnt_segs),
+      b->count_p = CountParams{c->d_lists, st.on_device<const uint32_t>(o_cnt_words), st.on_device<const CountSeg>(o_cnt_segs),
                                st.on_device<const Unit>(o_cnt_units), hits};
-    if (b->n_count_bool_units)
-      b->count_bool_p = CountBoolParams{c->d_lists, st.on_device<const uint32_t>(o_cntb_words), st.on_device<const CountBoolSeg>(o_cntb_segs),
-                                        st.on_device<const Unit>(o_cntb_units), hits};
   } else {
     b->hits_host.clear();
-    b->n_count_units = b->n_count_bool_units = 0;
+    b->n_count_units = 0;
   }
   TQ_CUDA(b->res_pin.ensure(b->res_bytes));
 
@@ -2111,7 +2096,7 @@ static int batch_prepare_impl(tq_ctx* c, const tq_query* queries, size_t nq, int
   b->stats.tile_postings = pl.tile_postings;
   for (auto& tg : pl.tgroups) b->stats.tile_list_bytes += tg.list_bytes;
   b->stats.tile_scratch_bytes = pl.tile_bytes;
-  b->stats.units_count_hits = (uint64_t)b->n_count_units + b->n_count_bool_units;
+  b->stats.units_count_hits = b->n_count_units;
   for (auto& g : b->groups) b->stats.units_count_hits += g.n_count_units;
   guard.ok = true;
   *out = b;
@@ -2224,8 +2209,8 @@ static int run_phase(tq_batch* b, int phase) {
     }
     if (b->count_hits) {
       // TQ_QUERY_COUNT_HITS: k_count_tiles reads the scored pairs and tile indexes, which nothing writes after k_score_lists, and
-      // adds to counters of its own -- it runs on the second stream next to the k_tile launches (as k_phrase does); the Count
-      // kernels of the queries on the per-query kernels go with it
+      // adds to counters of its own -- it runs on the second stream next to the k_tile launches (as k_phrase does); k_count for
+      // the queries on the per-query kernels goes with it
       const bool aside = tiles;
       cudaStream_t on = aside ? b->side : b->stream;
       if (aside) {
@@ -2235,8 +2220,7 @@ static int run_phase(tq_batch* b, int phase) {
       const int sp = span_begin(b, SPAN_COUNT, on);
       for (auto& g : b->groups)
         if (g.n_count_units) { k_count_tiles<<<g.n_count_units, kTileThreads, g.count_smem, on>>>(g.params, g.count); ++launches; }
-      if (b->n_count_bool_units) { k_count_bool<<<b->n_count_bool_units, kThreads, 0, on>>>(b->count_bool_p); ++launches; }
-      if (b->n_count_units) { k_count<<<b->n_count_units, kThreads, 0, on>>>(b->count_p); ++launches; }
+      if (b->n_count_units) { (b->count_mixed ? k_count<true> : k_count<false>)<<<b->n_count_units, kThreads, 0, on>>>(b->count_p); ++launches; }
       span_end(b, sp, on);
       TQ_CUDA(cudaGetLastError());
       if (aside) {
@@ -2472,7 +2456,7 @@ int tq_batch_fetch_hits(tq_batch* b, uint64_t* out_hits) {
   const uint64_t* hits = reinterpret_cast<const uint64_t*>(b->hits_pin.p);
   const uint32_t* ovf = reinterpret_cast<const uint32_t*>(hits + std::max<uint32_t>(b->nq, 1));
   for (uint32_t q = 0; q < b->nq; ++q) out_hits[q] = hits[q] + b->hits_host[q];
-  // a group whose tile held more sparse offsets than k_count_tiles keeps: its queries are counted again by the Count kernels
+  // a group whose tile held more sparse offsets than k_count_tiles keeps: its queries are counted again by k_count
   for (size_t gi = 0; gi < b->groups.size(); ++gi) {
     const std::vector<uint32_t>& qs = b->groups[gi].count_queries;
     if (!ovf[gi] || qs.empty()) continue;
@@ -2585,12 +2569,8 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
     if (rc != TQ_OK) return rc;
     hold_filters(c, b, queries, nq);  // (their views stay until the counts are in: the guard's tq_batch_destroy lets go)
   }
-  if (!cp.bool_units.empty()) {  // mixed boolean shapes: their own kernel, counts added to out_counts
-    const int rc = count_on_device(b, cp.bool_words, cp.bool_segs, cp.bool_units, nq, out_counts, k_count_bool);
-    if (rc != TQ_OK) return rc;
-  }
   if (cp.units.empty()) return TQ_OK;
-  return count_on_device(b, cp.list_ids, cp.segs, cp.units, nq, out_counts, k_count);
+  return count_on_device(b, cp.words, cp.segs, cp.units, cp.mixed, nq, out_counts);
 }
 
 // ---- codec-level access ---------------------------------------------------------------------------

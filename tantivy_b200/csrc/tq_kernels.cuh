@@ -1069,161 +1069,93 @@ __device__ __noinline__ void sort_pairs_desc(unsigned long long* a, uint32_t* b,
 }
 
 // ---- Count collector (N4): how many alive docs match, no scores ----------------------------------------------------
-// src/collector/count_collector.rs + Weight::count (term_weight.rs:179-219, boolean_weight.rs): one CTA walks its share
-// of a (query, segment)'s doc-id tiles; a tile is a bitmap in shared memory, a clause sets the bits of its postings
-// (OR: into the result, AND: into a scratch bitmap that is then intersected), the alive bitset is and-ed in, popcount.
+// src/collector/count_collector.rs + Weight::count (term_weight.rs:179-219; BooleanWeight::complex_scorer's scorer,
+// boolean_weight.rs:236-431): one CTA walks its share of a (query, segment)'s 8192-doc tiles.  Per tile a result bitmap in
+// shared memory = AND over the MUST groups of (OR of the group's clauses), SHOULD clauses counted per doc (byte counters, four
+// to a word) against `need`, MUST_NOT clauses cleared, alive bits and-ed in, popcount.  A term query is one MUST group of its
+// clause, an OR one group of all its clauses, an AND one group per clause.
+// words = [n_groups, need, n_should, n_not, (len, list ids..) per group, should list ids.., not list ids..] (32-bit).
 struct CountSeg {
-  uint32_t query, lists_base, n_lists, max_doc;
+  uint32_t query, words_base, max_doc, pad;
   const uint8_t* alive;
-  uint32_t op, pad;
 };
 struct CountParams {
   const ListDesc* lists;
-  const uint32_t* list_ids;
+  const uint32_t* words;
   const CountSeg* segs;
   const Unit* units;
   unsigned long long* counts;
 };
 
+// kMixed: some (query, segment) of the launch has SHOULD or MUST_NOT clauses.  Without them (every term, AND and OR query) every
+// pass is a MUST group: that instance has no SHOULD counters and no SHOULD or MUST_NOT pass per tile, which AND queries of
+// sparse lists otherwise pay for.
+template <bool kMixed>
 __global__ void __launch_bounds__(kThreads) k_count(const CountParams P) {
   constexpr uint32_t kWords = kTileDocs / 32u;
   __shared__ uint32_t s_acc[kWords], s_tmp[kWords];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
   __shared__ uint32_t s_part[kWarps];
   const Unit U = P.units[blockIdx.x];
   const CountSeg S = P.segs[U.qseg];
+  // (the words are read through P.words, a kernel parameter: no pointer of their own has to live through the posting walk)
+  const uint32_t wb = S.words_base, ng = P.words[wb], need = P.words[wb + 1u];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   uint32_t total = 0;
   for (uint32_t tile = U.begin; tile < U.end; ++tile) {
     const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
-    for (uint32_t c = 0; c < S.n_lists; ++c) {
-      uint32_t* bitmap = (S.op == 1u && c > 0) ? s_tmp : s_acc;  // 1 == TQ_OP_AND
-      if (c == 0 || S.op == 1u)
-        for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) bitmap[w] = 0;
+    // one pass per MUST group, then one over the SHOULD clauses and one over the MUST_NOT clauses: a pass marks its clauses'
+    // postings in s_tmp (SHOULD: counts them in s_cnt) and then narrows s_acc; the first MUST group marks s_acc itself.  One
+    // posting walk for every pass keeps the kernel's registers at those of a single inlined decode.
+    if (ng == 0u)
+      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] = 0xFFFFFFFFu;
+    uint32_t x = wb + 4u;
+    for (uint32_t p = 0; p < (kMixed ? ng + 2u : ng); ++p) {
+      const uint32_t kind = p < ng ? 0u : p - ng + 1u;  // 0: MUST group, 1: SHOULD, 2: MUST_NOT
+      const uint32_t len = kind == 0u ? P.words[x++] : P.words[wb + kind + 1u];
+      const bool should = kMixed && kind == 1u;
+      if (should ? need == 0u : len == 0u) { x += len; continue; }  // (a MUST group is never empty)
+      uint32_t* const bits = p == 0u ? s_acc : s_tmp;
+      if (should)
+        for (uint32_t w = threadIdx.x; w < kTileDocs / 4u; w += blockDim.x) s_cnt[w] = 0;
+      else
+        for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) bits[w] = 0;
       __syncthreads();
-      const ListDesc L = P.lists[P.list_ids[S.lists_base + c]];
-      const uint32_t j0 = first_block_ge(L.last_doc, 0, L.n_total, lo, lane);
-      for (uint32_t j = j0 + warp; j < L.n_total; j += kWarps) {
-        const uint32_t prev = __ldg(&L.tab4[j].w);
-        if (prev != 0xFFFFFFFFu && prev + 1u >= hi) break;  // the block starts at or after the tile's end
-        uint32_t doc[4], tf[4];
-        decode_block(L, j, lane, doc, tf);
+      for (const uint32_t end = x + len; x < end; ++x) {
+        const ListDesc L = P.lists[P.words[x]];
+        const uint32_t j0 = first_block_ge(L.last_doc, 0, L.n_total, lo, lane);
+        for (uint32_t j = j0 + warp; j < L.n_total; j += kWarps) {
+          const uint32_t prev = __ldg(&L.tab4[j].w);
+          if (prev != 0xFFFFFFFFu && prev + 1u >= hi) break;  // the block starts at or after the tile's end
+          uint32_t doc[4], tf[4];
+          decode_block(L, j, lane, doc, tf);
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (doc[i] >= lo && doc[i] < hi) atomicOr(&bitmap[(doc[i] - lo) >> 5], 1u << ((doc[i] - lo) & 31u));
-      }
-      __syncthreads();
-      if (S.op == 1u && c > 0) {
-        for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] &= s_tmp[w];
-        __syncthreads();
-      }
-    }
-    for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
-      uint32_t bits = s_acc[w];
-      if (bits && S.alive) bits &= __ldg(reinterpret_cast<const uint32_t*>(S.alive) + ((lo >> 5) + w));  // 32 docs per word, little endian
-      total += (uint32_t)__popc(bits);
-    }
-    __syncthreads();
-  }
-  total = __reduce_add_sync(kFull, total);
-  if (lane == 0) s_part[warp] = total;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long sum = 0;
-    for (int w = 0; w < kWarps; ++w) sum += s_part[w];
-    if (sum) atomicAdd(&P.counts[S.query], sum);
-  }
-}
-
-// Count for mixed boolean shapes (TQ_OP_BOOL; Weight::count over BooleanWeight::complex_scorer's scorer, boolean_weight.rs:236-431):
-// per 8192-doc tile a result bitmap = AND over the MUST groups of (OR of the group's clauses), SHOULD clauses counted per doc
-// (byte counters, four to a word) against `need`, MUST_NOT clauses cleared, alive bits and-ed in, popcount.
-// words = [n_groups, need, n_should, n_not, (len, list ids..) per group, should list ids.., not list ids..] (32-bit).
-struct CountBoolSeg {
-  uint32_t query, words_base, max_doc, pad;
-  const uint8_t* alive;
-};
-struct CountBoolParams {
-  const ListDesc* lists;
-  const uint32_t* words;
-  const CountBoolSeg* segs;
-  const Unit* units;
-  unsigned long long* counts;
-};
-
-template <class F>
-__device__ __forceinline__ void count_for_each_posting(const ListDesc& L, uint32_t lo, uint32_t hi, uint32_t lane, uint32_t warp, F f) {
-  const uint32_t j0 = first_block_ge(L.last_doc, 0, L.n_total, lo, lane);
-  for (uint32_t j = j0 + warp; j < L.n_total; j += kWarps) {
-    const uint32_t prev = __ldg(&L.tab4[j].w);
-    if (prev != 0xFFFFFFFFu && prev + 1u >= hi) break;  // the block starts at or after the tile's end
-    uint32_t doc[4], tf[4];
-    decode_block(L, j, lane, doc, tf);
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      if (doc[i] >= lo && doc[i] < hi) f(doc[i] - lo);
-  }
-}
-
-__global__ void __launch_bounds__(kThreads) k_count_bool(const CountBoolParams P) {
-  constexpr uint32_t kWords = kTileDocs / 32u;
-  __shared__ uint32_t s_acc[kWords], s_tmp[kWords];
-  __shared__ uint32_t s_cnt[kTileDocs / 4u];
-  __shared__ uint32_t s_part[kWarps];
-  const Unit U = P.units[blockIdx.x];
-  const CountBoolSeg S = P.segs[U.qseg];
-  const uint32_t* __restrict__ W = P.words + S.words_base;
-  const uint32_t ng = W[0], need = W[1], ns = W[2], nn = W[3];
-  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  uint32_t total = 0;
-  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
-    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
-    for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] = 0xFFFFFFFFu;
-    uint32_t x = 4;
-    for (uint32_t g = 0; g < ng; ++g) {
-      const uint32_t glen = W[x++];
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_tmp[w] = 0;
-      __syncthreads();
-      for (uint32_t e = 0; e < glen; ++e, ++x) {
-        const ListDesc L = P.lists[W[x]];
-        count_for_each_posting(L, lo, hi, lane, warp, [&](uint32_t o) { atomicOr(&s_tmp[o >> 5], 1u << (o & 31u)); });
-      }
-      __syncthreads();
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] &= s_tmp[w];
-      __syncthreads();
-    }
-    if (need) {
-      for (uint32_t w = threadIdx.x; w < kTileDocs / 4u; w += blockDim.x) s_cnt[w] = 0;
-      __syncthreads();
-      for (uint32_t e = 0; e < ns; ++e) {
-        const ListDesc L = P.lists[W[x + e]];
-        count_for_each_posting(L, lo, hi, lane, warp, [&](uint32_t o) { atomicAdd(&s_cnt[o >> 2], 1u << ((o & 3u) * 8u)); });  // <= 32 clauses: no carry
-      }
-      __syncthreads();
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
-        uint32_t m = 0;
-#pragma unroll
-        for (uint32_t b = 0; b < 8; ++b) {
-          const uint32_t c4 = s_cnt[w * 8u + b];
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) m |= (((c4 >> (8u * k)) & 255u) >= need ? 1u : 0u) << (b * 4u + k);
+          for (int i = 0; i < 4; ++i) {
+            const uint32_t o = doc[i] - lo;
+            if (doc[i] >= lo && doc[i] < hi) {
+              if (should) atomicAdd(&s_cnt[o >> 2], 1u << ((o & 3u) * 8u));  // <= 32 clauses: no carry
+              else atomicOr(&bits[o >> 5], 1u << (o & 31u));
+            }
+          }
         }
-        s_acc[w] &= m;
+      }
+      __syncthreads();
+      if (p == 0u && !should) continue;
+      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
+        uint32_t m = s_tmp[w];
+        if (should) {
+          m = 0;
+#pragma unroll
+          for (uint32_t b = 0; b < 8; ++b) {
+            const uint32_t c4 = s_cnt[w * 8u + b];
+#pragma unroll
+            for (uint32_t k = 0; k < 4; ++k) m |= (((c4 >> (8u * k)) & 255u) >= need ? 1u : 0u) << (b * 4u + k);
+          }
+        }
+        s_acc[w] &= kind == 2u ? ~m : m;
       }
       __syncthreads();
     }
-    x += ns;
-    if (nn) {
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_tmp[w] = 0;
-      __syncthreads();
-      for (uint32_t e = 0; e < nn; ++e) {
-        const ListDesc L = P.lists[W[x + e]];
-        count_for_each_posting(L, lo, hi, lane, warp, [&](uint32_t o) { atomicOr(&s_tmp[o >> 5], 1u << (o & 31u)); });
-      }
-      __syncthreads();
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] &= ~s_tmp[w];
-      __syncthreads();
-    }
-    __syncthreads();
     for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
       uint32_t bits = s_acc[w];
       const uint32_t first = lo + w * 32u;
@@ -1240,7 +1172,7 @@ __global__ void __launch_bounds__(kThreads) k_count_bool(const CountBoolParams P
   if (threadIdx.x == 0) {
     unsigned long long sum = 0;
     for (int w = 0; w < kWarps; ++w) sum += s_part[w];
-    if (sum) atomicAdd(&P.counts[S.query], sum);
+    if (sum) atomicAdd(&P.counts[P.segs[P.units[blockIdx.x].qseg].query], sum);  // (read here: nothing of it lives through the tiles)
   }
 }
 

@@ -1146,7 +1146,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
 // its clauses), keeps the docs that at least `need` SHOULD words list (a bit-sliced counter per lane: <= 32 clauses fit six words)
 // and clears the MUST_NOT words.  And-ed with the alive words (tq_segment_set_doc_range has cleared the docs outside the range in
 // them), popcount, a warp sum; one 64-bit add per (query, CTA).  A tile whose sparse offsets exceed kCountSparseCap sets the
-// group's overflow word: its flagged queries are then recounted by k_count / k_count_bool (tq_batch_fetch_hits).
+// group's overflow word: its flagged queries are then recounted by k_count (tq_batch_fetch_hits).
 constexpr uint8_t kTileQueryCount = 8;      // TQuery::flags bit 3: count the query's hits (k_tile does not read it)
 constexpr uint32_t kCountSparseCap = 8192;  // doc offsets of the sparse slots of one tile held in shared memory
 

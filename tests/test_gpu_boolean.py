@@ -28,7 +28,7 @@ def ctx(request):
 
 
 def _refused_but_counted(ctx, qb, oi):
-    """The per-query kernels have no TQ_OP_BOOL: the batch is refused (no silent fallback); Count (k_count_bool) answers."""
+    """The per-query kernels have no TQ_OP_BOOL: the batch is refused (no silent fallback); Count (k_count) answers."""
     with pytest.raises(T.TqError, match=_REFUSED):
         ctx.search_batch(qb)
     assert (ctx.count_batch(qb) == oi.count_batch(qb)).all()

@@ -246,7 +246,7 @@ def test_1025_query_batches(fx):
 
 def test_sparse_offsets_beyond_the_count_tile_buffer():
     """Ten lists that each hold every doc of the first tile, every list sparse (TQ_TILE_BIG_MIN): that tile has 10 240 sparse
-    offsets, more than k_count_tiles keeps; the group's queries are recounted by the Count kernels."""
+    offsets, more than k_count_tiles keeps; the group's queries are recounted by k_count."""
     rng = np.random.default_rng(77)
     max_doc = 300_000
     lengths = np.clip(np.round(np.exp(rng.normal(np.log(40), 0.7, size=max_doc))), 1, 4096).astype(np.uint32)

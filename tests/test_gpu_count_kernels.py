@@ -1,4 +1,4 @@
-"""The Count kernels (k_count, k_count_bool, k_count_tiles, k_filter_combine) against the score model at every tile, word and unit
+"""The Count kernels (k_count, k_count_tiles, k_filter_combine) against the score model at every tile, word and unit
 edge.  Every count is checked exactly against tests/score_model.py (the docs its scorers match, and-ed with the alive bits, the
 filter and the doc range, as M.count does); every batch that counts hits returns the same rows as the batch without the flag.
 
@@ -23,7 +23,7 @@ from tests.test_gpu_parity import _ctx_with_env, fresh_ord  # noqa: E402
 S, R, X = TQ_OCCUR_SHOULD, TQ_OCCUR_MUST, TQ_OCCUR_MUST_NOT
 NL = 32
 KS = (1, 10, 1000)
-TILE, CTILE = 1024, 8192  # k_count_tiles' tile (and 8 of them: its default unit), k_count / k_count_bool's tile
+TILE, CTILE = 1024, 8192  # k_count_tiles' tile (and 8 of them: its default unit), k_count's tile
 LADDER_DOCS = 34 * CTILE + 1003  # 273 tiles of 1024 docs, 35 of 8192 (the last ones partial), 11 docs in the last 32-doc word
 DENSE_MIN = 6  # TQ_TILE_BIG_MIN's default: a list with >= 6 postings per 1024-doc tile gets a presence map
 

@@ -897,7 +897,7 @@ def _bool_needs_the_tile_engine(ctx, qb):
     is refused as unsupported (no silent fallback), and the refusal leaves the context usable."""
     with pytest.raises(T.TqError, match="TQ_OP_BOOL needs term_occur and the tile engine"):
         ctx.search_batch(qb)
-    assert ctx.count_batch(qb).shape == (qb.nq,)  # Count (k_count_bool) runs on either engine
+    assert ctx.count_batch(qb).shape == (qb.nq,)  # Count (k_count) runs on either engine
 
 
 def test_mixed_boolean_shapes(ctx, synth):
@@ -937,7 +937,7 @@ def test_mixed_boolean_small_segments_with_deletes_and_absent_terms(ctx):
 
 
 def test_count_mixed_boolean_shapes(ctx, synth):
-    """searcher.search(&query, &Count) for the mixed shapes (k_count_bool): alive docs matching, vs the oracle's Count."""
+    """searcher.search(&query, &Count) for the mixed shapes (k_count): alive docs matching, vs the oracle's Count."""
     ix, oi, base = synth
     qs = [_bool_query(ix.query(TQ_OP_OR, terms, 1, segment_base=base), occ, grp, msm) for terms, occ, grp, msm in _BOOL_SHAPES]
     qb = QueryBatch(qs)
