@@ -13,6 +13,7 @@
 //
 // No tensor cores: the path is integer unpack + one f32 divide per posting (SURVEY.md §8d).
 #pragma once
+#include "tq_layout.h"
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -22,91 +23,10 @@ constexpr uint32_t kTerminated = 0x7FFFFFFFu;  // src/docset.rs:12
 constexpr uint32_t kNoList = 0xFFFFFFFFu;
 constexpr unsigned kFull = 0xFFFFFFFFu;
 
-constexpr int kThreads = 256;                 // 8 warps per CTA
-constexpr int kWarps = kThreads / 32;
 constexpr uint32_t kCap = 2048;               // CTA candidate buffer (u64 keys), power of two
 constexpr uint32_t kRoundMargin = kWarps * 128;  // most keys one round of 8 warps can push
-constexpr uint32_t kTileDocs = 8192;          // OR: doc-id tile width held in shared memory
-constexpr uint32_t kTfRows = 17;              // term frequencies below this use the precomputed factor table (tf_bits <= 4 => tf <= 16)
 
-// One posting list of one (segment, field, term), device resident.  Built once per term by
-// k_build_tables from the raw tantivy bytes and cached for the life of the segment (segments
-// are immutable, ARCHITECTURE.md "Searcher").
-struct ListDesc {
-  const uint8_t* blocks;      // the list's bit-packed blocks, copied 16-byte aligned when the table is built
-                              // (posting lists start at arbitrary byte offsets inside the .idx body)
-  const uint32_t* last_doc;   // [n_total] last doc id of every block; entry n_blocks = last tail doc
-  const uint2* blk;           // [n_blocks + 1] .x byte offset from `blocks`, .y packed meta
-  const uint4* tab4;          // [n_total] {last_doc, byte offset, meta, last doc of the previous block (0xFFFFFFFF: none)}
-                              // one 16-byte record per block so that a 32-wide probe yields position AND record
-  const uint32_t* tail_docs;  // [tail_n] the VInt tail, decoded at build time
-  const uint32_t* tail_tfs;   // [tail_n]
-  const uint8_t* fieldnorm;   // the segment's fieldnorm ids for this field; null => constant id 1
-  uint32_t n_blocks;          // full 128-doc blocks
-  uint32_t tail_n;            // docs in the VInt tail (0..127)
-  uint32_t n_total;           // n_blocks + (tail_n ? 1 : 0)
-  uint32_t doc_freq;
-  uint32_t has_freq;          // term frequencies are stored (else tf = 1)
-  uint32_t build_status;      // 0 ok, else corrupt
-};
-// meta bits: [0:5) doc_bits, bit 6 strict-delta, [8:14) tf_bits, [16:24) block-max fieldnorm id,
-// [24:32) block-max tf code (255 = saturated), see src/postings/skip.rs:16-22,205-253.
-
-struct QList {  // one clause of one query in one segment
-  uint32_t list_id;
-  float weight;        // Bm25Weight.weight
-  uint32_t cache_idx;  // which 256-entry tf-norm table
-  uint32_t pad;
-};
-struct QSeg {  // one (query, segment): what Collector::collect_segment sees
-  uint32_t query;
-  uint32_t lists_base;  // index into qlists; AND: ascending doc_freq (leader first); OR/TERM: clause order
-  uint32_t n_lists;
-  uint32_t max_doc;
-  uint32_t segment_ord;
-  uint32_t flags;        // bit 0: every clause reads the same fieldnorm array (`fieldnorm` below); bit 1: prunable (every
-                         // weight finite and >= 0); bit 2: AND in Intersection::score order, (s0 + s1) + (s2 + s3 + ...)
-  const uint8_t* alive;  // alive bitset bytes or null
-  const uint8_t* fieldnorm;  // shared fieldnorm ids (padded to a multiple of kTileDocs) when flags&1
-};
-struct Unit {  // one CTA's share of a QSeg
-  uint32_t qseg;
-  uint32_t begin, end;  // TERM/AND: block range of the (leader) list; OR: tile range
-  uint32_t pad;
-};
-struct DQuery {
-  uint32_t k;
-  uint32_t cand_base;  // first slot of this query's candidate region
-  uint32_t cand_cap;
-  uint32_t op;
-};
-struct QState {  // zeroed before every run
-  unsigned int theta;       // score key: lower bound of the final k-th best score
-  unsigned int cand_count;
-};
-struct Cand { uint32_t score_key, segment_ord, doc, pad; };
-
-struct BatchParams {
-  const ListDesc* lists;
-  const float* caches;  // [n_caches][256] tf-norm tables (bm25.rs:58-69)
-  const float* tf_tables;  // [n_caches][kTfRows][256]: tf / (tf + norm[id]) for tf < kTfRows
-  const QList* qlists;
-  const QSeg* qsegs;
-  const Unit* units;
-  const DQuery* queries;
-  QState* qstate;
-  Cand* cands;
-  float* res_scores;
-  uint32_t* res_segs;
-  uint32_t* res_docs;
-  uint32_t* res_counts;
-  uint32_t res_stride;
-  uint32_t n_queries;
-  unsigned long long* counters;  // [8] k_or_strip windows by route: 1 exhaustive, 2 hot, 3 cold; 5 bytes read
-  uint32_t reserved[4];          // unused: keeps the struct at 144 B.  At 128 B nvcc 12.9 loads the kernel parameters another
-                                 // way and the code of every kernel changes (k_or_strip measured 0.4% slower on an H100).
-  uint32_t* ovf;                 // set by k_final when a query was handed more candidates than its region holds (tile engine only), or null
-};
+// The descriptors (ListDesc, QList, QSeg, Unit, DQuery, QState, Cand) and BatchParams are in tq_layout.h.
 
 // ---- small helpers ---------------------------------------------------------------------------
 // Order preserving for every float, with -0.0 and +0.0 on ONE key (the reference compares scores with partial_cmp, which ties

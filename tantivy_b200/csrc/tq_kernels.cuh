@@ -15,14 +15,6 @@
 
 namespace tq {
 
-struct BuildJob {
-  const uint8_t* bytes;  // the term's postings range
-  uint32_t len;
-  uint32_t doc_freq;
-  uint32_t record_option;  // 0/1/2; bit 8: ignore term frequencies (score with tf = 1)
-  uint32_t list_id;
-};
-
 __device__ __forceinline__ uint32_t load_u32_unaligned(const uint8_t* p) {
   return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
@@ -613,22 +605,9 @@ __global__ void __launch_bounds__(kThreads, 3) k_or(const BatchParams P, uint32_
 //    16-byte block records gives position and record, the packed vectors follow (2 dependent loads);
 //  * thinner clauses keep their current block DECODED AND SCORED in shared memory (docs + scores); a window only
 //    looks at it when the block's next unread doc falls inside the window, so a block is decoded once per strip.
-// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or.
-constexpr uint32_t kWin = 1024;  // docs per window (multiple of 512)
+// Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or.  The limits
+// (kWin, kStripWarps, kStripMaxLists, ...) are in tq_layout.h.
 constexpr uint32_t kWBuf = 256;
-constexpr uint32_t kMaxCached = 6;
-constexpr uint32_t kStripWarps = 4;
-constexpr uint32_t kStripThreads = kStripWarps * 32;
-constexpr uint32_t kStripMaxLists = 8;
-constexpr uint32_t kStripMaxK = 128;
-// MaxScore split: a clause with at least one posting per kStripNeDiv docs may turn non-essential; in a union without
-// such a clause, the densest one may still go under the looser bound kStripNeDiv2.
-constexpr uint32_t kStripNeDiv = 8;
-constexpr uint32_t kStripNeDiv2 = 64;
-// Threshold sample: the three sample launches of a (query, segment) end at 1/32, 1/8 and 1/2 of its windows.
-constexpr uint32_t kStripSampleDiv = 32;
-constexpr uint32_t kStripSampleDiv2 = 8;
-constexpr uint32_t kStripSampleDiv3 = 2;
 constexpr uint32_t kNoDoc = 0xFFFFFFFFu;
 
 struct StripWarpFixed {  // per warp, dynamic shared memory; followed by n_cached x StripCache
@@ -644,9 +623,7 @@ struct StripCache {
   uint32_t doc[128];
   float score[128];
 };
-__host__ __device__ constexpr size_t strip_smem_bytes(uint32_t n_cached) {
-  return kStripWarps * (sizeof(StripWarpFixed) + (size_t)n_cached * sizeof(StripCache));
-}
+static_assert(sizeof(StripWarpFixed) == kStripWarpFixedBytes && sizeof(StripCache) == kStripCacheBytes, "strip_smem_bytes (tq_layout.h)");
 
 __device__ __forceinline__ void fetch_issue_rec(const ListDesc& L, const uint4 rec, uint32_t lane, BlockFetch& f) {
   f.meta = rec.z;
@@ -1074,18 +1051,7 @@ __device__ __noinline__ void sort_pairs_desc(unsigned long long* a, uint32_t* b,
 // shared memory = AND over the MUST groups of (OR of the group's clauses), SHOULD clauses counted per doc (byte counters, four
 // to a word) against `need`, MUST_NOT clauses cleared, alive bits and-ed in, popcount.  A term query is one MUST group of its
 // clause, an OR one group of all its clauses, an AND one group per clause.
-// words = [n_groups, need, n_should, n_not, (len, list ids..) per group, should list ids.., not list ids..] (32-bit).
-struct CountSeg {
-  uint32_t query, words_base, max_doc, pad;
-  const uint8_t* alive;
-};
-struct CountParams {
-  const ListDesc* lists;
-  const uint32_t* words;
-  const CountSeg* segs;
-  const Unit* units;
-  unsigned long long* counts;
-};
+// The structure words are CountParams::words (tq_layout.h).
 
 // kMixed: some (query, segment) of the launch has SHOULD or MUST_NOT clauses.  Without them (every term, AND and OR query) every
 // pass is a MUST group: that instance has no SHOULD counters and no SHOULD or MUST_NOT pass per tile, which AND queries of

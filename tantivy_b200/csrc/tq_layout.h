@@ -1,0 +1,307 @@
+// The host-device contract: every struct the host stages for the kernels (descriptors copied with one cudaMemcpyAsync, kernel
+// parameters), the capacities the planner sizes them by, and the shared-memory size of each kernel that takes a dynamic amount.
+// Host-only translation units include this header without the kernels (plain C++17 plus the CUDA include path); the kernel
+// headers include it instead of defining these themselves.  No kernel and no device-only function lives here.
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include "bm25_host.hpp"  // TQ_HD
+
+namespace tq {
+
+constexpr int kThreads = 256;                 // 8 warps per CTA
+constexpr int kWarps = kThreads / 32;
+constexpr uint32_t kTileDocs = 8192;          // OR: doc-id tile width held in shared memory
+constexpr uint32_t kTfRows = 17;              // term frequencies below this use the precomputed factor table (tf_bits <= 4 => tf <= 16)
+
+// ---- per-query kernels (tq_device.cuh, tq_kernels.cuh) ------------------------------------------------------------------
+
+// One posting list of one (segment, field, term), device resident.  Built once per term by
+// k_build_tables from the raw tantivy bytes and cached for the life of the segment (segments
+// are immutable, ARCHITECTURE.md "Searcher").
+struct ListDesc {
+  const uint8_t* blocks;      // the list's bit-packed blocks, copied 16-byte aligned when the table is built
+                              // (posting lists start at arbitrary byte offsets inside the .idx body)
+  const uint32_t* last_doc;   // [n_total] last doc id of every block; entry n_blocks = last tail doc
+  const uint2* blk;           // [n_blocks + 1] .x byte offset from `blocks`, .y packed meta
+  const uint4* tab4;          // [n_total] {last_doc, byte offset, meta, last doc of the previous block (0xFFFFFFFF: none)}
+                              // one 16-byte record per block so that a 32-wide probe yields position AND record
+  const uint32_t* tail_docs;  // [tail_n] the VInt tail, decoded at build time
+  const uint32_t* tail_tfs;   // [tail_n]
+  const uint8_t* fieldnorm;   // the segment's fieldnorm ids for this field; null => constant id 1
+  uint32_t n_blocks;          // full 128-doc blocks
+  uint32_t tail_n;            // docs in the VInt tail (0..127)
+  uint32_t n_total;           // n_blocks + (tail_n ? 1 : 0)
+  uint32_t doc_freq;
+  uint32_t has_freq;          // term frequencies are stored (else tf = 1)
+  uint32_t build_status;      // 0 ok, else corrupt
+};
+// meta bits: [0:5) doc_bits, bit 6 strict-delta, [8:14) tf_bits, [16:24) block-max fieldnorm id,
+// [24:32) block-max tf code (255 = saturated), see src/postings/skip.rs:16-22,205-253.
+
+struct BuildJob {
+  const uint8_t* bytes;  // the term's postings range
+  uint32_t len;
+  uint32_t doc_freq;
+  uint32_t record_option;  // 0/1/2; bit 8: ignore term frequencies (score with tf = 1)
+  uint32_t list_id;
+};
+
+struct QList {  // one clause of one query in one segment
+  uint32_t list_id;
+  float weight;        // Bm25Weight.weight
+  uint32_t cache_idx;  // which 256-entry tf-norm table
+  uint32_t pad;
+};
+struct QSeg {  // one (query, segment): what Collector::collect_segment sees
+  uint32_t query;
+  uint32_t lists_base;  // index into qlists; AND: ascending doc_freq (leader first); OR/TERM: clause order
+  uint32_t n_lists;
+  uint32_t max_doc;
+  uint32_t segment_ord;
+  uint32_t flags;        // bit 0: every clause reads the same fieldnorm array (`fieldnorm` below); bit 1: prunable (every
+                         // weight finite and >= 0); bit 2: AND in Intersection::score order, (s0 + s1) + (s2 + s3 + ...)
+  const uint8_t* alive;  // alive bitset bytes or null
+  const uint8_t* fieldnorm;  // shared fieldnorm ids (padded to a multiple of kTileDocs) when flags&1
+};
+struct Unit {  // one CTA's share of a QSeg
+  uint32_t qseg;
+  uint32_t begin, end;  // TERM/AND: block range of the (leader) list; OR: tile range
+  uint32_t pad;
+};
+struct DQuery {
+  uint32_t k;
+  uint32_t cand_base;  // first slot of this query's candidate region
+  uint32_t cand_cap;
+  uint32_t op;
+};
+struct QState {  // zeroed before every run
+  unsigned int theta;       // score key: lower bound of the final k-th best score
+  unsigned int cand_count;
+};
+struct Cand { uint32_t score_key, segment_ord, doc, pad; };
+
+struct BatchParams {
+  const ListDesc* lists;
+  const float* caches;  // [n_caches][256] tf-norm tables (bm25.rs:58-69)
+  const float* tf_tables;  // [n_caches][kTfRows][256]: tf / (tf + norm[id]) for tf < kTfRows
+  const QList* qlists;
+  const QSeg* qsegs;
+  const Unit* units;
+  const DQuery* queries;
+  QState* qstate;
+  Cand* cands;
+  float* res_scores;
+  uint32_t* res_segs;
+  uint32_t* res_docs;
+  uint32_t* res_counts;
+  uint32_t res_stride;
+  uint32_t n_queries;
+  unsigned long long* counters;  // [8] k_or_strip windows by route: 1 exhaustive, 2 hot, 3 cold; 5 bytes read
+  uint32_t reserved[4];          // unused: keeps the struct at 144 B.  At 128 B nvcc 12.9 loads the kernel parameters another
+                                 // way and the code of every kernel changes (k_or_strip measured 0.4% slower on an H100).
+  uint32_t* ovf;                 // set by k_final when a query was handed more candidates than its region holds (tile engine only), or null
+};
+
+static_assert(sizeof(ListDesc) == 80, "ListDesc layout");
+static_assert(sizeof(QList) == 16 && sizeof(QSeg) == 40 && sizeof(Unit) == 16 && sizeof(DQuery) == 16 && sizeof(Cand) == 16,
+              "per-query descriptor layout");
+static_assert(sizeof(BatchParams) == 144, "BatchParams must stay at 144 B (see `reserved`)");
+
+// k_or_strip (tq_kernels.cuh).  Eligible when k <= kStripMaxK, <= kStripMaxLists clauses and <= kMaxCached thin clauses; otherwise k_or.
+constexpr uint32_t kWin = 1024;  // docs per window (multiple of 512)
+constexpr uint32_t kMaxCached = 6;
+constexpr uint32_t kStripWarps = 4;
+constexpr uint32_t kStripThreads = kStripWarps * 32;
+constexpr uint32_t kStripMaxLists = 8;
+constexpr uint32_t kStripMaxK = 128;
+// MaxScore split: a clause with at least one posting per kStripNeDiv docs may turn non-essential; in a union without
+// such a clause, the densest one may still go under the looser bound kStripNeDiv2.
+constexpr uint32_t kStripNeDiv = 8;
+constexpr uint32_t kStripNeDiv2 = 64;
+// Threshold sample: the three sample launches of a (query, segment) end at 1/32, 1/8 and 1/2 of its windows.
+constexpr uint32_t kStripSampleDiv = 32;
+constexpr uint32_t kStripSampleDiv2 = 8;
+constexpr uint32_t kStripSampleDiv3 = 2;
+
+// Dynamic shared memory of k_or_strip: per warp a StripWarpFixed and n_cached StripCaches (sizes asserted beside the types).
+constexpr size_t kStripWarpFixedBytes = 7424, kStripCacheBytes = 1024;
+TQ_HD constexpr size_t strip_smem_bytes(uint32_t n_cached) {
+  return kStripWarps * (kStripWarpFixedBytes + (size_t)n_cached * kStripCacheBytes);
+}
+
+// words = [n_groups, need, n_should, n_not, (len, list ids..) per group, should list ids.., not list ids..] (32-bit).
+struct CountSeg {
+  uint32_t query, words_base, max_doc, pad;
+  const uint8_t* alive;
+};
+struct CountParams {
+  const ListDesc* lists;
+  const uint32_t* words;
+  const CountSeg* segs;
+  const Unit* units;
+  unsigned long long* counts;
+};
+
+// ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
+
+constexpr uint32_t kTile = 1024;            // docs per tile
+constexpr uint32_t kTileThreads = 256;
+constexpr uint32_t kTileWarps = kTileThreads / 32;
+constexpr uint32_t kTileMaxQueries = 1024;  // (query, segment) pairs of one group in one segment
+constexpr uint32_t kTileMaxSlots = 4096;    // distinct scored lists of one group in one segment
+constexpr uint32_t kTileMaxBig = 64;        // dense lists of one segment that get a tile index and a presence map
+constexpr uint32_t kTileMaxPairs = 12288;   // pairs of one tile held in shared memory (start | len are 16-bit fields)
+constexpr uint32_t kTileExactWindows = 2;   // warps that take heavy pairs in an exact launch (each owns a window of kTile f32 slots)
+constexpr uint32_t kNoSlot = 0xFFFFFFFFu;
+constexpr uint32_t kTileOpAnd = 1;  // TQ_OP_AND; term queries and unions share one evaluation (a union of one clause)
+constexpr uint32_t kTileOpBool = 3;  // TQ_OP_BOOL: the clause words are [n_groups, need_should, n_should, n_not, (len, slots..) per MUST group,
+                                     // SHOULD slots.., MUST_NOT slots..], groups by ascending cost, slots inside by descending weight
+
+struct TSlot {  // one distinct scored list of a group: (posting list, Bm25Weight.weight, tf-norm table)
+  uint32_t list_id;
+  float weight;
+  uint32_t cache_idx;
+  uint32_t doc_freq;
+  uint32_t pair_base;  // first element of this list's pairs in p_docs / p_scores (multiple of 128)
+  uint32_t big;        // column in the segment's tile index, kNoSlot for small lists
+  uint32_t tseg;
+  uint32_t pad;
+};
+struct TSeg {  // one segment of a group
+  uint32_t slot_base, n_slots, n_big;  // slots [0, n_big) have a tile index and are staged by whole warps
+  uint32_t query_base, n_queries;
+  uint32_t max_doc, segment_ord, n_tiles;
+  uint32_t clause_base, n_clause_words;  // this segment's share of TileParams::clauses (staged in shared memory when it fits)
+  uint32_t pad0, pad1;
+  const uint8_t* alive;
+  uint32_t* tix;  // [(n_tiles + 1)][n_big]: index of the list's first pair with doc >= tile * kTile (written by k_score_lists)
+};
+struct TQuery {  // one (query, segment): what Collector::collect_segment sees
+  uint32_t query;
+  uint32_t clause_base;  // into TileParams::clauses: slot ordinals (local to the segment) in canonical summation order
+  uint16_t n_clauses;
+  uint8_t op;
+  uint8_t flags;  // bit 0: prunable (every weight finite and >= 0);
+                  // bit 2: AND / BOOL groups in Intersection::score order, (s0 + s1) + (s2 + s3 + ...), not one after another
+};
+struct TUnit { uint32_t tseg, t0, t1, pad; };
+struct SChunk { uint32_t slot, b0, b1; };  // a CTA's share of k_score_lists: blocks [b0, b1) of one slot (global slot ordinal)
+
+static_assert(sizeof(TSlot) == 32 && sizeof(TSeg) == 64 && sizeof(TQuery) == 12 && sizeof(TUnit) == 16 && sizeof(SChunk) == 12,
+              "tile descriptor layout");
+
+struct TileParams {
+  const TSlot* slots;
+  const TSeg* segs;
+  const TQuery* queries;
+  const uint16_t* clauses;
+  const TUnit* units;
+  const SChunk* chunks;
+  uint32_t* p_docs;
+  float* p_scores;
+  uint32_t* samples;       // [n_queries of the batch][sample_cap] score keys
+  uint32_t* sample_count;  // [n_queries of the batch]
+  uint32_t* flags;         // [0]: a tile held more pairs than p_cap (the batch is re-run on the per-query kernels)
+  unsigned long long* counters;  // [16] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
+                                 //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold;
+                                 //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage);
+                                 //     [16, 16 + kOrExits) B2's union postings by exit (TileOrExit)
+                                 //     (null: the launch runs k_tile<*, false, *>)
+  uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
+  uint32_t sample_cap;
+  uint32_t p_cap;      // pairs of one tile that fit in shared memory
+  uint32_t max_slots;  // largest n_slots of any segment of the group
+  uint32_t max_big;    // ... n_big
+  uint32_t max_queries;  // ... n_queries
+  uint32_t cl_cap;     // clause words staged in shared memory per CTA (0: the segment's clauses are read from global memory)
+  uint32_t seg_cap;    // entries of the per-tile work list (essential clauses of the flat pairs)
+  uint32_t light_max;  // (query, tile) pairs with at most this many essential postings are evaluated posting by posting (flat path);
+                       // above it (and with more than one essential clause) a warp accumulates the query's window
+  uint32_t n_win;      // warps of a CTA that own a window (2: heavy pairs are rare; 8 for groups with wide queries)
+};
+
+// Sizes of k_tile's on-chip records (TileQ, TileSeg, TileTQ, TileStageA in tq_tile.cuh, asserted there).
+constexpr uint32_t kTileQBytes = 16, kTileSegBytes = 4, kTileTQBytes = 8, kTileStageABytes = 1056;
+
+// Shared memory of a k_tile CTA: byte offsets of its regions, in this order (the sparse slots' cursors are not on chip:
+// TileParams::cursors).  f32 scores [p_cap] at 0; the work list: TileQ records [max_queries] (`list`) + TileSeg segments [seg_cap]
+// (`seg`, which stage A uses for its TileStageA scratch), and in the same bytes the [n_win][kTile] f32 windows of the rare heavy
+// pairs (stage B3 starts after the last B2 of the tile); per slot: pair range start | len << 16 (`info`), largest score in the tile
+// (`max`, >= 0) and stripe mask [max_slots] each; presence maps [max_big][32]; TileTQ [max_queries]; u16 presence map ranks
+// [max_big][32], doc offsets [p_cap], heavy pairs [max_queries] and clause slots [cl_cap].
+struct TileSmem { uint32_t list, seg, info, max, mask, bits, tq, rank, off, heavy, cl, end; };
+TQ_HD constexpr TileSmem tile_smem_layout(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries,
+                                          uint32_t seg_cap, uint32_t cl_cap, uint32_t n_win) {
+  const uint32_t seg_bytes = seg_cap * kTileSegBytes > kTileStageABytes ? seg_cap * kTileSegBytes : kTileStageABytes;
+  const uint32_t list_bytes = max_queries * kTileQBytes + seg_bytes, win_bytes = n_win * kTile * 4u;
+  TileSmem L{};
+  L.list = p_cap * 4u;
+  L.seg = L.list + max_queries * kTileQBytes;
+  L.info = L.list + (((list_bytes > win_bytes ? list_bytes : win_bytes) + 15u) & ~15u);
+  L.max = L.info + max_slots * 4u; L.mask = L.max + max_slots * 4u; L.bits = L.mask + max_slots * 4u;
+  L.tq = L.bits + max_big * 128u;
+  L.rank = L.tq + max_queries * kTileTQBytes;
+  L.off = L.rank + max_big * 64u; L.heavy = L.off + p_cap * 2u; L.cl = L.heavy + max_queries * 2u;
+  L.end = L.cl + cl_cap * 2u + 64u;
+  return L;
+}
+TQ_HD constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries, uint32_t seg_cap,
+                                       uint32_t cl_cap, uint32_t n_win) {
+  return tile_smem_layout(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win).end;
+}
+
+// k_count_tiles
+constexpr uint8_t kTileQueryCount = 8;      // TQuery::flags bit 3: count the query's hits (k_tile does not read it)
+constexpr uint32_t kCountSparseCap = 8192;  // doc offsets of the sparse slots of one tile held in shared memory
+
+struct CountTileParams {
+  const TUnit* units;            // this group's count units
+  uint2* cursors;                // [CTAs][max_slots] sparse slots' cursors: (first pair not walked yet, its doc)
+  unsigned long long* hits;      // [queries of the batch]
+  uint32_t* overflow;            // this group's word: a tile held more sparse offsets than kCountSparseCap
+};
+
+// Shared memory of a k_count_tiles CTA: presence maps [max_big][32] | sparse slots' start | len << 16 [max_slots] |
+// per-query hit counts [max_queries] | sparse doc offsets (u16) [kCountSparseCap]
+TQ_HD constexpr size_t count_tiles_smem_bytes(uint32_t max_slots, uint32_t max_big, uint32_t max_queries) {
+  return (size_t)max_big * 128u + (size_t)max_slots * 4u + (size_t)max_queries * 4u + kCountSparseCap * 2u;
+}
+static_assert(count_tiles_smem_bytes(kTileMaxSlots, kTileMaxBig, kTileMaxQueries) <= 48u * 1024u,
+              "k_count_tiles launches without raising its dynamic shared memory limit");
+
+// ---- phrase queries (tq_phrase.cuh) ---------------------------------------------------------------------------------------
+
+constexpr uint32_t kPhraseMaxTerms = 8;
+constexpr uint32_t kPhraseWarps = 4;
+constexpr uint32_t kPhraseThreads = kPhraseWarps * 32;
+
+struct PosDesc {  // one term's position stream in one segment, built on first use and cached with the segment
+  const uint8_t* widths;                 // [n_blocks] bit width of every bit-packed block
+  const uint32_t* blk_off;               // [n_blocks + 1] byte offset of block b from `blocks`
+  const uint8_t* blocks;                 // the bit-packed blocks (in the `.pos` body, any alignment)
+  const uint32_t* tail;                  // [tail_n] the VInt-encoded rest, decoded
+  const unsigned long long* post_off;    // [n_posting_blocks + 1] positions that precede posting block b (last entry: the VInt tail block)
+  uint32_t n_blocks, tail_n, status, pad;
+};
+struct PosJob {
+  const uint8_t* pos_bytes;   // the term's positions range
+  uint32_t pos_len;
+  const uint8_t* list_bytes;  // the term's postings range (for the skip records)
+  uint32_t list_len;
+  uint32_t doc_freq;
+  uint32_t pos_id;
+  unsigned char* pool;        // the segment's table pool ...
+  unsigned long long* pool_cursor;  // ... bump-allocated on the device (the sizes are in the data)
+  unsigned long long pool_cap;
+};
+struct PhraseAux { uint32_t pos_id, offset, slop = 0; };  // per clause of a phrase (parallel to qlists): its position table, max_offset - its offset, the phrase's slop
+
+// dynamic shared memory: per warp [128][ct] PhraseCand (ct = most terms of a phrase in the batch) + [128 docs | 128 tfs | 128 prefixes]
+// of a decoded secondary block (reused for the compacted matches)
+constexpr size_t kPhraseCandBytes = 12;  // sizeof(PhraseCand), asserted beside it
+TQ_HD constexpr size_t phrase_smem_bytes(uint32_t ct) { return kPhraseWarps * (128u * ct * kPhraseCandBytes + 384u * 4u); }
+
+}  // namespace tq

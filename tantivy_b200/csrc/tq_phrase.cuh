@@ -17,30 +17,7 @@
 
 namespace tq {
 
-constexpr uint32_t kPhraseMaxTerms = 8;
-constexpr uint32_t kPhraseWarps = 4;
-constexpr uint32_t kPhraseThreads = kPhraseWarps * 32;
-
-struct PosDesc {  // one term's position stream in one segment, built on first use and cached with the segment
-  const uint8_t* widths;                 // [n_blocks] bit width of every bit-packed block
-  const uint32_t* blk_off;               // [n_blocks + 1] byte offset of block b from `blocks`
-  const uint8_t* blocks;                 // the bit-packed blocks (in the `.pos` body, any alignment)
-  const uint32_t* tail;                  // [tail_n] the VInt-encoded rest, decoded
-  const unsigned long long* post_off;    // [n_posting_blocks + 1] positions that precede posting block b (last entry: the VInt tail block)
-  uint32_t n_blocks, tail_n, status, pad;
-};
-struct PosJob {
-  const uint8_t* pos_bytes;   // the term's positions range
-  uint32_t pos_len;
-  const uint8_t* list_bytes;  // the term's postings range (for the skip records)
-  uint32_t list_len;
-  uint32_t doc_freq;
-  uint32_t pos_id;
-  unsigned char* pool;        // the segment's table pool ...
-  unsigned long long* pool_cursor;  // ... bump-allocated on the device (the sizes are in the data)
-  unsigned long long pool_cap;
-};
-struct PhraseAux { uint32_t pos_id, offset, slop = 0; };  // per clause of a phrase (parallel to qlists): its position table, max_offset - its offset, the phrase's slop
+// (kPhraseMaxTerms, PosDesc, PosJob, PhraseAux and phrase_smem_bytes: tq_layout.h)
 
 __global__ void __launch_bounds__(kThreads) k_build_pos_tables(const PosJob* __restrict__ jobs, PosDesc* __restrict__ descs, uint32_t* __restrict__ status_out) {
   const PosJob J = jobs[blockIdx.x];
@@ -186,6 +163,7 @@ __device__ __forceinline__ uint32_t pos_delta(const PosDesc& D, unsigned long lo
 }
 
 struct PhraseCand { uint32_t pos_lo, pos_hi, tf; };  // first delta of the doc in the term's stream (64-bit), its term frequency
+static_assert(sizeof(PhraseCand) == kPhraseCandBytes, "phrase_smem_bytes (tq_layout.h)");
 
 // Two terms with slop: intersection_count_with_slop (phrase_scorer.rs:145-186) over the two position streams, left = the term the
 // Intersection puts first (ascending size_hint).  A left position within `slop` of the right one matches; the left cursor first moves
@@ -264,10 +242,6 @@ __device__ __forceinline__ void tf_prefix(const uint32_t (&tf)[4], uint32_t lane
   const uint32_t incl = warp_incl_scan(s, lane);
   pre[0] = incl - s; pre[1] = pre[0] + tf[0]; pre[2] = pre[1] + tf[1]; pre[3] = pre[2] + tf[2];
 }
-
-// dynamic shared memory: per warp [128][ct] PhraseCand (ct = most terms of a phrase in the batch) + [128 docs | 128 tfs | 128 prefixes]
-// of a decoded secondary block (reused for the compacted matches)
-__host__ __device__ constexpr size_t phrase_smem_bytes(uint32_t ct) { return kPhraseWarps * (128u * ct * sizeof(PhraseCand) + 384u * 4u); }
 
 __global__ void __launch_bounds__(kPhraseThreads, 5) k_phrase(const BatchParams P, const PosDesc* __restrict__ pdescs, const PhraseAux* __restrict__ aux_all,
                                                            uint32_t unit_base, uint32_t ct) {

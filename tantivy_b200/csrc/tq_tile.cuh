@@ -42,80 +42,9 @@
 
 namespace tq {
 
-constexpr uint32_t kTile = 1024;            // docs per tile
-constexpr uint32_t kTileThreads = 256;
-constexpr uint32_t kTileWarps = kTileThreads / 32;
-constexpr uint32_t kTileMaxQueries = 1024;  // (query, segment) pairs of one group in one segment
-constexpr uint32_t kTileMaxSlots = 4096;    // distinct scored lists of one group in one segment
-constexpr uint32_t kTileMaxBig = 64;        // dense lists of one segment that get a tile index and a presence map
-constexpr uint32_t kTileMaxPairs = 12288;   // pairs of one tile held in shared memory (start | len are 16-bit fields)
-constexpr uint32_t kTileExactWindows = 2;   // warps that take heavy pairs in an exact launch (each owns a window of kTile f32 slots)
+// The tile engine's limits, descriptors (TSlot, TSeg, TQuery, TUnit, SChunk) and TileParams are in tq_layout.h.
 constexpr uint32_t kSampleSeg = 6;          // sample launch: postings scored per driving clause and (query, tile)
 constexpr uint32_t kSamplePerTile = 4;      // sample launch: the best few partial maxima of a (query, tile)
-constexpr uint32_t kNoSlot = 0xFFFFFFFFu;
-constexpr uint32_t kTileOpAnd = 1;  // TQ_OP_AND; term queries and unions share one evaluation (a union of one clause)
-constexpr uint32_t kTileOpBool = 3;  // TQ_OP_BOOL: the clause words are [n_groups, need_should, n_should, n_not, (len, slots..) per MUST group,
-                                     // SHOULD slots.., MUST_NOT slots..], groups by ascending cost, slots inside by descending weight
-
-struct TSlot {  // one distinct scored list of a group: (posting list, Bm25Weight.weight, tf-norm table)
-  uint32_t list_id;
-  float weight;
-  uint32_t cache_idx;
-  uint32_t doc_freq;
-  uint32_t pair_base;  // first element of this list's pairs in p_docs / p_scores (multiple of 128)
-  uint32_t big;        // column in the segment's tile index, kNoSlot for small lists
-  uint32_t tseg;
-  uint32_t pad;
-};
-struct TSeg {  // one segment of a group
-  uint32_t slot_base, n_slots, n_big;  // slots [0, n_big) have a tile index and are staged by whole warps
-  uint32_t query_base, n_queries;
-  uint32_t max_doc, segment_ord, n_tiles;
-  uint32_t clause_base, n_clause_words;  // this segment's share of TileParams::clauses (staged in shared memory when it fits)
-  uint32_t pad0, pad1;
-  const uint8_t* alive;
-  uint32_t* tix;  // [(n_tiles + 1)][n_big]: index of the list's first pair with doc >= tile * kTile (written by k_score_lists)
-};
-struct TQuery {  // one (query, segment): what Collector::collect_segment sees
-  uint32_t query;
-  uint32_t clause_base;  // into TileParams::clauses: slot ordinals (local to the segment) in canonical summation order
-  uint16_t n_clauses;
-  uint8_t op;
-  uint8_t flags;  // bit 0: prunable (every weight finite and >= 0);
-                  // bit 2: AND / BOOL groups in Intersection::score order, (s0 + s1) + (s2 + s3 + ...), not one after another
-};
-struct TUnit { uint32_t tseg, t0, t1, pad; };
-struct SChunk { uint32_t slot, b0, b1; };  // a CTA's share of k_score_lists: blocks [b0, b1) of one slot (global slot ordinal)
-
-struct TileParams {
-  const TSlot* slots;
-  const TSeg* segs;
-  const TQuery* queries;
-  const uint16_t* clauses;
-  const TUnit* units;
-  const SChunk* chunks;
-  uint32_t* p_docs;
-  float* p_scores;
-  uint32_t* samples;       // [n_queries of the batch][sample_cap] score keys
-  uint32_t* sample_count;  // [n_queries of the batch]
-  uint32_t* flags;         // [0]: a tile held more pairs than p_cap (the batch is re-run on the per-query kernels)
-  unsigned long long* counters;  // [16] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
-                                 //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold;
-                                 //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage);
-                                 //     [16, 16 + kOrExits) B2's union postings by exit (TileOrExit)
-                                 //     (null: the launch runs k_tile<*, false, *>)
-  uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
-  uint32_t sample_cap;
-  uint32_t p_cap;      // pairs of one tile that fit in shared memory
-  uint32_t max_slots;  // largest n_slots of any segment of the group
-  uint32_t max_big;    // ... n_big
-  uint32_t max_queries;  // ... n_queries
-  uint32_t cl_cap;     // clause words staged in shared memory per CTA (0: the segment's clauses are read from global memory)
-  uint32_t seg_cap;    // entries of the per-tile work list (essential clauses of the flat pairs)
-  uint32_t light_max;  // (query, tile) pairs with at most this many essential postings are evaluated posting by posting (flat path);
-                       // above it (and with more than one essential clause) a warp accumulates the query's window
-  uint32_t n_win;      // warps of a CTA that own a window (2: heavy pairs are rare; 8 for groups with wide queries)
-};
 
 
 // ---- K1 + K2, once per batch -------------------------------------------------------------------------------------------
@@ -404,32 +333,8 @@ struct TileStageA {
   uint32_t wa[kTileWarps][8];
 };
 
-// Shared memory of a k_tile CTA: byte offsets of its regions, in this order (the sparse slots' cursors are not on chip:
-// TileParams::cursors).  f32 scores [p_cap] at 0; the work list: TileQ records [max_queries] (`list`) + TileSeg segments [seg_cap]
-// (`seg`, which stage A uses for its TileStageA scratch), and in the same bytes the [n_win][kTile] f32 windows of the rare heavy
-// pairs (stage B3 starts after the last B2 of the tile); per slot: pair range start | len << 16 (`info`), largest score in the tile
-// (`max`, >= 0) and stripe mask [max_slots] each; presence maps [max_big][32]; TileTQ [max_queries]; u16 presence map ranks
-// [max_big][32], doc offsets [p_cap], heavy pairs [max_queries] and clause slots [cl_cap].
-struct TileSmem { uint32_t list, seg, info, max, mask, bits, tq, rank, off, heavy, cl, end; };
-__host__ __device__ constexpr TileSmem tile_smem_layout(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries,
-                                                        uint32_t seg_cap, uint32_t cl_cap, uint32_t n_win) {
-  const uint32_t seg_bytes = seg_cap * (uint32_t)sizeof(TileSeg) > (uint32_t)sizeof(TileStageA) ? seg_cap * (uint32_t)sizeof(TileSeg) : (uint32_t)sizeof(TileStageA);
-  const uint32_t list_bytes = max_queries * (uint32_t)sizeof(TileQ) + seg_bytes, win_bytes = n_win * kTile * 4u;
-  TileSmem L{};
-  L.list = p_cap * 4u;
-  L.seg = L.list + max_queries * (uint32_t)sizeof(TileQ);
-  L.info = L.list + (((list_bytes > win_bytes ? list_bytes : win_bytes) + 15u) & ~15u);
-  L.max = L.info + max_slots * 4u; L.mask = L.max + max_slots * 4u; L.bits = L.mask + max_slots * 4u;
-  L.tq = L.bits + max_big * 128u;
-  L.rank = L.tq + max_queries * (uint32_t)sizeof(TileTQ);
-  L.off = L.rank + max_big * 64u; L.heavy = L.off + p_cap * 2u; L.cl = L.heavy + max_queries * 2u;
-  L.end = L.cl + cl_cap * 2u + 64u;
-  return L;
-}
-__host__ __device__ constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t max_slots, uint32_t max_big, uint32_t max_queries, uint32_t seg_cap,
-                                                      uint32_t cl_cap, uint32_t n_win) {
-  return tile_smem_layout(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win).end;
-}
+static_assert(sizeof(TileQ) == kTileQBytes && sizeof(TileSeg) == kTileSegBytes && sizeof(TileTQ) == kTileTQBytes &&
+                  sizeof(TileStageA) == kTileStageABytes, "tile_smem_layout (tq_layout.h)");
 
 __device__ __forceinline__ TileView tile_view(unsigned char* s_dyn, const TileParams& TP, uint32_t n_big) {
   const TileSmem L = tile_smem_layout(TP.p_cap, TP.max_slots, TP.max_big, TP.max_queries, TP.seg_cap, TP.cl_cap, TP.n_win);
@@ -1147,23 +1052,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
 // and clears the MUST_NOT words.  And-ed with the alive words (tq_segment_set_doc_range has cleared the docs outside the range in
 // them), popcount, a warp sum; one 64-bit add per (query, CTA).  A tile whose sparse offsets exceed kCountSparseCap sets the
 // group's overflow word: its flagged queries are then recounted by k_count (tq_batch_fetch_hits).
-constexpr uint8_t kTileQueryCount = 8;      // TQuery::flags bit 3: count the query's hits (k_tile does not read it)
-constexpr uint32_t kCountSparseCap = 8192;  // doc offsets of the sparse slots of one tile held in shared memory
-
-struct CountTileParams {
-  const TUnit* units;            // this group's count units
-  uint2* cursors;                // [CTAs][max_slots] sparse slots' cursors: (first pair not walked yet, its doc)
-  unsigned long long* hits;      // [queries of the batch]
-  uint32_t* overflow;            // this group's word: a tile held more sparse offsets than kCountSparseCap
-};
-
-// Shared memory of a k_count_tiles CTA: presence maps [max_big][32] | sparse slots' start | len << 16 [max_slots] |
-// per-query hit counts [max_queries] | sparse doc offsets (u16) [kCountSparseCap]
-__host__ __device__ constexpr size_t count_tiles_smem_bytes(uint32_t max_slots, uint32_t max_big, uint32_t max_queries) {
-  return (size_t)max_big * 128u + (size_t)max_slots * 4u + (size_t)max_queries * 4u + kCountSparseCap * 2u;
-}
-static_assert(count_tiles_smem_bytes(kTileMaxSlots, kTileMaxBig, kTileMaxQueries) <= 48u * 1024u,
-              "k_count_tiles launches without raising its dynamic shared memory limit");
+// (kTileQueryCount, kCountSparseCap, CountTileParams and count_tiles_smem_bytes: tq_layout.h)
 
 // Lane `lane`'s stripe word of `slot` in this tile: bit i = the slot lists doc lo + 32 * lane + i.
 __device__ __forceinline__ uint32_t count_word(const uint32_t* bits, const uint32_t* info, const uint16_t* off, uint32_t n_big, uint32_t slot,

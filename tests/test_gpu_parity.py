@@ -887,6 +887,54 @@ def test_multi_handle_split_segment(synth):
         m.close()
 
 
+def _returns_within(fn, seconds=120):
+    """fn() on a daemon thread: a call that never returns fails the test instead of hanging the run."""
+    import threading
+    out = {}
+
+    def run():
+        try:
+            out["value"] = fn()
+        except BaseException as e:  # noqa: BLE001 (handed to the caller)
+            out["error"] = e
+    t = threading.Thread(target=run, daemon=True)
+    t.start()
+    t.join(seconds)
+    if t.is_alive():
+        return False, None
+    if "error" in out:
+        raise out["error"]
+    return True, out["value"]
+
+
+@pytest.mark.parametrize("bad_device", [0, 1])
+def test_multi_handle_prepare_fails_on_one_device(synth, bad_device):
+    """A batch whose prepare fails on one device of the handle only (a duplicated (term_idx, segment_ord) on a segment that device
+    owns) fails as a whole: the other devices' workers leave the key exchange, the call returns an error instead of waiting for
+    the failed worker, and the handle answers the next batch like one context."""
+    ix, oi, base = synth
+    m = T.MultiContext([0, 0])
+    hung = False
+    try:
+        for s in range(ix.n_segments):
+            m.segment_register(base + s, 0, ix.max_doc[s], ix.record_option, ix.body(s), ix.fieldnorm(s), None, device_index=s % 2)
+        good = ix.query(TQ_OP_OR, [0, 1, 2], 10, segment_base=base)
+        dup = next(ts for ts in good["term_segs"] if (ts[1] - base) % 2 == bad_device)
+        bad = dict(good, term_segs=good["term_segs"] + [dup])
+        with pytest.raises(T.TqError):
+            done, _ = _returns_within(lambda: m.search_batch(QueryBatch([good, bad])))
+            hung = not done
+            assert done, "tq_multi_search_batch did not return after a prepare failed on one device"
+        qb = QueryBatch([good, ix.query(TQ_OP_AND, [0, 1], 10, segment_base=base)])
+        done, rows = _returns_within(lambda: m.search_batch(qb))
+        hung = not done
+        assert done
+        assert_same(rows, oi.search_batch(qb, mode=0, n_threads=8), qb.nq)
+    finally:
+        if not hung:  # (a worker still blocked in the handle must not see it destroyed)
+            m.close()
+
+
 # ---- N4: mixed boolean shapes (TQ_OP_BOOL) --------------------------------------------------------------------------
 _bool_query = bool_query
 _BOOL_SHAPES = BOOL_SHAPES
