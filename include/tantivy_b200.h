@@ -203,6 +203,12 @@ typedef struct {
                                    non-essential walk, [3] completed */
   float count_hits_ms;          /* device time of the launches that count TQ_QUERY_COUNT_HITS queries (k_count_tiles, k_count) */
   uint64_t units_count_hits;    /* CTAs of those launches */
+  /* cumulative since ctx creation: tq_sort_batch.  Device time of k_sort + k_sort_final, their CTAs (one per unit of up to eight
+   * 8192-doc tiles, plus one per query), and the 8192-doc tiles the units came to and of those the ones skipped by the bound. */
+  float sort_ms;
+  uint64_t units_sort;
+  uint64_t sort_tiles_seen;
+  uint64_t sort_tiles_skipped;
 } tq_stats;
 
 /* ---- context ------------------------------------------------------------------------- */
@@ -256,6 +262,27 @@ int tq_filter_register(tq_ctx*, uint32_t filter_id, uint32_t segment_ord, const 
 /* Frees every bitset of the filter; TQ_ERR_NOT_FOUND if none is registered. */
 int tq_filter_unregister(tq_ctx*, uint32_t filter_id);
 
+/* Sort columns (TopDocs::order_by_fast_field / order_by_u64_field: SortByStaticFastValue, src/collector/sort_key/
+ * sort_by_static_fast_value.rs).  The caller materialises the segment's `Column::first(doc)` once: values[d] = the u64 image of
+ * doc d's first value (common/src/lib.rs: u64 as is; i64 and DateTime v ^ 1 << 63; f64 bits ^ 1 << 63 when the sign bit is clear,
+ * !bits when it is set; bool 0 / 1), and `present` in the `.del` layout (bit set = doc d has a value; NULL = every doc has one).
+ * Both are copied.  The rules are tq_filter_register's: a column belongs to a segment ordinal, not to a field; at least one field of
+ * the ordinal must be registered (else TQ_ERR_NOT_FOUND); n_values must equal max_doc and present_len * 8 >= max_doc (else
+ * TQ_ERR_INVALID_ARGUMENT); registering a (column, segment) again replaces it; unregistering the last field of a segment ordinal
+ * drops the ordinal's columns.  tq_sort_column_register / _unregister of a column return TQ_ERR_INVALID_ARGUMENT while a
+ * tq_sort_batch on another thread reads it. */
+int tq_sort_column_register(tq_ctx*, uint32_t column_id, uint32_t segment_ord, const uint64_t* values, size_t n_values,
+                            const uint8_t* present, size_t present_len);
+/* Frees every segment's column of column_id; TQ_ERR_NOT_FOUND if none is registered. */
+int tq_sort_column_unregister(tq_ctx*, uint32_t column_id);
+
+#define TQ_ORDER_DESC 0u /* Order::Desc (ComparatorEnum::Natural): larger values first */
+#define TQ_ORDER_ASC 1u  /* Order::Asc (ComparatorEnum::ReverseNoneLower): smaller values first */
+typedef struct {
+  uint32_t column_id; /* as given to tq_sort_column_register */
+  uint32_t order;     /* TQ_ORDER_DESC / TQ_ORDER_ASC */
+} tq_sort_spec;
+
 /* ---- search -------------------------------------------------------------------------- */
 /* The whole hot path for a batch of queries, host buffers in / host buffers out:
  * block decode -> AND/OR/term -> BM25 -> per-segment top-k -> merge_fruits.
@@ -272,6 +299,19 @@ int tq_search_batch(tq_ctx*, const tq_query* queries, size_t nq, uint32_t out_st
  * segment without deletes is answered from doc_freq, as the reference does -- unless it carries TQ_QUERY_FILTER (Count inside
  * FilterCollector): then only the docs its filter keeps are counted, over the 8192-doc tiles the filter leaves non-empty. */
 int tq_count_batch(tq_ctx*, const tq_query* queries, size_t nq, uint64_t* out_counts);
+
+/* TopDocs::with_limit(k).order_by_fast_field(column, order) for term / AND / OR / mixed boolean (TQ_OP_BOOL) queries, synchronous
+ * like tq_count_batch: the docs tq_count_batch counts (alive, inside the doc ranges, kept by the query's filter with
+ * TQ_QUERY_FILTER), keyed by sorts[q]'s column.  Row q (out_stride >= k entries apart) holds out_count[q] <= k hits: the docs with
+ * a value by value (desc or asc), then the docs without one; ties, None docs included, by (segment_ord asc, doc asc) in both orders
+ * (compare_for_top_k, top_score_collector.rs:591-600; order.rs:286-293).  out_values[i] = the u64 image of the hit's value (0 for
+ * a doc without one), out_present[i] = 1 if it has one.  `and_offset(o)` is k = limit + o and skipping o rows.  out_hits may be
+ * NULL; else out_hits[q] = tq_count_batch's answer for query q, (Count, TopDocs::order_by_fast_field), and every tile of the query
+ * is visited.  k must be in 1..TQ_MAX_K.  Weights are read where tq_count_batch reads them (TQ_OP_BOOL); thresholds and
+ * TQ_QUERY_COUNT_HITS are ignored.  TQ_OP_PHRASE returns TQ_ERR_UNSUPPORTED; a segment the query names without a column for
+ * sorts[q].column_id returns TQ_ERR_NOT_FOUND. */
+int tq_sort_batch(tq_ctx*, const tq_query* queries, const tq_sort_spec* sorts, size_t nq, uint32_t out_stride, uint64_t* out_values,
+                  uint8_t* out_present, uint32_t* out_segment_ord, uint32_t* out_doc, uint32_t* out_count, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

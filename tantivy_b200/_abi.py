@@ -18,6 +18,7 @@ TQ_TERM_IGNORE_FREQ = 1
 TQ_QUERY_HAS_THRESHOLD = 1
 TQ_QUERY_COUNT_HITS = 2
 TQ_QUERY_FILTER = 4
+TQ_ORDER_DESC, TQ_ORDER_ASC = 0, 1
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -131,7 +132,20 @@ class Stats(C.Structure):
         ("tile_b2_exits", C.c_uint64 * 4),
         ("count_hits_ms", C.c_float),
         ("units_count_hits", C.c_uint64),
+        ("sort_ms", C.c_float),
+        ("units_sort", C.c_uint64),
+        ("sort_tiles_seen", C.c_uint64),
+        ("sort_tiles_skipped", C.c_uint64),
     ]
+
+
+class SortSpec(C.Structure):
+    """tq_sort_spec — the column and Order of TopDocs::order_by_fast_field for one query."""
+    _fields_ = [("column_id", C.c_uint32), ("order", C.c_uint32)]
+
+
+SORT_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("order", "<u4")])
+assert SORT_SPEC_DTYPE.itemsize == C.sizeof(SortSpec) == 8
 
 
 def ptr(arr, typ):

@@ -159,6 +159,7 @@ struct tq_batch {
   PinBuf hits_pin;
   std::vector<std::pair<uint32_t, uint32_t>> held;  // the (segment, field)s its queries name, counted in tq_ctx::seg_users until destroyed
   std::vector<uint32_t> held_filters;               // the filters its queries name, counted in tq_ctx::filter_users until destroyed
+  std::vector<uint32_t> held_columns;               // tq_sort_batch: the sort columns it reads, counted in tq_ctx::sort_users
 };
 
 // host twin of score_to_key (tq_device.cuh): order-preserving u32 image of a float, -0.0 and +0.0 on one key
@@ -350,6 +351,7 @@ void tq_ctx_destroy(tq_ctx* c) {
     kv.second.arena.release();
   }
   for (auto& kv : c->filter_views) cudaFree(kv.second.d_bits);
+  for (auto& kv : c->sort_columns) kv.second.release();
   cudaFree(c->d_pos_descs);
   c->build_pin.release(); c->build_dev.release();
   if (c->build_stream) cudaStreamDestroy(c->build_stream);
@@ -371,6 +373,10 @@ int tq_get_stats(tq_ctx* c, tq_stats* out) {
   }
   out->tile_counters[7] = c->tile_smem_last;
   out->tile_ctas_per_sm = c->tile_ctas_last;
+  out->sort_ms = (float)c->sort_ms;
+  out->units_sort = c->sort_units;
+  out->sort_tiles_seen = c->sort_tiles_seen;
+  out->sort_tiles_skipped = c->sort_tiles_skipped;
   return TQ_OK;
 }
 
@@ -510,9 +516,12 @@ int tq_segment_unregister(tq_ctx* c, uint32_t segment_ord, uint32_t field) {
   c->list_tables.drop([&](const ListKey& k) { return k.segment_ord == segment_ord && k.field == field; });  // ... and their ids are reused
   drop_views(c, [&](const std::tuple<uint32_t, uint32_t, uint32_t>& k) { return std::get<1>(k) == segment_ord && std::get<2>(k) == field; });
   auto rest = c->segments.lower_bound({segment_ord, 0u});
-  if (rest == c->segments.end() || rest->first.first != segment_ord)  // the ordinal's last field: its filters go too (a reused ordinal starts clean)
-    for (auto fi = c->filters.begin(); fi != c->filters.end();)
+  if (rest == c->segments.end() || rest->first.first != segment_ord) {  // the ordinal's last field: its filters and sort columns go too
+    for (auto fi = c->filters.begin(); fi != c->filters.end();)                // (a reused ordinal starts clean)
       if (fi->first.second == segment_ord) fi = c->filters.erase(fi); else ++fi;
+    for (auto ci = c->sort_columns.begin(); ci != c->sort_columns.end();)
+      if (ci->first.second == segment_ord) { ci->second.release(); ci = c->sort_columns.erase(ci); } else ++ci;
+  }
   return TQ_OK;
 }
 
@@ -548,6 +557,67 @@ int tq_filter_unregister(tq_ctx* c, uint32_t filter_id) {
   cudaDeviceSynchronize();
   drop_views(c, [&](const std::tuple<uint32_t, uint32_t, uint32_t>& k) { return std::get<0>(k) == filter_id; });
   while (first != c->filters.end() && first->first.first == filter_id) first = c->filters.erase(first);
+  return TQ_OK;
+}
+
+// ---- sort columns (tq_sort_batch) ---------------------------------------------------------------------------------------------
+int tq_sort_column_register(tq_ctx* c, uint32_t column_id, uint32_t segment_ord, const uint64_t* values, size_t n_values,
+                            const uint8_t* present, size_t present_len) {
+  if (!c || (!values && n_values) || (!present && present_len)) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  std::lock_guard<std::mutex> g(c->mu);
+  uint32_t max_doc = 0;
+  bool any = false;
+  for (auto it = c->segments.lower_bound({segment_ord, 0u}); it != c->segments.end() && it->first.first == segment_ord; ++it) {
+    any = true;
+    max_doc = std::max(max_doc, it->second.max_doc);
+  }
+  if (!any) return fail(TQ_ERR_NOT_FOUND, "no field of the segment ordinal is registered");
+  if (n_values != max_doc) return fail(TQ_ERR_INVALID_ARGUMENT, "a sort column holds max_doc values");
+  if (present && present_len * 8 < max_doc) return fail(TQ_ERR_INVALID_ARGUMENT, "present bitset shorter than max_doc");
+  if (c->sort_users.count(column_id)) return fail(TQ_ERR_INVALID_ARGUMENT, "a sort run still reads the column");
+  // the bounds of every 8192-doc tile: the largest and the smallest value of its docs with a value, and which kinds it holds
+  const uint32_t n_tiles = (max_doc + kTileDocs - 1) / kTileDocs;
+  SortColumn col;
+  col.tiles.assign(n_tiles, SortTile{{0ull, 0ull}, 0u, 0u});
+  for (uint32_t t = 0; t < n_tiles; ++t) {
+    unsigned long long hi = 0, lo = ~0ull;
+    uint32_t flags = 0;
+    for (uint32_t d = t * kTileDocs, e = std::min(max_doc, d + kTileDocs); d < e; ++d) {
+      if (present && !((present[d >> 3] >> (d & 7u)) & 1u)) { flags |= kSortTileNone; continue; }
+      flags |= kSortTileValues;
+      hi = std::max<unsigned long long>(hi, values[d]);
+      lo = std::min<unsigned long long>(lo, values[d]);
+    }
+    col.tiles[t] = SortTile{{(flags & kSortTileValues) ? hi : 0ull, (flags & kSortTileValues) ? ~lo : 0ull}, flags, 0u};
+  }
+  const size_t present_bytes = (size_t)n_tiles * (kTileDocs / 8);
+  cudaError_t e = cudaMalloc(&col.d_values, std::max<size_t>((size_t)max_doc * 8, 8));
+  if (e == cudaSuccess && max_doc) e = cudaMemcpy(col.d_values, values, (size_t)max_doc * 8, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMalloc(&col.d_tiles, std::max<size_t>(n_tiles, 1) * sizeof(SortTile));
+  if (e == cudaSuccess && n_tiles) e = cudaMemcpy(col.d_tiles, col.tiles.data(), n_tiles * sizeof(SortTile), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && present && n_tiles) {
+    std::vector<uint8_t> bits(present_bytes, 0);
+    memcpy(bits.data(), present, ((size_t)max_doc + 7) / 8);
+    if (max_doc & 7u) bits[max_doc >> 3] &= (uint8_t)((1u << (max_doc & 7u)) - 1u);  // bits at and beyond max_doc are ignored
+    e = cudaMalloc(&col.d_present, present_bytes);
+    if (e == cudaSuccess) e = cudaMemcpy(col.d_present, bits.data(), present_bytes, cudaMemcpyHostToDevice);
+  }
+  if (e != cudaSuccess) { col.release(); return fail(TQ_ERR_CUDA, std::string("sort column upload: ") + cudaGetErrorString(e)); }
+  auto it = c->sort_columns.find({column_id, segment_ord});
+  if (it != c->sort_columns.end()) { it->second.release(); it->second = std::move(col); }  // (no run reads it: sort_users)
+  else c->sort_columns.emplace(std::make_pair(column_id, segment_ord), std::move(col));
+  return TQ_OK;
+}
+
+int tq_sort_column_unregister(tq_ctx* c, uint32_t column_id) {
+  if (!c) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  std::lock_guard<std::mutex> g(c->mu);
+  if (c->sort_users.count(column_id)) return fail(TQ_ERR_INVALID_ARGUMENT, "a sort run still reads the column");
+  auto first = c->sort_columns.lower_bound({column_id, 0u});
+  if (first == c->sort_columns.end() || first->first.first != column_id) return fail(TQ_ERR_NOT_FOUND, "sort column not registered");
+  while (first != c->sort_columns.end() && first->first.first == column_id) { first->second.release(); first = c->sort_columns.erase(first); }
   return TQ_OK;
 }
 
@@ -1094,6 +1164,11 @@ void tq_batch_destroy(tq_batch* b) {
     if (--it->second == 0) b->ctx->filter_users.erase(it);
   }
   b->held_filters.clear();
+  for (uint32_t col : b->held_columns) {
+    auto it = b->ctx->sort_users.find(col);
+    if (--it->second == 0) b->ctx->sort_users.erase(it);
+  }
+  b->held_columns.clear();
   b->ctx->pool.push_back(b);  // buffers are recycled by the next batch
 }
 
@@ -1517,6 +1592,143 @@ int tq_count_batch(tq_ctx* c, const tq_query* queries, size_t nq, uint64_t* out_
   }
   if (cp.units.empty()) return TQ_OK;
   return count_on_device(b, cp.words, cp.segs, cp.units, cp.mixed, nq, out_counts);
+}
+
+// ---- sort by a fast field -------------------------------------------------------------------------------------
+int tq_sort_batch(tq_ctx* c, const tq_query* queries, const tq_sort_spec* sorts, size_t nq, uint32_t out_stride, uint64_t* out_values,
+                  uint8_t* out_present, uint32_t* out_segment_ord, uint32_t* out_doc, uint32_t* out_count, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !sorts || !out_values || !out_present || !out_segment_ord || !out_doc || !out_count)))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  uint32_t kmax = 1;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "sorting phrase queries by a fast field is not on the device path");
+    if (queries[qi].k == 0 || queries[qi].k > TQ_MAX_K) return fail(TQ_ERR_INVALID_ARGUMENT, "k must be in 1..TQ_MAX_K");
+    if (sorts[qi].order != TQ_ORDER_DESC && sorts[qi].order != TQ_ORDER_ASC) return fail(TQ_ERR_INVALID_ARGUMENT, "order");
+    kmax = std::max(kmax, queries[qi].k);
+  }
+  if (out_stride < kmax) return fail(TQ_ERR_INVALID_ARGUMENT, "out_stride must hold k rows");
+  for (size_t qi = 0; qi < nq; ++qi) { out_count[qi] = 0; if (out_hits) out_hits[qi] = 0; }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<SortSeg> ssegs;
+  std::vector<SortQuery> sq(nq);
+  uint64_t n_cands = 0;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<std::pair<unsigned long long, Unit>> by_bound;
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      const bool asc = sorts[qi].order == TQ_ORDER_ASC;
+      std::vector<const SortColumn*> cols;
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        auto it = c->sort_columns.find({sorts[qi].column_id, cp.segment_ords[si]});
+        if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a sorted query names a segment without the sort column (tq_sort_column_register)");
+        const SortColumn& col = it->second;
+        if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "sort column and segment differ in max_doc");
+        ssegs.push_back(SortSeg{col.d_values, col.d_present, col.d_tiles, cp.segment_ords[si], 0u});
+        cols.push_back(&col);
+      }
+      // the units with the best possible keys first: they raise the bound that lets the later ones skip their tiles
+      by_bound.clear();
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const Unit& u = cp.units[ui];
+        const std::vector<SortTile>& tiles = cols[u.qseg - s0]->tiles;
+        unsigned long long best = 0;
+        bool none = false;
+        for (uint32_t t = u.begin; t < u.end; ++t) {
+          if (tiles[t].flags & kSortTileValues) best = std::max(best, tiles[t].best[asc ? 1 : 0]);
+          none = none || (tiles[t].flags & kSortTileNone);
+        }
+        // (a unit collects its None docs in doc order, so only a unit without any may walk backwards)
+        const bool backward = !none && tiles[u.end - 1].best[asc ? 1 : 0] > tiles[u.begin].best[asc ? 1 : 0];
+        by_bound.emplace_back(best, Unit{u.qseg, u.begin, u.end, backward ? kSortUnitBackward : 0u});
+      }
+      std::stable_sort(by_bound.begin(), by_bound.end(), [](const auto& x, const auto& y) { return x.first > y.first; });
+      for (size_t i = 0; i < by_bound.size(); ++i) cp.units[u0 + i] = by_bound[i].second;
+      sq[qi] = SortQuery{queries[qi].k, (asc ? kSortAsc : 0u) | (out_hits ? kSortAllTiles : 0u), (uint32_t)n_cands, 0u};
+      n_cands += (uint64_t)(cp.units.size() - u0) * queries[qi].k;
+    }
+    if (n_cands > 0xFFFFFFFFull) return fail(TQ_ERR_INVALID_ARGUMENT, "batch too large: split it");
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) b->held_columns.push_back(sorts[qi].column_id);
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // descriptors: one H2D copy; scratch: results | hits | tile counters (one D2H copy), then the per-query state and candidates
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(ssegs), o_q = st.add(sq);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  const size_t rows = nq * (size_t)kmax;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_values = take(rows * 8), r_hits = take(nq * 8), r_tiles = take(16), r_segs = take(rows * 4), r_docs = take(rows * 4),
+               r_counts = take(nq * 4), r_present = take(rows), res_bytes = off;
+  const size_t r_qstate = take(nq * sizeof(SortQState)), r_cands = take(n_cands * sizeof(SortCand)), r_nones = take(n_cands * sizeof(SortCand));
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(res_bytes));
+  uint8_t* const d = b->scratch.p;
+  SortParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.ssegs = st.on_device<const SortSeg>(o_z);
+  P.queries = st.on_device<const SortQuery>(o_q);
+  P.qstate = reinterpret_cast<SortQState*>(d + r_qstate);
+  P.cands = reinterpret_cast<SortCand*>(d + r_cands);
+  P.nones = reinterpret_cast<SortCand*>(d + r_nones);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.res_values = reinterpret_cast<unsigned long long*>(d + r_values);
+  P.res_present = d + r_present;
+  P.res_segs = reinterpret_cast<uint32_t*>(d + r_segs);
+  P.res_docs = reinterpret_cast<uint32_t*>(d + r_docs);
+  P.res_counts = reinterpret_cast<uint32_t*>(d + r_counts);
+  P.res_stride = kmax;
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d + r_hits, 0, r_segs - r_hits, b->stream));  // hits, tile counters
+  TQ_CUDA(cudaMemsetAsync(d + r_counts, 0, nq * 4, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d + r_qstate, 0, nq * sizeof(SortQState), b->stream));
+  TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+  (cp.mixed ? k_sort<true> : k_sort<false>)<<<(unsigned)cp.units.size(), kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  k_sort_final<<<(unsigned)nq, kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, res_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  const uint8_t* h = b->res_pin.p;
+  const uint32_t* counts = reinterpret_cast<const uint32_t*>(h + r_counts);
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const size_t src = qi * kmax, dst = qi * (size_t)out_stride, n = counts[qi];
+    out_count[qi] = counts[qi];
+    memcpy(out_values + dst, h + r_values + src * 8, n * 8);
+    memcpy(out_present + dst, h + r_present + src, n);
+    memcpy(out_segment_ord + dst, h + r_segs + src * 4, n * 4);
+    memcpy(out_doc + dst, h + r_docs + src * 4, n * 4);
+    if (out_hits) memcpy(&out_hits[qi], h + r_hits + qi * 8, 8);
+  }
+  float ms = 0;
+  cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_tiles, 16);
+  std::lock_guard<std::mutex> g(c->mu);
+  c->sort_ms += ms;
+  c->sort_units += cp.units.size() + nq;
+  c->sort_tiles_seen += tiles[0];
+  c->sort_tiles_skipped += tiles[1];
+  return TQ_OK;
 }
 
 // ---- codec-level access ---------------------------------------------------------------------------

@@ -154,6 +154,17 @@ struct FilterView {
   std::vector<TileRun> runs, count_runs;
 };
 
+// A sort column of one (column_id, segment_ord) (tq_sort_column_register): the u64 images on the device, the present bits (padded
+// to whole 8192-doc tiles: k_sort reads a tile's words whole) and the bounds of every 8192-doc tile, on the device for k_sort and
+// on the host for the planner, which runs a query's units by descending bound.
+struct SortColumn {
+  unsigned long long* d_values = nullptr;
+  uint32_t* d_present = nullptr;  // null: every doc has a value
+  SortTile* d_tiles = nullptr;
+  std::vector<SortTile> tiles;
+  void release() { cudaFree(d_values); cudaFree(d_present); cudaFree(d_tiles); d_values = nullptr; d_present = nullptr; d_tiles = nullptr; }
+};
+
 // A cache of device tables built at first use (block tables of posting lists, position tables): key -> table id, the ids of
 // dropped entries reused first.  An entry the current call schedules takes its id at once (later lookups of the same key share
 // it) and stays pending until the call builds the pending tables together (flush_tables, tq_engine.cu) or rolls them back: a
@@ -213,6 +224,11 @@ struct tq_ctx {
   std::map<std::pair<uint32_t, uint32_t>, std::vector<uint8_t>> filters;  // (filter_id, segment_ord) -> the caller's bits, ceil(max_doc / 8) bytes
   std::map<std::tuple<uint32_t, uint32_t, uint32_t>, tq::host::FilterView> filter_views;  // (filter_id, segment_ord, field)
   std::map<uint32_t, uint32_t> filter_users;  // filter_id -> prepared batches not yet destroyed that name it
+  std::map<std::pair<uint32_t, uint32_t>, tq::host::SortColumn> sort_columns;  // (column_id, segment_ord)
+  std::map<uint32_t, uint32_t> sort_users;  // column_id -> sort runs in progress that read it
+  // cumulative tq_stats fields of the sort runs (sort_ms, units_sort, sort_tiles_seen, sort_tiles_skipped)
+  double sort_ms = 0;
+  uint64_t sort_units = 0, sort_tiles_seen = 0, sort_tiles_skipped = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;

@@ -1020,8 +1020,9 @@ __global__ void __launch_bounds__(kStripThreads) k_or_strip(const BatchParams P,
 
 // ---- final per-query selection -----------------------------------------------------------------------------
 // Keys: a = score_key:32 | (0xFFFFFFFF - segment_ord):32, b = ~doc; descending (a, b) is
-// (score desc, segment_ord asc, doc asc) = compare_for_top_k (top_score_collector.rs:591-600).
-__device__ __noinline__ void sort_pairs_desc(unsigned long long* a, uint32_t* b, unsigned n) {
+// (score desc, segment_ord asc, doc asc) = compare_for_top_k (top_score_collector.rs:591-600).  k_sort_final sorts with a 64-bit b.
+template <class B>
+__device__ __noinline__ void sort_pairs_desc(unsigned long long* a, B* b, unsigned n) {
   unsigned size = 2;
   while (size < n) size <<= 1;
   for (unsigned i = threadIdx.x; i < size; i += blockDim.x)
@@ -1033,7 +1034,7 @@ __device__ __noinline__ void sort_pairs_desc(unsigned long long* a, uint32_t* b,
         const unsigned ixj = i ^ j;
         if (ixj > i) {
           const unsigned long long a1 = a[i], a2 = a[ixj];
-          const uint32_t b1 = b[i], b2 = b[ixj];
+          const B b1 = b[i], b2 = b[ixj];
           const bool first_less = a1 < a2 || (a1 == a2 && b1 < b2);
           const bool first_greater = a1 > a2 || (a1 == a2 && b1 > b2);
           const bool desc = (i & kk) == 0;
@@ -1053,13 +1054,82 @@ __device__ __noinline__ void sort_pairs_desc(unsigned long long* a, uint32_t* b,
 // clause, an OR one group of all its clauses, an AND one group per clause.
 // The structure words are CountParams::words (tq_layout.h).
 
+// One 8192-doc tile [lo, hi) of a (query, segment) evaluated as a boolean structure: one pass per MUST group, then one over the
+// SHOULD clauses and one over the MUST_NOT clauses.  A pass marks its clauses' postings in s_tmp (SHOULD: counts them in s_cnt) and
+// then narrows s_acc; the first MUST group marks s_acc itself.  One posting walk for every pass keeps the caller's registers at
+// those of a single inlined decode.  Then on_word(w, bits) for every 32-doc word of the tile: the matching docs, docs at and beyond
+// max_doc cleared, alive bits (or the filter view) and-ed in.  Every thread of the CTA calls it; the caller syncs before s_acc is
+// written again.  k_count and k_sort share it.
 // kMixed: some (query, segment) of the launch has SHOULD or MUST_NOT clauses.  Without them (every term, AND and OR query) every
 // pass is a MUST group: that instance has no SHOULD counters and no SHOULD or MUST_NOT pass per tile, which AND queries of
 // sparse lists otherwise pay for.
+template <bool kMixed, class OnWord>
+__device__ __forceinline__ void match_tile(const CountParams& P, const uint8_t* alive, uint32_t wb, uint32_t ng, uint32_t need,
+                                           uint32_t lo, uint32_t hi, uint32_t* s_acc, uint32_t* s_tmp, uint32_t* s_cnt, OnWord on_word) {
+  constexpr uint32_t kWords = kTileDocs / 32u;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  if (ng == 0u)
+    for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] = 0xFFFFFFFFu;
+  uint32_t x = wb + 4u;
+  for (uint32_t p = 0; p < (kMixed ? ng + 2u : ng); ++p) {
+    const uint32_t kind = p < ng ? 0u : p - ng + 1u;  // 0: MUST group, 1: SHOULD, 2: MUST_NOT
+    const uint32_t len = kind == 0u ? P.words[x++] : P.words[wb + kind + 1u];
+    const bool should = kMixed && kind == 1u;
+    if (should ? need == 0u : len == 0u) { x += len; continue; }  // (a MUST group is never empty)
+    uint32_t* const bits = p == 0u ? s_acc : s_tmp;
+    if (should)
+      for (uint32_t w = threadIdx.x; w < kTileDocs / 4u; w += blockDim.x) s_cnt[w] = 0;
+    else
+      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) bits[w] = 0;
+    __syncthreads();
+    for (const uint32_t end = x + len; x < end; ++x) {
+      const ListDesc L = P.lists[P.words[x]];
+      const uint32_t j0 = first_block_ge(L.last_doc, 0, L.n_total, lo, lane);
+      for (uint32_t j = j0 + warp; j < L.n_total; j += kWarps) {
+        const uint32_t prev = __ldg(&L.tab4[j].w);
+        if (prev != 0xFFFFFFFFu && prev + 1u >= hi) break;  // the block starts at or after the tile's end
+        uint32_t doc[4], tf[4];
+        decode_block(L, j, lane, doc, tf);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t o = doc[i] - lo;
+          if (doc[i] >= lo && doc[i] < hi) {
+            if (should) atomicAdd(&s_cnt[o >> 2], 1u << ((o & 3u) * 8u));  // <= 32 clauses: no carry
+            else atomicOr(&bits[o >> 5], 1u << (o & 31u));
+          }
+        }
+      }
+    }
+    __syncthreads();
+    if (p == 0u && !should) continue;
+    for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
+      uint32_t m = s_tmp[w];
+      if (should) {
+        m = 0;
+#pragma unroll
+        for (uint32_t b = 0; b < 8; ++b) {
+          const uint32_t c4 = s_cnt[w * 8u + b];
+#pragma unroll
+          for (uint32_t k = 0; k < 4; ++k) m |= (((c4 >> (8u * k)) & 255u) >= need ? 1u : 0u) << (b * 4u + k);
+        }
+      }
+      s_acc[w] &= kind == 2u ? ~m : m;
+    }
+    __syncthreads();
+  }
+  for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
+    uint32_t bits = s_acc[w];
+    const uint32_t first = lo + w * 32u;
+    if (first >= hi) bits = 0;
+    else if (hi - first < 32u) bits &= (1u << (hi - first)) - 1u;  // docs beyond max_doc
+    if (bits && alive) bits &= __ldg(reinterpret_cast<const uint32_t*>(alive) + ((lo >> 5) + w));
+    on_word(w, bits);
+  }
+}
+
 template <bool kMixed>
 __global__ void __launch_bounds__(kThreads) k_count(const CountParams P) {
-  constexpr uint32_t kWords = kTileDocs / 32u;
-  __shared__ uint32_t s_acc[kWords], s_tmp[kWords];
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
   __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
   __shared__ uint32_t s_part[kWarps];
   const Unit U = P.units[blockIdx.x];
@@ -1070,66 +1140,7 @@ __global__ void __launch_bounds__(kThreads) k_count(const CountParams P) {
   uint32_t total = 0;
   for (uint32_t tile = U.begin; tile < U.end; ++tile) {
     const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
-    // one pass per MUST group, then one over the SHOULD clauses and one over the MUST_NOT clauses: a pass marks its clauses'
-    // postings in s_tmp (SHOULD: counts them in s_cnt) and then narrows s_acc; the first MUST group marks s_acc itself.  One
-    // posting walk for every pass keeps the kernel's registers at those of a single inlined decode.
-    if (ng == 0u)
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) s_acc[w] = 0xFFFFFFFFu;
-    uint32_t x = wb + 4u;
-    for (uint32_t p = 0; p < (kMixed ? ng + 2u : ng); ++p) {
-      const uint32_t kind = p < ng ? 0u : p - ng + 1u;  // 0: MUST group, 1: SHOULD, 2: MUST_NOT
-      const uint32_t len = kind == 0u ? P.words[x++] : P.words[wb + kind + 1u];
-      const bool should = kMixed && kind == 1u;
-      if (should ? need == 0u : len == 0u) { x += len; continue; }  // (a MUST group is never empty)
-      uint32_t* const bits = p == 0u ? s_acc : s_tmp;
-      if (should)
-        for (uint32_t w = threadIdx.x; w < kTileDocs / 4u; w += blockDim.x) s_cnt[w] = 0;
-      else
-        for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) bits[w] = 0;
-      __syncthreads();
-      for (const uint32_t end = x + len; x < end; ++x) {
-        const ListDesc L = P.lists[P.words[x]];
-        const uint32_t j0 = first_block_ge(L.last_doc, 0, L.n_total, lo, lane);
-        for (uint32_t j = j0 + warp; j < L.n_total; j += kWarps) {
-          const uint32_t prev = __ldg(&L.tab4[j].w);
-          if (prev != 0xFFFFFFFFu && prev + 1u >= hi) break;  // the block starts at or after the tile's end
-          uint32_t doc[4], tf[4];
-          decode_block(L, j, lane, doc, tf);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t o = doc[i] - lo;
-            if (doc[i] >= lo && doc[i] < hi) {
-              if (should) atomicAdd(&s_cnt[o >> 2], 1u << ((o & 3u) * 8u));  // <= 32 clauses: no carry
-              else atomicOr(&bits[o >> 5], 1u << (o & 31u));
-            }
-          }
-        }
-      }
-      __syncthreads();
-      if (p == 0u && !should) continue;
-      for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
-        uint32_t m = s_tmp[w];
-        if (should) {
-          m = 0;
-#pragma unroll
-          for (uint32_t b = 0; b < 8; ++b) {
-            const uint32_t c4 = s_cnt[w * 8u + b];
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) m |= (((c4 >> (8u * k)) & 255u) >= need ? 1u : 0u) << (b * 4u + k);
-          }
-        }
-        s_acc[w] &= kind == 2u ? ~m : m;
-      }
-      __syncthreads();
-    }
-    for (uint32_t w = threadIdx.x; w < kWords; w += blockDim.x) {
-      uint32_t bits = s_acc[w];
-      const uint32_t first = lo + w * 32u;
-      if (first >= hi) bits = 0;
-      else if (hi - first < 32u) bits &= (1u << (hi - first)) - 1u;  // docs beyond max_doc
-      if (bits && S.alive) bits &= __ldg(reinterpret_cast<const uint32_t*>(S.alive) + ((lo >> 5) + w));
-      total += (uint32_t)__popc(bits);
-    }
+    match_tile<kMixed>(P, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t, uint32_t bits) { total += (uint32_t)__popc(bits); });
     __syncthreads();
   }
   total = __reduce_add_sync(kFull, total);
@@ -1140,6 +1151,270 @@ __global__ void __launch_bounds__(kThreads) k_count(const CountParams P) {
     for (int w = 0; w < kWarps; ++w) sum += s_part[w];
     if (sum) atomicAdd(&P.counts[P.segs[P.units[blockIdx.x].qseg].query], sum);  // (read here: nothing of it lives through the tiles)
   }
+}
+
+// ---- sort by a fast field (TopDocs::order_by_fast_field: SortByStaticFastValue, sort_by_static_fast_value.rs) ----------------
+// The docs Count counts, each keyed by its column value, top k.  One CTA per Count unit: per 8192-doc tile it first reads the
+// query's threshold and skips the tile when no doc of it can enter the top k -- every doc with a value is below the bound (the
+// tile's best v', SortTile) and the query already holds k docs with values or the tile has no None doc -- unless the query's hits
+// are counted.  Otherwise match_tile builds the tile's match bitmap, each matching doc with a value is keyed by v' (an 8-byte
+// gather) and kept in a shared buffer when v' >= the bound; a full buffer is sorted by (v' desc, doc asc) and cut to k, whose
+// k-th v' then bounds the query (atomicMax); so is the buffer at the end of the tile in which it first holds k docs.  A doc is
+// dropped only when k docs strictly precede it.  A unit walks its tiles backwards (kSortUnitBackward) when its bounds rise and it
+// has no None doc: a column ascending in doc id, sorted Desc, then finds its best docs first.  None docs all tie, so the
+// unit keeps its first k in doc order.  At exit each unit hands over at most k docs of each stream: the regions hold that much,
+// so nothing is ever dropped for capacity.
+
+// Sorts the buffer by (v' desc, doc asc), keeps its first k and, when it held k, raises the CTA's and the query's bounds.
+__device__ __forceinline__ void sort_compact(unsigned long long* s_key, uint32_t* s_doc, uint32_t& s_n, uint32_t k, unsigned long long& s_theta,
+                                             uint32_t& s_full, SortQState* qs) {
+  const uint32_t n = s_n;
+  sort_pairs_desc(s_key, s_doc, n);
+  if (threadIdx.x == 0) {
+    if (n >= k) {
+      const unsigned long long kth = s_key[k - 1];
+      if (kth > s_theta) { s_theta = kth; atomicMax(&qs->theta, kth); }
+      if (!s_full) { s_full = 1; atomicExch(&qs->full, 1u); }
+    }
+    s_n = min(n, k);
+  }
+  __syncthreads();
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads) k_sort(const SortParams P) {
+  static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ unsigned long long s_key[kCap];
+  __shared__ uint32_t s_doc[kCap];  // ~doc: descending (key, ~doc) is (v' desc, doc asc)
+  __shared__ uint32_t s_none[kSortMaxK];
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ unsigned long long s_theta;  // max(the k-th v' this CTA held, the query's bound when last read)
+  __shared__ uint32_t s_n, s_nn, s_full, s_skip, s_base, s_nbase;
+  const Unit U = P.c.units[blockIdx.x];
+  const CountSeg S = P.c.segs[U.qseg];
+  const SortSeg Z = P.ssegs[U.qseg];
+  const SortQuery Q = P.queries[S.query];
+  SortQState* const qs = P.qstate + S.query;
+  const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const bool asc = (Q.flags & kSortAsc) != 0;
+  if (threadIdx.x == 0) { s_theta = 0; s_n = 0; s_nn = 0; s_full = 0; }
+  uint32_t total = 0, seen = 0, skipped = 0;
+  for (uint32_t i = U.begin; i < U.end; ++i) {
+    const uint32_t tile = (U.pad & kSortUnitBackward) ? U.end - 1u - (i - U.begin) : i;
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const unsigned long long th = max(s_theta, *reinterpret_cast<volatile unsigned long long*>(&qs->theta));
+      const uint32_t full = s_full | *reinterpret_cast<volatile uint32_t*>(&qs->full);
+      s_theta = th;
+      s_full = full;
+      const SortTile T = Z.tiles[tile];
+      const bool skip = !(Q.flags & kSortAllTiles) && (!(T.flags & kSortTileValues) || T.best[asc ? 1 : 0] < th) &&
+                        (!(T.flags & kSortTileNone) || full);
+      s_skip = skip;
+      ++seen;
+      skipped += skip ? 1u : 0u;
+    }
+    __syncthreads();
+    if (s_skip) continue;
+    match_tile<kMixed>(P.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    total += (uint32_t)__popc(bits);
+    uint32_t with = bits, none = 0;
+    if (Z.present) {
+      const uint32_t pw = __ldg(Z.present + (lo >> 5) + threadIdx.x);
+      with = bits & pw;
+      none = bits & ~pw;
+    }
+    // None docs: the unit's first k in doc order (a CTA-wide prefix sum over the words), until k docs with values are known
+    if (Z.present && !s_full && s_nn < Q.k) {
+      const uint32_t c = (uint32_t)__popc(none);
+      uint32_t incl = c;
+#pragma unroll
+      for (uint32_t o = 1; o < 32u; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(kFull, incl, o);
+        if (lane >= o) incl += v;
+      }
+      if (lane == 31u) s_part[warp] = incl;
+      __syncthreads();
+      uint32_t at = s_nn + incl - c;
+      for (uint32_t w = 0; w < warp; ++w) at += s_part[w];
+      for (uint32_t m = none; m && at < Q.k; m &= m - 1u, ++at) s_none[at] = lo + threadIdx.x * 32u + (uint32_t)(__ffs(m) - 1);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        uint32_t sum = s_nn;
+        for (int w = 0; w < kWarps; ++w) sum += s_part[w];
+        s_nn = min(sum, Q.k);
+      }
+    }
+    // docs with values, one per thread and round: a round adds at most kThreads keys, so the buffer is cut before it can overflow
+    while (__syncthreads_or(with != 0u)) {
+      const unsigned long long th = s_theta;
+      if (with) {
+        const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(with) - 1);
+        with &= with - 1u;
+        const unsigned long long v = __ldg(Z.values + doc);
+        const unsigned long long key = asc ? ~v : v;
+        if (key >= th) {
+          const uint32_t slot = atomicAdd(&s_n, 1u);
+          s_key[slot] = key;
+          s_doc[slot] = ~doc;
+        }
+      }
+      __syncthreads();
+      if (s_n > kCap - (uint32_t)kThreads) sort_compact(s_key, s_doc, s_n, Q.k, s_theta, s_full, qs);
+    }
+    if (!s_full && s_n >= Q.k) sort_compact(s_key, s_doc, s_n, Q.k, s_theta, s_full, qs);  // the first k: a bound for the next tiles
+  }
+  __syncthreads();
+  if (s_n > Q.k) sort_compact(s_key, s_doc, s_n, Q.k, s_theta, s_full, qs);
+  if (Q.flags & kSortAllTiles) {
+    total = __reduce_add_sync(kFull, total);
+    if (lane == 0) s_part[warp] = total;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (Q.flags & kSortAllTiles) {
+      unsigned long long sum = 0;
+      for (int w = 0; w < kWarps; ++w) sum += s_part[w];
+      if (sum) atomicAdd(&P.c.counts[S.query], sum);
+    }
+    if (P.tiles && seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (skipped) atomicAdd(&P.tiles[1], (unsigned long long)skipped); }
+    s_base = s_n ? atomicAdd(&qs->n_cands, s_n) : 0u;
+    if (s_full) s_nn = 0;  // k docs with values are known: no None doc can make the top k
+    s_nbase = s_nn ? atomicAdd(&qs->n_nones, s_nn) : 0u;
+  }
+  __syncthreads();
+  SortCand* const cands = P.cands + Q.cand_base + s_base;
+  for (uint32_t i = threadIdx.x; i < s_n; i += blockDim.x) cands[i] = SortCand{s_key[i], Z.segment_ord, ~s_doc[i]};
+  SortCand* const nones = P.nones + Q.cand_base + s_nbase;
+  for (uint32_t i = threadIdx.x; i < s_nn; i += blockDim.x) nones[i] = SortCand{0ull, Z.segment_ord, s_none[i]};
+}
+
+// The first min(C, k) of C candidates by (a desc, b desc), (a, b) = key(candidate), sorted into s_a / s_b; returns how many.  A
+// 64-bit radix select of the k-th largest a (8 passes, as k_final's 4), then the candidates above it and its ties are sorted --
+// the ties slab by slab when they do not fit the buffer, as in k_final.
+template <class Key>
+__device__ uint32_t select_sorted(const SortCand* __restrict__ cands, uint32_t C, uint32_t k, Key key, unsigned long long* s_a,
+                                  unsigned long long* s_b, uint32_t* s_hist, unsigned long long& s_prefix, uint32_t& s_need,
+                                  uint32_t& s_ties, uint32_t& s_n) {
+  if (C <= kCap) {
+    for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) key(cands[i], s_a[i], s_b[i]);
+    __syncthreads();
+    sort_pairs_desc(s_a, s_b, C);
+    return min(C, k);
+  }
+  if (threadIdx.x == 0) { s_prefix = 0; s_need = k; s_n = 0; }
+  unsigned long long mask = 0;
+  for (int pass = 0; pass < 8; ++pass) {
+    const int shift = 56 - 8 * pass;
+    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
+    __syncthreads();
+    const unsigned long long prefix = s_prefix;
+    for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) {
+      unsigned long long a, b;
+      key(cands[i], a, b);
+      if ((a & mask) == prefix) atomicAdd(&s_hist[(a >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      uint32_t need = s_need, bsel = 0;
+      for (int bin = 255; bin >= 0; --bin) {
+        const uint32_t h = s_hist[bin];
+        if (h >= need) { bsel = (uint32_t)bin; s_ties = h; break; }
+        need -= h;
+      }
+      s_need = need;
+      s_prefix = prefix | ((unsigned long long)bsel << shift);
+    }
+    mask |= 0xFFull << shift;
+    __syncthreads();
+  }
+  const unsigned long long kth = s_prefix;  // exactly the k-th largest a
+  const uint32_t ties = s_ties, above = k - s_need;
+  const bool one_sweep = above + ties <= kCap;  // the usual case; else a flood of equal a: the ties slab by slab
+  for (uint32_t i = threadIdx.x; i < C; i += blockDim.x) {
+    unsigned long long a, b;
+    key(cands[i], a, b);
+    if (one_sweep ? a >= kth : a > kth) {
+      const uint32_t slot = atomicAdd(&s_n, 1u);
+      s_a[slot] = a;
+      s_b[slot] = b;
+    }
+  }
+  __syncthreads();
+  uint32_t have = s_n;
+  if (one_sweep) {
+    __syncthreads();
+    sort_pairs_desc(s_a, s_b, have);
+    return min(have, k);
+  }
+  for (uint32_t next = 0; next < C;) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_n = have;
+    __syncthreads();
+    const uint32_t slab_end = min(C, next + (kCap - have));
+    for (uint32_t i = next + threadIdx.x; i < slab_end; i += blockDim.x) {
+      unsigned long long a, b;
+      key(cands[i], a, b);
+      if (a == kth) {
+        const uint32_t slot = atomicAdd(&s_n, 1u);
+        s_a[slot] = a;
+        s_b[slot] = b;
+      }
+    }
+    __syncthreads();
+    const uint32_t n = s_n;
+    __syncthreads();
+    sort_pairs_desc(s_a, s_b, n);
+    have = min(n, k);
+    next = slab_end;
+  }
+  return have;
+}
+
+// The rows of every query: its docs with values by (v' desc, segment asc, doc asc), then, while the row has room, its None docs
+// by (segment asc, doc asc) (compare_for_top_k, top_score_collector.rs:591-600; Order::Asc = ReverseNoneLower, order.rs:286-293).
+__global__ void __launch_bounds__(kThreads) k_sort_final(const SortParams P) {
+  __shared__ unsigned long long s_a[kCap], s_b[kCap];
+  __shared__ uint32_t s_hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ uint32_t s_need, s_ties, s_n;
+  const uint32_t q = blockIdx.x;
+  const SortQuery Q = P.queries[q];
+  const uint32_t n_cands = P.qstate[q].n_cands, n_nones = P.qstate[q].n_nones;
+  const bool asc = (Q.flags & kSortAsc) != 0;
+  const size_t row = (size_t)q * P.res_stride;
+  auto address = [](const SortCand& c) { return ~((unsigned long long)c.segment_ord << 32 | c.doc); };  // descending = ascending address
+  const uint32_t have = select_sorted(P.cands + Q.cand_base, n_cands, Q.k,
+                                      [&](const SortCand& c, unsigned long long& a, unsigned long long& b) { a = c.key; b = address(c); },
+                                      s_a, s_b, s_hist, s_prefix, s_need, s_ties, s_n);
+  for (uint32_t i = threadIdx.x; i < have; i += blockDim.x) {
+    const unsigned long long addr = ~s_b[i];
+    P.res_values[row + i] = asc ? ~s_a[i] : s_a[i];
+    P.res_present[row + i] = 1;
+    P.res_segs[row + i] = (uint32_t)(addr >> 32);
+    P.res_docs[row + i] = (uint32_t)addr;
+  }
+  uint32_t n_none = 0;
+  if (have < Q.k && n_nones) {
+    __syncthreads();
+    n_none = select_sorted(P.nones + Q.cand_base, n_nones, Q.k - have,
+                           [&](const SortCand& c, unsigned long long& a, unsigned long long& b) { a = b = address(c); },
+                           s_a, s_b, s_hist, s_prefix, s_need, s_ties, s_n);
+    for (uint32_t i = threadIdx.x; i < n_none; i += blockDim.x) {
+      const unsigned long long addr = ~s_b[i];
+      P.res_values[row + have + i] = 0;
+      P.res_present[row + have + i] = 0;
+      P.res_segs[row + have + i] = (uint32_t)(addr >> 32);
+      P.res_docs[row + have + i] = (uint32_t)addr;
+    }
+  }
+  if (threadIdx.x == 0) P.res_counts[q] = have + n_none;
 }
 
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit

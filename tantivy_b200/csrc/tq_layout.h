@@ -145,6 +145,58 @@ struct CountParams {
   unsigned long long* counts;
 };
 
+// ---- sort by a fast field (k_sort, k_sort_final) ------------------------------------------------------------------------
+// The key of a doc with a value is v' = value (Desc) or ~value (Asc): larger v' first.  Docs without a value (None) come after
+// every doc with one, in (segment, doc) order, in both orders; they travel as a stream of their own.
+constexpr uint32_t kSortMaxK = 1024;  // TQ_MAX_K: a k_sort CTA keeps up to this many None docs on chip
+
+// One 8192-doc tile of a registered column: the best v' any doc with a value can have, per order ([0] Desc: the largest value,
+// [1] Asc: ~ the smallest), and which kinds of docs it holds.
+struct SortTile {
+  unsigned long long best[2];
+  uint32_t flags;  // kSortTileValues: some doc has a value; kSortTileNone: some doc has none
+  uint32_t pad;
+};
+constexpr uint32_t kSortTileValues = 1, kSortTileNone = 2;
+struct SortSeg {  // the column of one (query, segment), parallel to CountParams::segs
+  const unsigned long long* values;  // [max_doc] u64 images
+  const uint32_t* present;           // bitset in the alive layout (null: every doc has a value)
+  const SortTile* tiles;
+  uint32_t segment_ord, pad;
+};
+struct SortQuery {
+  uint32_t k;
+  uint32_t flags;      // kSortAsc; kSortAllTiles: the query's hits are counted, so no tile is skipped
+  uint32_t cand_base;  // first slot of the query's regions in SortParams::cands and ::nones (units of the query x k each)
+  uint32_t pad;
+};
+constexpr uint32_t kSortAsc = 1, kSortAllTiles = 2;
+constexpr uint32_t kSortUnitBackward = 1;  // Unit::pad of a k_sort unit: walk its tiles from the last to the first
+struct SortQState {  // zeroed before every run
+  unsigned long long theta;  // lower bound of the query's k-th v' (a CTA that held k docs with values published its k-th)
+  uint32_t full;             // some CTA held k docs with values: no None doc can make the top k
+  uint32_t n_cands, n_nones;
+  uint32_t pad;
+};
+struct SortCand { unsigned long long key; uint32_t segment_ord, doc; };  // key: v' (None stream: unused)
+struct SortParams {
+  CountParams c;  // structure words, (query, segment) pairs, units and hit counters: the Count plan
+  const SortSeg* ssegs;
+  const SortQuery* queries;
+  SortQState* qstate;
+  SortCand* cands;  // per query: the docs with values each unit kept (<= k per unit)
+  SortCand* nones;  // per query: the first k None docs of each unit in doc order
+  unsigned long long* tiles;  // [0] tiles seen, [1] of them skipped
+  unsigned long long* res_values;
+  uint8_t* res_present;
+  uint32_t* res_segs;
+  uint32_t* res_docs;
+  uint32_t* res_counts;
+  uint32_t res_stride;
+};
+static_assert(sizeof(SortTile) == 24 && sizeof(SortSeg) == 32 && sizeof(SortQuery) == 16 && sizeof(SortQState) == 24 && sizeof(SortCand) == 16,
+              "sort descriptor layout");
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

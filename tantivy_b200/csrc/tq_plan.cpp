@@ -406,7 +406,8 @@ void append_qsegs(const tq_ctx* c, BatchPlan& pl, size_t qi, int op) {
 // The Count work of query qi (Count collector, count_collector.rs; Weight::count, term_weight.rs:179-219): its (query, segment)
 // pairs go to cp; a term on a segment without deletes is answered from its doc_freq, added to *host_add (term_weight.rs:179-190).
 // ctx->mu held.
-int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_term_seg*>& order, CountPlan& cp, uint64_t* host_add) {
+int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_term_seg*>& order, CountPlan& cp, uint64_t* host_add,
+               bool all_docs) {
   int rc = check_shape(q, false);
   if (rc != TQ_OK) return rc;
   if (!q.term_segs && q.n_term_segs) return fail(TQ_ERR_INVALID_ARGUMENT, "query arrays");
@@ -445,7 +446,7 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_t
     const FilterView* view = nullptr;
     const int arc = query_alive(c, q, *seg, &cs.alive, &view);
     if (arc != TQ_OK) return arc;
-    if (q.op != TQ_OP_BOOL && n_here == 1 && !cs.alive) {  // TermWeight::count without deletes (nor a filter): the term's doc_freq (term_weight.rs:179-190)
+    if (q.op != TQ_OP_BOOL && n_here == 1 && !cs.alive && !all_docs) {  // TermWeight::count without deletes (nor a filter): the term's doc_freq (term_weight.rs:179-190)
       *host_add += ts[0]->doc_freq;
       return TQ_OK;
     }
@@ -462,6 +463,7 @@ int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_t
         for (uint32_t t0 = r.t0; t0 < r.t1; t0 += per) cp.units.push_back(Unit{seg_idx, t0, std::min(r.t1, t0 + per), 0});
     }
     cp.segs.push_back(cs);
+    cp.segment_ords.push_back(seg->segment_ord);
     return TQ_OK;
   });
 }

@@ -100,6 +100,7 @@ struct SegWork { UnitClass cls; uint32_t total; bool sample; };
 struct CountPlan {
   std::vector<uint32_t> words;
   std::vector<CountSeg> segs;
+  std::vector<uint32_t> segment_ords;  // parallel to segs
   std::vector<Unit> units;
   bool mixed = false;  // some pair has SHOULD or MUST_NOT clauses: k_count<true>
 };
@@ -149,7 +150,9 @@ int plan_query(tq_ctx* c, BatchPlan& pl, size_t qi);
 int cut_units(const tq_ctx* c, BatchPlan& pl);
 // Tile groups: slot order, pair bases, score chunks, tile ranges of the launches.
 int stage_tile_groups(const tq_ctx* c, BatchPlan& pl);
-// The Count work of query qi: its (query, segment) pairs go to cp, doc_freq shortcuts to *host_add.  ctx->mu held.
-int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_term_seg*>& order, CountPlan& cp, uint64_t* host_add);
+// The Count work of query qi: its (query, segment) pairs go to cp, doc_freq shortcuts to *host_add -- none with all_docs (a sort
+// needs every matching doc, not only how many there are).  ctx->mu held.
+int plan_count(tq_ctx* c, const tq_query& q, uint32_t qi, std::vector<const tq_term_seg*>& order, CountPlan& cp, uint64_t* host_add,
+               bool all_docs = false);
 
 }  // namespace tq::host

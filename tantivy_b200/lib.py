@@ -6,7 +6,7 @@ import os
 
 import numpy as np
 
-from ._abi import Query, QueryBatch, Stats, TermSeg, f32p, ptr, u8p, u32p, u64p
+from ._abi import SORT_SPEC_DTYPE, TQ_ORDER_ASC, TQ_ORDER_DESC, Query, QueryBatch, SortSpec, Stats, TermSeg, f32p, ptr, u8p, u32p, u64p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -39,6 +39,9 @@ def _load():
     lib.tq_search_batch.argtypes = [vp, C.POINTER(Query), sz, C.c_uint32, f32p, u32p, u32p, u32p]
     lib.tq_batch_prepare.argtypes = [vp, C.POINTER(Query), sz, C.POINTER(vp)]
     lib.tq_count_batch.argtypes = [vp, C.POINTER(Query), sz, u64p]
+    lib.tq_sort_column_register.argtypes = [vp, C.c_uint32, C.c_uint32, u64p, sz, u8p, sz]
+    lib.tq_sort_column_unregister.argtypes = [vp, C.c_uint32]
+    lib.tq_sort_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(SortSpec), sz, C.c_uint32, u64p, u8p, u32p, u32p, u32p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -103,6 +106,47 @@ LIB = _load()
 def _check(rc, ctx=None):
     if rc != 0:
         raise TqError(f"tantivy_b200 error {rc}: {LIB.tq_last_error(ctx).decode(errors='replace')}")
+
+
+_HIGHEST_BIT = np.uint64(1 << 63)
+FAST_VALUE_KINDS = ("u64", "i64", "f64", "bool", "date")
+
+
+def fast_value_to_u64(values, kind):
+    """The u64 image of fast-field values (MonotonicallyMappableToU64, common/src/lib.rs), what tq_sort_column_register takes:
+    u64 as is; i64 v ^ 2^63; f64 bits ^ 2^63 when the sign bit is clear (+0.0 included), !bits when it is set (-0.0 included);
+    bool 0 / 1; date (numpy datetime64, or int64 nanoseconds since the epoch) as its i64 nanoseconds.  Order-preserving."""
+    if kind == "u64":
+        return np.asarray(values, dtype=np.uint64).copy()
+    if kind == "i64":
+        return np.asarray(values, dtype=np.int64).view(np.uint64) ^ _HIGHEST_BIT
+    if kind == "date":
+        v = np.asarray(values)
+        if np.issubdtype(v.dtype, np.datetime64):
+            v = v.astype("datetime64[ns]").view(np.int64)
+        return np.asarray(v, dtype=np.int64).view(np.uint64) ^ _HIGHEST_BIT
+    if kind == "f64":
+        bits = np.asarray(values, dtype=np.float64).view(np.uint64)
+        neg = (bits & _HIGHEST_BIT) != 0
+        return np.where(neg, ~bits, bits ^ _HIGHEST_BIT)
+    if kind == "bool":
+        return np.asarray(values, dtype=bool).astype(np.uint64)
+    raise ValueError(f"kind must be one of {FAST_VALUE_KINDS}, got {kind!r}")
+
+
+def u64_to_fast_value(images, kind):
+    """The reverse of fast_value_to_u64 (MonotonicallyMappableToU64::from_u64): date gives datetime64[ns]."""
+    u = np.asarray(images, dtype=np.uint64)
+    if kind == "u64":
+        return u.copy()
+    if kind in ("i64", "date"):
+        v = (u ^ _HIGHEST_BIT).view(np.int64)
+        return v.view("datetime64[ns]") if kind == "date" else v
+    if kind == "f64":
+        return np.where((u & _HIGHEST_BIT) != 0, u ^ _HIGHEST_BIT, ~u).view(np.float64)
+    if kind == "bool":
+        return u > 0
+    raise ValueError(f"kind must be one of {FAST_VALUE_KINDS}, got {kind!r}")
 
 
 def bm25_idf(doc_freq, doc_count):
@@ -287,6 +331,41 @@ class Context:
 
     def filter_unregister(self, filter_id):
         _check(LIB.tq_filter_unregister(self.h, filter_id), self.h)
+
+    def sort_column_register(self, column_id, segment_ord, values, present=None):
+        """The sort column `column_id` of one segment (every field registered under the ordinal): `values` = the u64 images of
+        each doc's first value (max_doc of them, fast_value_to_u64), `present` = bits in the `.del` layout, set = the doc has a
+        value (np.packbits(mask, bitorder="little"); None: every doc has one)."""
+        v = np.ascontiguousarray(values, dtype=np.uint64)
+        p = None if present is None else np.ascontiguousarray(present, dtype=np.uint8)
+        _check(LIB.tq_sort_column_register(self.h, column_id, segment_ord, ptr(v, u64p), v.size, ptr(p, u8p), 0 if p is None else p.size), self.h)
+
+    def sort_column_unregister(self, column_id):
+        _check(LIB.tq_sort_column_unregister(self.h, column_id), self.h)
+
+    def sort_batch(self, qb: QueryBatch, specs, count_hits=False):
+        """TopDocs::with_limit(k).order_by_fast_field(column, order) per query (tq_sort_batch); specs = one (column_id, order) per
+        query, order TQ_ORDER_DESC / TQ_ORDER_ASC or "desc" / "asc".  Returns (values, present, segs, docs, counts) -- rows of the
+        batch's largest k, values as u64 images (u64_to_fast_value maps them back), present as bool -- and with count_hits=True the
+        Count of every query as well."""
+        specs = list(specs)
+        if len(specs) != qb.nq:
+            raise ValueError(f"one sort spec per query: {len(specs)} for {qb.nq} queries")
+        spec = np.zeros(max(qb.nq, 1), dtype=SORT_SPEC_DTYPE)
+        for i, (col, order) in enumerate(specs):
+            spec[i]["column_id"] = col
+            spec[i]["order"] = {"desc": TQ_ORDER_DESC, "asc": TQ_ORDER_ASC}.get(order, order)
+        n, stride = max(qb.nq, 1), qb.kmax
+        values = np.zeros((n, stride), dtype=np.uint64)
+        present = np.zeros((n, stride), dtype=np.uint8)
+        segs = np.zeros((n, stride), dtype=np.uint32)
+        docs = np.zeros((n, stride), dtype=np.uint32)
+        counts = np.zeros(n, dtype=np.uint32)
+        hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+        _check(LIB.tq_sort_batch(self.h, qb.ptr, spec.ctypes.data_as(C.POINTER(SortSpec)), qb.nq, stride, ptr(values, u64p), ptr(present, u8p),
+                                 ptr(segs, u32p), ptr(docs, u32p), ptr(counts, u32p), ptr(hits, u64p)), self.h)
+        out = (values, present.astype(bool), segs, docs, counts)
+        return out + (hits[:qb.nq],) if count_hits else out
 
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
