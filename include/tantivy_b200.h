@@ -217,6 +217,17 @@ int tq_ctx_create(int device, tq_ctx** out);
 void tq_ctx_destroy(tq_ctx*);
 const char* tq_last_error(tq_ctx*);
 int tq_get_stats(tq_ctx*, tq_stats* out);
+/* Cumulative since ctx creation: tq_histogram_batch.  Device time of k_hist + k_hist_final, their CTAs (one per unit of up to
+ * eight 8192-doc tiles, plus one per query), the 8192-doc tiles the units came to and of those the ones counted as one bucket
+ * (every value of the tile in one bucket: the tile's matches added without reading a value).  A struct of its own, so that
+ * tq_stats keeps its layout. */
+typedef struct {
+  float hist_ms;
+  uint64_t units_hist;
+  uint64_t hist_tiles_seen;
+  uint64_t hist_tiles_one_bucket;
+} tq_histogram_stats;
+int tq_get_histogram_stats(tq_ctx*, tq_histogram_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -283,6 +294,21 @@ typedef struct {
   uint32_t order;     /* TQ_ORDER_DESC / TQ_ORDER_ASC */
 } tq_sort_spec;
 
+/* Histogram aggregations (AggregationCollector with one `histogram` or `date_histogram` and no sub-aggregation, src/aggregation/
+ * bucket/histogram/histogram.rs) read the same registered columns.  Only single-valued columns: the reference counts every value
+ * of a multi-valued doc, a sort column holds its first, so a multi-valued field stays on the CPU path. */
+#define TQ_FAST_U64 0u  /* how a column's u64 image maps to f64 (f64_from_fastfield_u64, aggregation/mod.rs): u64 as f64 */
+#define TQ_FAST_I64 1u  /* i64 as f64 */
+#define TQ_FAST_F64 2u  /* the f64 itself */
+#define TQ_FAST_BOOL 3u /* 0.0 / 1.0 */
+#define TQ_FAST_DATE 4u /* i64 nanoseconds as f64 */
+typedef struct {
+  uint32_t column_id;        /* a column of tq_sort_column_register */
+  uint32_t kind;             /* TQ_FAST_* */
+  double interval, offset;   /* in the column's unit (DATE: nanoseconds -- the caller normalises the request's milliseconds) */
+  double hard_min, hard_max; /* collect-time bounds; -DBL_MAX / DBL_MAX when the request has none */
+} tq_histogram_spec;
+
 /* ---- search -------------------------------------------------------------------------- */
 /* The whole hot path for a batch of queries, host buffers in / host buffers out:
  * block decode -> AND/OR/term -> BM25 -> per-segment top-k -> merge_fruits.
@@ -312,6 +338,23 @@ int tq_count_batch(tq_ctx*, const tq_query* queries, size_t nq, uint64_t* out_co
  * sorts[q].column_id returns TQ_ERR_NOT_FOUND. */
 int tq_sort_batch(tq_ctx*, const tq_query* queries, const tq_sort_spec* sorts, size_t nq, uint32_t out_stride, uint64_t* out_values,
                   uint8_t* out_present, uint32_t* out_segment_ord, uint32_t* out_doc, uint32_t* out_count, uint64_t* out_hits);
+
+/* The segment part of a histogram aggregation for term / AND / OR / mixed boolean (TQ_OP_BOOL) queries, synchronous like
+ * tq_count_batch, over the docs tq_count_batch counts.  Per (query, segment) the bounds are [hard_min, hard_max], or every finite
+ * value when the segment's column already lies inside them (normalize_histogram_req, histogram.rs:672-699).  A doc with a value
+ * val (as f64, by specs[q].kind) inside them falls in bucket pos = floor((val - offset) / interval) as i64 (Rust `as`: saturating,
+ * NaN -> 0); docs without a value, NaN and, with the default bounds, +-inf are not counted.  Row q (out_stride entries apart)
+ * holds the intermediate result of query q over all its segments: its out_n[q] non-empty buckets in ascending pos, out_pos[i] and
+ * out_doc_count[i]; the key of a bucket is pos as f64 * interval + offset, and the final result (gap filling, min_doc_count,
+ * extended bounds, keys) is the caller's.  When some out_n[q] > out_stride, every out_n is written and the call returns
+ * TQ_ERR_INVALID_ARGUMENT: retry with a larger stride.  out_hits may be NULL; else out_hits[q] = tq_count_batch's answer for query
+ * q.  The counters of a query span the bucket range of the column's values in the 8192-doc tiles the query visits, clipped to its
+ * bounds: a range of more than 2^20 buckets returns TQ_ERR_UNSUPPORTED (the caller takes the CPU path).  TQ_OP_PHRASE returns
+ * TQ_ERR_UNSUPPORTED; a segment without the column TQ_ERR_NOT_FOUND; a kind outside TQ_FAST_* or an interval that is not finite and
+ * > 0 TQ_ERR_INVALID_ARGUMENT.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The run holds its columns as tq_sort_batch
+ * does. */
+int tq_histogram_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec* specs, size_t nq, uint32_t out_stride,
+                       int64_t* out_pos, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

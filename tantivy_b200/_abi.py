@@ -19,6 +19,7 @@ TQ_QUERY_HAS_THRESHOLD = 1
 TQ_QUERY_COUNT_HITS = 2
 TQ_QUERY_FILTER = 4
 TQ_ORDER_DESC, TQ_ORDER_ASC = 0, 1
+TQ_FAST_U64, TQ_FAST_I64, TQ_FAST_F64, TQ_FAST_BOOL, TQ_FAST_DATE = 0, 1, 2, 3, 4
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -139,6 +140,11 @@ class Stats(C.Structure):
     ]
 
 
+class HistogramStats(C.Structure):
+    """tq_histogram_stats — the cumulative counters of tq_histogram_batch (tq_get_histogram_stats)."""
+    _fields_ = [("hist_ms", C.c_float), ("units_hist", C.c_uint64), ("hist_tiles_seen", C.c_uint64), ("hist_tiles_one_bucket", C.c_uint64)]
+
+
 class SortSpec(C.Structure):
     """tq_sort_spec — the column and Order of TopDocs::order_by_fast_field for one query."""
     _fields_ = [("column_id", C.c_uint32), ("order", C.c_uint32)]
@@ -146,6 +152,17 @@ class SortSpec(C.Structure):
 
 SORT_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("order", "<u4")])
 assert SORT_SPEC_DTYPE.itemsize == C.sizeof(SortSpec) == 8
+
+
+class HistogramSpec(C.Structure):
+    """tq_histogram_spec — the column, its kind (TQ_FAST_*), the grid and the collect-time bounds of one query's histogram."""
+    _fields_ = [("column_id", C.c_uint32), ("kind", C.c_uint32), ("interval", C.c_double), ("offset", C.c_double),
+                ("hard_min", C.c_double), ("hard_max", C.c_double)]
+
+
+HISTOGRAM_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("kind", "<u4"), ("interval", "<f8"), ("offset", "<f8"), ("hard_min", "<f8"),
+                                 ("hard_max", "<f8")])
+assert HISTOGRAM_SPEC_DTYPE.itemsize == C.sizeof(HistogramSpec) == 40
 
 
 def ptr(arr, typ):

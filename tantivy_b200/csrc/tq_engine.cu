@@ -10,6 +10,8 @@
 //   TopBySortKeyCollector::merge_fruits       src/collector/sort_key_top_collector.rs:54-60
 // There is NO CPU fallback: without a CUDA device every entry point fails with TQ_ERR_CUDA.
 #include <algorithm>
+#include <cfloat>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -380,6 +382,16 @@ int tq_get_stats(tq_ctx* c, tq_stats* out) {
   return TQ_OK;
 }
 
+int tq_get_histogram_stats(tq_ctx* c, tq_histogram_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->hist_ms = (float)c->hist_ms;
+  out->units_hist = c->hist_units;
+  out->hist_tiles_seen = c->hist_tiles_seen;
+  out->hist_tiles_one_bucket = c->hist_tiles_one_bucket;
+  return TQ_OK;
+}
+
 int tq_segment_register(tq_ctx* c, uint32_t segment_ord, uint32_t field, uint32_t max_doc, int record_option,
                         const uint8_t* idx_body, size_t idx_len, const uint8_t* fieldnorm, size_t fieldnorm_len,
                         const uint8_t* alive_bitset, size_t alive_len) {
@@ -580,16 +592,24 @@ int tq_sort_column_register(tq_ctx* c, uint32_t column_id, uint32_t segment_ord,
   const uint32_t n_tiles = (max_doc + kTileDocs - 1) / kTileDocs;
   SortColumn col;
   col.tiles.assign(n_tiles, SortTile{{0ull, 0ull}, 0u, 0u});
+  col.finite.assign(n_tiles, FiniteTile{0ull, 0ull, 0u});
+  // images of the f64 infinities: finite values lie strictly between them, NaNs beyond them
+  constexpr unsigned long long kNegInf = 0x000FFFFFFFFFFFFFull, kPosInf = 0xFFF0000000000000ull;
   for (uint32_t t = 0; t < n_tiles; ++t) {
-    unsigned long long hi = 0, lo = ~0ull;
-    uint32_t flags = 0;
+    unsigned long long hi = 0, lo = ~0ull, fhi = 0, flo = ~0ull;
+    uint32_t flags = 0, fflags = 0;
     for (uint32_t d = t * kTileDocs, e = std::min(max_doc, d + kTileDocs); d < e; ++d) {
       if (present && !((present[d >> 3] >> (d & 7u)) & 1u)) { flags |= kSortTileNone; continue; }
       flags |= kSortTileValues;
-      hi = std::max<unsigned long long>(hi, values[d]);
-      lo = std::min<unsigned long long>(lo, values[d]);
+      const unsigned long long v = values[d];
+      hi = std::max<unsigned long long>(hi, v);
+      lo = std::min<unsigned long long>(lo, v);
+      if (v > kNegInf && v < kPosInf) { fflags |= kFiniteAny; fhi = std::max(fhi, v); flo = std::min(flo, v); }
+      else fflags |= v == kNegInf ? kFiniteNegInf : v == kPosInf ? kFinitePosInf : 0u;
     }
     col.tiles[t] = SortTile{{(flags & kSortTileValues) ? hi : 0ull, (flags & kSortTileValues) ? ~lo : 0ull}, flags, 0u};
+    col.finite[t] = FiniteTile{flo, fhi, fflags};
+    if (flags & kSortTileValues) { col.min_image = std::min<unsigned long long>(col.min_image, lo); col.max_image = std::max<unsigned long long>(col.max_image, hi); }
   }
   const size_t present_bytes = (size_t)n_tiles * (kTileDocs / 8);
   cudaError_t e = cudaMalloc(&col.d_values, std::max<size_t>((size_t)max_doc * 8, 8));
@@ -1728,6 +1748,178 @@ int tq_sort_batch(tq_ctx* c, const tq_query* queries, const tq_sort_spec* sorts,
   c->sort_units += cp.units.size() + nq;
   c->sort_tiles_seen += tiles[0];
   c->sort_tiles_skipped += tiles[1];
+  return TQ_OK;
+}
+
+// ---- histogram of a fast field ---------------------------------------------------------------------------------
+int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* specs, size_t nq, uint32_t out_stride,
+                       int64_t* out_pos, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !specs || !out_n || (out_stride && (!out_pos || !out_doc_count)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "histograms of phrase queries are not on the device path");
+    if (specs[qi].kind > TQ_FAST_DATE) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram kind");
+    if (!(specs[qi].interval > 0.0) || !std::isfinite(specs[qi].interval)) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram interval must be finite and > 0");
+  }
+  for (size_t qi = 0; qi < nq; ++qi) { out_n[qi] = 0; if (out_hits) out_hits[qi] = 0; }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<HistSeg> hsegs;
+  std::vector<HistQuery> hq(nq);
+  std::vector<HistUnit> hunits;  // parallel to cp.units
+  uint64_t n_counters = 0;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<long long, long long>> uwin;  // per unit of the query: its first and last pos (first > last: none)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_histogram_spec& sp = specs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      cols.clear();
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
+        if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a histogram query names a segment without the column (tq_sort_column_register)");
+        const SortColumn& col = it->second;
+        if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+        // normalize_histogram_req: the hard bounds collapse to every finite value when the segment's column lies inside them
+        double lo = sp.hard_min, hi = sp.hard_max;
+        if (col.min_image <= col.max_image && hist_value(col.min_image, sp.kind) >= lo && hist_value(col.max_image, sp.kind) <= hi) {
+          lo = -DBL_MAX;
+          hi = DBL_MAX;
+        }
+        hsegs.push_back(HistSeg{col.d_values, col.d_present, col.d_tiles, lo, hi});
+        cols.push_back(&col);
+      }
+      // per unit: the buckets of its tiles' values, clipped to its segment's bounds; the query's dense range (compute_dense_range,
+      // histogram.rs:751-769, over the visited tiles only) is their union
+      uwin.clear();
+      long long base = 0, top = -1;
+      bool any = false;
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const Unit& u = cp.units[ui];
+        const size_t k = u.qseg - s0;
+        const HistSeg& z = hsegs[u.qseg];
+        double umin = INFINITY, umax = -INFINITY;
+        for (uint32_t t = u.begin; t < u.end; ++t) {
+          double vmin, vmax;
+          if (sp.kind == TQ_FAST_F64) {  // an infinity widens the range only when it is in bounds; a NaN never is
+            const FiniteTile& f = cols[k]->finite[t];
+            vmin = INFINITY; vmax = -INFINITY;
+            if (f.flags & kFiniteAny) { vmin = hist_value(f.lo, sp.kind); vmax = hist_value(f.hi, sp.kind); }
+            if ((f.flags & kFiniteNegInf) && z.lo == -INFINITY) vmin = -INFINITY;
+            if ((f.flags & kFinitePosInf) && z.hi == INFINITY) vmax = INFINITY;
+          } else {
+            const SortTile& st = cols[k]->tiles[t];
+            if (!(st.flags & kSortTileValues)) continue;
+            vmin = hist_value(~st.best[1], sp.kind);
+            vmax = hist_value(st.best[0], sp.kind);
+          }
+          umin = std::min(umin, vmin);
+          umax = std::max(umax, vmax);
+        }
+        const double lo = std::max(umin, z.lo), hi = std::min(umax, z.hi);
+        if (!(lo <= hi)) { uwin.emplace_back(1, 0); continue; }  // no value of the unit can pass the bounds
+        const long long p0 = hist_pos(lo, sp.offset, sp.interval), p1 = hist_pos(hi, sp.offset, sp.interval);
+        uwin.emplace_back(p0, p1);
+        base = any ? std::min(base, p0) : p0;
+        top = any ? std::max(top, p1) : p1;
+        any = true;
+      }
+      const __int128 len = any ? (__int128)top - base + 1 : 0;
+      if (len > kHistMaxBins)
+        return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its histogram spans more than 2^20 buckets (take the CPU path)");
+      for (const auto& w : uwin)
+        hunits.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - base), (uint32_t)(w.second - w.first + 1)} : HistUnit{0u, 0u});
+      hq[qi] = HistQuery{sp.interval, sp.offset, base, n_counters, (uint32_t)len, sp.kind, out_hits ? kHistHits : 0u, 0u};
+      n_counters += (uint64_t)len;
+    }
+    if (n_counters > (1ull << 27)) return fail(TQ_ERR_INVALID_ARGUMENT, "batch too large: its histograms hold more than 2^27 buckets, split it");
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) b->held_columns.push_back(specs[qi].column_id);
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // descriptors: one H2D copy; scratch: row lengths | hits | tile counters (read back first), the rows (read back as wide as the
+  // longest), then the counters
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(hsegs), o_q = st.add(hq),
+               o_h = st.add(hunits);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  const size_t rows = nq * (size_t)out_stride;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_n = take(nq * 4), r_hits = take(nq * 8), r_tiles = take(16), head_bytes = off;
+  const size_t r_pos = take(rows * 8), r_count = take(rows * 8), r_counters = take(n_counters * 8);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(r_counters));
+  uint8_t* const d = b->scratch.p;
+  HistParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.hsegs = st.on_device<const HistSeg>(o_z);
+  P.queries = st.on_device<const HistQuery>(o_q);
+  P.hunits = st.on_device<const HistUnit>(o_h);
+  P.counts = reinterpret_cast<unsigned long long*>(d + r_counters);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.res_pos = reinterpret_cast<long long*>(d + r_pos);
+  P.res_count = reinterpret_cast<unsigned long long*>(d + r_count);
+  P.res_n = reinterpret_cast<uint32_t*>(d + r_n);
+  P.res_stride = out_stride;
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d + r_hits, 0, head_bytes - r_hits, b->stream));  // hits, tile counters
+  TQ_CUDA(cudaMemsetAsync(d + r_counters, 0, n_counters * 8, b->stream));
+  TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+  (cp.mixed ? k_hist<true> : k_hist<false>)<<<(unsigned)cp.units.size(), kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  k_hist_final<<<(unsigned)nq, kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  const uint8_t* h = b->res_pin.p;
+  memcpy(out_n, h + r_n, nq * 4);
+  uint32_t widest = 0;
+  for (size_t qi = 0; qi < nq; ++qi) widest = std::max(widest, out_n[qi]);
+  const bool fits = widest <= out_stride;
+  if (fits && widest) {  // the rows, only as wide as the longest
+    TQ_CUDA(cudaMemcpy2DAsync(b->res_pin.p + r_pos, (size_t)out_stride * 8, d + r_pos, (size_t)out_stride * 8, (size_t)widest * 8, nq,
+                              cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpy2DAsync(b->res_pin.p + r_count, (size_t)out_stride * 8, d + r_count, (size_t)out_stride * 8, (size_t)widest * 8, nq,
+                              cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+  }
+  for (size_t qi = 0; fits && qi < nq; ++qi) {
+    const size_t at = qi * (size_t)out_stride;
+    memcpy(out_pos + at, h + r_pos + at * 8, (size_t)out_n[qi] * 8);
+    memcpy(out_doc_count + at, h + r_count + at * 8, (size_t)out_n[qi] * 8);
+    if (out_hits) memcpy(&out_hits[qi], h + r_hits + qi * 8, 8);
+  }
+  float ms = 0;
+  cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_tiles, 16);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->hist_ms += ms;
+    c->hist_units += cp.units.size() + nq;
+    c->hist_tiles_seen += tiles[0];
+    c->hist_tiles_one_bucket += tiles[1];
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a histogram has more non-empty buckets than out_stride: out_n holds how many");
   return TQ_OK;
 }
 

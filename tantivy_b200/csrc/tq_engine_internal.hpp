@@ -157,11 +157,20 @@ struct FilterView {
 // A sort column of one (column_id, segment_ord) (tq_sort_column_register): the u64 images on the device, the present bits (padded
 // to whole 8192-doc tiles: k_sort reads a tile's words whole) and the bounds of every 8192-doc tile, on the device for k_sort and
 // on the host for the planner, which runs a query's units by descending bound.
+// A histogram reads the same column as f64; for TQ_FAST_F64 the planner also needs the bounds of each tile's finite values and
+// whether it holds -inf / +inf (finite), since the image bounds of a tile with an infinity or a NaN say nothing of its range.
+struct FiniteTile {
+  unsigned long long lo, hi;  // smallest and largest image of the tile's finite f64 values (kFiniteAny)
+  uint32_t flags;
+};
+constexpr uint32_t kFiniteAny = 1, kFiniteNegInf = 2, kFinitePosInf = 4;
 struct SortColumn {
   unsigned long long* d_values = nullptr;
   uint32_t* d_present = nullptr;  // null: every doc has a value
   SortTile* d_tiles = nullptr;
   std::vector<SortTile> tiles;
+  std::vector<FiniteTile> finite;
+  unsigned long long min_image = ~0ull, max_image = 0;  // over every doc with a value (none: min_image > max_image)
   void release() { cudaFree(d_values); cudaFree(d_present); cudaFree(d_tiles); d_values = nullptr; d_present = nullptr; d_tiles = nullptr; }
 };
 
@@ -229,6 +238,9 @@ struct tq_ctx {
   // cumulative tq_stats fields of the sort runs (sort_ms, units_sort, sort_tiles_seen, sort_tiles_skipped)
   double sort_ms = 0;
   uint64_t sort_units = 0, sort_tiles_seen = 0, sort_tiles_skipped = 0;
+  // ... and of the histogram runs (hist_ms, units_hist, hist_tiles_seen, hist_tiles_one_bucket)
+  double hist_ms = 0;
+  uint64_t hist_units = 0, hist_tiles_seen = 0, hist_tiles_one_bucket = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;

@@ -1417,6 +1417,125 @@ __global__ void __launch_bounds__(kThreads) k_sort_final(const SortParams P) {
   if (threadIdx.x == 0) P.res_counts[q] = have + n_none;
 }
 
+// ---- histogram of a fast field (AggregationCollector: histogram / date_histogram, bucket/histogram/histogram.rs) ------------
+// The docs Count counts, each with a value in its bounds counted in bucket pos(val).  One CTA per Count unit: per 8192-doc tile
+// match_tile builds the match bitmap, and-ed with the present bits.  When the tile's smallest and largest values (SortTile) are
+// both in bounds and in one bucket, so is every value between them (pos is monotone in the image): the tile's matches go to that
+// bucket without a gather.  Otherwise each thread walks the matches of its own 32-doc word: an 8-byte gather, the conversion, the
+// bounds test and pos, one counter increment.  A unit counts into its own window of the query's counters (HistUnit: the buckets of
+// its tiles' values in bounds), per CTA in shared memory when the window has kHistSmemBins or fewer (flushed with one 64-bit
+// atomicAdd per non-zero bucket at exit), else global.  A timestamp unit of eight tiles spans a few minutes of the column, so even a
+// query of many thousand buckets counts on chip.
+
+// (3 CTAs per SM: the division's slow path is a call, and at the 64 registers of 4 CTAs the kernel spills around it)
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
+  static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ uint32_t s_bins[kHistSmemBins];
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ uint32_t s_one;  // the tile's one bucket (index into the unit's window), or ~0u
+  const Unit U = P.c.units[blockIdx.x];
+  const CountSeg S = P.c.segs[U.qseg];
+  const HistSeg Z = P.hsegs[U.qseg];
+  const HistQuery Q = P.queries[S.query];
+  const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const HistUnit W = P.hunits[blockIdx.x];
+  const long long base = Q.base + (long long)W.first;  // pos of the unit's first counter
+  const bool shared = W.n_bins <= kHistSmemBins;
+  unsigned long long* const counts = P.counts + Q.counters + W.first;
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x) s_bins[i] = 0;
+  uint32_t total = 0, one = 0;
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      const SortTile T = Z.tiles[tile];
+      uint32_t idx = 0xFFFFFFFFu;
+      if (W.n_bins && (T.flags & kSortTileValues)) {
+        const double vmin = hist_value(~T.best[1], Q.kind), vmax = hist_value(T.best[0], Q.kind);
+        if (vmin >= Z.lo && vmax <= Z.hi) {
+          const long long p = hist_pos(vmin, Q.offset, Q.interval);
+          if (p == hist_pos(vmax, Q.offset, Q.interval) && p >= base && p - base < (long long)W.n_bins) idx = (uint32_t)(p - base);
+        }
+      }
+      s_one = idx;
+      one += idx != 0xFFFFFFFFu ? 1u : 0u;
+    }
+    match_tile<kMixed>(P.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    total += (uint32_t)__popc(bits);
+    uint32_t with = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
+    if (s_one < W.n_bins) {  // one bucket: every value of the tile, matching or not, lies in bounds and in one bucket
+      const uint32_t c = __reduce_add_sync(kFull, (uint32_t)__popc(with));
+      const uint32_t idx = s_one;
+      if (lane == 0 && c) {
+        if (shared) atomicAdd(&s_bins[idx], c);
+        else atomicAdd(&counts[idx], (unsigned long long)c);
+      }
+    } else if (W.n_bins) {
+      for (; with; with &= with - 1u) {
+        const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(with) - 1);
+        const double val = hist_value(__ldg(Z.values + doc), Q.kind);
+        if (!(val >= Z.lo && val <= Z.hi)) continue;  // HistogramBounds::contains (NaN never passes)
+        const unsigned long long idx = (unsigned long long)(hist_pos(val, Q.offset, Q.interval) - base);
+        if (idx < W.n_bins) {  // (always: the window covers every value in bounds of the unit's tiles)
+          if (shared) atomicAdd(&s_bins[idx], 1u);
+          else atomicAdd(&counts[idx], 1ull);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x)
+      if (s_bins[i]) atomicAdd(&counts[i], (unsigned long long)s_bins[i]);
+  if (Q.flags & kHistHits) {
+    total = __reduce_add_sync(kFull, total);
+    if (lane == 0) s_part[warp] = total;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (Q.flags & kHistHits) {
+      unsigned long long sum = 0;
+      for (int w = 0; w < kWarps; ++w) sum += s_part[w];
+      if (sum) atomicAdd(&P.c.counts[S.query], sum);
+    }
+    const uint32_t seen = U.end - U.begin;
+    if (seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (one) atomicAdd(&P.tiles[1], (unsigned long long)one); }
+  }
+}
+
+// One CTA per query: the non-zero counters of its range, in ascending pos, into its row (a CTA-wide prefix sum per 256 counters).
+__global__ void __launch_bounds__(kThreads) k_hist_final(const HistParams P) {
+  __shared__ uint32_t s_part[kWarps];
+  const uint32_t q = blockIdx.x;
+  const HistQuery Q = P.queries[q];
+  const unsigned long long* const counts = P.counts + Q.counters;
+  const size_t row = (size_t)q * P.res_stride;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t base = 0;  // non-empty buckets before this round of counters (the same on every thread)
+  for (uint32_t i0 = 0; i0 < Q.n_bins; i0 += blockDim.x) {
+    const uint32_t i = i0 + threadIdx.x;
+    const unsigned long long c = i < Q.n_bins ? counts[i] : 0ull;
+    const uint32_t mask = __ballot_sync(kFull, c != 0ull);
+    if (lane == 0) s_part[warp] = (uint32_t)__popc(mask);
+    __syncthreads();
+    uint32_t at = base + (uint32_t)__popc(mask & ((1u << lane) - 1u));
+    for (uint32_t w = 0; w < warp; ++w) at += s_part[w];
+    if (c && at < P.res_stride) {
+      P.res_pos[row + at] = Q.base + (long long)i;
+      P.res_count[row + at] = c;
+    }
+    for (int w = 0; w < kWarps; ++w) base += s_part[w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) P.res_n[q] = base;
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

@@ -7,6 +7,10 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <math.h>
+#include <string.h>
+
+#include "../../include/tantivy_b200.h"  // TQ_FAST_*
 #include "bm25_host.hpp"  // TQ_HD
 
 namespace tq {
@@ -196,6 +200,75 @@ struct SortParams {
 };
 static_assert(sizeof(SortTile) == 24 && sizeof(SortSeg) == 32 && sizeof(SortQuery) == 16 && sizeof(SortQState) == 24 && sizeof(SortCand) == 16,
               "sort descriptor layout");
+
+// ---- histogram of a fast field (k_hist, k_hist_final) -------------------------------------------------------------------
+// Doc counts per bucket pos = as_i64(floor((val - offset) / interval)) of the docs Count counts whose value lies in the (query,
+// segment)'s bounds.  A query's counters cover its dense range [base, base + n_bins); a unit counts into its own window of them
+// (HistUnit): kHistSmemBins or fewer are kept per CTA in shared memory, more go straight to the global u64 counters.  A range above kHistMaxBins is refused (TQ_ERR_UNSUPPORTED).
+// The value and the bucket are computed by the same code on the host (the planner's ranges) and on the device (k_hist).
+// f64_from_fastfield_u64 (aggregation/mod.rs:374) of a u64 image
+TQ_HD inline double hist_value(unsigned long long v, uint32_t kind) {
+  constexpr unsigned long long kHigh = 1ull << 63;
+  if (kind == TQ_FAST_F64) {
+    const unsigned long long bits = (v & kHigh) ? v ^ kHigh : ~v;
+#ifdef __CUDA_ARCH__
+    return __longlong_as_double((long long)bits);
+#else
+    double d;
+    memcpy(&d, &bits, 8);
+    return d;
+#endif
+  }
+  if (kind == TQ_FAST_I64 || kind == TQ_FAST_DATE) return (double)(long long)(v ^ kHigh);
+  return (double)v;  // u64, bool
+}
+// get_bucket_pos_f64(val, interval, offset) as i64 (histogram.rs:739-741): Rust's `as` saturates and maps NaN to 0
+TQ_HD inline long long hist_pos(double val, double offset, double interval) {
+#ifdef __CUDA_ARCH__
+  const double f = floor(__ddiv_rn(__dsub_rn(val, offset), interval));
+#else
+  const double f = floor((val - offset) / interval);  // (the host units build with -ffp-contract=off)
+#endif
+  if (f != f) return 0;
+  if (f >= 9223372036854775808.0) return 0x7FFFFFFFFFFFFFFFll;
+  if (f < -9223372036854775808.0) return (long long)0x8000000000000000ull;
+  return (long long)f;
+}
+constexpr uint32_t kHistSmemBins = 4096;
+constexpr uint32_t kHistMaxBins = 1u << 20;
+struct HistSeg {  // the column and bounds of one (query, segment), parallel to CountParams::segs
+  const unsigned long long* values;  // [max_doc] u64 images
+  const uint32_t* present;           // bitset in the alive layout (null: every doc has a value)
+  const SortTile* tiles;             // the column's per-tile bounds (tq_sort_column_register)
+  double lo, hi;                     // collect-time bounds after the per-segment collapse: val counts iff lo <= val <= hi
+};
+struct HistQuery {
+  double interval, offset;
+  long long base;              // pos of counter 0
+  unsigned long long counters; // first counter of the query in HistParams::counts
+  uint32_t n_bins;             // 0: no doc of the query can pass its bounds
+  uint32_t kind;               // TQ_FAST_*
+  uint32_t flags;              // kHistHits: the query's Count is asked for as well
+  uint32_t pad;
+};
+constexpr uint32_t kHistHits = 1;
+struct HistUnit {  // the buckets one k_hist unit can count into, parallel to CountParams::units
+  uint32_t first;   // its first counter, relative to the query's base
+  uint32_t n_bins;  // 0: no value of the unit's tiles passes the bounds
+};
+struct HistParams {
+  CountParams c;  // structure words, (query, segment) pairs, units and hit counters: the Count plan
+  const HistSeg* hsegs;
+  const HistQuery* queries;
+  const HistUnit* hunits;
+  unsigned long long* counts;   // every query's counters, zeroed before the run
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them counted as one bucket
+  long long* res_pos;           // [nq][res_stride]: the non-empty buckets in ascending pos
+  unsigned long long* res_count;
+  uint32_t* res_n;              // [nq]: how many there are (may exceed res_stride: only res_stride are written)
+  uint32_t res_stride;
+};
+static_assert(sizeof(HistSeg) == 40 && sizeof(HistQuery) == 48 && sizeof(HistUnit) == 8, "histogram descriptor layout");
 
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 

@@ -6,7 +6,8 @@ import os
 
 import numpy as np
 
-from ._abi import SORT_SPEC_DTYPE, TQ_ORDER_ASC, TQ_ORDER_DESC, Query, QueryBatch, SortSpec, Stats, TermSeg, f32p, ptr, u8p, u32p, u64p
+from ._abi import (HISTOGRAM_SPEC_DTYPE, SORT_SPEC_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64, TQ_ORDER_ASC,
+                   TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, f32p, ptr, u8p, u32p, u64p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -28,6 +29,7 @@ def _load():
     lib.tq_ctx_create.argtypes = [C.c_int, C.POINTER(vp)]
     lib.tq_ctx_destroy.argtypes = [vp]
     lib.tq_get_stats.argtypes = [vp, C.POINTER(Stats)]
+    lib.tq_get_histogram_stats.argtypes = [vp, C.POINTER(HistogramStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -42,6 +44,7 @@ def _load():
     lib.tq_sort_column_register.argtypes = [vp, C.c_uint32, C.c_uint32, u64p, sz, u8p, sz]
     lib.tq_sort_column_unregister.argtypes = [vp, C.c_uint32]
     lib.tq_sort_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(SortSpec), sz, C.c_uint32, u64p, u8p, u32p, u32p, u32p, u64p]
+    lib.tq_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), sz, C.c_uint32, C.POINTER(C.c_int64), u64p, u32p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -110,6 +113,7 @@ def _check(rc, ctx=None):
 
 _HIGHEST_BIT = np.uint64(1 << 63)
 FAST_VALUE_KINDS = ("u64", "i64", "f64", "bool", "date")
+_FAST_KIND = {"u64": TQ_FAST_U64, "i64": TQ_FAST_I64, "f64": TQ_FAST_F64, "bool": TQ_FAST_BOOL, "date": TQ_FAST_DATE}
 
 
 def fast_value_to_u64(values, kind):
@@ -367,6 +371,37 @@ class Context:
         out = (values, present.astype(bool), segs, docs, counts)
         return out + (hits[:qb.nq],) if count_hits else out
 
+    def histogram_batch(self, qb: QueryBatch, specs, count_hits=False, stride=4096):
+        """The segment part of a histogram aggregation per query (tq_histogram_batch) over sort columns; specs = one
+        (column_id, kind, interval, offset[, hard_min, hard_max]) per query, kind "u64" / "i64" / "f64" / "bool" / "date" or a
+        TQ_FAST_* value, interval, offset and bounds in the column's unit (date: nanoseconds; tantivy_b200.histogram turns requests
+        into specs).  Returns (pos, doc_count, n): row q holds the n[q] non-empty buckets of query q in ascending pos, over all its
+        segments -- and with count_hits=True the Count of every query as well.  Raises TqError with code -4 (TQ_ERR_UNSUPPORTED)
+        when a query's bucket range is too wide for the device.  `stride` is the row width tried first: a longer row runs the
+        batch again at its width."""
+        specs = list(specs)
+        if len(specs) != qb.nq:
+            raise ValueError(f"one histogram spec per query: {len(specs)} for {qb.nq} queries")
+        spec = np.zeros(max(qb.nq, 1), dtype=HISTOGRAM_SPEC_DTYPE)
+        for i, sp in enumerate(specs):
+            col, kind, interval, offset = sp[:4]
+            hard_min, hard_max = sp[4:6] if len(sp) > 4 else (-np.finfo(np.float64).max, np.finfo(np.float64).max)
+            spec[i] = (col, _FAST_KIND.get(kind, kind), interval, offset, hard_min, hard_max)
+        n = max(qb.nq, 1)
+        while True:
+            pos = np.empty((n, stride), dtype=np.int64)  # (only the first n[q] entries of row q are written)
+            counts = np.empty((n, stride), dtype=np.uint64)
+            nb = np.zeros(n, dtype=np.uint32)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_histogram_batch(self.h, qb.ptr, spec.ctypes.data_as(C.POINTER(HistogramSpec)), qb.nq, stride,
+                                        pos.ctypes.data_as(C.POINTER(C.c_int64)), ptr(counts, u64p), ptr(nb, u32p), ptr(hits, u64p))
+            if rc == -1 and int(nb.max()) > stride:  # TQ_ERR_INVALID_ARGUMENT with the row lengths: a wider row
+                stride = int(nb.max())
+                continue
+            _check(rc, self.h)
+            out = (pos, counts, nb)
+            return out + (hits[:qb.nq],) if count_hits else out
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -400,7 +435,11 @@ class Context:
     def stats(self):
         s = Stats()
         _check(LIB.tq_get_stats(self.h, C.byref(s)), self.h)
-        return {name: (list(getattr(s, name)) if name in ("or_windows", "tile_counters", "tile_cycles", "tile_b2_exits") else getattr(s, name)) for name, _ in Stats._fields_}
+        hs = HistogramStats()
+        _check(LIB.tq_get_histogram_stats(self.h, C.byref(hs)), self.h)
+        out = {name: (list(getattr(s, name)) if name in ("or_windows", "tile_counters", "tile_cycles", "tile_b2_exits") else getattr(s, name)) for name, _ in Stats._fields_}
+        out.update({name: getattr(hs, name) for name, _ in HistogramStats._fields_})
+        return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
         """All arguments are raw device addresses (int), e.g. torch tensors' data_ptr()."""
