@@ -187,14 +187,16 @@ typedef struct {
   uint64_t tile_groups;         /* query groups evaluated together (one decode-and-score pass each) */
   uint64_t tile_postings;       /* postings decoded and scored by k_score_lists (every distinct list once) */
   uint64_t tile_list_bytes;     /* bytes of those lists' postings ranges (skip data + packed blocks + VInt tails) */
-  uint64_t tile_scratch_bytes;  /* HBM scratch of the pair arrays, tile indexes, samples and k_tile's sparse-slot cursors */
+  uint64_t tile_scratch_bytes;  /* HBM scratch of the pair arrays, tile indexes, samples, key histograms and the sparse-slot cursors */
   uint64_t tile_fallbacks;      /* 1 if the run overflowed a tile engine buffer and was repeated (TQ_OP_BOOL on the tile engine, the rest on the per-query kernels) */
   uint64_t tile_counters[8];    /* cumulative, with TQ_TILE_COUNTERS=1: (query, tile) pairs seen / skipped / light / heavy,
                                    essential postings applied, docs completed, docs at or above the threshold;
                                    [7] (always): dynamic shared memory bytes of a k_tile CTA of the last prepared group */
   uint64_t tile_ctas_per_sm;    /* k_tile CTAs an SM holds at once in the exact launches of the last prepared group (occupancy API) */
   uint64_t tile_cycles[8];      /* cumulative, with TQ_TILE_COUNTERS=1: k_tile warp cycles (clock64) by stage: [0] cursor prologue,
-                                   [1] A (staging), [2] B1 (routing), [3] B2 (flat evaluation), [4] B3 (windows), [5] barrier waits */
+                                   [1] A (staging), [2] B1 (routing), [3] B2 (flat evaluation), [4] B3 (windows and running-threshold
+                                   refreshes), [5] barrier waits; not cycles: [6] running-threshold refreshes of the exact launches,
+                                   [7] of them those that raised the query's threshold */
   uint64_t tile_groups_union_only; /* of tile_groups: groups whose queries are all term queries and unions, which run the
                                       union-only k_tile instances (k_tile<*, *, true>); the rest run the general instances */
   uint64_t tile_b2_exits[4];    /* cumulative, with TQ_TILE_COUNTERS=1: union postings of the exact k_tile launches' flat evaluation

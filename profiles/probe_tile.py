@@ -60,6 +60,7 @@ for i in range(steps + 2):
                       "groups": st["tile_groups"], "smem": int(c1[7]), "tile_ctas_per_sm": st["tile_ctas_per_sm"],
                       "counters(pairs,skip,light,heavy,ess,compl,pass)": (c1 - c0)[:7].tolist(),
                       "b2_union_exits(bound,not_owner,walk,completed)": (x1 - x0).tolist(),
+                      "theta_refresh(refreshes,raises)": (y1 - y0)[6:8].tolist(),
                       "stage_shares": stage_shares(y1 - y0)}), flush=True)
     c0, y0, x0 = c1, y1, x1
     bt.close()

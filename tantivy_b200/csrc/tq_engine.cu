@@ -284,7 +284,7 @@ int tq_ctx_create(int device, tq_ctx** out) {
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
   c->tile_scratch_mb = env_u32("TQ_TILE_SCRATCH_MB", (uint32_t)(total_bytes / 8 >> 20));
-  c->tile_sample_div = env_u32("TQ_TILE_SAMPLE_DIV", 16);    // share of the tiles in the sample launch (0/1: none)
+  c->tile_sample_div = env_u32("TQ_TILE_SAMPLE_DIV", 32);    // share of the tiles in the sample launch (0/1: none)
   c->tile_round_div1 = env_u32("TQ_TILE_ROUND_DIV1", 8);     // the exact launches end at 1/8, 1/2 and all of a segment's tiles
   c->tile_round_div2 = env_u32("TQ_TILE_ROUND_DIV2", 2);
   c->tile_light_max = env_u32("TQ_TILE_LIGHT_MAX", 96);      // essential postings up to which a (query, tile) pair is evaluated posting by posting
@@ -918,9 +918,9 @@ static int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
   b->desc_bytes = st.bytes;
   TQ_CUDA(st.reserve(b->pin, b->dev));
 
-  // ---- tile scratch: pair arrays | tile indexes | samples | sample counts | flags + counters --------------------------------
+  // ---- tile scratch: pair arrays | tile indexes | samples | sample counts | key histograms | flags + counters ---------------
   uint32_t sample_cap = 0;
-  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_flags = 0, to_cursors = 0, to_count_cursors = 0;
+  size_t to_docs = 0, to_scores = 0, to_tix = 0, to_samples = 0, to_scount = 0, to_th_hist = 0, to_flags = 0, to_cursors = 0, to_count_cursors = 0;
   if (!pl.gstage.empty()) {
     uint64_t sample_units_tiles = 0;
     for (auto& gs : pl.gstage) for (auto& u : gs.units[0]) sample_units_tiles += u.t1 - u.t0;
@@ -931,6 +931,7 @@ static int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     to_tix = so2; so2 = align256(so2 + pl.tix_total_words * 4);
     to_samples = so2; so2 = align256(so2 + nq1 * sample_cap * 4);
     to_scount = so2; so2 = align256(so2 + nq1 * 4);
+    to_th_hist = so2; so2 = align256(so2 + nq1 * kThHistWords * 4);
     to_flags = so2; so2 = align256(so2 + 256);
     size_t cursors = 0;  // k_tile's sparse-slot cursors: max_slots per CTA of the largest launch (launches of a batch run one after another)
     for (auto& gs : pl.gstage)
@@ -978,6 +979,7 @@ static int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     TP.p_scores = reinterpret_cast<float*>(b->tile_dev.p + to_scores);
     TP.samples = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_samples);
     TP.sample_count = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_scount);
+    TP.th_hist = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_th_hist);
     TP.flags = reinterpret_cast<uint32_t*>(b->tile_dev.p + to_flags);
     TP.counters = c->tile_counters ? c->d_counters + 8 : nullptr;
     TP.cursors = reinterpret_cast<uint2*>(b->tile_dev.p + to_cursors);
@@ -1310,7 +1312,7 @@ static int run_phase(tq_batch* b, int phase) {
     if ((b->n_units[r] || (tile_round && phase > 0)) && b->nq) timed(SPAN_THETA, [&] { k_theta<<<(unsigned)b->nq, kThreads, 0, b->stream>>>(P); });
     if (tile_round && phase == 0 && b->nq) {
       const TileParams& TP = b->groups[0].params;
-      timed(SPAN_THETA, [&] { k_theta_samples<<<(unsigned)b->nq, kThreads, 0, b->stream>>>(P, TP.samples, TP.sample_count, TP.sample_cap); });
+      timed(SPAN_THETA, [&] { k_theta_samples<<<(unsigned)b->nq, kThreads, 0, b->stream>>>(P, TP.samples, TP.sample_count, TP.sample_cap, TP.th_hist); });
     }
     TQ_CUDA(cudaGetLastError());
     b->stats.kernel_launches += launches;

@@ -318,6 +318,26 @@ struct SChunk { uint32_t slot, b0, b1; };  // a CTA's share of k_score_lists: bl
 static_assert(sizeof(TSlot) == 32 && sizeof(TSeg) == 64 && sizeof(TQuery) == 12 && sizeof(TUnit) == 16 && sizeof(SChunk) == 12,
               "tile descriptor layout");
 
+// Running threshold of the exact k_tile launches: per query of the batch, a count of its pushed candidates' score keys by
+// bucket of key >> 16 (1/128 of a binade, 0.8 %) above a per-query base, kThHistFine buckets in kThHistCoarse coarse buckets of 32,
+// so that one warp finds the k-th from the top with two reads of one word per lane.  A query's words: fine counts [0, 2048),
+// coarse counts [2048, 2112), the base word at kThHistBaseWord (k_theta_samples writes the threshold's key >> 16 there; 0 = no
+// threshold yet: kThHistFallbackBase, the key of 2^-4 >> 16, so the window spans 2^-4 .. 2^12).  Zeroed at the start of every run.
+constexpr uint32_t kThHistFine = 2048, kThHistCoarse = 64, kThHistBaseWord = kThHistFine + kThHistCoarse;
+constexpr uint32_t kThHistWords = kThHistBaseWord + 32u;  // (a multiple of 32 words: every query's region starts on a 128-B line)
+constexpr uint32_t kThHistFallbackBase = 0xBD80u;
+TQ_HD inline uint32_t th_hist_base(uint32_t base_word) { return base_word ? base_word : kThHistFallbackBase; }
+// The bucket of a key: 0 at or below the base, the top bucket above the window.  edge(b) is a key no larger than any key of
+// bucket b (0 for bucket 0), and grows with b: edge(bucket(key)) <= key, so k candidates in buckets >= b hold k keys >= edge(b).
+TQ_HD inline uint32_t th_hist_bucket(uint32_t key, uint32_t base) {
+  const uint32_t hi = key >> 16;
+  return hi <= base ? 0u : (hi - base < kThHistFine - 1u ? hi - base : kThHistFine - 1u);
+}
+TQ_HD inline uint32_t th_hist_edge(uint32_t b, uint32_t base) {
+  const uint32_t hi = base + b;
+  return b ? (hi < 0xFFFFu ? hi : 0xFFFFu) << 16 : 0u;
+}
+
 struct TileParams {
   const TSlot* slots;
   const TSeg* segs;
@@ -333,8 +353,10 @@ struct TileParams {
   unsigned long long* counters;  // [16] diagnostics: 0 (query, tile) pairs seen, 1 skipped (bound / no essential posting / cold window),
                                  //     2 light pairs, 3 heavy pairs, 4 essential postings applied, 5 docs completed, 6 docs at or above the threshold;
                                  //     [8, 8 + kTileStages) clock64() cycles summed over warps, by stage (TileStage);
-                                 //     [16, 16 + kOrExits) B2's union postings by exit (TileOrExit)
+                                 //     [16, 16 + kOrExits) B2's union postings by exit (TileOrExit);
+                                 //     14 running-threshold refreshes, 15 of them that raised the threshold
                                  //     (null: the launch runs k_tile<*, false, *>)
+  uint32_t* th_hist;   // [n_queries of the batch][kThHistWords]: the exact launches' candidate keys by bucket (th_hist_bucket)
   uint2* cursors;      // [CTAs of the largest launch][max_slots] sparse slots' cursors (k_tile)
   uint32_t sample_cap;
   uint32_t p_cap;      // pairs of one tile that fit in shared memory

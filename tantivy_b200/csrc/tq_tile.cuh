@@ -30,7 +30,7 @@
 //                       give bit-identical scores;
 //                     * survivors (score key >= the query's threshold) go to the query's candidate region, k_final
 //                       (TopNHeap / merge_fruits) selects exactly.
-//   thresholds      a first launch over 1/16 of the tiles only SAMPLES scores (the complete scores of the docs that hold one of
+//   thresholds      a first launch over 1/32 of the tiles only SAMPLES scores (the complete scores of the docs that hold one of
 //                   a union's two heaviest clauses / a conjunction's matches); the k-th best sample is a valid lower bound of
 //                   the final k-th score (k_theta_samples).  The exact launches follow,
 //                   each ending in k_theta (exact k-th best candidate so far), so most tiles are visited under a
@@ -149,14 +149,74 @@ __device__ __forceinline__ float tile_find(const TileView& V, uint32_t slot, uin
   return found ? V.score[lo] : 0.0f;
 }
 
-__device__ __forceinline__ void tile_push(const BatchParams& P, uint32_t query, float score, uint32_t doc, uint32_t segment_ord,
-                                          uint32_t th_key, const uint8_t* __restrict__ alive) {
+// A CTA's counters of the current tile: pairs staged (A); heavy pairs (B1) and those a window took (B3); flat pairs (B1); work-list
+// segments claimed (B1), taken by a warp (B2) and written (the list filled up from `segvalid` on); whether queries were deferred
+// to another round of B1 + B2, and which; the queries whose running threshold is refreshed after the tile (tile_push).
+constexpr uint32_t kTileRefreshCap = 16;
+struct TileCtl {
+  uint32_t total, nheavy, hpos, nflat, nseg, segpos, segvalid, ndefer, defer[kTileMaxQueries / 32u];
+  uint32_t nref, ref[kTileRefreshCap];
+};
+
+// A candidate of an exact launch: appended to the query's region when its key reaches th_key and the doc is alive, and counted in
+// the query's key histogram (TileParams::th_hist).  The k-th push and every max(k / 4, 16)-th after it put the query on the CTA's
+// refresh list (a full list drops the entry: the next trigger comes soon enough).
+__device__ __forceinline__ void tile_push(const BatchParams& P, const TileParams& TP, TileCtl& C, uint32_t query, float score, uint32_t doc,
+                                          uint32_t segment_ord, uint32_t th_key, const uint8_t* __restrict__ alive) {
   const uint32_t key = score_to_key(score);
   if (key < th_key) return;
   if (alive && !is_alive(alive, doc)) return;
   const DQuery Q = P.queries[query];
   const uint32_t idx = atomicAdd(&P.qstate[query].cand_count, 1u);
   if (idx < Q.cand_cap) P.cands[Q.cand_base + idx] = Cand{key, segment_ord, doc, 0u};
+  uint32_t* H = TP.th_hist + (size_t)query * kThHistWords;
+  const uint32_t b = th_hist_bucket(key, th_hist_base(__ldg(H + kThHistBaseWord)));
+  atomicAdd(H + b, 1u);
+  atomicAdd(H + kThHistFine + (b >> 5), 1u);
+  const uint32_t n = idx + 1u;
+  if (n >= Q.k && (n - Q.k) % max(Q.k >> 2, 16u) == 0u) {
+    const uint32_t r = atomicAdd(&C.nref, 1u);
+    if (r < kTileRefreshCap) C.ref[r] = query;
+  }
+}
+
+// The running threshold of query `query`, one warp: the highest bucket b whose suffix count (candidates in buckets >= b) reaches
+// k, from the coarse counts (two per lane) and then that coarse bucket's 32 fine counts; the threshold rises to edge(b).
+// Why this is exact: every candidate counted is a real, alive doc that passes the query's filter, with its complete score; a doc is
+// pushed at most once per query and run (the exact launches cover disjoint tile ranges, a (query, tile) pair has one owner per
+// doc in B2 and one window in B3, and the sample launch pushes nothing); every count is a lower bound of what its bucket holds,
+// however the reads interleave with other CTAs' atomics.  So k docs have keys >= edge(b), and the final k-th key is >= edge(b):
+// docs tied at the k-th key still pass `key >= th_key`.  The same holds per rank under the sharded key exchange.  Returns whether
+// the threshold rose.
+__device__ __forceinline__ bool tile_theta_refresh(const BatchParams& P, const TileParams& TP, uint32_t query, uint32_t lane) {
+  const uint32_t* H = TP.th_hist + (size_t)query * kThHistWords;
+  const uint32_t k = P.queries[query].k;
+  const uint32_t c0 = __ldcg(H + kThHistFine + 2u * lane), c1 = __ldcg(H + kThHistFine + 2u * lane + 1u);
+  uint32_t suf = c0 + c1;  // -> the count of coarse buckets >= 2 * lane
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t v = __shfl_down_sync(kFull, suf, o);
+    if (lane + o < 32u) suf += v;
+  }
+  const uint32_t hit = __ballot_sync(kFull, suf >= k);
+  if (!hit) return false;
+  const uint32_t L = 31u - __clz(hit);
+  const uint32_t sL = __shfl_sync(kFull, suf, L), c0L = __shfl_sync(kFull, c0, L), c1L = __shfl_sync(kFull, c1, L);
+  const bool odd = sL - c0L >= k;
+  const uint32_t cb = 2u * L + (odd ? 1u : 0u);
+  const uint32_t need = k - (odd ? sL - c0L - c1L : sL - c0L);  // (> 0: the coarse buckets above cb hold fewer than k)
+  uint32_t fsuf = __ldcg(H + cb * 32u + lane);
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t v = __shfl_down_sync(kFull, fsuf, o);
+    if (lane + o < 32u) fsuf += v;
+  }
+  const uint32_t fhit = __ballot_sync(kFull, fsuf >= need);  // (0 when the fine counts trail the coarse ones: take cb's first)
+  const uint32_t b = cb * 32u + (fhit ? 31u - __clz(fhit) : 0u);
+  const uint32_t edge = th_hist_edge(b, th_hist_base(__ldg(H + kThHistBaseWord)));
+  uint32_t old = 0xFFFFFFFFu;
+  if (lane == 0 && edge) old = atomicMax(&P.qstate[query].theta, edge);
+  return __shfl_sync(kFull, old, 0) < edge;
 }
 
 // One (query, tile) pair that is evaluated posting by posting: what every posting's thread needs to know (16 bytes).
@@ -348,14 +408,10 @@ __device__ __forceinline__ TileView tile_view(unsigned char* s_dyn, const TilePa
                   n_big};
 }
 
-// A CTA's counters of the current tile: pairs staged (A); heavy pairs (B1) and those a window took (B3); flat pairs (B1); work-list
-// segments claimed (B1), taken by a warp (B2) and written (the list filled up from `segvalid` on); whether queries were deferred
-// to another round of B1 + B2, and which.
-struct TileCtl { uint32_t total, nheavy, hpos, nflat, nseg, segpos, segvalid, ndefer, defer[kTileMaxQueries / 32u]; };
-// Per-thread diagnostics of k_tile<*, true, *> (TileParams::counters[0, 7), and or_exit: [16, 20)); the other instances compile
-// them out.  or_exit: the exact launches' B2 union postings by how tile_eval_or left them (TileOrExit; 32 bits: a thread's share of
-// one launch).
-struct TileStats { unsigned long long pairs, skipped, flat, heavy, ess, completed, pushed; uint32_t or_exit[kOrExits]; };
+// Per-thread diagnostics of k_tile<*, true, *> (TileParams::counters[0, 7), refreshes and raises: [14, 16), or_exit: [16, 20)); the
+// other instances compile them out.  or_exit: the exact launches' B2 union postings by how tile_eval_or left them (TileOrExit; 32
+// bits: a thread's share of one launch).
+struct TileStats { unsigned long long pairs, skipped, flat, heavy, ess, completed, pushed; uint32_t or_exit[kOrExits], refreshes, raises; };
 // Stages of a tile as the cycle counters of k_tile<*, true, *> split a warp's time (TileParams::counters[8 + stage],
 // tq_stats.tile_cycles): the cursor prologue, A, B1, B2, B3, and the waits at the barriers between them.
 enum TileStage : int { kStPrologue, kStA, kStB1, kStB2, kStB3, kStBarrier, kTileStages };
@@ -788,7 +844,7 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
           ++st.completed;
           const uint32_t key = score_to_key(sum);
           if (key >= th_key) ++st.pushed;
-          if (!kSample) tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive);
+          if (!kSample) tile_push(P, TP, C, query, sum, lo + off, G.segment_ord, th_key, G.alive);
           else if (key >= th_key && key != 0u && (!G.alive || is_alive(G.alive, lo + off))) { s_query = query; s_key = key; }  // (a deleted doc bounds nothing)
         }
       }
@@ -810,7 +866,7 @@ __device__ __forceinline__ void tile_flat(const BatchParams& P, const TileParams
 // Stage B3 of a conjunction or TQ_OP_BOOL query: the lanes share the postings of the driving words [d0, d0 + dn) of cl, and each
 // evaluates its docs with eval(word, posting, doc offset, sum).
 template <bool kSample, typename Eval>
-__device__ __forceinline__ void tile_heavy_driven(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, const uint16_t* __restrict__ cl,
+__device__ __forceinline__ void tile_heavy_driven(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C, const uint16_t* __restrict__ cl,
                                                   uint32_t d0, uint32_t dn, uint32_t query, uint32_t th_key, uint32_t lo, uint32_t lane, TileStats& st, Eval eval) {
   uint32_t best = 0;
   for (uint32_t w = d0; w < d0 + dn; ++w) {
@@ -821,7 +877,7 @@ __device__ __forceinline__ void tile_heavy_driven(const BatchParams& P, const Ti
       float sum;
       if (!eval(w, p, off, sum)) continue;
       if (kSample) { if (!G.alive || is_alive(G.alive, lo + off)) best = max(best, score_to_key(sum)); }  // (a deleted doc bounds nothing)
-      else { ++st.completed; tile_push(P, query, sum, lo + off, G.segment_ord, th_key, G.alive); }
+      else { ++st.completed; tile_push(P, TP, C, query, sum, lo + off, G.segment_ord, th_key, G.alive); }
     }
     if (lane == 0) st.ess += e - a;
   }
@@ -831,7 +887,7 @@ __device__ __forceinline__ void tile_heavy_driven(const BatchParams& P, const Ti
 // Stage B3: heavy pair qi, evaluated by one warp.  A union accumulates its essential clauses into the warp's window `acc` of f32
 // score slots, clause by clause (the f32 summation order), then completes each touched doc with the non-essential suffix.
 template <bool kSample, bool kUnionOnly>
-__device__ __forceinline__ void tile_heavy(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V,
+__device__ __forceinline__ void tile_heavy(const BatchParams& P, const TileParams& TP, const TSeg& G, const TileView& V, TileCtl& C,
                                            const uint16_t* __restrict__ cl0, uint32_t qi, float* acc, uint32_t lo, uint32_t lane, TileStats& st) {
   const TileTQ tq = V.tq[qi];
   const uint16_t* __restrict__ cl = cl0 + tq.clause_base;
@@ -847,13 +903,13 @@ __device__ __forceinline__ void tile_heavy(const BatchParams& P, const TileParam
   if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpBool) {
     uint32_t d0 = 0, dn = 0;
     tile_bool_drive(V, cl, d0, dn, bound);
-    return tile_heavy_driven<kSample>(P, TP, G, V, cl, d0, dn, tq.query, th_key, lo, lane, st,
+    return tile_heavy_driven<kSample>(P, TP, G, V, C, cl, d0, dn, tq.query, th_key, lo, lane, st,
                                       [&](uint32_t w, uint32_t p, uint32_t off, float& sum) { return tile_eval_bool(V, cl, d0, w, p, off, io, sum); });
   }
   if (!kUnionOnly && (tq.op_flags & 3u) == kTileOpAnd) {
     uint32_t drv;
     tile_and_drive(V, cl, n, drv, bound);
-    return tile_heavy_driven<kSample>(P, TP, G, V, cl, drv, 1u, tq.query, th_key, lo, lane, st,
+    return tile_heavy_driven<kSample>(P, TP, G, V, C, cl, drv, 1u, tq.query, th_key, lo, lane, st,
                                       [&](uint32_t w, uint32_t p, uint32_t off, float& sum) { return tile_eval_and(V, cl, n, w, p, off, io, sum); });
   }
   const uint32_t n_e = tile_essential(V, cl, n, prune, theta_f, ne);
@@ -913,7 +969,7 @@ __device__ __forceinline__ void tile_heavy(const BatchParams& P, const TileParam
       if (dead) continue;
       ++st.completed;
       if (score_to_key(sum) >= th_key) ++st.pushed;
-      tile_push(P, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive);
+      tile_push(P, TP, C, tq.query, sum, lo + off, G.segment_ord, th_key, G.alive);
     }
   }
 }
@@ -947,6 +1003,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
   uint2* cursor = TP.cursors + (size_t)blockIdx.x * TP.max_slots;
   if (kCounters && tid < kTileStatWords) s_stat[tid] = 0ull;
   if (tid < kTileMaxQueries / 32u) C.defer[tid] = 0u;
+  if (tid == 0) C.nref = 0u;
   const bool cl_staged = G.n_clause_words <= TP.cl_cap;
   const uint16_t* __restrict__ cl0 = cl_staged ? V.cl : TP.clauses + G.clause_base;
   tile_prologue(TP, G, slots, V, cl_staged, cursor, U.t0, tid);
@@ -970,6 +1027,7 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
     mark(kStA);
     __syncthreads();
     mark(kStBarrier);
+    if (tid == 0) C.nref = 0u;  // (every warp has read the previous tile's refresh list: nothing is pushed before B2)
     // ---- stage A: this tile's pairs of every slot -> shared memory ----------------------------------------------------------
     if (warp < G.n_big) tile_stage_dense(TP, G, V, C.total, lo, warp, lane);
     tile_stage_sparse(TP, G, slots, V, cursor, C.total, lo, tid);
@@ -1014,23 +1072,33 @@ __global__ void __launch_bounds__(kTileThreads, kSample || kCounters ? 3 : 4) k_
       if (lane == 0) h = atomicAdd(&C.hpos, 1u);
       h = __shfl_sync(kFull, h, 0);
       if (h >= n_heavy) break;
-      tile_heavy<kSample, kUnionOnly>(P, TP, G, V, cl0, V.heavy[h], acc, lo, lane, st);
+      tile_heavy<kSample, kUnionOnly>(P, TP, G, V, C, cl0, V.heavy[h], acc, lo, lane, st);
       __syncwarp();
     }
     mark(kStB3);
     __syncthreads();
     mark(kStBarrier);
+    // ---- the running thresholds of the queries this tile's pushes put on the refresh list (tile_push): a warp per query -------
+    if constexpr (!kSample) {
+      const uint32_t n_ref = min(C.nref, kTileRefreshCap);
+      for (uint32_t i = warp; i < n_ref; i += kTileWarps) {
+        const bool raised = tile_theta_refresh(P, TP, C.ref[i], lane);
+        if (kCounters && lane == 0) { ++st.refreshes; st.raises += raised ? 1u : 0u; }
+      }
+      mark(kStB3);
+    }
   }
   if constexpr (kCounters) {
-    // warp-aggregated diagnostics (s_stat / TileParams::counters: the 7 of TileStats, 8 + the stages, 16 + the union exits)
-    unsigned long long v[7 + kOrExits] = {st.pairs, st.skipped, st.flat, st.heavy, st.ess, st.completed, st.pushed,
-                                          st.or_exit[0], st.or_exit[1], st.or_exit[2], st.or_exit[3]};
+    // warp-aggregated diagnostics (s_stat / TileParams::counters: the 7 of TileStats, 8 + the stages, 14 the refreshes, 15 the raises,
+    // 16 + the union exits)
+    unsigned long long v[9 + kOrExits] = {st.pairs, st.skipped, st.flat, st.heavy, st.ess, st.completed, st.pushed,
+                                          st.refreshes, st.raises, st.or_exit[0], st.or_exit[1], st.or_exit[2], st.or_exit[3]};
 #pragma unroll
-    for (int i = 0; i < 7 + kOrExits; ++i) {
+    for (int i = 0; i < 9 + kOrExits; ++i) {
       unsigned long long x = v[i];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(kFull, x, o);
-      if (lane == 0 && x) atomicAdd(&s_stat[i < 7 ? i : 16 + (i - 7)], x);
+      if (lane == 0 && x) atomicAdd(&s_stat[i < 7 ? i : i < 9 ? 14 + (i - 7) : 16 + (i - 9)], x);
     }
     if (lane == 0)
       for (int k = 0; k < kTileStages; ++k) atomicAdd(&s_stat[8 + k], cyc[k]);
@@ -1233,15 +1301,17 @@ __device__ __forceinline__ uint32_t block_kth_key(const uint32_t* __restrict__ k
   return *s_prefix;
 }
 
-// After the sample launch: the k-th best sampled score of a query bounds its final k-th score from below.
+// After the sample launch: the k-th best sampled score of a query bounds its final k-th score from below.  The threshold it leaves
+// is the base of the query's key histogram in the exact launches (th_hist: fixed for the run, before anything is counted).
 __global__ void __launch_bounds__(kThreads) k_theta_samples(const BatchParams P, const uint32_t* __restrict__ samples,
-                                                            const uint32_t* __restrict__ sample_count, uint32_t sample_cap) {
+                                                            const uint32_t* __restrict__ sample_count, uint32_t sample_cap,
+                                                            uint32_t* __restrict__ th_hist) {
   __shared__ uint32_t s_hist[256];
   __shared__ uint32_t s_prefix, s_need;
   const uint32_t q = blockIdx.x;
   const uint32_t n = min(sample_count[q], sample_cap);
   const uint32_t kth = block_kth_key(samples + (size_t)q * sample_cap, n, 1u, P.queries[q].k, s_hist, &s_prefix, &s_need);
-  if (threadIdx.x == 0 && kth) atomicMax(&P.qstate[q].theta, kth);
+  if (threadIdx.x == 0) th_hist[(size_t)q * kThHistWords + kThHistBaseWord] = max(atomicMax(&P.qstate[q].theta, kth), kth) >> 16;
 }
 
 // Cross-shard exchange, export side: the k best score keys a query holds so far (samples after the sample launch, else
