@@ -230,6 +230,17 @@ typedef struct {
   uint64_t hist_tiles_one_bucket;
 } tq_histogram_stats;
 int tq_get_histogram_stats(tq_ctx*, tq_histogram_stats* out);
+/* Cumulative since ctx creation: tq_terms_batch.  Device time of k_terms + k_terms_select over all waves, their CTAs (one per unit
+ * of up to eight 8192-doc tiles, plus one per (query, segment)), the 8192-doc tiles the units came to and of those the ones counted
+ * as one key (every value of the tile equal: the tile's matches added without reading a value).  A struct of its own, so that
+ * tq_stats and tq_histogram_stats keep their layouts. */
+typedef struct {
+  float terms_ms;
+  uint64_t units_terms;
+  uint64_t terms_tiles_seen;
+  uint64_t terms_tiles_one_key;
+} tq_terms_stats;
+int tq_get_terms_stats(tq_ctx*, tq_terms_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -311,6 +322,24 @@ typedef struct {
   double hard_min, hard_max; /* collect-time bounds; -DBL_MAX / DBL_MAX when the request has none */
 } tq_histogram_spec;
 
+/* Terms aggregations (AggregationCollector with one `terms` and no sub-aggregation, src/aggregation/bucket/term_agg/mod.rs) read the
+ * same registered columns, single-valued only: the key of a doc is its u64 image (for a str column the term ordinal, registered as
+ * ords().first(doc)), so key order is the image order, which is the reference's ordinal and value order. */
+#define TQ_TERMS_BY_COUNT 0u      /* order target `_count` */
+#define TQ_TERMS_BY_KEY 1u        /* order target `_key` */
+#define TQ_TERMS_MISSING_NONE 0u  /* docs without a value are not counted */
+#define TQ_TERMS_MISSING_IMAGE 1u /* ... count under missing_image (a numeric `missing`, as the column's image of it) */
+#define TQ_TERMS_MISSING_AFTER_MAX 2u /* ... count under the segment's largest image + 1 (0 + 1 without a value): a str `missing` */
+typedef struct {
+  uint32_t column_id;     /* a column of tq_sort_column_register */
+  uint32_t target;        /* TQ_TERMS_BY_COUNT / TQ_TERMS_BY_KEY */
+  uint32_t order;         /* TQ_ORDER_DESC / TQ_ORDER_ASC */
+  uint32_t segment_size;  /* entries kept per segment, >= 1: max(size, segment_size), as TermsAggregationInternal::from_req */
+  uint32_t missing_mode;  /* TQ_TERMS_MISSING_* */
+  uint32_t pad;
+  uint64_t missing_image; /* TQ_TERMS_MISSING_IMAGE: the key of a doc without a value */
+} tq_terms_spec;
+
 /* ---- search -------------------------------------------------------------------------- */
 /* The whole hot path for a batch of queries, host buffers in / host buffers out:
  * block decode -> AND/OR/term -> BM25 -> per-segment top-k -> merge_fruits.
@@ -357,6 +386,30 @@ int tq_sort_batch(tq_ctx*, const tq_query* queries, const tq_sort_spec* sorts, s
  * does. */
 int tq_histogram_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec* specs, size_t nq, uint32_t out_stride,
                        int64_t* out_pos, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_hits);
+
+/* The segment part of a terms aggregation for term / AND / OR / mixed boolean (TQ_OP_BOOL) queries, synchronous like
+ * tq_count_batch, over the docs tq_count_batch counts.  Per (query, segment): each doc's key is its image (a doc without a value
+ * counts under the missing key of specs[q].missing_mode, or not at all); the entries are the keys with a non-zero count, u32 counts
+ * as the reference's Bucket::count.  When there are more than segment_size, segment_size are kept by the order (count or key, desc
+ * or asc), ties at the cut by key ascending (the reference's select_nth_unstable leaves them unspecified), and the segment reports
+ * the count of the entry at position segment_size in that order (term_doc_count_before_cutoff) and the sum of the counts cut
+ * (sum_other_doc_count) -- into_intermediate_bucket_result / cut_off_buckets, term_agg/mod.rs:1000-1111, 1328-1353.  Row q
+ * (out_stride entries apart) holds query q's kept entries over all its segments, ascending by (segment_ord, key): out_segment_ord[i],
+ * out_key[i] (the image) and out_doc_count[i]; out_sum_other[q] and out_error_bound[q] are the sums of the two scalars over its
+ * segments.  A segment this context evaluates only part of (tq_segment_set_doc_range narrowed it) is not cut: its entries are all in
+ * the row and it adds 0 to both scalars, so that the caller can sum the ranges of the segment and cut once, as the reference cuts
+ * each segment once.  Mapping keys to terms or values, the merge and the final result (min_doc_count, order, size) are the caller's.  When
+ * some out_n[q] > out_stride, every out_n is written and the call returns TQ_ERR_INVALID_ARGUMENT: retry with a larger stride.
+ * out_hits may be NULL; else out_hits[q] = tq_count_batch's answer for query q.  A (query, segment)'s counters span the images of
+ * the 8192-doc tiles the query visits there: more than 2^20 keys returns TQ_ERR_UNSUPPORTED naming the query (the caller takes the
+ * CPU path).  Queries whose counters exceed the ctx's budget (TQ_TERMS_COUNTER_BUDGET at ctx creation, in counters) run in
+ * consecutive waves on one scratch region.  TQ_OP_PHRASE returns TQ_ERR_UNSUPPORTED; a segment without the column
+ * TQ_ERR_NOT_FOUND; a target, order or missing mode outside its defines, segment_size 0, or TQ_TERMS_MISSING_AFTER_MAX on a
+ * segment whose largest image is 2^64 - 1 TQ_ERR_INVALID_ARGUMENT.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The run
+ * holds its columns as tq_sort_batch does. */
+int tq_terms_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec* specs, size_t nq, uint32_t out_stride,
+                   uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_sum_other,
+                   uint64_t* out_error_bound, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

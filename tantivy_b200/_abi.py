@@ -20,6 +20,8 @@ TQ_QUERY_COUNT_HITS = 2
 TQ_QUERY_FILTER = 4
 TQ_ORDER_DESC, TQ_ORDER_ASC = 0, 1
 TQ_FAST_U64, TQ_FAST_I64, TQ_FAST_F64, TQ_FAST_BOOL, TQ_FAST_DATE = 0, 1, 2, 3, 4
+TQ_TERMS_BY_COUNT, TQ_TERMS_BY_KEY = 0, 1
+TQ_TERMS_MISSING_NONE, TQ_TERMS_MISSING_IMAGE, TQ_TERMS_MISSING_AFTER_MAX = 0, 1, 2
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -145,6 +147,11 @@ class HistogramStats(C.Structure):
     _fields_ = [("hist_ms", C.c_float), ("units_hist", C.c_uint64), ("hist_tiles_seen", C.c_uint64), ("hist_tiles_one_bucket", C.c_uint64)]
 
 
+class TermsStats(C.Structure):
+    """tq_terms_stats — the cumulative counters of tq_terms_batch (tq_get_terms_stats)."""
+    _fields_ = [("terms_ms", C.c_float), ("units_terms", C.c_uint64), ("terms_tiles_seen", C.c_uint64), ("terms_tiles_one_key", C.c_uint64)]
+
+
 class SortSpec(C.Structure):
     """tq_sort_spec — the column and Order of TopDocs::order_by_fast_field for one query."""
     _fields_ = [("column_id", C.c_uint32), ("order", C.c_uint32)]
@@ -163,6 +170,17 @@ class HistogramSpec(C.Structure):
 HISTOGRAM_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("kind", "<u4"), ("interval", "<f8"), ("offset", "<f8"), ("hard_min", "<f8"),
                                  ("hard_max", "<f8")])
 assert HISTOGRAM_SPEC_DTYPE.itemsize == C.sizeof(HistogramSpec) == 40
+
+
+class TermsSpec(C.Structure):
+    """tq_terms_spec — the column, order target and direction, segment_size and missing key of one query's terms aggregation."""
+    _fields_ = [("column_id", C.c_uint32), ("target", C.c_uint32), ("order", C.c_uint32), ("segment_size", C.c_uint32),
+                ("missing_mode", C.c_uint32), ("pad", C.c_uint32), ("missing_image", C.c_uint64)]
+
+
+TERMS_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("target", "<u4"), ("order", "<u4"), ("segment_size", "<u4"), ("missing_mode", "<u4"),
+                             ("pad", "<u4"), ("missing_image", "<u8")])
+assert TERMS_SPEC_DTYPE.itemsize == C.sizeof(TermsSpec) == 32
 
 
 def ptr(arr, typ):

@@ -280,6 +280,8 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->strip_windows_per_unit = std::max<uint32_t>(1u, env_u32("TQ_STRIP_WINDOWS_PER_UNIT", kStripWarps * 64u));
   // test hook: smallest k_count_tiles unit, in tiles (1: every tile edge is a unit edge, where the sparse cursors are searched)
   c->count_hits_tiles_per_unit = std::max<uint32_t>(1u, env_u32("TQ_COUNT_HITS_TILES_PER_UNIT", 8));
+  // terms counters per wave of tq_terms_batch (256 MB); test hook: a small budget runs a batch in many waves
+  c->terms_counter_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_COUNTER_BUDGET", 1u << 26));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -389,6 +391,16 @@ int tq_get_histogram_stats(tq_ctx* c, tq_histogram_stats* out) {
   out->units_hist = c->hist_units;
   out->hist_tiles_seen = c->hist_tiles_seen;
   out->hist_tiles_one_bucket = c->hist_tiles_one_bucket;
+  return TQ_OK;
+}
+
+int tq_get_terms_stats(tq_ctx* c, tq_terms_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->terms_ms = (float)c->terms_ms;
+  out->units_terms = c->terms_units;
+  out->terms_tiles_seen = c->terms_tiles_seen;
+  out->terms_tiles_one_key = c->terms_tiles_one_key;
   return TQ_OK;
 }
 
@@ -1754,6 +1766,21 @@ int tq_sort_batch(tq_ctx* c, const tq_query* queries, const tq_sort_spec* sorts,
 }
 
 // ---- histogram of a fast field ---------------------------------------------------------------------------------
+// The smallest and largest image of the unit's tiles that hold a value; false: none does.
+static bool unit_images(const SortColumn& col, const Unit& u, unsigned long long& lo, unsigned long long& hi) {
+  bool any = false;
+  lo = ~0ull;
+  hi = 0;
+  for (uint32_t t = u.begin; t < u.end; ++t) {
+    const SortTile& st = col.tiles[t];
+    if (!(st.flags & kSortTileValues)) continue;
+    lo = std::min<unsigned long long>(lo, ~st.best[1]);
+    hi = std::max<unsigned long long>(hi, st.best[0]);
+    any = true;
+  }
+  return any;
+}
+
 int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* specs, size_t nq, uint32_t out_stride,
                        int64_t* out_pos, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_hits) {
   if (!c || (nq && (!queries || !specs || !out_n || (out_stride && (!out_pos || !out_doc_count)))))
@@ -1811,22 +1838,19 @@ int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_sp
         const size_t k = u.qseg - s0;
         const HistSeg& z = hsegs[u.qseg];
         double umin = INFINITY, umax = -INFINITY;
-        for (uint32_t t = u.begin; t < u.end; ++t) {
-          double vmin, vmax;
-          if (sp.kind == TQ_FAST_F64) {  // an infinity widens the range only when it is in bounds; a NaN never is
+        if (sp.kind == TQ_FAST_F64) {
+          for (uint32_t t = u.begin; t < u.end; ++t) {  // an infinity widens the range only when it is in bounds; a NaN never is
             const FiniteTile& f = cols[k]->finite[t];
-            vmin = INFINITY; vmax = -INFINITY;
+            double vmin = INFINITY, vmax = -INFINITY;
             if (f.flags & kFiniteAny) { vmin = hist_value(f.lo, sp.kind); vmax = hist_value(f.hi, sp.kind); }
             if ((f.flags & kFiniteNegInf) && z.lo == -INFINITY) vmin = -INFINITY;
             if ((f.flags & kFinitePosInf) && z.hi == INFINITY) vmax = INFINITY;
-          } else {
-            const SortTile& st = cols[k]->tiles[t];
-            if (!(st.flags & kSortTileValues)) continue;
-            vmin = hist_value(~st.best[1], sp.kind);
-            vmax = hist_value(st.best[0], sp.kind);
+            umin = std::min(umin, vmin);
+            umax = std::max(umax, vmax);
           }
-          umin = std::min(umin, vmin);
-          umax = std::max(umax, vmax);
+        } else {
+          unsigned long long ilo, ihi;  // (hist_value is monotone in the image for every other kind)
+          if (unit_images(*cols[k], u, ilo, ihi)) { umin = hist_value(ilo, sp.kind); umax = hist_value(ihi, sp.kind); }
         }
         const double lo = std::max(umin, z.lo), hi = std::min(umax, z.hi);
         if (!(lo <= hi)) { uwin.emplace_back(1, 0); continue; }  // no value of the unit can pass the bounds
@@ -1922,6 +1946,242 @@ int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_sp
     c->hist_tiles_one_bucket += tiles[1];
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a histogram has more non-empty buckets than out_stride: out_n holds how many");
+  return TQ_OK;
+}
+
+// ---- terms of a fast field ------------------------------------------------------------------------------------
+int tq_terms_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* specs, size_t nq, uint32_t out_stride,
+                   uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_sum_other,
+                   uint64_t* out_error_bound, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !specs || !out_n || !out_sum_other || !out_error_bound ||
+                    (out_stride && (!out_segment_ord || !out_key || !out_doc_count)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const tq_terms_spec& sp = specs[qi];
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "terms of phrase queries are not on the device path");
+    if (sp.target > TQ_TERMS_BY_KEY || sp.order > TQ_ORDER_ASC || sp.missing_mode > TQ_TERMS_MISSING_AFTER_MAX || !sp.segment_size)
+      return fail(TQ_ERR_INVALID_ARGUMENT, "terms spec: target, order, missing mode or segment_size");
+  }
+  for (size_t qi = 0; qi < nq; ++qi) {
+    out_n[qi] = 0;
+    out_sum_other[qi] = out_error_bound[qi] = 0;
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<TermsSeg> tsegs;    // parallel to cp.segs
+  std::vector<HistUnit> windows;  // parallel to cp.units
+  std::vector<size_t> q_seg(nq + 1), q_unit(nq + 1);
+  std::vector<uint64_t> q_counters(nq, 0), q_region(nq, 0);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<unsigned long long, unsigned long long>> uwin;  // per unit of the query: its smallest and largest image
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_terms_spec& sp = specs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_seg[qi] = s0;
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      cols.clear();
+      uint32_t flags = (out_hits ? kTermsHits : 0u) | (sp.missing_mode != TQ_TERMS_MISSING_NONE ? kTermsMissing : 0u) |
+                       (sp.target == TQ_TERMS_BY_KEY ? kTermsByKey : 0u) | (sp.order == TQ_ORDER_ASC ? kTermsAsc : 0u);
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
+        if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a terms query names a segment without the column (tq_sort_column_register)");
+        const SortColumn& col = it->second;
+        if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+        unsigned long long missing = sp.missing_image;
+        if (sp.missing_mode == TQ_TERMS_MISSING_AFTER_MAX) {  // get_missing_val_as_u64_lenient: the column's max_value + 1 (0 without values)
+          const unsigned long long top = col.min_image <= col.max_image ? col.max_image : 0ull;
+          if (top == ~0ull) return fail(TQ_ERR_INVALID_ARGUMENT, "query " + std::to_string(qi) + ": a str column whose largest image is 2^64 - 1 has no missing key");
+          missing = top + 1;
+        }
+        // a segment this context evaluates only part of (tq_segment_set_doc_range) is not cut here: the reference cuts a segment
+        // once, so the caller cuts after summing its ranges; segment_size 0 marks it (every entry is kept, both scalars stay 0)
+        bool part = false;
+        for (auto s = c->segments.lower_bound({cp.segment_ords[si], 0u}); s != c->segments.end() && s->first.first == cp.segment_ords[si]; ++s)
+          part = part || s->second.doc_lo != 0 || s->second.doc_hi != s->second.max_doc;
+        tsegs.push_back(TermsSeg{col.d_values, col.d_present, col.d_tiles, 0ull, missing, 0ull, 0ull, 0u, part ? 0u : sp.segment_size, flags, 0u});
+        cols.push_back(&col);
+      }
+      // per unit the images of its tiles; per (query, segment) their union
+      uwin.clear();
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const Unit& u = cp.units[ui];
+        unsigned long long lo, hi;
+        if (!unit_images(*cols[u.qseg - s0], u, lo, hi)) { uwin.emplace_back(1ull, 0ull); continue; }
+        uwin.emplace_back(lo, hi);
+        TermsSeg& z = tsegs[u.qseg];
+        if (!z.n_keys) { z.base = lo; z.n_keys = 1; z.region = hi; }  // (region holds the top until the span is known)
+        else { z.base = std::min(z.base, lo); z.region = std::max<unsigned long long>(z.region, hi); }
+      }
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        TermsSeg& z = tsegs[si];
+        if (z.n_keys) {
+          const unsigned long long span_m1 = z.region - z.base;  // (images up to 2^64 - 1: the span is never formed as top + 1)
+          if (span_m1 >= kTermsMaxKeys)
+            return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its terms span more than 2^20 keys in a segment (take the CPU path)");
+          z.n_keys = (uint32_t)span_m1 + 1u;
+        }
+        if (!z.segment_size) z.segment_size = z.n_keys + 1u;  // more than its entries: no cut
+        z.counters = q_counters[qi];
+        z.region = q_region[qi];
+        q_counters[qi] += z.n_keys;
+        q_region[qi] += std::min<uint64_t>(z.segment_size, (uint64_t)z.n_keys + ((z.flags & kTermsMissing) ? 1u : 0u));
+      }
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const auto& w = uwin[ui - u0];
+        windows.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - tsegs[cp.units[ui].qseg].base), (uint32_t)(w.second - w.first + 1)}
+                                              : HistUnit{0u, 0u});
+      }
+    }
+    q_seg[nq] = cp.segs.size();
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) b->held_columns.push_back(specs[qi].column_id);
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // waves of consecutive queries whose counters fit the budget (a query above it runs alone); counters and regions relative to it
+  struct Wave { size_t q0, q1; uint64_t counters, region; };
+  std::vector<Wave> waves;
+  uint64_t max_counters = 0, max_region = 0;
+  size_t max_segs = 0;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (waves.empty() || (waves.back().counters && waves.back().counters + q_counters[qi] > c->terms_counter_budget))
+      waves.push_back(Wave{qi, qi, 0, 0});
+    Wave& w = waves.back();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) { tsegs[si].counters += w.counters; tsegs[si].region += w.region; }
+    w.q1 = qi + 1;
+    w.counters += q_counters[qi];
+    w.region += q_region[qi];
+    max_counters = std::max(max_counters, w.counters);
+    max_region = std::max(max_region, w.region);
+    max_segs = std::max(max_segs, q_seg[w.q1] - q_seg[w.q0]);
+  }
+  // descriptors: one H2D copy; scratch: hits | tile counters, then one wave's per-(query, segment) results | kept entries |
+  // missing counters | counters
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(tsegs), o_h = st.add(windows);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(16), head_bytes = off;
+  const size_t r_n = take(max_segs * 4), r_other = take(max_segs * 8), r_err = take(max_segs * 8), r_key = take(max_region * 8),
+               r_count = take(max_region * 4), wave_bytes = off - head_bytes;
+  const size_t r_missing = take(max_segs * 4), r_counters = take(max_counters * 4);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  TermsParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.tsegs = st.on_device<const TermsSeg>(o_z);
+  P.windows = st.on_device<const HistUnit>(o_h);
+  P.counts = reinterpret_cast<uint32_t*>(d + r_counters);
+  P.missing = reinterpret_cast<uint32_t*>(d + r_missing);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.res_key = reinterpret_cast<unsigned long long*>(d + r_key);
+  P.res_count = reinterpret_cast<uint32_t*>(d + r_count);
+  P.res_n = reinterpret_cast<uint32_t*>(d + r_n);
+  P.res_other = reinterpret_cast<unsigned long long*>(d + r_other);
+  P.res_error = reinterpret_cast<unsigned long long*>(d + r_err);
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  // per (query, segment): its kept entries (ascending key) and scalars, gathered wave by wave
+  std::vector<std::vector<std::pair<unsigned long long, uint32_t>>> kept(cp.segs.size());
+  std::vector<uint64_t> seg_other(cp.segs.size()), seg_err(cp.segs.size());
+  float ms_total = 0;
+  const uint8_t* h = b->res_pin.p;
+  for (const Wave& w : waves) {
+    const size_t sa = q_seg[w.q0], sb = q_seg[w.q1], ua = q_unit[w.q0], ub = q_unit[w.q1];
+    if (sa == sb) continue;
+    P.unit_base = (uint32_t)ua;
+    P.seg_base = (uint32_t)sa;
+    TQ_CUDA(cudaMemsetAsync(d + r_missing, 0, (sb - sa) * 4, b->stream));
+    TQ_CUDA(cudaMemsetAsync(d + r_counters, 0, w.counters * 4, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    if (ub > ua) {
+      (cp.mixed ? k_terms<true> : k_terms<false>)<<<(unsigned)(ub - ua), kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    k_terms_select<<<(unsigned)(sb - sa), kThreads, 0, b->stream>>>(P);
+    TQ_CUDA(cudaGetLastError());
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + head_bytes, r_key - head_bytes + w.region * 8, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_count - head_bytes), d + r_count, w.region * 4, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    for (size_t si = sa; si < sb; ++si) {
+      const size_t rel = si - sa;
+      uint32_t n;
+      memcpy(&n, h + (r_n - head_bytes) + rel * 4, 4);
+      memcpy(&seg_other[si], h + (r_other - head_bytes) + rel * 8, 8);
+      memcpy(&seg_err[si], h + (r_err - head_bytes) + rel * 8, 8);
+      kept[si].resize(n);
+      for (uint32_t j = 0; j < n; ++j) {
+        const size_t e = tsegs[si].region + j;
+        unsigned long long key;
+        uint32_t count;
+        memcpy(&key, h + (r_key - head_bytes) + e * 8, 8);
+        memcpy(&count, h + (r_count - head_bytes) + e * 4, 4);
+        kept[si][j] = {key, count};
+      }
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_tiles, 16);
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  // rows: each query's segments by segment_ord, each in ascending key
+  bool fits = true;
+  std::vector<size_t> by_ord;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    by_ord.clear();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) by_ord.push_back(si);
+    std::sort(by_ord.begin(), by_ord.end(), [&](size_t x, size_t y) { return cp.segment_ords[x] < cp.segment_ords[y]; });
+    uint32_t n = 0;
+    for (size_t si : by_ord) {
+      out_sum_other[qi] += seg_other[si];
+      out_error_bound[qi] += seg_err[si];
+      for (const auto& e : kept[si]) {
+        if (n < out_stride) {
+          const size_t at = qi * (size_t)out_stride + n;
+          out_segment_ord[at] = cp.segment_ords[si];
+          out_key[at] = e.first;
+          out_doc_count[at] = e.second;
+        }
+        ++n;
+      }
+    }
+    out_n[qi] = n;
+    fits = fits && n <= out_stride;
+  }
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->terms_ms += ms_total;
+    c->terms_units += cp.units.size() + cp.segs.size();
+    c->terms_tiles_seen += tiles[0];
+    c->terms_tiles_one_key += tiles[1];
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride: out_n holds how many");
   return TQ_OK;
 }
 

@@ -241,12 +241,16 @@ struct tq_ctx {
   // ... and of the histogram runs (hist_ms, units_hist, hist_tiles_seen, hist_tiles_one_bucket)
   double hist_ms = 0;
   uint64_t hist_units = 0, hist_tiles_seen = 0, hist_tiles_one_bucket = 0;
+  // ... and of the terms runs (terms_ms, units_terms, terms_tiles_seen, terms_tiles_one_key)
+  double terms_ms = 0;
+  uint64_t terms_units = 0, terms_tiles_seen = 0, terms_tiles_one_key = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;
   std::vector<tq_batch*> pool;
   tq_stats stats{};
   uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit, strip_windows_per_unit, count_hits_tiles_per_unit;
+  uint32_t terms_counter_budget;  // u32 counters one tq_terms_batch wave may hold
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 32, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;

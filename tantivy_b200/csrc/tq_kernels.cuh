@@ -1427,40 +1427,38 @@ __global__ void __launch_bounds__(kThreads) k_sort_final(const SortParams P) {
 // atomicAdd per non-zero bucket at exit), else global.  A timestamp unit of eight tiles spans a few minutes of the column, so even a
 // query of many thousand buckets counts on chip.
 
-// (3 CTAs per SM: the division's slow path is a call, and at the 64 registers of 4 CTAs the kernel spills around it)
-template <bool kMixed>
-__global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
+// The body of k_hist and k_terms: one CTA per Count unit counts its matching docs by key into its window of counters.  K is the
+// key policy, static functions over the (query, segment)'s descriptor Z, the query's Q and the unit's window W (from the origin
+// `base`): the one key of a tile with values, if it has one (every value of the tile, matching or not, has it: the tile's matches are added without a gather;
+// ~0u: none), whether a value is counted and the index of its counter, and whether matching docs without a value are counted as
+// well (K::kMissing: one add per warp at exit).
+template <class K, bool kMixed, class Params>
+__device__ __forceinline__ void count_unit_keys(const Params& P, const uint32_t unit) {
   static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
   __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
   __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
   __shared__ uint32_t s_bins[kHistSmemBins];
   __shared__ uint32_t s_part[kWarps];
-  __shared__ uint32_t s_one;  // the tile's one bucket (index into the unit's window), or ~0u
-  const Unit U = P.c.units[blockIdx.x];
+  __shared__ uint32_t s_one;  // the tile's one key (index into the unit's window), or ~0u
+  const Unit U = P.c.units[unit];
   const CountSeg S = P.c.segs[U.qseg];
-  const HistSeg Z = P.hsegs[U.qseg];
-  const HistQuery Q = P.queries[S.query];
+  const typename K::Seg Z = K::seg(P, U);
+  const typename K::Query Q = K::query(P, S, Z);
   const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const HistUnit W = P.hunits[blockIdx.x];
-  const long long base = Q.base + (long long)W.first;  // pos of the unit's first counter
+  const HistUnit W = K::window(P, unit);
+  const typename K::Base base = K::base(Z, Q, W);  // the key of the unit's first counter
   const bool shared = W.n_bins <= kHistSmemBins;
-  unsigned long long* const counts = P.counts + Q.counters + W.first;
+  typename K::Counter* const counts = K::counts(P, Z, Q, W);
   if (shared)
     for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x) s_bins[i] = 0;
-  uint32_t total = 0, one = 0;
+  uint32_t total = 0, one = 0, missing = 0;
   for (uint32_t tile = U.begin; tile < U.end; ++tile) {
     const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
     if (threadIdx.x == 0) {
       const SortTile T = Z.tiles[tile];
       uint32_t idx = 0xFFFFFFFFu;
-      if (W.n_bins && (T.flags & kSortTileValues)) {
-        const double vmin = hist_value(~T.best[1], Q.kind), vmax = hist_value(T.best[0], Q.kind);
-        if (vmin >= Z.lo && vmax <= Z.hi) {
-          const long long p = hist_pos(vmin, Q.offset, Q.interval);
-          if (p == hist_pos(vmax, Q.offset, Q.interval) && p >= base && p - base < (long long)W.n_bins) idx = (uint32_t)(p - base);
-        }
-      }
+      if (W.n_bins && (T.flags & kSortTileValues)) K::one(T, Z, Q, W, base, idx);
       s_one = idx;
       one += idx != 0xFFFFFFFFu ? 1u : 0u;
     }
@@ -1469,22 +1467,23 @@ __global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
     const uint32_t bits = s_acc[threadIdx.x];
     total += (uint32_t)__popc(bits);
     uint32_t with = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
-    if (s_one < W.n_bins) {  // one bucket: every value of the tile, matching or not, lies in bounds and in one bucket
+    if constexpr (K::kMissing) missing += (uint32_t)__popc(bits ^ with);
+    if (s_one < W.n_bins) {
       const uint32_t c = __reduce_add_sync(kFull, (uint32_t)__popc(with));
       const uint32_t idx = s_one;
       if (lane == 0 && c) {
         if (shared) atomicAdd(&s_bins[idx], c);
-        else atomicAdd(&counts[idx], (unsigned long long)c);
+        else atomicAdd(&counts[idx], (typename K::Counter)c);
       }
     } else if (W.n_bins) {
       for (; with; with &= with - 1u) {
         const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(with) - 1);
-        const double val = hist_value(__ldg(Z.values + doc), Q.kind);
-        if (!(val >= Z.lo && val <= Z.hi)) continue;  // HistogramBounds::contains (NaN never passes)
-        const unsigned long long idx = (unsigned long long)(hist_pos(val, Q.offset, Q.interval) - base);
-        if (idx < W.n_bins) {  // (always: the window covers every value in bounds of the unit's tiles)
+        const typename K::Value val = K::value(__ldg(Z.values + doc), Q);
+        if (!K::counted(val, Z)) continue;
+        const unsigned long long idx = K::index(val, Q, base);
+        if (idx < W.n_bins) {  // (always: the window covers every counted value of the unit's tiles)
           if (shared) atomicAdd(&s_bins[idx], 1u);
-          else atomicAdd(&counts[idx], 1ull);
+          else atomicAdd(&counts[idx], (typename K::Counter)1);
         }
       }
     }
@@ -1492,14 +1491,14 @@ __global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
   }
   if (shared)
     for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x)
-      if (s_bins[i]) atomicAdd(&counts[i], (unsigned long long)s_bins[i]);
-  if (Q.flags & kHistHits) {
+      if (s_bins[i]) atomicAdd(&counts[i], (typename K::Counter)s_bins[i]);
+  if (K::hits(Q)) {
     total = __reduce_add_sync(kFull, total);
     if (lane == 0) s_part[warp] = total;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (Q.flags & kHistHits) {
+    if (K::hits(Q)) {
       unsigned long long sum = 0;
       for (int w = 0; w < kWarps; ++w) sum += s_part[w];
       if (sum) atomicAdd(&P.c.counts[S.query], sum);
@@ -1507,6 +1506,49 @@ __global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
     const uint32_t seen = U.end - U.begin;
     if (seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (one) atomicAdd(&P.tiles[1], (unsigned long long)one); }
   }
+  if constexpr (K::kMissing) {
+    if (Z.flags & kTermsMissing) {
+      missing = __reduce_add_sync(kFull, missing);
+      if (lane == 0 && missing) atomicAdd(&P.missing[U.qseg - P.seg_base], missing);
+    }
+  }
+}
+
+// The histogram's keys: bucket pos(val) of the values in the (query, segment)'s bounds.
+struct HistKeys {
+  typedef HistSeg Seg;
+  typedef HistQuery Query;
+  typedef long long Base;
+  typedef double Value;
+  typedef unsigned long long Counter;
+  static constexpr bool kMissing = false;
+  static __device__ __forceinline__ HistSeg seg(const HistParams& P, const Unit& U) { return P.hsegs[U.qseg]; }
+  static __device__ __forceinline__ HistQuery query(const HistParams& P, const CountSeg& S, const HistSeg&) { return P.queries[S.query]; }
+  static __device__ __forceinline__ HistUnit window(const HistParams& P, uint32_t unit) { return P.hunits[unit]; }
+  static __device__ __forceinline__ long long base(const HistSeg&, const HistQuery& Q, const HistUnit& W) { return Q.base + (long long)W.first; }
+  static __device__ __forceinline__ Counter* counts(const HistParams& P, const HistSeg&, const HistQuery& Q, const HistUnit& W) { return P.counts + Q.counters + W.first; }
+  // one bucket: the tile's smallest and largest values both in bounds and in one bucket (pos is monotone in the image)
+  static __device__ __forceinline__ void one(const SortTile T, const HistSeg& Z, const HistQuery& Q, const HistUnit& W, const long long base, uint32_t& idx) {
+    const double vmin = hist_value(~T.best[1], Q.kind), vmax = hist_value(T.best[0], Q.kind);
+    if (vmin >= Z.lo && vmax <= Z.hi) {
+      const long long p = hist_pos(vmin, Q.offset, Q.interval);
+      if (p == hist_pos(vmax, Q.offset, Q.interval) && p >= base && p - base < (long long)W.n_bins) idx = (uint32_t)(p - base);
+    }
+  }
+  static __device__ __forceinline__ double value(unsigned long long v, const HistQuery& Q) { return hist_value(v, Q.kind); }
+  static __device__ __forceinline__ bool counted(double val, const HistSeg& Z) {
+    return val >= Z.lo && val <= Z.hi;  // HistogramBounds::contains (NaN never passes)
+  }
+  static __device__ __forceinline__ unsigned long long index(double val, const HistQuery& Q, long long base) {
+    return (unsigned long long)(hist_pos(val, Q.offset, Q.interval) - base);
+  }
+  static __device__ __forceinline__ bool hits(const HistQuery& Q) { return Q.flags & kHistHits; }
+};
+
+// (3 CTAs per SM: the division's slow path is a call, and at the 64 registers of 4 CTAs the kernel spills around it)
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 3) k_hist(const HistParams P) {
+  count_unit_keys<HistKeys, kMixed>(P, blockIdx.x);
 }
 
 // One CTA per query: the non-zero counters of its range, in ascending pos, into its row (a CTA-wide prefix sum per 256 counters).
@@ -1534,6 +1576,184 @@ __global__ void __launch_bounds__(kThreads) k_hist_final(const HistParams P) {
     __syncthreads();
   }
   if (threadIdx.x == 0) P.res_n[q] = base;
+}
+
+// ---- terms of a fast field (AggregationCollector: terms, bucket/term_agg/mod.rs) ---------------------------------------------
+// The docs Count counts, each counted under its image, through count_unit_keys: a tile whose smallest and largest image are equal
+// adds its matches to that key without a gather, a matching doc without a value goes to the (query, segment)'s missing counter.
+struct TermsKeys {
+  typedef TermsSeg Seg;
+  typedef uint32_t Query;  // the (query, segment)'s flags
+  typedef unsigned long long Base;
+  typedef unsigned long long Value;
+  typedef uint32_t Counter;  // Bucket::count is a u32
+  static constexpr bool kMissing = true;
+  static __device__ __forceinline__ TermsSeg seg(const TermsParams& P, const Unit& U) { return P.tsegs[U.qseg]; }
+  static __device__ __forceinline__ uint32_t query(const TermsParams&, const CountSeg&, const TermsSeg& Z) { return Z.flags; }
+  static __device__ __forceinline__ HistUnit window(const TermsParams& P, uint32_t unit) { return P.windows[unit]; }
+  static __device__ __forceinline__ unsigned long long base(const TermsSeg& Z, uint32_t, const HistUnit& W) { return Z.base + W.first; }
+  static __device__ __forceinline__ Counter* counts(const TermsParams& P, const TermsSeg& Z, uint32_t, const HistUnit& W) { return P.counts + Z.counters + W.first; }
+  static __device__ __forceinline__ void one(const SortTile T, const TermsSeg&, uint32_t, const HistUnit& W, const unsigned long long base, uint32_t& idx) {
+    if (T.best[0] == ~T.best[1] && T.best[0] - base < W.n_bins) idx = (uint32_t)(T.best[0] - base);
+  }
+  static __device__ __forceinline__ unsigned long long value(unsigned long long v, uint32_t) { return v; }
+  static __device__ __forceinline__ bool counted(unsigned long long, const TermsSeg&) { return true; }
+  static __device__ __forceinline__ unsigned long long index(unsigned long long v, uint32_t, unsigned long long base) { return v - base; }
+  static __device__ __forceinline__ bool hits(uint32_t flags) { return flags & kTermsHits; }
+};
+
+// (4 CTAs per SM: no division here, and the 64 registers hold the loop without spilling)
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 4) k_terms(const TermsParams P) {
+  count_unit_keys<TermsKeys, kMixed>(P, P.unit_base + blockIdx.x);
+}
+
+// Exclusive CTA-wide prefix sum of v (fields packed in v add independently while each total fits its field); *total = the sum.
+__device__ __forceinline__ uint32_t cta_scan_excl(const uint32_t v, uint32_t* s_part, uint32_t& total) {
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (uint32_t d = 1; d < 32u; d <<= 1) {
+    const uint32_t y = __shfl_up_sync(kFull, x, d);
+    if (lane >= d) x += y;
+  }
+  if (lane == 31u) s_part[warp] = x;
+  __syncthreads();
+  uint32_t before = 0, sum = 0;
+  for (int w = 0; w < kWarps; ++w) {
+    const uint32_t p = s_part[w];
+    before += w < (int)warp ? p : 0u;
+    sum += p;
+  }
+  __syncthreads();
+  total = sum;
+  return before + x - v;
+}
+
+// One CTA per (query, segment) of a wave: the segment's cut (into_intermediate_bucket_result + cut_off_buckets).  A missing key
+// inside the counters' range is folded into its counter; one outside it is one more entry, before or after them in key order.  The
+// entries are the non-zero ones.  More than segment_size of them: by count, a radix select (4 passes of 8 bits) finds the count t
+// of the segment_size-th entry (t over ~count for asc: the segment_size-th largest t either way) and the entries beyond it are kept
+// with the lowest keys at t; by key, the first or last segment_size entries.  The kept entries go to the region in ascending key.
+__global__ void __launch_bounds__(kThreads) k_terms_select(const TermsParams P) {
+  __shared__ uint32_t s_hist[256];
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ unsigned long long s_wide[kWarps];
+  __shared__ uint32_t s_sel[3];  // the select's prefix, the rank left within it, the entries equal to it
+  __shared__ uint32_t s_error;
+  const uint32_t rel = blockIdx.x;
+  const TermsSeg Z = P.tsegs[P.seg_base + rel];
+  uint32_t* const cnt = P.counts + Z.counters;
+  const uint32_t n = Z.n_keys, ss = Z.segment_size;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t mc = (Z.flags & kTermsMissing) ? P.missing[rel] : 0u;
+  const bool inside = mc && Z.missing - Z.base < (unsigned long long)n;
+  const uint32_t extra = mc && !inside ? 1u : 0u, off = extra && Z.missing < Z.base ? 1u : 0u;
+  if (inside && threadIdx.x == 0) cnt[Z.missing - Z.base] += mc;
+  __syncthreads();
+  const uint32_t L = n + extra;  // entries in key order: [missing,] counters[0..n) [, missing]
+  auto count_at = [&](uint32_t i) -> uint32_t { i -= off; return i < n ? cnt[i] : mc; };
+  auto key_at = [&](uint32_t i) -> unsigned long long { i -= off; return i < n ? Z.base + i : Z.missing; };
+  const bool asc = Z.flags & kTermsAsc, by_key = Z.flags & kTermsByKey;
+  auto rank_key = [&](uint32_t c) -> uint32_t { return asc ? ~c : c; };  // larger first
+  // the entries and their doc count
+  uint32_t nz = 0;
+  unsigned long long sum = 0;
+  for (uint32_t i = threadIdx.x; i < L; i += blockDim.x) {
+    const uint32_t c = count_at(i);
+    nz += c ? 1u : 0u;
+    sum += c;
+  }
+  nz = __reduce_add_sync(kFull, nz);
+  for (int d = 16; d; d >>= 1) sum += __shfl_xor_sync(kFull, sum, d);
+  if (lane == 0) { s_part[warp] = nz; s_wide[warp] = sum; }
+  __syncthreads();
+  uint32_t N = 0;
+  unsigned long long total = 0;
+  for (int w = 0; w < kWarps; ++w) { N += s_part[w]; total += s_wide[w]; }
+  __syncthreads();
+  const bool cut = N > ss;
+  uint32_t t_cut = 0, need = 0;
+  if (cut && !by_key) {
+    uint32_t prefix = 0, mask = 0, k = ss;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      s_hist[threadIdx.x] = 0;
+      __syncthreads();
+      for (uint32_t i = threadIdx.x; i < L; i += blockDim.x) {
+        const uint32_t c = count_at(i);
+        const uint32_t t = rank_key(c);
+        if (c && (t & mask) == prefix) atomicAdd(&s_hist[(t >> shift) & 255u], 1u);
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        uint32_t b = 255, acc = 0;
+        for (; acc + s_hist[b] < k; --b) acc += s_hist[b];
+        s_sel[0] = prefix | (b << shift);
+        s_sel[1] = k - acc;
+        s_sel[2] = s_hist[b];
+      }
+      __syncthreads();
+      prefix = s_sel[0];
+      k = s_sel[1];
+      mask |= 255u << shift;
+      __syncthreads();
+    }
+    t_cut = prefix;
+    need = k;  // entries at t_cut to keep, the lowest keys first
+    // term_doc_count_before_cutoff: t_cut itself when more entries tie at it, else the largest t below it
+    if (threadIdx.x == 0) s_error = s_sel[2] > need ? t_cut : 0u;
+    uint32_t below = 0;
+    const bool more = s_sel[2] > need;
+    __syncthreads();
+    if (!more) {
+      for (uint32_t i = threadIdx.x; i < L; i += blockDim.x) {
+        const uint32_t c = count_at(i);
+        const uint32_t t = rank_key(c);
+        if (c && t < t_cut) below = max(below, t);
+      }
+      below = __reduce_max_sync(kFull, below);
+      if (lane == 0) atomicMax(&s_error, below);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) s_error = rank_key(s_error);
+  } else if (threadIdx.x == 0) {
+    s_error = 0;
+  }
+  __syncthreads();
+  // by key: the entry ranks kept and the rank whose count is reported
+  const uint32_t r0 = cut && by_key && !asc ? N - ss : 0u, r_err = cut && by_key ? (asc ? ss : N - ss - 1u) : 0xFFFFFFFFu;
+  uint32_t base_nz = 0, base_eq = 0, base_keep = 0;
+  unsigned long long kept = 0;
+  for (uint32_t i0 = 0; i0 < L; i0 += blockDim.x) {
+    const uint32_t i = i0 + threadIdx.x;
+    const uint32_t c = i < L ? count_at(i) : 0u;
+    const bool eq = c && cut && !by_key && rank_key(c) == t_cut;
+    uint32_t tot;
+    const uint32_t ex = cta_scan_excl((c ? 1u : 0u) | (eq ? 1u << 16 : 0u), s_part, tot);
+    const uint32_t r_nz = base_nz + (ex & 0xFFFFu), r_eq = base_eq + (ex >> 16);
+    base_nz += tot & 0xFFFFu;
+    base_eq += tot >> 16;
+    bool keep = c != 0;
+    if (cut) keep = keep && (by_key ? r_nz - r0 < ss : (rank_key(c) > t_cut || (eq && r_eq < need)));
+    if (c && r_nz == r_err) s_error = c;
+    const uint32_t at = base_keep + cta_scan_excl(keep ? 1u : 0u, s_part, tot);
+    base_keep += tot;
+    if (keep) {
+      P.res_key[Z.region + at] = key_at(i);
+      P.res_count[Z.region + at] = c;
+      kept += c;
+    }
+  }
+  for (int d = 16; d; d >>= 1) kept += __shfl_xor_sync(kFull, kept, d);
+  if (lane == 0) s_wide[warp] = kept;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long k_sum = 0;
+    for (int w = 0; w < kWarps; ++w) k_sum += s_wide[w];
+    P.res_n[rel] = base_keep;
+    P.res_other[rel] = total - k_sum;
+    P.res_error[rel] = cut ? s_error : 0u;
+  }
 }
 
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit

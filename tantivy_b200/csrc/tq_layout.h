@@ -270,6 +270,42 @@ struct HistParams {
 };
 static_assert(sizeof(HistSeg) == 40 && sizeof(HistQuery) == 48 && sizeof(HistUnit) == 8, "histogram descriptor layout");
 
+// ---- terms of a fast field (k_terms, k_terms_select) ----------------------------------------------------------------------
+// Doc counts per image of the docs Count counts.  Each (query, segment) has u32 counters over [base, base + n_keys), the images
+// of the 8192-doc tiles its units visit (at most kTermsMaxKeys, else TQ_ERR_UNSUPPORTED), and one counter of its matching docs
+// without a value; a unit counts into its own window of them (a HistUnit), on chip when it has kHistSmemBins or fewer.  Queries run
+// in waves whose counters fit the ctx's budget: a TermsSeg's counters and region are relative to its wave.
+constexpr uint32_t kTermsMaxKeys = 1u << 20;
+struct TermsSeg {  // one (query, segment), parallel to CountParams::segs
+  const unsigned long long* values;  // [max_doc] u64 images
+  const uint32_t* present;           // bitset in the alive layout (null: every doc has a value)
+  const SortTile* tiles;             // the column's per-tile bounds
+  unsigned long long base;           // image of counter 0
+  unsigned long long missing;        // the key of a doc without a value (kTermsMissing)
+  unsigned long long counters;       // first counter in TermsParams::counts
+  unsigned long long region;         // first kept entry in TermsParams::res_key / res_count
+  uint32_t n_keys;                   // counters (0: no visited tile holds a value)
+  uint32_t segment_size;             // entries kept, >= 1
+  uint32_t flags;                    // kTerms*
+  uint32_t pad;
+};
+constexpr uint32_t kTermsHits = 1, kTermsMissing = 2, kTermsByKey = 4, kTermsAsc = 8;
+struct TermsParams {
+  CountParams c;                // structure words, (query, segment) pairs, units and hit counters: the Count plan of the batch
+  const TermsSeg* tsegs;        // parallel to c.segs
+  const HistUnit* windows;      // parallel to c.units: each unit's window of its (query, segment)'s counters
+  uint32_t* counts;             // the wave's counters, zeroed before it
+  uint32_t* missing;            // [wave's (query, segment)s]: their matching docs without a value, zeroed before the wave
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them counted as one key
+  unsigned long long* res_key;  // the wave's kept entries, each (query, segment) in its region, ascending key
+  uint32_t* res_count;
+  uint32_t* res_n;              // [wave's (query, segment)s]: kept entries
+  unsigned long long* res_other;  // ... sum_other_doc_count
+  unsigned long long* res_error;  // ... term_doc_count_before_cutoff
+  uint32_t unit_base, seg_base;   // the wave's first unit and first (query, segment)
+};
+static_assert(sizeof(TermsSeg) == 72, "terms descriptor layout");
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

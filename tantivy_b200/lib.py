@@ -6,8 +6,9 @@ import os
 
 import numpy as np
 
-from ._abi import (HISTOGRAM_SPEC_DTYPE, SORT_SPEC_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64, TQ_ORDER_ASC,
-                   TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, f32p, ptr, u8p, u32p, u64p)
+from ._abi import (HISTOGRAM_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
+                   TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
+                   f32p, ptr, u8p, u32p, u64p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -30,6 +31,7 @@ def _load():
     lib.tq_ctx_destroy.argtypes = [vp]
     lib.tq_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.tq_get_histogram_stats.argtypes = [vp, C.POINTER(HistogramStats)]
+    lib.tq_get_terms_stats.argtypes = [vp, C.POINTER(TermsStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -45,6 +47,7 @@ def _load():
     lib.tq_sort_column_unregister.argtypes = [vp, C.c_uint32]
     lib.tq_sort_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(SortSpec), sz, C.c_uint32, u64p, u8p, u32p, u32p, u32p, u64p]
     lib.tq_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), sz, C.c_uint32, C.POINTER(C.c_int64), u64p, u32p, u64p]
+    lib.tq_terms_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), sz, C.c_uint32, u32p, u64p, u64p, u32p, u64p, u64p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -402,6 +405,41 @@ class Context:
             out = (pos, counts, nb)
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def terms_batch(self, qb: QueryBatch, specs, count_hits=False, stride=1024):
+        """The segment part of a terms aggregation per query (tq_terms_batch) over sort columns; specs = one
+        (column_id, target, order, segment_size[, missing_mode, missing_image]) per query, target TQ_TERMS_BY_*, order TQ_ORDER_*,
+        missing_mode TQ_TERMS_MISSING_* (tantivy_b200.terms turns requests into specs).  Returns (segment_ord, key, doc_count, n,
+        sum_other, error_bound): row q holds the n[q] kept entries of query q, ascending by (segment_ord, key image), over all its
+        segments, and sum_other[q] / error_bound[q] the sums of sum_other_doc_count / term_doc_count_before_cutoff over them -- and
+        with count_hits=True the Count of every query as well.  Raises TqError with code -4 (TQ_ERR_UNSUPPORTED) when a
+        (query, segment)'s keys span too wide a range for the device.  `stride` is the row width tried first: a longer row runs the
+        batch again at its width."""
+        specs = list(specs)
+        if len(specs) != qb.nq:
+            raise ValueError(f"one terms spec per query: {len(specs)} for {qb.nq} queries")
+        spec = np.zeros(max(qb.nq, 1), dtype=TERMS_SPEC_DTYPE)
+        for i, sp in enumerate(specs):
+            col, target, order, segment_size = sp[:4]
+            mode, image = sp[4:6] if len(sp) > 4 else (0, 0)
+            spec[i] = (col, target, order, segment_size, mode, 0, image)
+        n = max(qb.nq, 1)
+        while True:
+            segs = np.empty((n, stride), dtype=np.uint32)  # (only the first n[q] entries of row q are written)
+            keys = np.empty((n, stride), dtype=np.uint64)
+            counts = np.empty((n, stride), dtype=np.uint64)
+            nb = np.zeros(n, dtype=np.uint32)
+            other = np.zeros(n, dtype=np.uint64)
+            error = np.zeros(n, dtype=np.uint64)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_terms_batch(self.h, qb.ptr, spec.ctypes.data_as(C.POINTER(TermsSpec)), qb.nq, stride, ptr(segs, u32p), ptr(keys, u64p),
+                                    ptr(counts, u64p), ptr(nb, u32p), ptr(other, u64p), ptr(error, u64p), ptr(hits, u64p))
+            if rc == -1 and int(nb.max()) > stride:  # TQ_ERR_INVALID_ARGUMENT with the row lengths: a wider row
+                stride = int(nb.max())
+                continue
+            _check(rc, self.h)
+            out = (segs, keys, counts, nb, other[:qb.nq], error[:qb.nq])
+            return out + (hits[:qb.nq],) if count_hits else out
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -439,6 +477,9 @@ class Context:
         _check(LIB.tq_get_histogram_stats(self.h, C.byref(hs)), self.h)
         out = {name: (list(getattr(s, name)) if name in ("or_windows", "tile_counters", "tile_cycles", "tile_b2_exits") else getattr(s, name)) for name, _ in Stats._fields_}
         out.update({name: getattr(hs, name) for name, _ in HistogramStats._fields_})
+        ts = TermsStats()
+        _check(LIB.tq_get_terms_stats(self.h, C.byref(ts)), self.h)
+        out.update({name: getattr(ts, name) for name, _ in TermsStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
