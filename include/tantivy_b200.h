@@ -241,6 +241,16 @@ typedef struct {
   uint64_t terms_tiles_one_key;
 } tq_terms_stats;
 int tq_get_terms_stats(tq_ctx*, tq_terms_stats* out);
+/* Cumulative since ctx creation: tq_metrics_batch.  Device time of k_metrics, its CTAs (one per unit of up to eight 8192-doc
+ * tiles), the (tile, column) pairs the units came to and of those the ones added as one value (every value of the tile's column
+ * equal: its matches added without reading a value).  A struct of its own, so that the other stats keep their layouts. */
+typedef struct {
+  float metrics_ms;
+  uint64_t units_metrics;
+  uint64_t metrics_tiles_seen;
+  uint64_t metrics_tiles_one_value;
+} tq_metrics_stats;
+int tq_get_metrics_stats(tq_ctx*, tq_metrics_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -340,6 +350,56 @@ typedef struct {
   uint64_t missing_image; /* TQ_TERMS_MISSING_IMAGE: the key of a doc without a value */
 } tq_terms_spec;
 
+/* Metric aggregations (avg, sum, min, max, stats, value_count: src/aggregation/metric/stats.rs) over the same registered columns,
+ * single-valued only.  One spec per query names up to TQ_METRICS_MAX_COLUMNS columns, all fed by one match pass; each collects the
+ * value f64_from_fastfield_u64(image) of every doc the query collects that has one, and, with TQ_METRIC_MISSING, that of
+ * missing_image for every such doc without one (fetch_block_with_missing).  The column types a metric reads follow
+ * agg_data.rs:529-543: value_count reads str, bool and ip columns too, and those collect 0.0 per value (is_number_or_date_type
+ * false, stats.rs:372-375): a TQ_METRIC_COUNT_ONLY column, never read.  Every other metric reads numeric and date columns only;
+ * on any other column tantivy reads an empty u64 column (get_ff_reader, accessor_helpers.rs:59-74): a TQ_METRIC_EMPTY column,
+ * in which no doc has a value and column_id is not looked up. */
+#define TQ_METRICS_MAX_COLUMNS 4
+#define TQ_METRIC_MISSING 1u    /* docs without a value collect missing_image (f64_to_fastfield_u64 of `missing`, agg_data.rs:568) */
+#define TQ_METRIC_COUNT_ONLY 2u /* every collected value is 0.0: only the count is kept */
+#define TQ_METRIC_EMPTY 4u      /* no doc has a value (kind TQ_FAST_U64): only TQ_METRIC_MISSING collects anything */
+typedef struct {
+  uint32_t column_id;     /* a column of tq_sort_column_register (ignored with TQ_METRIC_EMPTY) */
+  uint32_t kind;          /* TQ_FAST_*: how an image maps to f64 */
+  uint32_t flags;         /* TQ_METRIC_* */
+  uint32_t pad;
+  uint64_t missing_image; /* TQ_METRIC_MISSING: the image a doc without a value collects */
+} tq_metric_column;
+typedef struct {
+  uint32_t n_columns;  /* 1 .. TQ_METRICS_MAX_COLUMNS; the same column may appear twice */
+  uint32_t pad;
+  tq_metric_column columns[TQ_METRICS_MAX_COLUMNS];
+} tq_metrics_spec;
+/* The intermediate result of one (query, column): IntermediateStats, without the order-dependent Kahan state.
+ *   count      values collected, NaN and +-inf included (a count-only column: every value)
+ *   n_nan      of them NaN; n_inf of them +-inf
+ *   min_image / max_image   the smallest / largest image of the non-NaN values (~0 / 0 when there is none; a count-only column
+ *              keeps them so): min and max are the values of these images, f64::MAX / f64::MIN when there is none (the reference's
+ *              starting values: NaN never lowers min, and +inf never does either since f64::MAX <= +inf).  -0.0 sorts before +0.0.
+ *   sum        the f64 sum of the finite values, added in no particular order; magnitude the f64 sum of their |v|
+ *   quantum_exp  Q: the least exponent of the lowest set bit over the finite non-zero values (every one is a multiple of 2^Q);
+ *              INT32_MAX when there is none
+ * Parts of one query (split segments, several contexts) merge field by field: counts add, min_image takes the min, max_image the
+ * max, sum and magnitude add, quantum_exp takes the min.
+ * The guard: the merged sum is the reference's Kahan sum, bit for bit, when n_nan == n_inf == 0 and magnitude < 2^(53 + Q), or
+ * magnitude is finite when 53 + Q > 1023.  Then every partial sum, in any order, is a multiple of 2^Q below 2^(53 + Q) in magnitude,
+ * hence exact: Kahan's compensation stays 0 and every order gives the exact sum (DESIGN §3.8).  Otherwise sum, avg and stats take the
+ * CPU path; count, min and max are exact always. */
+typedef struct {
+  uint64_t count, n_nan, n_inf;
+  uint64_t min_image, max_image;
+  double sum, magnitude;
+  int32_t quantum_exp;
+  uint32_t pad;
+} tq_metric_part;
+#ifdef __cplusplus
+static_assert(sizeof(tq_metric_column) == 24 && sizeof(tq_metrics_spec) == 104 && sizeof(tq_metric_part) == 64, "metrics ABI layout");
+#endif
+
 /* ---- search -------------------------------------------------------------------------- */
 /* The whole hot path for a batch of queries, host buffers in / host buffers out:
  * block decode -> AND/OR/term -> BM25 -> per-segment top-k -> merge_fruits.
@@ -410,6 +470,15 @@ int tq_histogram_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec
 int tq_terms_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec* specs, size_t nq, uint32_t out_stride,
                    uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_sum_other,
                    uint64_t* out_error_bound, uint64_t* out_hits);
+
+/* The intermediate metric results of term / AND / OR / mixed boolean (TQ_OP_BOOL) queries, synchronous like tq_count_batch, over
+ * the docs tq_count_batch counts: out[q * TQ_METRICS_MAX_COLUMNS + i] is query q's tq_metric_part of specs[q].columns[i] over all
+ * its segments (parts past n_columns are written empty: count 0, images ~0 / 0, sums 0, quantum_exp INT32_MAX).  out_hits may be
+ * NULL; else out_hits[q] = tq_count_batch's answer for query q.  Applying the guard, merging parts of other contexts and the final
+ * values are the caller's.  TQ_OP_PHRASE returns TQ_ERR_UNSUPPORTED; a segment without a column TQ_ERR_NOT_FOUND; n_columns outside
+ * 1 .. TQ_METRICS_MAX_COLUMNS, a kind outside TQ_FAST_* or a flag outside TQ_METRIC_* TQ_ERR_INVALID_ARGUMENT.  k, thresholds and
+ * TQ_QUERY_COUNT_HITS are ignored.  The run holds its columns as tq_sort_batch does. */
+int tq_metrics_batch(tq_ctx*, const tq_query* queries, const tq_metrics_spec* specs, size_t nq, tq_metric_part* out, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

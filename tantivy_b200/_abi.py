@@ -22,6 +22,8 @@ TQ_ORDER_DESC, TQ_ORDER_ASC = 0, 1
 TQ_FAST_U64, TQ_FAST_I64, TQ_FAST_F64, TQ_FAST_BOOL, TQ_FAST_DATE = 0, 1, 2, 3, 4
 TQ_TERMS_BY_COUNT, TQ_TERMS_BY_KEY = 0, 1
 TQ_TERMS_MISSING_NONE, TQ_TERMS_MISSING_IMAGE, TQ_TERMS_MISSING_AFTER_MAX = 0, 1, 2
+TQ_METRICS_MAX_COLUMNS = 4
+TQ_METRIC_MISSING, TQ_METRIC_COUNT_ONLY, TQ_METRIC_EMPTY = 1, 2, 4
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -181,6 +183,36 @@ class TermsSpec(C.Structure):
 TERMS_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("target", "<u4"), ("order", "<u4"), ("segment_size", "<u4"), ("missing_mode", "<u4"),
                              ("pad", "<u4"), ("missing_image", "<u8")])
 assert TERMS_SPEC_DTYPE.itemsize == C.sizeof(TermsSpec) == 32
+
+
+class MetricsStats(C.Structure):
+    """tq_metrics_stats — the cumulative counters of tq_metrics_batch (tq_get_metrics_stats)."""
+    _fields_ = [("metrics_ms", C.c_float), ("units_metrics", C.c_uint64), ("metrics_tiles_seen", C.c_uint64), ("metrics_tiles_one_value", C.c_uint64)]
+
+
+class MetricColumn(C.Structure):
+    """tq_metric_column — one column of a metrics spec: its kind, TQ_METRIC_* flags and missing image."""
+    _fields_ = [("column_id", C.c_uint32), ("kind", C.c_uint32), ("flags", C.c_uint32), ("pad", C.c_uint32), ("missing_image", C.c_uint64)]
+
+
+class MetricsSpec(C.Structure):
+    """tq_metrics_spec — the 1..TQ_METRICS_MAX_COLUMNS columns one query's metrics read."""
+    _fields_ = [("n_columns", C.c_uint32), ("pad", C.c_uint32), ("columns", MetricColumn * TQ_METRICS_MAX_COLUMNS)]
+
+
+class MetricPart(C.Structure):
+    """tq_metric_part — the intermediate result of one (query, column)."""
+    _fields_ = [("count", C.c_uint64), ("n_nan", C.c_uint64), ("n_inf", C.c_uint64), ("min_image", C.c_uint64), ("max_image", C.c_uint64),
+                ("sum", C.c_double), ("magnitude", C.c_double), ("quantum_exp", C.c_int32), ("pad", C.c_uint32)]
+
+
+METRIC_COLUMN_DTYPE = np.dtype([("column_id", "<u4"), ("kind", "<u4"), ("flags", "<u4"), ("pad", "<u4"), ("missing_image", "<u8")])
+METRICS_SPEC_DTYPE = np.dtype([("n_columns", "<u4"), ("pad", "<u4"), ("columns", METRIC_COLUMN_DTYPE, (TQ_METRICS_MAX_COLUMNS,))])
+METRIC_PART_DTYPE = np.dtype([("count", "<u8"), ("n_nan", "<u8"), ("n_inf", "<u8"), ("min_image", "<u8"), ("max_image", "<u8"), ("sum", "<f8"),
+                              ("magnitude", "<f8"), ("quantum_exp", "<i4"), ("pad", "<u4")])
+assert METRIC_COLUMN_DTYPE.itemsize == C.sizeof(MetricColumn) == 24
+assert METRICS_SPEC_DTYPE.itemsize == C.sizeof(MetricsSpec) == 104
+assert METRIC_PART_DTYPE.itemsize == C.sizeof(MetricPart) == 64
 
 
 def ptr(arr, typ):

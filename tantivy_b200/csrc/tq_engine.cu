@@ -404,6 +404,16 @@ int tq_get_terms_stats(tq_ctx* c, tq_terms_stats* out) {
   return TQ_OK;
 }
 
+int tq_get_metrics_stats(tq_ctx* c, tq_metrics_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->metrics_ms = (float)c->metrics_ms;
+  out->units_metrics = c->metrics_units;
+  out->metrics_tiles_seen = c->metrics_tiles_seen;
+  out->metrics_tiles_one_value = c->metrics_tiles_one_value;
+  return TQ_OK;
+}
+
 int tq_segment_register(tq_ctx* c, uint32_t segment_ord, uint32_t field, uint32_t max_doc, int record_option,
                         const uint8_t* idx_body, size_t idx_len, const uint8_t* fieldnorm, size_t fieldnorm_len,
                         const uint8_t* alive_bitset, size_t alive_len) {
@@ -2182,6 +2192,115 @@ int tq_terms_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* spec
     c->terms_tiles_one_key += tiles[1];
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride: out_n holds how many");
+  return TQ_OK;
+}
+
+// ---- metrics of fast fields ----------------------------------------------------------------------------------
+int tq_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_metrics_spec* specs, size_t nq, tq_metric_part* out, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !specs || !out))) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const tq_metrics_spec& sp = specs[qi];
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "metrics of phrase queries are not on the device path");
+    if (sp.n_columns < 1 || sp.n_columns > TQ_METRICS_MAX_COLUMNS) return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: n_columns must be 1..4");
+    for (uint32_t i = 0; i < sp.n_columns; ++i)
+      if (sp.columns[i].kind > TQ_FAST_DATE || (sp.columns[i].flags & ~(TQ_METRIC_MISSING | TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY)) ||
+          ((sp.columns[i].flags & TQ_METRIC_EMPTY) && ((sp.columns[i].flags & TQ_METRIC_COUNT_ONLY) || sp.columns[i].kind != TQ_FAST_U64)))
+        return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: column kind or flags");
+  }
+  const tq_metric_part empty{0ull, 0ull, 0ull, ~0ull, 0ull, 0.0, 0.0, INT32_MAX, 0u};
+  for (size_t qi = 0; qi < nq; ++qi) {
+    for (uint32_t i = 0; i < kMetricsMaxColumns; ++i) out[qi * kMetricsMaxColumns + i] = empty;
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<MetricsSeg> msegs;  // parallel to cp.segs
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_metrics_spec& sp = specs[qi];
+      const size_t s0 = cp.segs.size();
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        MetricsSeg z{};
+        z.n_columns = sp.n_columns;
+        z.flags = out_hits ? kMetricsHits : 0u;
+        for (uint32_t i = 0; i < sp.n_columns; ++i) {
+          const tq_metric_column& mc = sp.columns[i];
+          if (mc.flags & TQ_METRIC_EMPTY) {  // (tantivy's empty column: no values, no tiles)
+            z.col[i] = MetricsCol{nullptr, nullptr, nullptr, mc.missing_image, mc.kind, mc.flags};
+            continue;
+          }
+          auto it = c->sort_columns.find({mc.column_id, cp.segment_ords[si]});
+          if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a metrics query names a segment without the column (tq_sort_column_register)");
+          const SortColumn& col = it->second;
+          if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+          z.col[i] = MetricsCol{col.d_values, col.d_present, col.d_tiles, mc.missing_image, mc.kind, mc.flags};
+        }
+        msegs.push_back(z);
+      }
+    }
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the parts are in)
+    for (size_t qi = 0; qi < nq; ++qi)
+      for (uint32_t i = 0; i < specs[qi].n_columns; ++i)
+        if (!(specs[qi].columns[i].flags & TQ_METRIC_EMPTY)) b->held_columns.push_back(specs[qi].columns[i].column_id);
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // descriptors and the empty accumulators: one H2D copy; scratch: hits | tile counters
+  std::vector<tq_metric_part> parts(nq * kMetricsMaxColumns, empty);
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(msegs), o_p = st.add(parts);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(16), head_bytes = off;
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(head_bytes + parts.size() * sizeof(tq_metric_part)));
+  uint8_t* const d = b->scratch.p;
+  MetricsParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.msegs = st.on_device<const MetricsSeg>(o_z);
+  P.parts = st.on_device<tq_metric_part>(o_p);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+  (cp.mixed ? k_metrics<true> : k_metrics<false>)<<<(unsigned)cp.units.size(), kThreads, 0, b->stream>>>(P);
+  TQ_CUDA(cudaGetLastError());
+  TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + head_bytes, st.on_device<const uint8_t>(o_p), parts.size() * sizeof(tq_metric_part),
+                          cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  const uint8_t* h = b->res_pin.p;
+  memcpy(out, h + head_bytes, parts.size() * sizeof(tq_metric_part));
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  float ms = 0;
+  cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_tiles, 16);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->metrics_ms += ms;
+    c->metrics_units += cp.units.size();
+    c->metrics_tiles_seen += tiles[0];
+    c->metrics_tiles_one_value += tiles[1];
+  }
   return TQ_OK;
 }
 

@@ -244,6 +244,9 @@ struct tq_ctx {
   // ... and of the terms runs (terms_ms, units_terms, terms_tiles_seen, terms_tiles_one_key)
   double terms_ms = 0;
   uint64_t terms_units = 0, terms_tiles_seen = 0, terms_tiles_one_key = 0;
+  // ... and of the metrics runs (metrics_ms, units_metrics, metrics_tiles_seen, metrics_tiles_one_value)
+  double metrics_ms = 0;
+  uint64_t metrics_units = 0, metrics_tiles_seen = 0, metrics_tiles_one_value = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;

@@ -1756,6 +1756,176 @@ __global__ void __launch_bounds__(kThreads) k_terms_select(const TermsParams P) 
   }
 }
 
+// ---- metrics of fast fields (AggregationCollector: avg / sum / min / max / stats / value_count, metric/stats.rs) -------------
+// The docs Count counts, each collecting its value in every column of the query's spec: one match pass feeds up to four columns.
+// One CTA per Count unit: per 8192-doc tile match_tile builds the match bitmap; per column, a tile whose smallest and largest images
+// are equal (SortTile: every value of the tile, matching or not, is that one) adds popc(match & present) copies of its value
+// without a gather, any other tile has each thread walk the matches of its own 32-doc word with one 8-byte gather per doc.  A
+// count-only column is never read, and an empty one (TQ_METRIC_EMPTY) has no value in any doc.  Matching docs without a value are counted per thread and added at exit as copies of the
+// missing value.  The accumulators of the four columns live in registers per thread; NaN and +-inf, which only ever decide a
+// refusal, are counted in shared memory.  At exit each quantity is reduced per warp, then per CTA, and flushed with one set of
+// atomics per (unit, column).  Every add is one f64 operation on exact operands, so under the guard (tantivy_b200.h) every
+// partial sum is exact and the order of the adds and atomics cannot change the result.
+struct MetricAcc {
+  unsigned long long lo, hi;  // smallest / largest image of the non-NaN values
+  double sum, mag;            // sum and sum of |v| of the finite values
+  uint32_t count, missing;    // values seen; matching docs without a value
+  int q;                      // least exponent of the lowest set bit of a finite non-zero value
+};
+
+// n copies of the value of `image`
+__device__ __forceinline__ void metric_add(MetricAcc& a, const unsigned long long image, const uint32_t kind, const uint32_t n,
+                                           uint32_t* s_nan_inf) {
+  const double v = hist_value(image, kind);
+  if (v != v) { atomicAdd(&s_nan_inf[0], n); return; }
+  a.lo = min(a.lo, image);
+  a.hi = max(a.hi, image);
+  const double av = fabs(v);
+  if (av == INFINITY) { atomicAdd(&s_nan_inf[1], n); return; }
+  a.sum = __dadd_rn(a.sum, __dmul_rn((double)n, v));
+  a.mag = __dadd_rn(a.mag, __dmul_rn((double)n, av));
+  if (av != 0.0) a.q = min(a.q, metric_quantum_exp((unsigned long long)__double_as_longlong(av)));
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads) k_metrics(const MetricsParams P) {
+  static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
+  static_assert(sizeof(MetricsSeg) % 8u == 0 && sizeof(MetricsSeg) / 8u <= (uint32_t)kThreads, "one word of the descriptor per thread");
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ MetricsSeg s_z;
+  __shared__ unsigned long long s_one[kC];  // per column: the tile's one image, when s_has_one
+  __shared__ uint32_t s_has_one[kC];
+  __shared__ uint32_t s_nan_inf[kC][2];
+  __shared__ unsigned long long s_lo[kWarps][kC], s_hi[kWarps][kC];
+  __shared__ double s_sum[kWarps][kC], s_mag[kWarps][kC];
+  __shared__ uint32_t s_count[kWarps][kC], s_part[kWarps];
+  __shared__ int s_q[kWarps][kC];
+  const Unit U = P.c.units[blockIdx.x];
+  const CountSeg S = P.c.segs[U.qseg];
+  if (threadIdx.x < sizeof(MetricsSeg) / 8u)
+    reinterpret_cast<unsigned long long*>(&s_z)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(P.msegs + U.qseg)[threadIdx.x];
+  if (threadIdx.x < 2u * kC) (&s_nan_inf[0][0])[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t nc = s_z.n_columns;
+  const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  MetricAcc acc[kC];
+#pragma unroll
+  for (uint32_t c = 0; c < kC; ++c) acc[c] = MetricAcc{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};
+  uint32_t total = 0, one = 0, seen = 0;
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x < nc) {  // (warp 0)
+      const MetricsCol& C = s_z.col[threadIdx.x];
+      uint32_t has = 0;
+      if (!(C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY))) {
+        const SortTile T = C.tiles[tile];
+        has = (T.flags & kSortTileValues) && T.best[0] == ~T.best[1] ? 1u : 0u;
+        s_one[threadIdx.x] = T.best[0];
+        ++seen;
+        one += has;
+      }
+      s_has_one[threadIdx.x] = has;
+    }
+    match_tile<kMixed>(P.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    total += (uint32_t)__popc(bits);
+#pragma unroll
+    for (uint32_t c = 0; c < kC; ++c) {
+      if (c >= nc) break;
+      const MetricsCol& C = s_z.col[c];
+      const uint32_t with = (C.flags & TQ_METRIC_EMPTY) ? 0u : C.present ? bits & __ldg(C.present + (lo >> 5) + threadIdx.x) : bits;
+      const uint32_t n = (uint32_t)__popc(with);
+      acc[c].count += n;
+      acc[c].missing += (uint32_t)__popc(bits ^ with);
+      if (C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY)) continue;
+      if (s_has_one[c]) {
+        if (n) metric_add(acc[c], s_one[c], C.kind, n, s_nan_inf[c]);
+      } else {
+        for (uint32_t m = with; m; m &= m - 1u) {
+          const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(m) - 1);
+          metric_add(acc[c], __ldg(C.values + doc), C.kind, 1u, s_nan_inf[c]);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  // missing values, then the warp's figures
+#pragma unroll
+  for (uint32_t c = 0; c < kC; ++c) {
+    if (c >= nc) break;
+    const MetricsCol& C = s_z.col[c];
+    if ((C.flags & TQ_METRIC_MISSING) && acc[c].missing) {
+      acc[c].count += acc[c].missing;
+      if (!(C.flags & TQ_METRIC_COUNT_ONLY)) metric_add(acc[c], C.missing, C.kind, acc[c].missing, s_nan_inf[c]);
+    }
+    uint32_t count = __reduce_add_sync(kFull, acc[c].count);
+    int q = __reduce_min_sync(kFull, acc[c].q);
+    unsigned long long vlo = acc[c].lo, vhi = acc[c].hi;
+    double sum = acc[c].sum, mag = acc[c].mag;
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {
+      vlo = min(vlo, __shfl_xor_sync(kFull, vlo, d));
+      vhi = max(vhi, __shfl_xor_sync(kFull, vhi, d));
+      sum = __dadd_rn(sum, __shfl_xor_sync(kFull, sum, d));
+      mag = __dadd_rn(mag, __shfl_xor_sync(kFull, mag, d));
+    }
+    if (lane == 0) {
+      s_count[warp][c] = count;
+      s_q[warp][c] = q;
+      s_lo[warp][c] = vlo;
+      s_hi[warp][c] = vhi;
+      s_sum[warp][c] = sum;
+      s_mag[warp][c] = mag;
+    }
+  }
+  if (warp == 0) {
+    one = __reduce_add_sync(kFull, one);
+    seen = __reduce_add_sync(kFull, seen);
+  }
+  total = __reduce_add_sync(kFull, total);
+  if (lane == 0) s_part[warp] = total;
+  __syncthreads();
+  if (threadIdx.x < nc) {  // one set of atomics per (unit, column)
+    const uint32_t c = threadIdx.x;
+    unsigned long long count = 0, vlo = ~0ull, vhi = 0;
+    double sum = 0.0, mag = 0.0;
+    int q = INT32_MAX;
+    for (int w = 0; w < kWarps; ++w) {
+      count += s_count[w][c];
+      q = min(q, s_q[w][c]);
+      vlo = min(vlo, s_lo[w][c]);
+      vhi = max(vhi, s_hi[w][c]);
+      sum = __dadd_rn(sum, s_sum[w][c]);
+      mag = __dadd_rn(mag, s_mag[w][c]);
+    }
+    tq_metric_part* const out = P.parts + (size_t)S.query * kC + c;
+    if (count) {
+      atomicAdd(reinterpret_cast<unsigned long long*>(&out->count), count);
+      if (s_nan_inf[c][0]) atomicAdd(reinterpret_cast<unsigned long long*>(&out->n_nan), (unsigned long long)s_nan_inf[c][0]);
+      if (s_nan_inf[c][1]) atomicAdd(reinterpret_cast<unsigned long long*>(&out->n_inf), (unsigned long long)s_nan_inf[c][1]);
+      if (vlo <= vhi) {
+        atomicMin(reinterpret_cast<unsigned long long*>(&out->min_image), vlo);
+        atomicMax(reinterpret_cast<unsigned long long*>(&out->max_image), vhi);
+      }
+      atomicAdd(&out->sum, sum);
+      atomicAdd(&out->magnitude, mag);
+      if (q != INT32_MAX) atomicMin(&out->quantum_exp, q);
+    }
+  }
+  if (threadIdx.x == 0) {
+    if (s_z.flags & kMetricsHits) {
+      unsigned long long hits = 0;
+      for (int w = 0; w < kWarps; ++w) hits += s_part[w];
+      if (hits) atomicAdd(&P.c.counts[S.query], hits);
+    }
+    if (seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (one) atomicAdd(&P.tiles[1], (unsigned long long)one); }
+  }
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

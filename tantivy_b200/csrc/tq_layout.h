@@ -306,6 +306,44 @@ struct TermsParams {
 };
 static_assert(sizeof(TermsSeg) == 72, "terms descriptor layout");
 
+// ---- metrics of fast fields (k_metrics) -----------------------------------------------------------------------------------
+// One tq_metric_part accumulator per (query, column), fed by every unit of the query: no counters, so no waves and no size limit.
+constexpr uint32_t kMetricsMaxColumns = 4;  // TQ_METRICS_MAX_COLUMNS
+struct MetricsCol {  // one column of one (query, segment)
+  const unsigned long long* values;  // [max_doc] u64 images
+  const uint32_t* present;           // bitset in the alive layout (null: every doc has a value)
+  const SortTile* tiles;             // the column's per-tile bounds
+  unsigned long long missing;        // the image a doc without a value collects (TQ_METRIC_MISSING)
+  uint32_t kind;                     // TQ_FAST_*
+  uint32_t flags;                    // TQ_METRIC_*
+};
+struct MetricsSeg {  // one (query, segment), parallel to CountParams::segs
+  MetricsCol col[kMetricsMaxColumns];
+  uint32_t n_columns;
+  uint32_t flags;  // kMetricsHits
+  uint32_t pad[2];
+};
+constexpr uint32_t kMetricsHits = 1;
+struct MetricsParams {
+  CountParams c;                // structure words, (query, segment) pairs, units and hit counters: the Count plan of the batch
+  const MetricsSeg* msegs;      // parallel to c.segs
+  tq_metric_part* parts;        // [query][kMetricsMaxColumns], initialised empty by the host
+  unsigned long long* tiles;    // [0] (tile, column) pairs seen, [1] of them added as one value
+};
+static_assert(sizeof(MetricsCol) == 40 && sizeof(MetricsSeg) == 176, "metrics descriptor layout");
+// The exponent of the lowest set bit of a finite non-zero |v| (v is a multiple of 2^that); the guard's Q is its minimum.
+TQ_HD inline int metric_quantum_exp(unsigned long long abs_bits) {
+  const int e = (int)(abs_bits >> 52);
+  unsigned long long m = abs_bits & ((1ull << 52) - 1ull);
+  if (e) m |= 1ull << 52;
+#ifdef __CUDA_ARCH__
+  const int tz = __ffsll((long long)m) - 1;
+#else
+  const int tz = __builtin_ctzll(m);
+#endif
+  return (e ? e - 1075 : -1074) + tz;
+}
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

@@ -6,7 +6,8 @@ import os
 
 import numpy as np
 
-from ._abi import (HISTOGRAM_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
+from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
+                   MetricsSpec, MetricsStats, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
                    f32p, ptr, u8p, u32p, u64p)
 
@@ -32,6 +33,7 @@ def _load():
     lib.tq_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.tq_get_histogram_stats.argtypes = [vp, C.POINTER(HistogramStats)]
     lib.tq_get_terms_stats.argtypes = [vp, C.POINTER(TermsStats)]
+    lib.tq_get_metrics_stats.argtypes = [vp, C.POINTER(MetricsStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -48,6 +50,7 @@ def _load():
     lib.tq_sort_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(SortSpec), sz, C.c_uint32, u64p, u8p, u32p, u32p, u32p, u64p]
     lib.tq_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), sz, C.c_uint32, C.POINTER(C.c_int64), u64p, u32p, u64p]
     lib.tq_terms_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), sz, C.c_uint32, u32p, u64p, u64p, u32p, u64p, u64p, u64p]
+    lib.tq_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(MetricsSpec), sz, C.POINTER(MetricPart), u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -440,6 +443,28 @@ class Context:
             out = (segs, keys, counts, nb, other[:qb.nq], error[:qb.nq])
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def metrics_batch(self, qb: QueryBatch, specs, count_hits=False):
+        """The intermediate metric results per query (tq_metrics_batch) over sort columns; specs = one list per query of 1..4
+        (column_id, kind[, flags, missing_image]) columns, kind TQ_FAST_*, flags TQ_METRIC_* (tantivy_b200.metrics turns requests into
+        specs).  Returns a structured array [nq, TQ_METRICS_MAX_COLUMNS] of METRIC_PART_DTYPE (count, n_nan, n_inf, min_image,
+        max_image, sum, magnitude, quantum_exp), columns past a query's spec empty -- and with count_hits=True the Count of every query
+        as well."""
+        specs = list(specs)
+        if len(specs) != qb.nq:
+            raise ValueError(f"one metrics spec per query: {len(specs)} for {qb.nq} queries")
+        spec = np.zeros(max(qb.nq, 1), dtype=METRICS_SPEC_DTYPE)
+        for i, cols in enumerate(specs):
+            cols = list(cols)
+            spec[i]["n_columns"] = len(cols)
+            for j, col in enumerate(cols[:TQ_METRICS_MAX_COLUMNS]):
+                flags, image = (tuple(col[2:4]) + (0, 0))[:2]
+                spec[i]["columns"][j] = (col[0], col[1], flags, 0, image)
+        parts = np.zeros((max(qb.nq, 1), TQ_METRICS_MAX_COLUMNS), dtype=METRIC_PART_DTYPE)
+        hits = np.zeros(max(qb.nq, 1), dtype=np.uint64) if count_hits else None
+        _check(LIB.tq_metrics_batch(self.h, qb.ptr, spec.ctypes.data_as(C.POINTER(MetricsSpec)), qb.nq, parts.ctypes.data_as(C.POINTER(MetricPart)),
+                                    ptr(hits, u64p)), self.h)
+        return (parts[:qb.nq], hits[:qb.nq]) if count_hits else parts[:qb.nq]
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -480,6 +505,9 @@ class Context:
         ts = TermsStats()
         _check(LIB.tq_get_terms_stats(self.h, C.byref(ts)), self.h)
         out.update({name: getattr(ts, name) for name, _ in TermsStats._fields_})
+        ms = MetricsStats()
+        _check(LIB.tq_get_metrics_stats(self.h, C.byref(ms)), self.h)
+        out.update({name: getattr(ms, name) for name, _ in MetricsStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
