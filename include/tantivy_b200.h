@@ -251,6 +251,21 @@ typedef struct {
   uint64_t metrics_tiles_one_value;
 } tq_metrics_stats;
 int tq_get_metrics_stats(tq_ctx*, tq_metrics_stats* out);
+/* Cumulative since ctx creation: tq_histogram_metrics_batch.  Device time of k_hist_metrics + k_hist_metrics_final over all waves,
+ * their CTAs (one per unit of up to eight 8192-doc tiles, plus one per query), the 8192-doc tiles the units came to and of those
+ * the ones in one bucket (every value of the tile in one bucket: its metrics accumulated in registers as tq_metrics_batch does),
+ * and the (unit, bucket) accumulators flushed from shared memory at a unit's exit versus the runs of one-bucket tiles flushed
+ * straight to global memory (units whose window is too wide for shared memory).  A struct of its own, so that the other stats
+ * keep their layouts. */
+typedef struct {
+  float hist_metrics_ms;
+  uint64_t units_hist_metrics;
+  uint64_t hist_metrics_tiles_seen;
+  uint64_t hist_metrics_tiles_one_bucket;
+  uint64_t hist_metrics_flush_shared;
+  uint64_t hist_metrics_flush_global;
+} tq_hist_metrics_stats;
+int tq_get_hist_metrics_stats(tq_ctx*, tq_hist_metrics_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -479,6 +494,26 @@ int tq_terms_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec* specs,
  * 1 .. TQ_METRICS_MAX_COLUMNS, a kind outside TQ_FAST_* or a flag outside TQ_METRIC_* TQ_ERR_INVALID_ARGUMENT.  k, thresholds and
  * TQ_QUERY_COUNT_HITS are ignored.  The run holds its columns as tq_sort_batch does. */
 int tq_metrics_batch(tq_ctx*, const tq_query* queries, const tq_metrics_spec* specs, size_t nq, tq_metric_part* out, uint64_t* out_hits);
+
+/* A histogram with metric sub-aggregations (one `histogram` / `date_histogram` whose `aggs` are avg, sum, min, max, stats and
+ * value_count: SegmentHistogramCollector::collect pushing each counted doc to its bucket's sub-aggregation, histogram.rs:490-505),
+ * synchronous like tq_count_batch, over the docs tq_count_batch counts.  hspecs[q] is query q's histogram exactly as in
+ * tq_histogram_batch, mspecs[q] its metric columns exactly as in tq_metrics_batch; the docs a bucket's metrics collect are the docs
+ * the histogram counts in it (a doc without a histogram value, or with one outside the bounds, feeds no metric).  Row q (out_stride
+ * buckets apart) holds query q's out_n[q] non-empty buckets over all its segments in ascending pos: out_pos[i] and out_doc_count[i]
+ * as tq_histogram_batch writes them, and out_parts[i * TQ_METRICS_MAX_COLUMNS + c] the bucket's tq_metric_part of column c (parts
+ * past n_columns are written empty), with tq_metrics_batch's merge rules and guard, applied per (bucket, column) by the caller.
+ * When some out_n[q] > out_stride, every out_n is written and the call returns TQ_ERR_INVALID_ARGUMENT: retry with a larger
+ * stride.  out_hits may be NULL; else out_hits[q] = tq_count_batch's answer for query q.  A query's accumulators span its bucket
+ * range as in tq_histogram_batch, one tq_metric_part per (bucket, column): a range of more than 2^16 buckets returns
+ * TQ_ERR_UNSUPPORTED naming the query (the caller takes the CPU path).  Queries whose accumulators exceed the ctx's budget
+ * (TQ_HIST_METRICS_BUDGET at ctx creation, in (bucket, column) accumulators) run in consecutive waves on one scratch region.  The
+ * errors are those of tq_histogram_batch and tq_metrics_batch: TQ_OP_PHRASE returns TQ_ERR_UNSUPPORTED, a segment without a column
+ * TQ_ERR_NOT_FOUND, a bad histogram kind or interval, metric kind, flag or column count TQ_ERR_INVALID_ARGUMENT.  k, thresholds
+ * and TQ_QUERY_COUNT_HITS are ignored.  The run holds its columns as tq_sort_batch does. */
+int tq_histogram_metrics_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_metrics_spec* mspecs, size_t nq,
+                               uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
+                               uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

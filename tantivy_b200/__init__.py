@@ -13,3 +13,5 @@ from . import terms  # noqa: E402  (the terms aggregation's request and result s
 from .terms import TermsRefused  # noqa: E402
 from . import metrics  # noqa: E402  (the metric aggregations' request and result side)
 from .metrics import MetricsRefused  # noqa: E402
+from . import hist_metrics  # noqa: E402  (histograms with metric sub-aggregations: request and result side)
+from .hist_metrics import HistMetricsRefused  # noqa: E402

@@ -190,6 +190,12 @@ class MetricsStats(C.Structure):
     _fields_ = [("metrics_ms", C.c_float), ("units_metrics", C.c_uint64), ("metrics_tiles_seen", C.c_uint64), ("metrics_tiles_one_value", C.c_uint64)]
 
 
+class HistMetricsStats(C.Structure):
+    """tq_hist_metrics_stats — the cumulative counters of tq_histogram_metrics_batch (tq_get_hist_metrics_stats)."""
+    _fields_ = [("hist_metrics_ms", C.c_float), ("units_hist_metrics", C.c_uint64), ("hist_metrics_tiles_seen", C.c_uint64),
+                ("hist_metrics_tiles_one_bucket", C.c_uint64), ("hist_metrics_flush_shared", C.c_uint64), ("hist_metrics_flush_global", C.c_uint64)]
+
+
 class MetricColumn(C.Structure):
     """tq_metric_column — one column of a metrics spec: its kind, TQ_METRIC_* flags and missing image."""
     _fields_ = [("column_id", C.c_uint32), ("kind", C.c_uint32), ("flags", C.c_uint32), ("pad", C.c_uint32), ("missing_image", C.c_uint64)]

@@ -282,6 +282,7 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->count_hits_tiles_per_unit = std::max<uint32_t>(1u, env_u32("TQ_COUNT_HITS_TILES_PER_UNIT", 8));
   // terms counters per wave of tq_terms_batch (256 MB); test hook: a small budget runs a batch in many waves
   c->terms_counter_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_COUNTER_BUDGET", 1u << 26));
+  c->hist_metrics_budget = std::max<uint32_t>(1u, env_u32("TQ_HIST_METRICS_BUDGET", 1u << 22));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -411,6 +412,18 @@ int tq_get_metrics_stats(tq_ctx* c, tq_metrics_stats* out) {
   out->units_metrics = c->metrics_units;
   out->metrics_tiles_seen = c->metrics_tiles_seen;
   out->metrics_tiles_one_value = c->metrics_tiles_one_value;
+  return TQ_OK;
+}
+
+int tq_get_hist_metrics_stats(tq_ctx* c, tq_hist_metrics_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->hist_metrics_ms = (float)c->hist_metrics_ms;
+  out->units_hist_metrics = c->hist_metrics_units;
+  out->hist_metrics_tiles_seen = c->hist_metrics_tiles_seen;
+  out->hist_metrics_tiles_one_bucket = c->hist_metrics_tiles_one_bucket;
+  out->hist_metrics_flush_shared = c->hist_metrics_flush_shared;
+  out->hist_metrics_flush_global = c->hist_metrics_flush_global;
   return TQ_OK;
 }
 
@@ -1791,6 +1804,69 @@ static bool unit_images(const SortColumn& col, const Unit& u, unsigned long long
   return any;
 }
 
+// The histogram side of one query's plan, after plan_count added its (query, segment)s from s0 and units from u0: per (query,
+// segment) its column and bounds after normalize_histogram_req's collapse (hsegs, cols), per unit the first and last pos its tiles'
+// values in bounds can take (uwin; first > last: none), and the query's dense range [base, base + len) (compute_dense_range,
+// histogram.rs:751-769, over the visited tiles only).  A range above max_bins is TQ_ERR_UNSUPPORTED.
+static int plan_hist_query(tq_ctx* c, const tq_histogram_spec& sp, size_t qi, const CountPlan& cp, size_t s0, size_t u0, uint32_t max_bins,
+                           std::vector<HistSeg>& hsegs, std::vector<const SortColumn*>& cols, std::vector<std::pair<long long, long long>>& uwin,
+                           long long& base, uint64_t& len) {
+  cols.clear();
+  for (size_t si = s0; si < cp.segs.size(); ++si) {
+    auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
+    if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a histogram query names a segment without the column (tq_sort_column_register)");
+    const SortColumn& col = it->second;
+    if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+    // normalize_histogram_req: the hard bounds collapse to every finite value when the segment's column lies inside them
+    double lo = sp.hard_min, hi = sp.hard_max;
+    if (col.min_image <= col.max_image && hist_value(col.min_image, sp.kind) >= lo && hist_value(col.max_image, sp.kind) <= hi) {
+      lo = -DBL_MAX;
+      hi = DBL_MAX;
+    }
+    hsegs.push_back(HistSeg{col.d_values, col.d_present, col.d_tiles, lo, hi});
+    cols.push_back(&col);
+  }
+  // per unit: the buckets of its tiles' values, clipped to its segment's bounds; the query's dense range (compute_dense_range,
+  // histogram.rs:751-769, over the visited tiles only) is their union
+  uwin.clear();
+  long long top = -1;
+  base = 0;
+  bool any = false;
+  for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+    const Unit& u = cp.units[ui];
+    const size_t k = u.qseg - s0;
+    const HistSeg& z = hsegs[u.qseg];
+    double umin = INFINITY, umax = -INFINITY;
+    if (sp.kind == TQ_FAST_F64) {
+      for (uint32_t t = u.begin; t < u.end; ++t) {  // an infinity widens the range only when it is in bounds; a NaN never is
+        const FiniteTile& f = cols[k]->finite[t];
+        double vmin = INFINITY, vmax = -INFINITY;
+        if (f.flags & kFiniteAny) { vmin = hist_value(f.lo, sp.kind); vmax = hist_value(f.hi, sp.kind); }
+        if ((f.flags & kFiniteNegInf) && z.lo == -INFINITY) vmin = -INFINITY;
+        if ((f.flags & kFinitePosInf) && z.hi == INFINITY) vmax = INFINITY;
+        umin = std::min(umin, vmin);
+        umax = std::max(umax, vmax);
+      }
+    } else {
+      unsigned long long ilo, ihi;  // (hist_value is monotone in the image for every other kind)
+      if (unit_images(*cols[k], u, ilo, ihi)) { umin = hist_value(ilo, sp.kind); umax = hist_value(ihi, sp.kind); }
+    }
+    const double lo = std::max(umin, z.lo), hi = std::min(umax, z.hi);
+    if (!(lo <= hi)) { uwin.emplace_back(1, 0); continue; }  // no value of the unit can pass the bounds
+    const long long p0 = hist_pos(lo, sp.offset, sp.interval), p1 = hist_pos(hi, sp.offset, sp.interval);
+    uwin.emplace_back(p0, p1);
+    base = any ? std::min(base, p0) : p0;
+    top = any ? std::max(top, p1) : p1;
+    any = true;
+  }
+  const __int128 n = any ? (__int128)top - base + 1 : 0;
+  if (n > max_bins)
+    return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its histogram spans more than 2^" + std::to_string(31 - __builtin_clz(max_bins)) +
+                                        " buckets (take the CPU path)");
+  len = (uint64_t)n;
+  return TQ_OK;
+}
+
 int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* specs, size_t nq, uint32_t out_stride,
                        int64_t* out_pos, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_hits) {
   if (!c || (nq && (!queries || !specs || !out_n || (out_stride && (!out_pos || !out_doc_count)))))
@@ -1823,56 +1899,10 @@ int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_sp
       const size_t s0 = cp.segs.size(), u0 = cp.units.size();
       int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
       if (rc != TQ_OK) return rc;
-      cols.clear();
-      for (size_t si = s0; si < cp.segs.size(); ++si) {
-        auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
-        if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a histogram query names a segment without the column (tq_sort_column_register)");
-        const SortColumn& col = it->second;
-        if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
-        // normalize_histogram_req: the hard bounds collapse to every finite value when the segment's column lies inside them
-        double lo = sp.hard_min, hi = sp.hard_max;
-        if (col.min_image <= col.max_image && hist_value(col.min_image, sp.kind) >= lo && hist_value(col.max_image, sp.kind) <= hi) {
-          lo = -DBL_MAX;
-          hi = DBL_MAX;
-        }
-        hsegs.push_back(HistSeg{col.d_values, col.d_present, col.d_tiles, lo, hi});
-        cols.push_back(&col);
-      }
-      // per unit: the buckets of its tiles' values, clipped to its segment's bounds; the query's dense range (compute_dense_range,
-      // histogram.rs:751-769, over the visited tiles only) is their union
-      uwin.clear();
-      long long base = 0, top = -1;
-      bool any = false;
-      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
-        const Unit& u = cp.units[ui];
-        const size_t k = u.qseg - s0;
-        const HistSeg& z = hsegs[u.qseg];
-        double umin = INFINITY, umax = -INFINITY;
-        if (sp.kind == TQ_FAST_F64) {
-          for (uint32_t t = u.begin; t < u.end; ++t) {  // an infinity widens the range only when it is in bounds; a NaN never is
-            const FiniteTile& f = cols[k]->finite[t];
-            double vmin = INFINITY, vmax = -INFINITY;
-            if (f.flags & kFiniteAny) { vmin = hist_value(f.lo, sp.kind); vmax = hist_value(f.hi, sp.kind); }
-            if ((f.flags & kFiniteNegInf) && z.lo == -INFINITY) vmin = -INFINITY;
-            if ((f.flags & kFinitePosInf) && z.hi == INFINITY) vmax = INFINITY;
-            umin = std::min(umin, vmin);
-            umax = std::max(umax, vmax);
-          }
-        } else {
-          unsigned long long ilo, ihi;  // (hist_value is monotone in the image for every other kind)
-          if (unit_images(*cols[k], u, ilo, ihi)) { umin = hist_value(ilo, sp.kind); umax = hist_value(ihi, sp.kind); }
-        }
-        const double lo = std::max(umin, z.lo), hi = std::min(umax, z.hi);
-        if (!(lo <= hi)) { uwin.emplace_back(1, 0); continue; }  // no value of the unit can pass the bounds
-        const long long p0 = hist_pos(lo, sp.offset, sp.interval), p1 = hist_pos(hi, sp.offset, sp.interval);
-        uwin.emplace_back(p0, p1);
-        base = any ? std::min(base, p0) : p0;
-        top = any ? std::max(top, p1) : p1;
-        any = true;
-      }
-      const __int128 len = any ? (__int128)top - base + 1 : 0;
-      if (len > kHistMaxBins)
-        return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its histogram spans more than 2^20 buckets (take the CPU path)");
+      long long base = 0;
+      uint64_t len = 0;
+      rc = plan_hist_query(c, sp, qi, cp, s0, u0, kHistMaxBins, hsegs, cols, uwin, base, len);
+      if (rc != TQ_OK) return rc;
       for (const auto& w : uwin)
         hunits.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - base), (uint32_t)(w.second - w.first + 1)} : HistUnit{0u, 0u});
       hq[qi] = HistQuery{sp.interval, sp.offset, base, n_counters, (uint32_t)len, sp.kind, out_hits ? kHistHits : 0u, 0u};
@@ -2196,17 +2226,52 @@ int tq_terms_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* spec
 }
 
 // ---- metrics of fast fields ----------------------------------------------------------------------------------
+// A metrics spec's column count, kinds and flags (TQ_ERR_INVALID_ARGUMENT).
+static int check_metrics_spec(const tq_metrics_spec& sp) {
+  if (sp.n_columns < 1 || sp.n_columns > TQ_METRICS_MAX_COLUMNS) return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: n_columns must be 1..4");
+  for (uint32_t i = 0; i < sp.n_columns; ++i)
+    if (sp.columns[i].kind > TQ_FAST_DATE || (sp.columns[i].flags & ~(TQ_METRIC_MISSING | TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY)) ||
+        ((sp.columns[i].flags & TQ_METRIC_EMPTY) && ((sp.columns[i].flags & TQ_METRIC_COUNT_ONLY) || sp.columns[i].kind != TQ_FAST_U64)))
+      return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: column kind or flags");
+  return TQ_OK;
+}
+
+// One MetricsSeg per (query, segment) plan_count added from s0: the spec's columns in that segment.
+static int plan_metrics_segs(tq_ctx* c, const tq_metrics_spec& sp, const CountPlan& cp, size_t s0, bool hits, std::vector<MetricsSeg>& msegs) {
+  for (size_t si = s0; si < cp.segs.size(); ++si) {
+    MetricsSeg z{};
+    z.n_columns = sp.n_columns;
+    z.flags = hits ? kMetricsHits : 0u;
+    for (uint32_t i = 0; i < sp.n_columns; ++i) {
+      const tq_metric_column& mc = sp.columns[i];
+      if (mc.flags & TQ_METRIC_EMPTY) {  // (tantivy's empty column: no values, no tiles)
+        z.col[i] = MetricsCol{nullptr, nullptr, nullptr, mc.missing_image, mc.kind, mc.flags};
+        continue;
+      }
+      auto it = c->sort_columns.find({mc.column_id, cp.segment_ords[si]});
+      if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a metrics query names a segment without the column (tq_sort_column_register)");
+      const SortColumn& col = it->second;
+      if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+      z.col[i] = MetricsCol{col.d_values, col.d_present, col.d_tiles, mc.missing_image, mc.kind, mc.flags};
+    }
+    msegs.push_back(z);
+  }
+  return TQ_OK;
+}
+
+// The registered columns a metrics spec reads, for the batch to hold (the caller sorts and dedups b->held_columns).
+static void hold_metric_columns(tq_batch* b, const tq_metrics_spec& sp) {
+  for (uint32_t i = 0; i < sp.n_columns; ++i)
+    if (!(sp.columns[i].flags & TQ_METRIC_EMPTY)) b->held_columns.push_back(sp.columns[i].column_id);
+}
+
 int tq_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_metrics_spec* specs, size_t nq, tq_metric_part* out, uint64_t* out_hits) {
   if (!c || (nq && (!queries || !specs || !out))) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
   TQ_CUDA(cudaSetDevice(c->device));
   for (size_t qi = 0; qi < nq; ++qi) {
-    const tq_metrics_spec& sp = specs[qi];
     if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "metrics of phrase queries are not on the device path");
-    if (sp.n_columns < 1 || sp.n_columns > TQ_METRICS_MAX_COLUMNS) return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: n_columns must be 1..4");
-    for (uint32_t i = 0; i < sp.n_columns; ++i)
-      if (sp.columns[i].kind > TQ_FAST_DATE || (sp.columns[i].flags & ~(TQ_METRIC_MISSING | TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY)) ||
-          ((sp.columns[i].flags & TQ_METRIC_EMPTY) && ((sp.columns[i].flags & TQ_METRIC_COUNT_ONLY) || sp.columns[i].kind != TQ_FAST_U64)))
-        return fail(TQ_ERR_INVALID_ARGUMENT, "metrics spec: column kind or flags");
+    int rc = check_metrics_spec(specs[qi]);
+    if (rc != TQ_OK) return rc;
   }
   const tq_metric_part empty{0ull, 0ull, 0ull, ~0ull, 0ull, 0.0, 0.0, INT32_MAX, 0u};
   for (size_t qi = 0; qi < nq; ++qi) {
@@ -2229,31 +2294,13 @@ int tq_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_metrics_spec* 
       const size_t s0 = cp.segs.size();
       int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
       if (rc != TQ_OK) return rc;
-      for (size_t si = s0; si < cp.segs.size(); ++si) {
-        MetricsSeg z{};
-        z.n_columns = sp.n_columns;
-        z.flags = out_hits ? kMetricsHits : 0u;
-        for (uint32_t i = 0; i < sp.n_columns; ++i) {
-          const tq_metric_column& mc = sp.columns[i];
-          if (mc.flags & TQ_METRIC_EMPTY) {  // (tantivy's empty column: no values, no tiles)
-            z.col[i] = MetricsCol{nullptr, nullptr, nullptr, mc.missing_image, mc.kind, mc.flags};
-            continue;
-          }
-          auto it = c->sort_columns.find({mc.column_id, cp.segment_ords[si]});
-          if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a metrics query names a segment without the column (tq_sort_column_register)");
-          const SortColumn& col = it->second;
-          if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
-          z.col[i] = MetricsCol{col.d_values, col.d_present, col.d_tiles, mc.missing_image, mc.kind, mc.flags};
-        }
-        msegs.push_back(z);
-      }
+      rc = plan_metrics_segs(c, sp, cp, s0, out_hits != nullptr, msegs);
+      if (rc != TQ_OK) return rc;
     }
     int rc = flush_builds(c, &built);
     if (rc != TQ_OK) return rc;
     hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the parts are in)
-    for (size_t qi = 0; qi < nq; ++qi)
-      for (uint32_t i = 0; i < specs[qi].n_columns; ++i)
-        if (!(specs[qi].columns[i].flags & TQ_METRIC_EMPTY)) b->held_columns.push_back(specs[qi].columns[i].column_id);
+    for (size_t qi = 0; qi < nq; ++qi) hold_metric_columns(b, specs[qi]);
     std::sort(b->held_columns.begin(), b->held_columns.end());
     b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
     for (uint32_t col : b->held_columns) ++c->sort_users[col];
@@ -2301,6 +2348,195 @@ int tq_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_metrics_spec* 
     c->metrics_tiles_seen += tiles[0];
     c->metrics_tiles_one_value += tiles[1];
   }
+  return TQ_OK;
+}
+
+// ---- metrics per histogram bucket ----------------------------------------------------------------------------
+int tq_histogram_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_metrics_spec* mspecs, size_t nq,
+                               uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
+                               uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !hspecs || !mspecs || !out_n || (out_stride && (!out_pos || !out_doc_count || !out_parts)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "histograms of phrase queries are not on the device path");
+    if (hspecs[qi].kind > TQ_FAST_DATE) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram kind");
+    if (!(hspecs[qi].interval > 0.0) || !std::isfinite(hspecs[qi].interval)) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram interval must be finite and > 0");
+    int rc = check_metrics_spec(mspecs[qi]);
+    if (rc != TQ_OK) return rc;
+  }
+  for (size_t qi = 0; qi < nq; ++qi) { out_n[qi] = 0; if (out_hits) out_hits[qi] = 0; }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<HistSeg> hsegs;     // parallel to cp.segs
+  std::vector<MetricsSeg> msegs;  // parallel to cp.segs
+  std::vector<HistQuery> hq(nq);
+  std::vector<HistUnit> hunits;   // parallel to cp.units
+  std::vector<size_t> q_unit(nq + 1);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<long long, long long>> uwin;  // per unit of the query: its first and last pos (first > last: none)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_histogram_spec& sp = hspecs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      long long base = 0;
+      uint64_t len = 0;
+      rc = plan_hist_query(c, sp, qi, cp, s0, u0, kHistMetricsMaxBins, hsegs, cols, uwin, base, len);
+      if (rc != TQ_OK) return rc;
+      rc = plan_metrics_segs(c, mspecs[qi], cp, s0, out_hits != nullptr, msegs);
+      if (rc != TQ_OK) return rc;
+      for (const auto& w : uwin)
+        hunits.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - base), (uint32_t)(w.second - w.first + 1)} : HistUnit{0u, 0u});
+      hq[qi] = HistQuery{sp.interval, sp.offset, base, 0ull, (uint32_t)len, sp.kind, out_hits ? kHistHits : 0u, 0u};
+    }
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      b->held_columns.push_back(hspecs[qi].column_id);
+      hold_metric_columns(b, mspecs[qi]);
+    }
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // waves of consecutive queries whose accumulators (kC per bucket) fit the budget (a query above it runs alone); counters and rows
+  // relative to the wave.  A query's row holds min(out_stride, n_bins) entries (it has at most n_bins non-empty buckets), so a
+  // wave's rows, on the device and in pinned memory, are bounded by its counters and the budget as well.
+  struct Wave { size_t q0, q1; uint64_t counters, rows; };
+  std::vector<Wave> waves;
+  std::vector<unsigned long long> row_at(nq);
+  uint64_t max_counters = 0, max_rows = 0;
+  size_t max_queries = 0;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (waves.empty() || (waves.back().counters && (waves.back().counters + hq[qi].n_bins) * kC > c->hist_metrics_budget))
+      waves.push_back(Wave{qi, qi, 0, 0});
+    Wave& w = waves.back();
+    hq[qi].counters = w.counters;
+    row_at[qi] = w.rows;
+    w.q1 = qi + 1;
+    w.counters += hq[qi].n_bins;
+    w.rows += std::min<uint64_t>(out_stride, hq[qi].n_bins);
+    max_counters = std::max(max_counters, w.counters);
+    max_rows = std::max(max_rows, w.rows);
+    max_queries = std::max(max_queries, w.q1 - w.q0);
+  }
+  // descriptors: one H2D copy; scratch: hits | tile counters, then one wave's row lengths | rows (pos | doc counts | parts) |
+  // doc counters | accumulators
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(hsegs), o_m = st.add(msegs),
+               o_q = st.add(hq), o_h = st.add(hunits), o_r = st.add(row_at);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  const size_t part_row = (size_t)kC * sizeof(tq_metric_part);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(32), head_bytes = off;
+  const size_t r_n = take(max_queries * 4), r_pos = take(max_rows * 8), r_count = take(max_rows * 8), r_parts = take(max_rows * part_row),
+               wave_bytes = off - head_bytes;
+  const size_t r_counters = take(max_counters * 8), r_acc = take(max_counters * part_row);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  HistMetricsParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.hsegs = st.on_device<const HistSeg>(o_z);
+  P.msegs = st.on_device<const MetricsSeg>(o_m);
+  P.queries = st.on_device<const HistQuery>(o_q);
+  P.hunits = st.on_device<const HistUnit>(o_h);
+  P.rows = st.on_device<const unsigned long long>(o_r);
+  P.counts = reinterpret_cast<unsigned long long*>(d + r_counters);
+  P.parts = reinterpret_cast<tq_metric_part*>(d + r_acc);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.res_pos = reinterpret_cast<long long*>(d + r_pos);
+  P.res_count = reinterpret_cast<unsigned long long*>(d + r_count);
+  P.res_parts = reinterpret_cast<tq_metric_part*>(d + r_parts);
+  P.res_n = reinterpret_cast<uint32_t*>(d + r_n);
+  P.res_stride = out_stride;
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  const uint8_t* h = b->res_pin.p;
+  const size_t p_pos = r_pos - head_bytes, p_count = r_count - head_bytes, p_parts = r_parts - head_bytes;
+  float ms_total = 0;
+  bool fits = true;
+  for (const Wave& w : waves) {
+    const size_t ua = q_unit[w.q0], ub = q_unit[w.q1], wq = w.q1 - w.q0;
+    P.unit_base = (uint32_t)ua;
+    P.query_base = (uint32_t)w.q0;
+    TQ_CUDA(cudaMemsetAsync(d + r_counters, 0, w.counters * 8, b->stream));
+    TQ_CUDA(cudaMemsetAsync(d + r_acc, 0, w.counters * part_row, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    if (ub > ua) {
+      (cp.mixed ? k_hist_metrics<true> : k_hist_metrics<false>)<<<(unsigned)(ub - ua), kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    k_hist_metrics_final<<<(unsigned)wq, kThreads, 0, b->stream>>>(P);
+    TQ_CUDA(cudaGetLastError());
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + r_n, wq * 4, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    memcpy(out_n + w.q0, h, wq * 4);
+    for (size_t qi = w.q0; qi < w.q1; ++qi) fits = fits && out_n[qi] <= out_stride;
+    if (!fits) continue;  // (a row too long: only the lengths of the remaining waves)
+    // the rows: the wave's whole region when they fill half of it or more, else each query's row only as long as it is
+    uint64_t filled = 0;
+    for (size_t qi = w.q0; qi < w.q1; ++qi) filled += out_n[qi];
+    auto fetch = [&](size_t at, size_t n) {
+      TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + p_pos + at * 8, d + r_pos + at * 8, n * 8, cudaMemcpyDeviceToHost, b->stream));
+      TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + p_count + at * 8, d + r_count + at * 8, n * 8, cudaMemcpyDeviceToHost, b->stream));
+      TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + p_parts + at * part_row, d + r_parts + at * part_row, n * part_row, cudaMemcpyDeviceToHost,
+                              b->stream));
+      return TQ_OK;
+    };
+    if (2 * filled >= w.rows) {
+      int rc = fetch(0, w.rows);
+      if (rc != TQ_OK) return rc;
+    } else {
+      for (size_t qi = w.q0; qi < w.q1; ++qi) {
+        int rc = out_n[qi] ? fetch(row_at[qi], out_n[qi]) : TQ_OK;
+        if (rc != TQ_OK) return rc;
+      }
+    }
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    for (size_t qi = w.q0; qi < w.q1; ++qi) {
+      const size_t at = row_at[qi], dst = qi * (size_t)out_stride, n = out_n[qi];
+      memcpy(out_pos + dst, h + p_pos + at * 8, n * 8);
+      memcpy(out_doc_count + dst, h + p_count + at * 8, n * 8);
+      memcpy(out_parts + dst * kC, h + p_parts + at * part_row, n * part_row);
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  unsigned long long tiles[4];
+  memcpy(tiles, h + r_tiles, 32);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->hist_metrics_ms += ms_total;
+    c->hist_metrics_units += cp.units.size() + nq;
+    c->hist_metrics_tiles_seen += tiles[0];
+    c->hist_metrics_tiles_one_bucket += tiles[1];
+    c->hist_metrics_flush_shared += tiles[2];
+    c->hist_metrics_flush_global += tiles[3];
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a histogram has more non-empty buckets than out_stride: out_n holds how many");
   return TQ_OK;
 }
 

@@ -1926,6 +1926,311 @@ __global__ void __launch_bounds__(kThreads) k_metrics(const MetricsParams P) {
   }
 }
 
+// ---- metrics per histogram bucket (histogram / date_histogram with metric sub-aggregations, histogram.rs:490-505) -------------
+// The docs k_hist counts, each feeding the metric columns of the (query, segment)'s MetricsSeg in its bucket.  One CTA per Count
+// unit on match_tile.  A tile whose values are all in bounds and in one bucket (HistKeys::one) accumulates as k_metrics does, in
+// registers, with its one-value tiles and missing copies; the registers carry over consecutive tiles of that bucket (the bucket is
+// CTA-uniform there) and are reduced per warp, then per CTA, and flushed with one set of atomics per (run of tiles, column) when
+// the bucket changes or the unit ends.  Any other tile has each thread walk the matches of its own 32-doc word: a gather of the
+// histogram value, the bounds test and pos (hist_value / hist_pos, as k_hist), then per column a gather and atomics on that
+// bucket's accumulators.  A unit's window of kHistMetricsSmemBins or fewer buckets lives in shared memory and is flushed per
+// non-empty bucket at exit; a wider one goes to global memory.  The accumulators are tq_metric_parts with min_image and
+// quantum_exp stored complemented (~min_image, INT32_MAX - quantum_exp as u32), so that zeroed memory is an empty part and every
+// field merges with an add or a max; k_hist_metrics_final undoes the complement.  As in k_metrics every add is one f64 operation
+// on exact operands, so under the guard, applied per (bucket, column), the order of the adds cannot change the result.
+__device__ __forceinline__ void hm_merge(tq_metric_part* p, const unsigned long long count, const unsigned long long n_nan,
+                                         const unsigned long long n_inf, const unsigned long long lo, const unsigned long long hi,
+                                         const double sum, const double mag, const int q) {
+  if (!count) return;
+  atomicAdd(reinterpret_cast<unsigned long long*>(&p->count), count);
+  if (n_nan) atomicAdd(reinterpret_cast<unsigned long long*>(&p->n_nan), n_nan);
+  if (n_inf) atomicAdd(reinterpret_cast<unsigned long long*>(&p->n_inf), n_inf);
+  if (lo <= hi) {
+    atomicMax(reinterpret_cast<unsigned long long*>(&p->min_image), ~lo);
+    atomicMax(reinterpret_cast<unsigned long long*>(&p->max_image), hi);
+  }
+  if (mag != 0.0) {  // (finite values all +-0 add nothing to a sum that starts at +0)
+    atomicAdd(&p->sum, sum);
+    atomicAdd(&p->magnitude, mag);
+  }
+  if (q != INT32_MAX) atomicMax(reinterpret_cast<unsigned*>(&p->quantum_exp), 0x7FFFFFFFu - (unsigned)q);
+}
+
+// one doc of one column into its bucket's accumulator: its value, the missing value, or (count-only) just the count
+__device__ __forceinline__ void hm_collect(tq_metric_part* p, const MetricsCol& C, const uint32_t doc, const bool has) {
+  if (!has && !(C.flags & TQ_METRIC_MISSING)) return;
+  if (C.flags & TQ_METRIC_COUNT_ONLY) {
+    atomicAdd(reinterpret_cast<unsigned long long*>(&p->count), 1ull);
+    return;
+  }
+  const unsigned long long image = has ? __ldg(C.values + doc) : C.missing;
+  const double v = hist_value(image, C.kind);
+  if (v != v) { hm_merge(p, 1ull, 1ull, 0ull, ~0ull, 0ull, 0.0, 0.0, INT32_MAX); return; }
+  const double av = fabs(v);
+  if (av == INFINITY) { hm_merge(p, 1ull, 0ull, 1ull, image, image, 0.0, 0.0, INT32_MAX); return; }
+  hm_merge(p, 1ull, 0ull, 0ull, image, image, v, av, av != 0.0 ? metric_quantum_exp((unsigned long long)__double_as_longlong(av)) : INT32_MAX);
+}
+
+// one counted doc of a straddling tile: its bucket's doc counter and every column (cw: the thread's present words per column)
+template <class Docs>
+__device__ __forceinline__ void hm_doc(Docs* docs, tq_metric_part* parts, const MetricsSeg& z, const uint32_t* cw, const uint32_t doc,
+                                       const uint32_t bit) {
+  atomicAdd(docs, (Docs)1);
+#pragma unroll
+  for (uint32_t c = 0; c < kMetricsMaxColumns; ++c) {
+    if (c >= z.n_columns) break;
+    hm_collect(parts + c, z.col[c], doc, (cw[c] >> bit) & 1u);
+  }
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsParams P) {
+  static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
+  static_assert(sizeof(MetricsSeg) % 8u == 0 && sizeof(MetricsSeg) / 8u <= (uint32_t)kThreads, "one word of the descriptor per thread");
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ MetricsSeg s_z;
+  __shared__ tq_metric_part s_parts[kHistMetricsSmemBins * kC];  // the window's accumulators, when it fits
+  __shared__ uint32_t s_docs[kHistMetricsSmemBins];
+  __shared__ unsigned long long s_one[kC];  // per column: the tile's one image, when s_has_one
+  __shared__ uint32_t s_has_one[kC];
+  __shared__ uint32_t s_bucket;             // the tile's one bucket (index into the window), or ~0u
+  __shared__ uint32_t s_nan_inf[kC][2];     // the run's NaN and +-inf values per column
+  __shared__ unsigned long long s_lo[kWarps][kC], s_hi[kWarps][kC];
+  __shared__ double s_sum[kWarps][kC], s_mag[kWarps][kC];
+  __shared__ uint32_t s_count[kWarps][kC], s_part[kWarps], s_rdocs[kWarps];
+  __shared__ int s_q[kWarps][kC];
+  const uint32_t unit = P.unit_base + blockIdx.x;
+  const Unit U = P.c.units[unit];
+  const CountSeg S = P.c.segs[U.qseg];
+  const HistSeg Z = P.hsegs[U.qseg];
+  const HistQuery Q = P.queries[S.query];
+  const HistUnit W = P.hunits[unit];
+  if (threadIdx.x < sizeof(MetricsSeg) / 8u)
+    reinterpret_cast<unsigned long long*>(&s_z)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(P.msegs + U.qseg)[threadIdx.x];
+  if (threadIdx.x < 2u * kC) (&s_nan_inf[0][0])[threadIdx.x] = 0;
+  const bool shared = W.n_bins <= kHistMetricsSmemBins;
+  if (shared) {
+    for (uint32_t i = threadIdx.x; i < W.n_bins * (uint32_t)(sizeof(tq_metric_part) / 8u) * kC; i += blockDim.x)
+      reinterpret_cast<unsigned long long*>(s_parts)[i] = 0ull;
+    for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x) s_docs[i] = 0;
+  }
+  __syncthreads();
+  const uint32_t nc = s_z.n_columns;
+  const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const long long base = Q.base + (long long)W.first;  // pos of the window's first bucket
+  unsigned long long* const gdocs = P.counts + Q.counters + W.first;
+  tq_metric_part* const gparts = P.parts + (Q.counters + W.first) * kC;
+  MetricAcc acc[kC];
+#pragma unroll
+  for (uint32_t c = 0; c < kC; ++c) acc[c] = MetricAcc{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};
+  uint32_t rdocs = 0, total = 0, one = 0, flushed_global = 0;
+  uint32_t run = 0xFFFFFFFFu;  // the bucket of the register run (CTA-uniform), or none
+  // the run into its bucket: missing copies, per warp, per CTA, one merge per column (CTA-uniform: every thread calls it)
+  auto flush = [&]() {
+#pragma unroll
+    for (uint32_t c = 0; c < kC; ++c) {
+      if (c >= nc) break;
+      const MetricsCol& C = s_z.col[c];
+      if ((C.flags & TQ_METRIC_MISSING) && acc[c].missing) {
+        acc[c].count += acc[c].missing;
+        if (!(C.flags & TQ_METRIC_COUNT_ONLY)) metric_add(acc[c], C.missing, C.kind, acc[c].missing, s_nan_inf[c]);
+      }
+      uint32_t count = __reduce_add_sync(kFull, acc[c].count);
+      int q = __reduce_min_sync(kFull, acc[c].q);
+      unsigned long long vlo = acc[c].lo, vhi = acc[c].hi;
+      double sum = acc[c].sum, mag = acc[c].mag;
+#pragma unroll
+      for (int d = 16; d; d >>= 1) {
+        vlo = min(vlo, __shfl_xor_sync(kFull, vlo, d));
+        vhi = max(vhi, __shfl_xor_sync(kFull, vhi, d));
+        sum = __dadd_rn(sum, __shfl_xor_sync(kFull, sum, d));
+        mag = __dadd_rn(mag, __shfl_xor_sync(kFull, mag, d));
+      }
+      if (lane == 0) {
+        s_count[warp][c] = count;
+        s_q[warp][c] = q;
+        s_lo[warp][c] = vlo;
+        s_hi[warp][c] = vhi;
+        s_sum[warp][c] = sum;
+        s_mag[warp][c] = mag;
+      }
+      acc[c] = MetricAcc{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};
+    }
+    rdocs = __reduce_add_sync(kFull, rdocs);
+    if (lane == 0) s_rdocs[warp] = rdocs;
+    rdocs = 0;
+    __syncthreads();
+    if (threadIdx.x < nc) {
+      const uint32_t c = threadIdx.x;
+      unsigned long long count = 0, vlo = ~0ull, vhi = 0;
+      double sum = 0.0, mag = 0.0;
+      int q = INT32_MAX;
+      for (int w = 0; w < kWarps; ++w) {
+        count += s_count[w][c];
+        q = min(q, s_q[w][c]);
+        vlo = min(vlo, s_lo[w][c]);
+        vhi = max(vhi, s_hi[w][c]);
+        sum = __dadd_rn(sum, s_sum[w][c]);
+        mag = __dadd_rn(mag, s_mag[w][c]);
+      }
+      const unsigned long long n_nan = s_nan_inf[c][0], n_inf = s_nan_inf[c][1];
+      s_nan_inf[c][0] = s_nan_inf[c][1] = 0;  // (only this thread reads or resets column c's until the next barrier)
+      if (shared) hm_merge(s_parts + run * kC + c, count, n_nan, n_inf, vlo, vhi, sum, mag, q);
+      else hm_merge(gparts + (size_t)run * kC + c, count, n_nan, n_inf, vlo, vhi, sum, mag, q);
+    } else if (threadIdx.x == 32u) {  // (warp 1: the columns are warp 0's)
+      unsigned long long d = 0;
+      for (int w = 0; w < kWarps; ++w) d += s_rdocs[w];
+      if (d) {
+        if (shared) s_docs[run] += (uint32_t)d;
+        else atomicAdd(&gdocs[run], d);
+      }
+    }
+    flushed_global += shared ? 0u : 1u;
+    __syncthreads();
+  };
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      const SortTile T = Z.tiles[tile];
+      uint32_t idx = 0xFFFFFFFFu;
+      if (W.n_bins && (T.flags & kSortTileValues)) HistKeys::one(T, Z, Q, W, base, idx);
+      s_bucket = idx;
+      one += idx != 0xFFFFFFFFu ? 1u : 0u;
+    }
+    if (threadIdx.x < nc) {  // (warp 0)
+      const MetricsCol& C = s_z.col[threadIdx.x];
+      uint32_t has = 0;
+      if (!(C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY))) {
+        const SortTile T = C.tiles[tile];
+        has = (T.flags & kSortTileValues) && T.best[0] == ~T.best[1] ? 1u : 0u;
+        s_one[threadIdx.x] = T.best[0];
+      }
+      s_has_one[threadIdx.x] = has;
+    }
+    match_tile<kMixed>(P.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    total += (uint32_t)__popc(bits);
+    const uint32_t b = s_bucket;
+    if (b < W.n_bins) {  // one bucket: every matching doc with a histogram value is in it
+      if (b != run) {
+        if (run != 0xFFFFFFFFu) flush();
+        run = b;
+      }
+      const uint32_t hw = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
+      rdocs += (uint32_t)__popc(hw);
+#pragma unroll
+      for (uint32_t c = 0; c < kC; ++c) {
+        if (c >= nc) break;
+        const MetricsCol& C = s_z.col[c];
+        const uint32_t with = (C.flags & TQ_METRIC_EMPTY) ? 0u : C.present ? hw & __ldg(C.present + (lo >> 5) + threadIdx.x) : hw;
+        const uint32_t n = (uint32_t)__popc(with);
+        acc[c].count += n;
+        acc[c].missing += (uint32_t)__popc(hw ^ with);
+        if (C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY)) continue;
+        if (s_has_one[c]) {
+          if (n) metric_add(acc[c], s_one[c], C.kind, n, s_nan_inf[c]);
+        } else {
+          for (uint32_t m = with; m; m &= m - 1u) {
+            const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(m) - 1);
+            metric_add(acc[c], __ldg(C.values + doc), C.kind, 1u, s_nan_inf[c]);
+          }
+        }
+      }
+    } else if (W.n_bins) {  // straddling: each doc to its own bucket
+      uint32_t hw = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
+      if (hw) {
+        uint32_t cw[kC];
+#pragma unroll
+        for (uint32_t c = 0; c < kC; ++c) {
+          const MetricsCol& C = s_z.col[c];
+          cw[c] = c >= nc || (C.flags & TQ_METRIC_EMPTY) ? 0u : C.present ? __ldg(C.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+        }
+        for (; hw; hw &= hw - 1u) {
+          const uint32_t bit = (uint32_t)(__ffs(hw) - 1), doc = lo + threadIdx.x * 32u + bit;
+          const double val = hist_value(__ldg(Z.values + doc), Q.kind);
+          if (!(val >= Z.lo && val <= Z.hi)) continue;  // HistogramBounds::contains (NaN never passes)
+          const unsigned long long idx = (unsigned long long)(hist_pos(val, Q.offset, Q.interval) - base);
+          if (idx >= W.n_bins) continue;  // (never: the window covers every counted value of the unit's tiles)
+          if (shared) hm_doc(s_docs + idx, s_parts + idx * kC, s_z, cw, doc, bit);
+          else hm_doc(gdocs + idx, gparts + idx * kC, s_z, cw, doc, bit);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (run != 0xFFFFFFFFu) flush();
+  uint32_t flushed_shared = 0;
+  if (shared) {  // every non-empty (bucket, column) of the window, and its doc counter, into the global accumulators
+    for (uint32_t i = threadIdx.x; i < W.n_bins * kC; i += blockDim.x) {
+      const uint32_t bin = i / kC, c = i % kC;
+      const tq_metric_part& a = s_parts[i];
+      if (c == 0 && s_docs[bin]) {
+        atomicAdd(&gdocs[bin], (unsigned long long)s_docs[bin]);
+        ++flushed_shared;
+      }
+      hm_merge(gparts + i, a.count, a.n_nan, a.n_inf, ~a.min_image, a.max_image, a.sum, a.magnitude,
+               (int)(0x7FFFFFFFu - (unsigned)a.quantum_exp));
+    }
+    flushed_shared = __reduce_add_sync(kFull, flushed_shared);
+  }
+  total = __reduce_add_sync(kFull, total);
+  if (lane == 0) { s_part[warp] = total; s_rdocs[warp] = flushed_shared; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (Q.flags & kHistHits) {
+      unsigned long long hits = 0;
+      for (int w = 0; w < kWarps; ++w) hits += s_part[w];
+      if (hits) atomicAdd(&P.c.counts[S.query], hits);
+    }
+    unsigned long long fs = 0;
+    for (int w = 0; w < kWarps; ++w) fs += s_rdocs[w];
+    const uint32_t seen = U.end - U.begin;
+    if (seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (one) atomicAdd(&P.tiles[1], (unsigned long long)one); }
+    if (fs) atomicAdd(&P.tiles[2], fs);
+    if (flushed_global) atomicAdd(&P.tiles[3], (unsigned long long)flushed_global);
+  }
+}
+
+// One CTA per query of the wave: its non-empty buckets in ascending pos into its row (the prefix sum of k_hist_final; at most
+// res_stride of them, and never more than its n_bins), each with its kMetricsMaxColumns parts, the complement of min_image and
+// quantum_exp undone.
+__global__ void __launch_bounds__(kThreads) k_hist_metrics_final(const HistMetricsParams P) {
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  __shared__ uint32_t s_part[kWarps];
+  const HistQuery Q = P.queries[P.query_base + blockIdx.x];
+  const unsigned long long* const counts = P.counts + Q.counters;
+  const tq_metric_part* const parts = P.parts + Q.counters * kC;
+  const size_t row = P.rows[P.query_base + blockIdx.x];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t base = 0;  // non-empty buckets before this round of counters (the same on every thread)
+  for (uint32_t i0 = 0; i0 < Q.n_bins; i0 += blockDim.x) {
+    const uint32_t i = i0 + threadIdx.x;
+    const unsigned long long c = i < Q.n_bins ? counts[i] : 0ull;
+    const uint32_t mask = __ballot_sync(kFull, c != 0ull);
+    if (lane == 0) s_part[warp] = (uint32_t)__popc(mask);
+    __syncthreads();
+    uint32_t at = base + (uint32_t)__popc(mask & ((1u << lane) - 1u));
+    for (uint32_t w = 0; w < warp; ++w) at += s_part[w];
+    if (c && at < P.res_stride) {
+      P.res_pos[row + at] = Q.base + (long long)i;
+      P.res_count[row + at] = c;
+      for (uint32_t k = 0; k < kC; ++k) {
+        tq_metric_part p = parts[(size_t)i * kC + k];
+        p.min_image = ~p.min_image;
+        p.quantum_exp = (int)(0x7FFFFFFFu - (unsigned)p.quantum_exp);
+        P.res_parts[(row + at) * kC + k] = p;
+      }
+    }
+    for (int w = 0; w < kWarps; ++w) base += s_part[w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) P.res_n[blockIdx.x] = base;
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

@@ -344,6 +344,33 @@ TQ_HD inline int metric_quantum_exp(unsigned long long abs_bits) {
   return (e ? e - 1075 : -1074) + tz;
 }
 
+// ---- metrics per histogram bucket (k_hist_metrics, k_hist_metrics_final) ------------------------------------------------------
+// The histogram's buckets (HistSeg, HistQuery, HistUnit as in k_hist) with one doc counter and kMetricsMaxColumns tq_metric_part
+// accumulators per bucket, fed by the columns of the (query, segment)'s MetricsSeg.  A unit whose window has kHistMetricsSmemBins
+// or fewer buckets accumulates in shared memory (tq_metric_part layout, flushed per non-empty bucket at exit), a wider one in
+// global memory.  A range above kHistMetricsMaxBins is refused (TQ_ERR_UNSUPPORTED); queries run in waves whose accumulators fit
+// the ctx's budget, and a HistQuery's counters are relative to its wave.
+constexpr uint32_t kHistMetricsSmemBins = 128;
+constexpr uint32_t kHistMetricsMaxBins = 1u << 16;
+struct HistMetricsParams {
+  CountParams c;                // structure words, (query, segment) pairs, units and hit counters: the Count plan of the batch
+  const HistSeg* hsegs;         // parallel to c.segs: the histogram column and bounds
+  const MetricsSeg* msegs;      // parallel to c.segs: the metric columns
+  const HistQuery* queries;     // [nq]: counters relative to the wave
+  const HistUnit* hunits;       // parallel to c.units
+  unsigned long long* counts;   // the wave's doc counters, zeroed before it
+  tq_metric_part* parts;        // [wave's counters][kMetricsMaxColumns], initialised empty before the wave
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them in one bucket, [2] buckets flushed from shared, [3] runs flushed to global
+  const unsigned long long* rows;  // [nq]: first entry of the query's row in res_*, relative to its wave; the row holds
+                                   // min(res_stride, n_bins) entries, so a wave's rows never outnumber its counters
+  long long* res_pos;           // the wave's rows: the non-empty buckets in ascending pos
+  unsigned long long* res_count;
+  tq_metric_part* res_parts;    // [wave's row entries][kMetricsMaxColumns]
+  uint32_t* res_n;              // [wave's queries]
+  uint32_t res_stride;
+  uint32_t unit_base, query_base;  // the wave's first unit and first query
+};
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

@@ -248,12 +248,12 @@ def rust_f64_display(v):
     return np.format_float_positional(v, trim="-")
 
 
-def finalize(req: HistogramAggregation, intermediate, kind, bucket_limit=DEFAULT_BUCKET_LIMIT):
-    """intermediate_histogram_buckets_to_final_buckets: {pos: doc_count} (merge_intermediate; pos on the device's grid, i.e. of
-    device_request(req, kind)) -> tantivy's histogram result.  is_date_agg is kind == "date"."""
+def final_buckets(req: HistogramAggregation, intermediate, kind, bucket_limit=DEFAULT_BUCKET_LIMIT):
+    """The buckets of intermediate_histogram_buckets_to_final_buckets, in key order: (key on the device's grid, doc_count, pos) for
+    each bucket of {pos: doc_count} that is kept, and (key, 0, None) for each bucket the gap filling or extended_bounds add."""
     r = device_request(req, kind)
     offset = r.offset or 0.0
-    buckets = sorted(((bucket_key(p, r.interval, offset), c) for p, c in intermediate.items() if c), key=lambda b: _total_order(b[0]))
+    buckets = sorted(((bucket_key(p, r.interval, offset), c, p) for p, c in intermediate.items() if c), key=lambda b: _total_order(b[0]))
     min_doc_count = r.min_doc_count or 0
     if min_doc_count == 0:
         lo, hi = (buckets[0][0], buckets[-1][0]) if buckets else (F64_MAX, -F64_MAX)
@@ -270,7 +270,7 @@ def finalize(req: HistogramAggregation, intermediate, kind, bucket_limit=DEFAULT
             if j == len(fill) or (i < len(buckets) and buckets[i][0] < fill[j]):
                 out.append(buckets[i]); i += 1  # noqa: E702
             elif i == len(buckets) or fill[j] < buckets[i][0]:
-                out.append((fill[j], 0)); j += 1  # noqa: E702
+                out.append((fill[j], 0, None)); j += 1  # noqa: E702
             else:
                 out.append(buckets[i]); i += 1; j += 1  # noqa: E702
         buckets = out
@@ -278,16 +278,26 @@ def finalize(req: HistogramAggregation, intermediate, kind, bucket_limit=DEFAULT
         buckets = [b for b in buckets if b[1] >= min_doc_count]
     if len(buckets) > bucket_limit:
         raise AggregationError(f"Aborting aggregation because bucket limit was exceeded. Limit: {bucket_limit}, Current: {len(buckets)}")
-    entries = []
-    for key, count in buckets:
-        e = {"key": key, "doc_count": count}
-        if kind == "date":
-            e["key_as_string"] = format_date(as_i64(key))
-            e["key"] = key / 1_000_000.0
-        entries.append(e)
-    if req.keyed:
-        return {"buckets": {rust_f64_display(e["key"]): e for e in entries}}
-    return {"buckets": entries}
+    return buckets
+
+
+def bucket_entry(key, count, kind):
+    """One final bucket {"key", "doc_count"[, "key_as_string"]}: a date key in milliseconds with its RFC 3339 string."""
+    e = {"key": key, "doc_count": count}
+    if kind == "date":
+        e["key_as_string"] = format_date(as_i64(key))
+        e["key"] = key / 1_000_000.0
+    return e
+
+
+def keyed_or_list(req: HistogramAggregation, entries):
+    return {"buckets": {rust_f64_display(e["key"]): e for e in entries}} if req.keyed else {"buckets": entries}
+
+
+def finalize(req: HistogramAggregation, intermediate, kind, bucket_limit=DEFAULT_BUCKET_LIMIT):
+    """intermediate_histogram_buckets_to_final_buckets: {pos: doc_count} (merge_intermediate; pos on the device's grid, i.e. of
+    device_request(req, kind)) -> tantivy's histogram result.  is_date_agg is kind == "date"."""
+    return keyed_or_list(req, [bucket_entry(key, count, kind) for key, count, _ in final_buckets(req, intermediate, kind, bucket_limit)])
 
 
 def _total_order(x):

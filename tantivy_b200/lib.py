@@ -7,7 +7,7 @@ import os
 import numpy as np
 
 from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
-                   MetricsSpec, MetricsStats, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
+                   MetricsSpec, MetricsStats, HistMetricsStats, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
                    f32p, ptr, u8p, u32p, u64p)
 
@@ -34,6 +34,7 @@ def _load():
     lib.tq_get_histogram_stats.argtypes = [vp, C.POINTER(HistogramStats)]
     lib.tq_get_terms_stats.argtypes = [vp, C.POINTER(TermsStats)]
     lib.tq_get_metrics_stats.argtypes = [vp, C.POINTER(MetricsStats)]
+    lib.tq_get_hist_metrics_stats.argtypes = [vp, C.POINTER(HistMetricsStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -51,6 +52,8 @@ def _load():
     lib.tq_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), sz, C.c_uint32, C.POINTER(C.c_int64), u64p, u32p, u64p]
     lib.tq_terms_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), sz, C.c_uint32, u32p, u64p, u64p, u32p, u64p, u64p, u64p]
     lib.tq_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(MetricsSpec), sz, C.POINTER(MetricPart), u64p]
+    lib.tq_histogram_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), C.POINTER(MetricsSpec), sz, C.c_uint32,
+                                               C.POINTER(C.c_int64), u64p, C.POINTER(MetricPart), u32p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -121,6 +124,27 @@ _HIGHEST_BIT = np.uint64(1 << 63)
 FAST_VALUE_KINDS = ("u64", "i64", "f64", "bool", "date")
 _FAST_KIND = {"u64": TQ_FAST_U64, "i64": TQ_FAST_I64, "f64": TQ_FAST_F64, "bool": TQ_FAST_BOOL, "date": TQ_FAST_DATE}
 
+
+def _histogram_specs(specs, nq):
+    """HISTOGRAM_SPEC_DTYPE rows of (column_id, kind, interval, offset[, hard_min, hard_max]) tuples."""
+    spec = np.zeros(max(nq, 1), dtype=HISTOGRAM_SPEC_DTYPE)
+    for i, sp in enumerate(specs):
+        col, kind, interval, offset = sp[:4]
+        hard_min, hard_max = sp[4:6] if len(sp) > 4 else (-np.finfo(np.float64).max, np.finfo(np.float64).max)
+        spec[i] = (col, _FAST_KIND.get(kind, kind), interval, offset, hard_min, hard_max)
+    return spec
+
+
+def _metrics_specs(specs, nq):
+    """METRICS_SPEC_DTYPE rows of lists of (column_id, kind[, flags, missing_image]) columns."""
+    spec = np.zeros(max(nq, 1), dtype=METRICS_SPEC_DTYPE)
+    for i, cols in enumerate(specs):
+        cols = list(cols)
+        spec[i]["n_columns"] = len(cols)
+        for j, col in enumerate(cols[:TQ_METRICS_MAX_COLUMNS]):
+            flags, image = (tuple(col[2:4]) + (0, 0))[:2]
+            spec[i]["columns"][j] = (col[0], col[1], flags, 0, image)
+    return spec
 
 def fast_value_to_u64(values, kind):
     """The u64 image of fast-field values (MonotonicallyMappableToU64, common/src/lib.rs), what tq_sort_column_register takes:
@@ -312,6 +336,7 @@ class Context:
         _check(LIB.tq_ctx_create(device, C.byref(h)))
         self.h = h
         self.device = device
+        self._hist_metrics_stride = 0  # the widest row hist_metrics_batch has returned (its next first try)
 
     def segment_register(self, segment_ord, field, max_doc, record_option, idx_body, fieldnorm=None, alive=None):
         idx_body = np.ascontiguousarray(idx_body, dtype=np.uint8)
@@ -388,11 +413,7 @@ class Context:
         specs = list(specs)
         if len(specs) != qb.nq:
             raise ValueError(f"one histogram spec per query: {len(specs)} for {qb.nq} queries")
-        spec = np.zeros(max(qb.nq, 1), dtype=HISTOGRAM_SPEC_DTYPE)
-        for i, sp in enumerate(specs):
-            col, kind, interval, offset = sp[:4]
-            hard_min, hard_max = sp[4:6] if len(sp) > 4 else (-np.finfo(np.float64).max, np.finfo(np.float64).max)
-            spec[i] = (col, _FAST_KIND.get(kind, kind), interval, offset, hard_min, hard_max)
+        spec = _histogram_specs(specs, qb.nq)
         n = max(qb.nq, 1)
         while True:
             pos = np.empty((n, stride), dtype=np.int64)  # (only the first n[q] entries of row q are written)
@@ -452,18 +473,46 @@ class Context:
         specs = list(specs)
         if len(specs) != qb.nq:
             raise ValueError(f"one metrics spec per query: {len(specs)} for {qb.nq} queries")
-        spec = np.zeros(max(qb.nq, 1), dtype=METRICS_SPEC_DTYPE)
-        for i, cols in enumerate(specs):
-            cols = list(cols)
-            spec[i]["n_columns"] = len(cols)
-            for j, col in enumerate(cols[:TQ_METRICS_MAX_COLUMNS]):
-                flags, image = (tuple(col[2:4]) + (0, 0))[:2]
-                spec[i]["columns"][j] = (col[0], col[1], flags, 0, image)
+        spec = _metrics_specs(specs, qb.nq)
         parts = np.zeros((max(qb.nq, 1), TQ_METRICS_MAX_COLUMNS), dtype=METRIC_PART_DTYPE)
         hits = np.zeros(max(qb.nq, 1), dtype=np.uint64) if count_hits else None
         _check(LIB.tq_metrics_batch(self.h, qb.ptr, spec.ctypes.data_as(C.POINTER(MetricsSpec)), qb.nq, parts.ctypes.data_as(C.POINTER(MetricPart)),
                                     ptr(hits, u64p)), self.h)
         return (parts[:qb.nq], hits[:qb.nq]) if count_hits else parts[:qb.nq]
+
+    def hist_metrics_batch(self, qb: QueryBatch, hspecs, mspecs, count_hits=False, stride=None):
+        """A histogram with metric sub-aggregations per query (tq_histogram_metrics_batch) over sort columns; hspecs = one histogram
+        spec per query as histogram_batch takes them, mspecs = one list of 1..4 metric columns per query as metrics_batch takes them
+        (tantivy_b200.hist_metrics turns requests into both).  Returns (pos, doc_count, parts, n): row q holds the n[q] non-empty
+        buckets of query q in ascending pos over all its segments, parts[q, j] the [TQ_METRICS_MAX_COLUMNS] METRIC_PART_DTYPE parts
+        of bucket j (columns past the query's spec empty) -- and with count_hits=True the Count of every query as well.  Raises
+        TqError with code -4 (TQ_ERR_UNSUPPORTED) when a query's bucket range is too wide for the device.  `stride` is the row width
+        tried first (default: the widest row this context has returned, at least 256): a longer row runs the batch again at its
+        width, so a context serving the same dashboard shapes runs each batch once."""
+        hspecs, mspecs = list(hspecs), list(mspecs)
+        if stride is None:
+            stride = max(256, self._hist_metrics_stride)
+        if len(hspecs) != qb.nq or len(mspecs) != qb.nq:
+            raise ValueError(f"one histogram and one metrics spec per query: {len(hspecs)} and {len(mspecs)} for {qb.nq} queries")
+        hspec, mspec = _histogram_specs(hspecs, qb.nq), _metrics_specs(mspecs, qb.nq)
+        n = max(qb.nq, 1)
+        while True:
+            pos = np.empty((n, stride), dtype=np.int64)  # (only the first n[q] entries of row q are written)
+            counts = np.empty((n, stride), dtype=np.uint64)
+            parts = np.empty((n, stride, TQ_METRICS_MAX_COLUMNS), dtype=METRIC_PART_DTYPE)
+            nb = np.zeros(n, dtype=np.uint32)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_histogram_metrics_batch(self.h, qb.ptr, hspec.ctypes.data_as(C.POINTER(HistogramSpec)),
+                                                mspec.ctypes.data_as(C.POINTER(MetricsSpec)), qb.nq, stride,
+                                                pos.ctypes.data_as(C.POINTER(C.c_int64)), ptr(counts, u64p),
+                                                parts.ctypes.data_as(C.POINTER(MetricPart)), ptr(nb, u32p), ptr(hits, u64p))
+            if rc == -1 and int(nb.max()) > stride:  # TQ_ERR_INVALID_ARGUMENT with the row lengths: a wider row
+                stride = int(nb.max())
+                continue
+            _check(rc, self.h)
+            self._hist_metrics_stride = max(self._hist_metrics_stride, int(nb[:qb.nq].max(initial=0)))
+            out = (pos[:qb.nq], counts[:qb.nq], parts[:qb.nq], nb[:qb.nq])
+            return out + (hits[:qb.nq],) if count_hits else out
 
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
@@ -508,6 +557,9 @@ class Context:
         ms = MetricsStats()
         _check(LIB.tq_get_metrics_stats(self.h, C.byref(ms)), self.h)
         out.update({name: getattr(ms, name) for name, _ in MetricsStats._fields_})
+        hm = HistMetricsStats()
+        _check(LIB.tq_get_hist_metrics_stats(self.h, C.byref(hm)), self.h)
+        out.update({name: getattr(hm, name) for name, _ in HistMetricsStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
