@@ -266,6 +266,18 @@ typedef struct {
   uint64_t hist_metrics_flush_global;
 } tq_hist_metrics_stats;
 int tq_get_hist_metrics_stats(tq_ctx*, tq_hist_metrics_stats* out);
+/* Cumulative since ctx creation: tq_terms_metrics_batch.  Device time of its kernels over all waves (k_terms, k_terms_order,
+ * k_terms_select, k_terms_select_metric, k_terms_mark, k_terms_metrics), their CTAs, the 8192-doc tiles k_terms_metrics came to and
+ * of those the ones whose docs with a value all hold one kept key (their metrics reduced per warp without a slot lookup), and the
+ * waves.  A struct of its own, so that the other stats keep their layouts. */
+typedef struct {
+  float terms_metrics_ms;
+  uint64_t units_terms_metrics;
+  uint64_t terms_metrics_tiles_seen;
+  uint64_t terms_metrics_tiles_one_key;
+  uint64_t terms_metrics_waves;
+} tq_terms_metrics_stats;
+int tq_get_terms_metrics_stats(tq_ctx*, tq_terms_metrics_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -352,6 +364,8 @@ typedef struct {
  * ords().first(doc)), so key order is the image order, which is the reference's ordinal and value order. */
 #define TQ_TERMS_BY_COUNT 0u      /* order target `_count` */
 #define TQ_TERMS_BY_KEY 1u        /* order target `_key` */
+#define TQ_TERMS_BY_METRIC 2u     /* order target: a metric sub-aggregation (tq_terms_metrics_batch only; tq_terms_batch returns
+                                     TQ_ERR_INVALID_ARGUMENT for it, as for any target outside its defines) */
 #define TQ_TERMS_MISSING_NONE 0u  /* docs without a value are not counted */
 #define TQ_TERMS_MISSING_IMAGE 1u /* ... count under missing_image (a numeric `missing`, as the column's image of it) */
 #define TQ_TERMS_MISSING_AFTER_MAX 2u /* ... count under the segment's largest image + 1 (0 + 1 without a value): a str `missing` */
@@ -514,6 +528,47 @@ int tq_metrics_batch(tq_ctx*, const tq_query* queries, const tq_metrics_spec* sp
 int tq_histogram_metrics_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_metrics_spec* mspecs, size_t nq,
                                uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
                                uint64_t* out_hits);
+
+/* A terms aggregation with metric sub-aggregations (one `terms` whose `aggs` are avg, sum, min, max, stats and value_count:
+ * collect_terms_with_docs pushing every doc the terms count to its term's sub-aggregation, term_agg/mod.rs), synchronous like
+ * tq_count_batch, over the docs tq_count_batch counts.  tspecs[q] is query q's terms exactly as in tq_terms_batch, except that its
+ * target may also be TQ_TERMS_BY_METRIC; mspecs[q] its metric columns exactly as in tq_metrics_batch.  The docs a term's metrics
+ * collect are the docs the terms count under its key, the missing key's included.
+ *   Order.  TQ_TERMS_BY_COUNT / TQ_TERMS_BY_KEY cut each segment exactly as tq_terms_batch does.  TQ_TERMS_BY_METRIC reads
+ *   orders[q]: the per-segment value of metric orders[q].metric of spec column orders[q].column (compute_metric_value(...)
+ *   .unwrap_or(0.0): count as f64; the sum, 0 without values; sum / count, min, max, 0 without values; f64::MAX / f64::MIN for a min
+ *   / max of NaN values only), compared as partial_cmp does (-0.0 equals +0.0).  Equal values at the cut keep the lowest keys, and
+ *   the two scalars follow that order: term_doc_count_before_cutoff is the doc count of the entry at position segment_size and
+ *   sum_other_doc_count the sum of the cut entries' doc counts (the reference's select_nth_unstable_by leaves ties unspecified).
+ *   out_order_part[q] is then the ordering column's tq_metric_part over every doc query q's terms collect, cut entries included,
+ *   over all its segments: the caller's guard on it decides whether the cut was exact (written empty for the other orders).
+ *   Rows.  Row q (out_stride entries apart) holds query q's kept entries over all its segments, ascending by (segment_ord, key), as
+ *   tq_terms_batch writes them, and out_parts[i * TQ_METRICS_MAX_COLUMNS + c] the entry's tq_metric_part of column c (parts past
+ *   n_columns are written empty); out_sum_other / out_error_bound as in tq_terms_batch.  A segment this context evaluates only part
+ *   of is not cut, as in tq_terms_batch.  When some out_n[q] > out_stride, every out_n is written and the call returns
+ *   TQ_ERR_INVALID_ARGUMENT: retry with a larger stride.  out_hits may be NULL; else out_hits[q] = tq_count_batch's answer.
+ *   Limits.  A (query, segment) whose keys span more than 2^20 returns TQ_ERR_UNSUPPORTED naming the query, as does one whose
+ *   kept entries' parts alone exceed the ctx's metrics budget.  Queries run in waves whose counters fit TQ_TERMS_COUNTER_BUDGET and
+ *   whose (kept entry, column) parts fit TQ_TERMS_METRICS_BUDGET (at ctx creation).
+ *   Errors.  Those of tq_terms_batch and tq_metrics_batch, and TQ_ERR_INVALID_ARGUMENT for TQ_TERMS_BY_METRIC with orders NULL, an
+ *   order column >= n_columns or an order metric outside TQ_TERMS_ORDER_*.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The
+ *   run holds its columns as tq_sort_batch does. */
+#define TQ_TERMS_ORDER_COUNT 0u /* value_count, stats.count */
+#define TQ_TERMS_ORDER_SUM 1u   /* sum, stats.sum */
+#define TQ_TERMS_ORDER_AVG 2u   /* avg, stats.avg */
+#define TQ_TERMS_ORDER_MIN 3u   /* min, stats.min */
+#define TQ_TERMS_ORDER_MAX 4u   /* max, stats.max */
+typedef struct {
+  uint32_t column;  /* index into the query's tq_metrics_spec columns */
+  uint32_t metric;  /* TQ_TERMS_ORDER_* */
+} tq_terms_metric_order;
+#ifdef __cplusplus
+static_assert(sizeof(tq_terms_metric_order) == 8, "terms metric order ABI layout");
+#endif
+int tq_terms_metrics_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec* tspecs, const tq_metrics_spec* mspecs,
+                           const tq_terms_metric_order* orders, size_t nq, uint32_t out_stride, uint32_t* out_segment_ord,
+                           uint64_t* out_key, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
+                           uint64_t* out_sum_other, uint64_t* out_error_bound, tq_metric_part* out_order_part, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

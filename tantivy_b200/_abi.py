@@ -20,7 +20,8 @@ TQ_QUERY_COUNT_HITS = 2
 TQ_QUERY_FILTER = 4
 TQ_ORDER_DESC, TQ_ORDER_ASC = 0, 1
 TQ_FAST_U64, TQ_FAST_I64, TQ_FAST_F64, TQ_FAST_BOOL, TQ_FAST_DATE = 0, 1, 2, 3, 4
-TQ_TERMS_BY_COUNT, TQ_TERMS_BY_KEY = 0, 1
+TQ_TERMS_BY_COUNT, TQ_TERMS_BY_KEY, TQ_TERMS_BY_METRIC = 0, 1, 2
+TQ_TERMS_ORDER_COUNT, TQ_TERMS_ORDER_SUM, TQ_TERMS_ORDER_AVG, TQ_TERMS_ORDER_MIN, TQ_TERMS_ORDER_MAX = 0, 1, 2, 3, 4
 TQ_TERMS_MISSING_NONE, TQ_TERMS_MISSING_IMAGE, TQ_TERMS_MISSING_AFTER_MAX = 0, 1, 2
 TQ_METRICS_MAX_COLUMNS = 4
 TQ_METRIC_MISSING, TQ_METRIC_COUNT_ONLY, TQ_METRIC_EMPTY = 1, 2, 4
@@ -219,6 +220,21 @@ METRIC_PART_DTYPE = np.dtype([("count", "<u8"), ("n_nan", "<u8"), ("n_inf", "<u8
 assert METRIC_COLUMN_DTYPE.itemsize == C.sizeof(MetricColumn) == 24
 assert METRICS_SPEC_DTYPE.itemsize == C.sizeof(MetricsSpec) == 104
 assert METRIC_PART_DTYPE.itemsize == C.sizeof(MetricPart) == 64
+
+
+class TermsMetricsStats(C.Structure):
+    """tq_terms_metrics_stats — the cumulative counters of tq_terms_metrics_batch (tq_get_terms_metrics_stats)."""
+    _fields_ = [("terms_metrics_ms", C.c_float), ("units_terms_metrics", C.c_uint64), ("terms_metrics_tiles_seen", C.c_uint64),
+                ("terms_metrics_tiles_one_key", C.c_uint64), ("terms_metrics_waves", C.c_uint64)]
+
+
+class TermsMetricOrder(C.Structure):
+    """tq_terms_metric_order — the spec column and TQ_TERMS_ORDER_* metric a TQ_TERMS_BY_METRIC query is ordered by."""
+    _fields_ = [("column", C.c_uint32), ("metric", C.c_uint32)]
+
+
+TERMS_METRIC_ORDER_DTYPE = np.dtype([("column", "<u4"), ("metric", "<u4")])
+assert TERMS_METRIC_ORDER_DTYPE.itemsize == C.sizeof(TermsMetricOrder) == 8
 
 
 def ptr(arr, typ):

@@ -283,6 +283,7 @@ int tq_ctx_create(int device, tq_ctx** out) {
   // terms counters per wave of tq_terms_batch (256 MB); test hook: a small budget runs a batch in many waves
   c->terms_counter_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_COUNTER_BUDGET", 1u << 26));
   c->hist_metrics_budget = std::max<uint32_t>(1u, env_u32("TQ_HIST_METRICS_BUDGET", 1u << 22));
+  c->terms_metrics_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_METRICS_BUDGET", 1u << 22));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -424,6 +425,17 @@ int tq_get_hist_metrics_stats(tq_ctx* c, tq_hist_metrics_stats* out) {
   out->hist_metrics_tiles_one_bucket = c->hist_metrics_tiles_one_bucket;
   out->hist_metrics_flush_shared = c->hist_metrics_flush_shared;
   out->hist_metrics_flush_global = c->hist_metrics_flush_global;
+  return TQ_OK;
+}
+
+int tq_get_terms_metrics_stats(tq_ctx* c, tq_terms_metrics_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->terms_metrics_ms = (float)c->terms_metrics_ms;
+  out->units_terms_metrics = c->terms_metrics_units;
+  out->terms_metrics_tiles_seen = c->terms_metrics_tiles_seen;
+  out->terms_metrics_tiles_one_key = c->terms_metrics_tiles_one_key;
+  out->terms_metrics_waves = c->terms_metrics_waves;
   return TQ_OK;
 }
 
@@ -1990,6 +2002,64 @@ int tq_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_sp
 }
 
 // ---- terms of a fast field ------------------------------------------------------------------------------------
+// The terms of query qi (tq_terms_batch, tq_terms_metrics_batch): one TermsSeg per (query, segment) plan_count added from s0, its
+// counters and region relative to the query (counters / region: the query's totals), and one window per unit added from u0.
+static int plan_terms_query(tq_ctx* c, const tq_terms_spec& sp, size_t qi, uint32_t flags, const CountPlan& cp, size_t s0, size_t u0,
+                            std::vector<TermsSeg>& tsegs, std::vector<HistUnit>& windows, std::vector<const SortColumn*>& cols,
+                            std::vector<std::pair<unsigned long long, unsigned long long>>& uwin, uint64_t& counters, uint64_t& region) {
+  cols.clear();
+  for (size_t si = s0; si < cp.segs.size(); ++si) {
+    auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
+    if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a terms query names a segment without the column (tq_sort_column_register)");
+    const SortColumn& col = it->second;
+    if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+    unsigned long long missing = sp.missing_image;
+    if (sp.missing_mode == TQ_TERMS_MISSING_AFTER_MAX) {  // get_missing_val_as_u64_lenient: the column's max_value + 1 (0 without values)
+      const unsigned long long top = col.min_image <= col.max_image ? col.max_image : 0ull;
+      if (top == ~0ull) return fail(TQ_ERR_INVALID_ARGUMENT, "query " + std::to_string(qi) + ": a str column whose largest image is 2^64 - 1 has no missing key");
+      missing = top + 1;
+    }
+    // a segment this context evaluates only part of (tq_segment_set_doc_range) is not cut here: the reference cuts a segment
+    // once, so the caller cuts after summing its ranges; segment_size 0 marks it (every entry is kept, both scalars stay 0)
+    bool part = false;
+    for (auto s = c->segments.lower_bound({cp.segment_ords[si], 0u}); s != c->segments.end() && s->first.first == cp.segment_ords[si]; ++s)
+      part = part || s->second.doc_lo != 0 || s->second.doc_hi != s->second.max_doc;
+    tsegs.push_back(TermsSeg{col.d_values, col.d_present, col.d_tiles, 0ull, missing, 0ull, 0ull, 0u, part ? 0u : sp.segment_size, flags, 0u});
+    cols.push_back(&col);
+  }
+  // per unit the images of its tiles; per (query, segment) their union
+  uwin.clear();
+  for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+    const Unit& u = cp.units[ui];
+    unsigned long long lo, hi;
+    if (!unit_images(*cols[u.qseg - s0], u, lo, hi)) { uwin.emplace_back(1ull, 0ull); continue; }
+    uwin.emplace_back(lo, hi);
+    TermsSeg& z = tsegs[u.qseg];
+    if (!z.n_keys) { z.base = lo; z.n_keys = 1; z.region = hi; }  // (region holds the top until the span is known)
+    else { z.base = std::min(z.base, lo); z.region = std::max<unsigned long long>(z.region, hi); }
+  }
+  for (size_t si = s0; si < cp.segs.size(); ++si) {
+    TermsSeg& z = tsegs[si];
+    if (z.n_keys) {
+      const unsigned long long span_m1 = z.region - z.base;  // (images up to 2^64 - 1: the span is never formed as top + 1)
+      if (span_m1 >= kTermsMaxKeys)
+        return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its terms span more than 2^20 keys in a segment (take the CPU path)");
+      z.n_keys = (uint32_t)span_m1 + 1u;
+    }
+    if (!z.segment_size) z.segment_size = z.n_keys + 1u;  // more than its entries: no cut
+    z.counters = counters;
+    z.region = region;
+    counters += z.n_keys;
+    region += std::min<uint64_t>(z.segment_size, (uint64_t)z.n_keys + ((z.flags & kTermsMissing) ? 1u : 0u));
+  }
+  for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+    const auto& w = uwin[ui - u0];
+    windows.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - tsegs[cp.units[ui].qseg].base), (uint32_t)(w.second - w.first + 1)}
+                                          : HistUnit{0u, 0u});
+  }
+  return TQ_OK;
+}
+
 int tq_terms_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* specs, size_t nq, uint32_t out_stride,
                    uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n, uint64_t* out_sum_other,
                    uint64_t* out_error_bound, uint64_t* out_hits) {
@@ -2031,58 +2101,10 @@ int tq_terms_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* spec
       q_unit[qi] = u0;
       int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
       if (rc != TQ_OK) return rc;
-      cols.clear();
       uint32_t flags = (out_hits ? kTermsHits : 0u) | (sp.missing_mode != TQ_TERMS_MISSING_NONE ? kTermsMissing : 0u) |
                        (sp.target == TQ_TERMS_BY_KEY ? kTermsByKey : 0u) | (sp.order == TQ_ORDER_ASC ? kTermsAsc : 0u);
-      for (size_t si = s0; si < cp.segs.size(); ++si) {
-        auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
-        if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a terms query names a segment without the column (tq_sort_column_register)");
-        const SortColumn& col = it->second;
-        if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
-        unsigned long long missing = sp.missing_image;
-        if (sp.missing_mode == TQ_TERMS_MISSING_AFTER_MAX) {  // get_missing_val_as_u64_lenient: the column's max_value + 1 (0 without values)
-          const unsigned long long top = col.min_image <= col.max_image ? col.max_image : 0ull;
-          if (top == ~0ull) return fail(TQ_ERR_INVALID_ARGUMENT, "query " + std::to_string(qi) + ": a str column whose largest image is 2^64 - 1 has no missing key");
-          missing = top + 1;
-        }
-        // a segment this context evaluates only part of (tq_segment_set_doc_range) is not cut here: the reference cuts a segment
-        // once, so the caller cuts after summing its ranges; segment_size 0 marks it (every entry is kept, both scalars stay 0)
-        bool part = false;
-        for (auto s = c->segments.lower_bound({cp.segment_ords[si], 0u}); s != c->segments.end() && s->first.first == cp.segment_ords[si]; ++s)
-          part = part || s->second.doc_lo != 0 || s->second.doc_hi != s->second.max_doc;
-        tsegs.push_back(TermsSeg{col.d_values, col.d_present, col.d_tiles, 0ull, missing, 0ull, 0ull, 0u, part ? 0u : sp.segment_size, flags, 0u});
-        cols.push_back(&col);
-      }
-      // per unit the images of its tiles; per (query, segment) their union
-      uwin.clear();
-      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
-        const Unit& u = cp.units[ui];
-        unsigned long long lo, hi;
-        if (!unit_images(*cols[u.qseg - s0], u, lo, hi)) { uwin.emplace_back(1ull, 0ull); continue; }
-        uwin.emplace_back(lo, hi);
-        TermsSeg& z = tsegs[u.qseg];
-        if (!z.n_keys) { z.base = lo; z.n_keys = 1; z.region = hi; }  // (region holds the top until the span is known)
-        else { z.base = std::min(z.base, lo); z.region = std::max<unsigned long long>(z.region, hi); }
-      }
-      for (size_t si = s0; si < cp.segs.size(); ++si) {
-        TermsSeg& z = tsegs[si];
-        if (z.n_keys) {
-          const unsigned long long span_m1 = z.region - z.base;  // (images up to 2^64 - 1: the span is never formed as top + 1)
-          if (span_m1 >= kTermsMaxKeys)
-            return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its terms span more than 2^20 keys in a segment (take the CPU path)");
-          z.n_keys = (uint32_t)span_m1 + 1u;
-        }
-        if (!z.segment_size) z.segment_size = z.n_keys + 1u;  // more than its entries: no cut
-        z.counters = q_counters[qi];
-        z.region = q_region[qi];
-        q_counters[qi] += z.n_keys;
-        q_region[qi] += std::min<uint64_t>(z.segment_size, (uint64_t)z.n_keys + ((z.flags & kTermsMissing) ? 1u : 0u));
-      }
-      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
-        const auto& w = uwin[ui - u0];
-        windows.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - tsegs[cp.units[ui].qseg].base), (uint32_t)(w.second - w.first + 1)}
-                                              : HistUnit{0u, 0u});
-      }
+      rc = plan_terms_query(c, sp, qi, flags, cp, s0, u0, tsegs, windows, cols, uwin, q_counters[qi], q_region[qi]);
+      if (rc != TQ_OK) return rc;
     }
     q_seg[nq] = cp.segs.size();
     q_unit[nq] = cp.units.size();
@@ -2537,6 +2559,272 @@ int tq_histogram_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_hist
     c->hist_metrics_flush_global += tiles[3];
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a histogram has more non-empty buckets than out_stride: out_n holds how many");
+  return TQ_OK;
+}
+
+// ---- metrics per term ----------------------------------------------------------------------------------------
+// A tq_metric_part as the accumulators hold it (min_image and quantum_exp complemented) back to the ABI's form.
+static tq_metric_part uncomplement(tq_metric_part p) {
+  p.min_image = ~p.min_image;
+  p.quantum_exp = (int)(0x7FFFFFFFu - (unsigned)p.quantum_exp);
+  return p;
+}
+
+int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* tspecs, const tq_metrics_spec* mspecs,
+                           const tq_terms_metric_order* orders, size_t nq, uint32_t out_stride, uint32_t* out_segment_ord,
+                           uint64_t* out_key, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
+                           uint64_t* out_sum_other, uint64_t* out_error_bound, tq_metric_part* out_order_part, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !tspecs || !mspecs || !out_n || !out_sum_other || !out_error_bound || !out_order_part ||
+                    (out_stride && (!out_segment_ord || !out_key || !out_doc_count || !out_parts)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const tq_terms_spec& sp = tspecs[qi];
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "terms of phrase queries are not on the device path");
+    if (sp.target > TQ_TERMS_BY_METRIC || sp.order > TQ_ORDER_ASC || sp.missing_mode > TQ_TERMS_MISSING_AFTER_MAX || !sp.segment_size)
+      return fail(TQ_ERR_INVALID_ARGUMENT, "terms spec: target, order, missing mode or segment_size");
+    int rc = check_metrics_spec(mspecs[qi]);
+    if (rc != TQ_OK) return rc;
+    if (sp.target == TQ_TERMS_BY_METRIC &&
+        (!orders || orders[qi].column >= mspecs[qi].n_columns || orders[qi].metric > TQ_TERMS_ORDER_MAX))
+      return fail(TQ_ERR_INVALID_ARGUMENT, "query " + std::to_string(qi) + ": a metric order needs orders[q] with a column of its spec and a TQ_TERMS_ORDER_* metric");
+  }
+  const tq_metric_part empty{0ull, 0ull, 0ull, ~0ull, 0ull, 0.0, 0.0, INT32_MAX, 0u};
+  for (size_t qi = 0; qi < nq; ++qi) {
+    out_n[qi] = 0;
+    out_sum_other[qi] = out_error_bound[qi] = 0;
+    out_order_part[qi] = empty;
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<TermsSeg> tsegs;    // parallel to cp.segs
+  std::vector<MetricsSeg> msegs;  // parallel to cp.segs
+  std::vector<HistUnit> windows;  // parallel to cp.units
+  std::vector<TermsOrder> ord(nq, TermsOrder{0u, 0u});
+  std::vector<size_t> q_seg(nq + 1), q_unit(nq + 1);
+  std::vector<uint64_t> q_counters(nq, 0), q_region(nq, 0);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<unsigned long long, unsigned long long>> uwin;
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_terms_spec& sp = tspecs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_seg[qi] = s0;
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      const uint32_t flags = (out_hits ? kTermsHits : 0u) | (sp.missing_mode != TQ_TERMS_MISSING_NONE ? kTermsMissing : 0u) |
+                             (sp.target == TQ_TERMS_BY_KEY ? kTermsByKey : 0u) | (sp.target == TQ_TERMS_BY_METRIC ? kTermsByMetric : 0u) |
+                             (sp.order == TQ_ORDER_ASC ? kTermsAsc : 0u);
+      rc = plan_terms_query(c, sp, qi, flags, cp, s0, u0, tsegs, windows, cols, uwin, q_counters[qi], q_region[qi]);
+      if (rc != TQ_OK) return rc;
+      rc = plan_metrics_segs(c, mspecs[qi], cp, s0, false, msegs);
+      if (rc != TQ_OK) return rc;
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        const TermsSeg& z = tsegs[si];
+        if ((uint64_t)std::min<uint64_t>(z.segment_size, (uint64_t)z.n_keys + ((z.flags & kTermsMissing) ? 1u : 0u)) * kC > c->terms_metrics_budget)
+          return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": the metric parts of its entries in a segment exceed the device budget (take the CPU path)");
+      }
+      if (sp.target == TQ_TERMS_BY_METRIC) ord[qi] = TermsOrder{orders[qi].column, orders[qi].metric};
+    }
+    q_seg[nq] = cp.segs.size();
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      b->held_columns.push_back(tspecs[qi].column_id);
+      hold_metric_columns(b, mspecs[qi]);
+    }
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // waves of consecutive queries whose counters fit the counter budget and whose kept entries' parts fit the metrics budget (a query
+  // above either runs alone); counters and regions relative to the wave
+  struct Wave { size_t q0, q1; uint64_t counters, region; bool by_metric; };
+  std::vector<Wave> waves;
+  uint64_t max_counters = 0, max_region = 0;
+  size_t max_segs = 0;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (waves.empty() || (waves.back().counters && (waves.back().counters + q_counters[qi] > c->terms_counter_budget ||
+                                                    (waves.back().region + q_region[qi]) * kC > c->terms_metrics_budget)))
+      waves.push_back(Wave{qi, qi, 0, 0, false});
+    Wave& w = waves.back();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) { tsegs[si].counters += w.counters; tsegs[si].region += w.region; }
+    w.q1 = qi + 1;
+    w.counters += q_counters[qi];
+    w.region += q_region[qi];
+    w.by_metric = w.by_metric || tspecs[qi].target == TQ_TERMS_BY_METRIC;
+    max_counters = std::max(max_counters, w.counters);
+    max_region = std::max(max_region, w.region);
+    max_segs = std::max(max_segs, q_seg[w.q1] - q_seg[w.q0]);
+  }
+  // descriptors: one H2D copy; scratch: hits | tile counters | order parts, then one wave's per-(query, segment) results | kept
+  // entries | their parts, then the wave's accumulators: missing counters and slots | the missing keys' order accumulators |
+  // counters | order accumulators
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(tsegs), o_h = st.add(windows),
+               o_m = st.add(msegs), o_o = st.add(ord);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  const size_t part_row = (size_t)kC * sizeof(tq_metric_part);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(16), r_mtiles = take(16), r_opart = take(nq * sizeof(tq_metric_part)), head_bytes = off;
+  const size_t r_n = take(max_segs * 4), r_other = take(max_segs * 8), r_err = take(max_segs * 8), r_key = take(max_region * 8),
+               r_count = take(max_region * 4), r_parts = take(max_region * part_row), wave_bytes = off - head_bytes;
+  const size_t r_missing = take(max_segs * 4), r_mslot = take(max_segs * 4), r_omc = take(max_segs * 4), r_omq = take(max_segs * 8),
+               r_counters = take(max_counters * 4), r_ocount = take(max_counters * 4), r_oq = take(max_counters * 8);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  TermsMetricsParams P{};
+  P.t.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                      reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.t.tsegs = st.on_device<const TermsSeg>(o_z);
+  P.t.windows = st.on_device<const HistUnit>(o_h);
+  P.t.counts = reinterpret_cast<uint32_t*>(d + r_counters);
+  P.t.missing = reinterpret_cast<uint32_t*>(d + r_missing);
+  P.t.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.t.res_key = reinterpret_cast<unsigned long long*>(d + r_key);
+  P.t.res_count = reinterpret_cast<uint32_t*>(d + r_count);
+  P.t.res_n = reinterpret_cast<uint32_t*>(d + r_n);
+  P.t.res_other = reinterpret_cast<unsigned long long*>(d + r_other);
+  P.t.res_error = reinterpret_cast<unsigned long long*>(d + r_err);
+  P.msegs = st.on_device<const MetricsSeg>(o_m);
+  P.orders = st.on_device<const TermsOrder>(o_o);
+  P.ocount = reinterpret_cast<uint32_t*>(d + r_ocount);
+  P.oq = reinterpret_cast<unsigned long long*>(d + r_oq);
+  P.ocount_missing = reinterpret_cast<uint32_t*>(d + r_omc);
+  P.oq_missing = reinterpret_cast<unsigned long long*>(d + r_omq);
+  P.order_parts = reinterpret_cast<tq_metric_part*>(d + r_opart);
+  P.mslot = reinterpret_cast<uint32_t*>(d + r_mslot);
+  P.parts = reinterpret_cast<tq_metric_part*>(d + r_parts);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_mtiles);
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters, order parts (zero: the empty complemented part)
+  // per (query, segment): its kept entries (ascending key) with their parts, and its scalars, gathered wave by wave
+  struct Entry { unsigned long long key; uint32_t count; tq_metric_part parts[kC]; };
+  std::vector<std::vector<Entry>> kept(cp.segs.size());
+  std::vector<uint64_t> seg_other(cp.segs.size()), seg_err(cp.segs.size());
+  float ms_total = 0;
+  uint64_t ctas = 0;
+  const uint8_t* h = b->res_pin.p;
+  for (const Wave& w : waves) {
+    const size_t sa = q_seg[w.q0], sb = q_seg[w.q1], ua = q_unit[w.q0], ub = q_unit[w.q1];
+    if (sa == sb) continue;
+    P.t.unit_base = (uint32_t)ua;
+    P.t.seg_base = (uint32_t)sa;
+    TQ_CUDA(cudaMemsetAsync(d + r_missing, 0, r_counters + w.counters * 4 - r_missing, b->stream));  // missing .. counters
+    TQ_CUDA(cudaMemsetAsync(d + r_parts, 0, w.region * part_row, b->stream));
+    if (w.by_metric) TQ_CUDA(cudaMemsetAsync(d + r_ocount, 0, r_oq + w.counters * 8 - r_ocount, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    const unsigned nu = (unsigned)(ub - ua), ns = (unsigned)(sb - sa);
+    if (nu) {
+      (cp.mixed ? k_terms<true> : k_terms<false>)<<<nu, kThreads, 0, b->stream>>>(P.t);
+      TQ_CUDA(cudaGetLastError());
+      if (w.by_metric) {
+        (cp.mixed ? k_terms_order<true> : k_terms_order<false>)<<<nu, kThreads, 0, b->stream>>>(P);
+        TQ_CUDA(cudaGetLastError());
+      }
+    }
+    k_terms_select<<<ns, kThreads, 0, b->stream>>>(P.t);
+    TQ_CUDA(cudaGetLastError());
+    if (w.by_metric) {
+      k_terms_select_metric<<<ns, kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    k_terms_mark<<<ns, kThreads, 0, b->stream>>>(P);
+    TQ_CUDA(cudaGetLastError());
+    if (nu) {
+      (cp.mixed ? k_terms_metrics<true> : k_terms_metrics<false>)<<<nu, kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    ctas += (w.by_metric ? 3u : 2u) * (uint64_t)nu + (w.by_metric ? 3u : 2u) * (uint64_t)ns;
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + head_bytes, r_key - head_bytes + w.region * 8, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_count - head_bytes), d + r_count, w.region * 4, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_parts - head_bytes), d + r_parts, w.region * part_row, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    for (size_t si = sa; si < sb; ++si) {
+      const size_t rel = si - sa;
+      uint32_t n;
+      memcpy(&n, h + (r_n - head_bytes) + rel * 4, 4);
+      memcpy(&seg_other[si], h + (r_other - head_bytes) + rel * 8, 8);
+      memcpy(&seg_err[si], h + (r_err - head_bytes) + rel * 8, 8);
+      kept[si].resize(n);
+      for (uint32_t j = 0; j < n; ++j) {
+        const size_t e = tsegs[si].region + j;
+        Entry& x = kept[si][j];
+        memcpy(&x.key, h + (r_key - head_bytes) + e * 8, 8);
+        memcpy(&x.count, h + (r_count - head_bytes) + e * 4, 4);
+        for (uint32_t k = 0; k < kC; ++k) {
+          tq_metric_part p;
+          memcpy(&p, h + (r_parts - head_bytes) + e * part_row + k * sizeof(tq_metric_part), sizeof(p));
+          x.parts[k] = uncomplement(p);
+        }
+      }
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_mtiles, 16);
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  for (size_t qi = 0; qi < nq; ++qi)
+    if (tspecs[qi].target == TQ_TERMS_BY_METRIC) {
+      tq_metric_part p;
+      memcpy(&p, h + r_opart + qi * sizeof(tq_metric_part), sizeof(p));
+      out_order_part[qi] = uncomplement(p);
+    }
+  // rows: each query's segments by segment_ord, each in ascending key
+  bool fits = true;
+  std::vector<size_t> by_ord;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    by_ord.clear();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) by_ord.push_back(si);
+    std::sort(by_ord.begin(), by_ord.end(), [&](size_t x, size_t y) { return cp.segment_ords[x] < cp.segment_ords[y]; });
+    uint32_t n = 0;
+    for (size_t si : by_ord) {
+      out_sum_other[qi] += seg_other[si];
+      out_error_bound[qi] += seg_err[si];
+      for (const Entry& e : kept[si]) {
+        if (n < out_stride) {
+          const size_t at = qi * (size_t)out_stride + n;
+          out_segment_ord[at] = cp.segment_ords[si];
+          out_key[at] = e.key;
+          out_doc_count[at] = e.count;
+          for (uint32_t k = 0; k < kC; ++k) out_parts[at * kC + k] = k < mspecs[qi].n_columns ? e.parts[k] : empty;
+        }
+        ++n;
+      }
+    }
+    out_n[qi] = n;
+    fits = fits && n <= out_stride;
+  }
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->terms_metrics_ms += ms_total;
+    c->terms_metrics_units += ctas;
+    c->terms_metrics_tiles_seen += tiles[0];
+    c->terms_metrics_tiles_one_key += tiles[1];
+    c->terms_metrics_waves += waves.size();
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride: out_n holds how many");
   return TQ_OK;
 }
 

@@ -251,6 +251,9 @@ struct tq_ctx {
   double hist_metrics_ms = 0;
   uint64_t hist_metrics_units = 0, hist_metrics_tiles_seen = 0, hist_metrics_tiles_one_bucket = 0, hist_metrics_flush_shared = 0,
            hist_metrics_flush_global = 0;
+  // ... and of the terms-with-metrics runs (terms_metrics_ms, units, tiles seen / with one kept key, waves)
+  double terms_metrics_ms = 0;
+  uint64_t terms_metrics_units = 0, terms_metrics_tiles_seen = 0, terms_metrics_tiles_one_key = 0, terms_metrics_waves = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;
@@ -259,6 +262,7 @@ struct tq_ctx {
   uint32_t term_blocks_per_unit, and_blocks_per_unit, or_tiles_per_unit, strip_windows_per_unit, count_hits_tiles_per_unit;
   uint32_t terms_counter_budget;  // u32 counters one tq_terms_batch wave may hold
   uint32_t hist_metrics_budget;   // (bucket, column) accumulators one tq_histogram_metrics_batch wave may hold
+  uint32_t terms_metrics_budget;  // (kept entry, column) parts one tq_terms_metrics_batch wave may hold
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 32, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;

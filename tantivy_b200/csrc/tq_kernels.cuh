@@ -2231,6 +2231,470 @@ __global__ void __launch_bounds__(kThreads) k_hist_metrics_final(const HistMetri
   if (threadIdx.x == 0) P.res_n[blockIdx.x] = base;
 }
 
+// ---- metrics per term (terms with metric sub-aggregations: collect_terms_with_docs, term_agg/mod.rs) -------------------------
+// The docs k_terms counts under a key feed the metric columns of the (query, segment)'s MetricsSeg in that key's entry.  k_terms
+// counts and k_terms_select cuts as for tq_terms_batch; a metric order (kTermsByMetric) adds k_terms_order before the cut, which
+// accumulates per key the ordering column's value count and quantity, and k_terms_select_metric, which recuts those (query,
+// segment)s by the metric.  k_terms_mark gives each kept key its slot, and k_terms_metrics makes the second match pass that feeds
+// the slots' parts.
+
+// The image a collected doc gives column C, or false when the column collects nothing for it (no value and no missing).  The
+// image of a count-only column is never read.
+__device__ __forceinline__ bool terms_metric_image(const MetricsCol& C, const uint32_t doc, unsigned long long& image) {
+  const bool has = !(C.flags & TQ_METRIC_EMPTY) && (!C.present || ((__ldg(C.present + (doc >> 5)) >> (doc & 31u)) & 1u));
+  if (!has && !(C.flags & TQ_METRIC_MISSING)) return false;
+  image = has && !(C.flags & TQ_METRIC_COUNT_ONLY) ? __ldg(C.values + doc) : C.missing;
+  return true;
+}
+
+// The ordering quantity of one collected value: its f64 bits for a sum or avg, ~image for a min, the image for a max, 0 for a count,
+// a count-only column or a NaN (an order on a column that saw NaN is refused by the caller's check of the total part).  Quantities
+// combine with an f64 add (sum, avg) or a max (the rest), and 0 is the empty quantity of either.
+__device__ __forceinline__ unsigned long long terms_order_q(const unsigned long long image, const MetricsCol& C, const uint32_t metric) {
+  if (metric == TQ_TERMS_ORDER_COUNT || (C.flags & TQ_METRIC_COUNT_ONLY)) return 0ull;
+  const double v = hist_value(image, C.kind);
+  if (v != v) return 0ull;
+  if (metric == TQ_TERMS_ORDER_MIN) return ~image;
+  if (metric == TQ_TERMS_ORDER_MAX) return image;
+  return (unsigned long long)__double_as_longlong(v);
+}
+__device__ __forceinline__ unsigned long long terms_order_combine(const unsigned long long a, const unsigned long long b, const bool sum) {
+  return sum ? (unsigned long long)__double_as_longlong(__dadd_rn(__longlong_as_double((long long)a), __longlong_as_double((long long)b)))
+             : max(a, b);
+}
+__device__ __forceinline__ void terms_order_atomic(uint32_t* count, unsigned long long* q, const uint32_t n, const unsigned long long v,
+                                                   const bool sum) {
+  if (!n) return;
+  atomicAdd(count, n);
+  if (!v) return;
+  if (sum) atomicAdd(reinterpret_cast<double*>(q), __longlong_as_double((long long)v));
+  else atomicMax(q, v);
+}
+
+// compute_metric_value(...).unwrap_or(0.0) of a key's ordering count and quantity (metric/stats.rs:325-356, with the stats' min /
+// max starting at f64::MAX / f64::MIN), as the rank k_terms_select_metric selects on: the value's monotone image with -0.0 taken as
+// +0.0 (partial_cmp's equality), complemented for an ascending order, so that the larger rank comes first.
+__device__ __forceinline__ unsigned long long terms_order_rank(const uint32_t oc, const unsigned long long oq, const MetricsCol& C,
+                                                               const uint32_t metric, const bool asc) {
+  constexpr double kMax = 1.7976931348623157e308;
+  double v = 0.0;
+  if (metric == TQ_TERMS_ORDER_COUNT) v = (double)oc;
+  else if (oc && !(C.flags & TQ_METRIC_COUNT_ONLY)) {
+    if (metric == TQ_TERMS_ORDER_SUM) v = __longlong_as_double((long long)oq);
+    else if (metric == TQ_TERMS_ORDER_AVG) v = __ddiv_rn(__longlong_as_double((long long)oq), (double)oc);
+    else if (metric == TQ_TERMS_ORDER_MIN) { const double m = hist_value(~oq, C.kind); v = m < kMax ? m : kMax; }
+    else { const double m = hist_value(oq, C.kind); v = m > -kMax ? m : -kMax; }
+  }
+  unsigned long long b = v == 0.0 ? 0ull : (unsigned long long)__double_as_longlong(v);
+  b = (b >> 63) ? ~b : b | (1ull << 63);
+  return asc ? ~b : b;
+}
+
+// One CTA per Count unit of a metric-ordered (query, segment) (the others exit): per counted doc the ordering column's value count
+// and quantity into its key's accumulators (the unit's window: in shared memory when it has kTermsOrderSmemKeys keys or fewer), and
+// the column's part over every collected doc, reduced per CTA and merged into the query's order part.  A tile whose values are
+// all one key, and the docs without a value (the missing key), accumulate in registers and are reduced per warp.
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads) k_terms_order(const TermsMetricsParams P) {
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ uint32_t s_oc[kTermsOrderSmemKeys];
+  __shared__ unsigned long long s_oq[kTermsOrderSmemKeys];
+  __shared__ uint32_t s_one;  // the tile's one key (index into the unit's window), or ~0u
+  __shared__ uint32_t s_nan_inf[2];
+  __shared__ unsigned long long s_lo[kWarps], s_hi[kWarps];
+  __shared__ double s_sum[kWarps], s_mag[kWarps];
+  __shared__ uint32_t s_count[kWarps];
+  __shared__ int s_q[kWarps];
+  const uint32_t unit = P.t.unit_base + blockIdx.x;
+  const Unit U = P.t.c.units[unit];
+  const TermsSeg Z = P.t.tsegs[U.qseg];
+  if (!(Z.flags & kTermsByMetric)) return;
+  const CountSeg S = P.t.c.segs[U.qseg];
+  const TermsOrder O = P.orders[S.query];
+  const MetricsCol C = P.msegs[U.qseg].col[O.column];
+  const HistUnit W = P.t.windows[unit];
+  const bool shared = W.n_bins <= kTermsOrderSmemKeys, sum = O.metric == TQ_TERMS_ORDER_SUM || O.metric == TQ_TERMS_ORDER_AVG;
+  const bool with_missing = (Z.flags & kTermsMissing) != 0;
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x) { s_oc[i] = 0; s_oq[i] = 0ull; }
+  if (threadIdx.x < 2u) s_nan_inf[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t wb = S.words_base, ng = P.t.c.words[wb], need = P.t.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const unsigned long long base = Z.base + W.first;
+  uint32_t* const gcnt = P.ocount + Z.counters + W.first;
+  unsigned long long* const gq = P.oq + Z.counters + W.first;
+  MetricAcc tot{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};  // the column over every collected doc
+  uint32_t m_n = 0;                                        // the missing key's values and quantity
+  unsigned long long m_q = 0ull;
+  // one collected doc into the total part; true with its quantity when the column collects it
+  auto collect = [&](const uint32_t doc, unsigned long long& q) -> bool {
+    unsigned long long image;
+    if (!terms_metric_image(C, doc, image)) return false;
+    ++tot.count;
+    if (!(C.flags & TQ_METRIC_COUNT_ONLY)) metric_add(tot, image, C.kind, 1u, s_nan_inf);
+    q = terms_order_q(image, C, O.metric);
+    return true;
+  };
+  // a warp's register count and quantity into one key's accumulators
+  auto flush_warp = [&](uint32_t n, unsigned long long q, uint32_t* pc, unsigned long long* pq) {
+    n = __reduce_add_sync(kFull, n);
+#pragma unroll
+    for (int d = 16; d; d >>= 1) q = terms_order_combine(q, __shfl_xor_sync(kFull, q, d), sum);
+    if (lane == 0) terms_order_atomic(pc, pq, n, q, sum);
+  };
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      const SortTile T = Z.tiles[tile];
+      uint32_t idx = 0xFFFFFFFFu;
+      if (W.n_bins && (T.flags & kSortTileValues)) TermsKeys::one(T, Z, 0u, W, base, idx);
+      s_one = idx;
+    }
+    match_tile<kMixed>(P.t.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    uint32_t with = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
+    if (with_missing)
+      for (uint32_t m = bits ^ with; m; m &= m - 1u) {
+        unsigned long long q;
+        if (collect(lo + threadIdx.x * 32u + (uint32_t)(__ffs(m) - 1), q)) { ++m_n; m_q = terms_order_combine(m_q, q, sum); }
+      }
+    const uint32_t one = s_one;
+    if (one < W.n_bins) {  // one key: registers, one flush per warp
+      uint32_t n = 0;
+      unsigned long long qs = 0ull;
+      for (; with; with &= with - 1u) {
+        unsigned long long q;
+        if (collect(lo + threadIdx.x * 32u + (uint32_t)(__ffs(with) - 1), q)) { ++n; qs = terms_order_combine(qs, q, sum); }
+      }
+      flush_warp(n, qs, shared ? &s_oc[one] : &gcnt[one], shared ? &s_oq[one] : &gq[one]);
+    } else if (W.n_bins) {
+      for (; with; with &= with - 1u) {
+        const uint32_t doc = lo + threadIdx.x * 32u + (uint32_t)(__ffs(with) - 1);
+        unsigned long long q;
+        if (!collect(doc, q)) continue;
+        const unsigned long long idx = __ldg(Z.values + doc) - base;
+        if (idx < W.n_bins) {  // (always: the window covers every value of the unit's tiles)
+          if (shared) terms_order_atomic(&s_oc[idx], &s_oq[idx], 1u, q, sum);
+          else terms_order_atomic(&gcnt[idx], &gq[idx], 1u, q, sum);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins; i += blockDim.x) terms_order_atomic(&gcnt[i], &gq[i], s_oc[i], s_oq[i], sum);
+  if (with_missing) {
+    const bool inside = Z.missing - Z.base < (unsigned long long)Z.n_keys;
+    const uint32_t rel = U.qseg - P.t.seg_base;
+    flush_warp(m_n, m_q, inside ? P.ocount + Z.counters + (Z.missing - Z.base) : P.ocount_missing + rel,
+               inside ? P.oq + Z.counters + (Z.missing - Z.base) : P.oq_missing + rel);
+  }
+  // the total part: per warp, per CTA, one merge
+  const uint32_t count = __reduce_add_sync(kFull, tot.count);
+  const int q = __reduce_min_sync(kFull, tot.q);
+  unsigned long long vlo = tot.lo, vhi = tot.hi;
+  double s = tot.sum, mag = tot.mag;
+#pragma unroll
+  for (int d = 16; d; d >>= 1) {
+    vlo = min(vlo, __shfl_xor_sync(kFull, vlo, d));
+    vhi = max(vhi, __shfl_xor_sync(kFull, vhi, d));
+    s = __dadd_rn(s, __shfl_xor_sync(kFull, s, d));
+    mag = __dadd_rn(mag, __shfl_xor_sync(kFull, mag, d));
+  }
+  if (lane == 0) { s_count[warp] = count; s_q[warp] = q; s_lo[warp] = vlo; s_hi[warp] = vhi; s_sum[warp] = s; s_mag[warp] = mag; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long n = 0, a = ~0ull, b = 0;
+    double x = 0.0, y = 0.0;
+    int e = INT32_MAX;
+    for (int w = 0; w < kWarps; ++w) {
+      n += s_count[w];
+      e = min(e, s_q[w]);
+      a = min(a, s_lo[w]);
+      b = max(b, s_hi[w]);
+      x = __dadd_rn(x, s_sum[w]);
+      y = __dadd_rn(y, s_mag[w]);
+    }
+    hm_merge(P.order_parts + S.query, n, s_nan_inf[0], s_nan_inf[1], a, b, x, y, e);
+  }
+}
+
+// One CTA per (query, segment) of a wave, after k_terms_select: a metric-ordered one with more than segment_size entries is cut
+// again by its metric (the others exit, k_terms_select's rows standing).  The entries are those of k_terms_select (the missing
+// count already folded into its counter when inside the counters); a radix select (8 passes of 8 bits) over the 64-bit rank of
+// terms_order_rank finds the rank t of the segment_size-th entry, and the entries above it are kept with the lowest keys at t.  The
+// entry at position segment_size in that order gives term_doc_count_before_cutoff; the doc counts of the entries cut add up to
+// sum_other_doc_count.  The kept entries overwrite the (query, segment)'s region in ascending key.
+__global__ void __launch_bounds__(kThreads) k_terms_select_metric(const TermsMetricsParams P) {
+  __shared__ uint32_t s_hist[256];
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ unsigned long long s_wide[kWarps];
+  __shared__ unsigned long long s_prefix;
+  __shared__ uint32_t s_k, s_error;
+  const uint32_t rel = blockIdx.x, si = P.t.seg_base + rel;
+  const TermsSeg Z = P.t.tsegs[si];
+  if (!(Z.flags & kTermsByMetric)) return;
+  const TermsOrder O = P.orders[P.t.c.segs[si].query];
+  const MetricsCol C = P.msegs[si].col[O.column];
+  const uint32_t* const cnt = P.t.counts + Z.counters;
+  const uint32_t n = Z.n_keys, ss = Z.segment_size;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t mc = (Z.flags & kTermsMissing) ? P.t.missing[rel] : 0u;
+  const bool inside = mc && Z.missing - Z.base < (unsigned long long)n;
+  const uint32_t extra = mc && !inside ? 1u : 0u, off = extra && Z.missing < Z.base ? 1u : 0u;
+  const uint32_t L = n + extra;  // entries in key order: [missing,] counters[0..n) [, missing]
+  const bool asc = Z.flags & kTermsAsc;
+  auto count_at = [&](uint32_t i) -> uint32_t { i -= off; return i < n ? cnt[i] : mc; };
+  auto key_at = [&](uint32_t i) -> unsigned long long { i -= off; return i < n ? Z.base + i : Z.missing; };
+  auto rank_at = [&](uint32_t i) -> unsigned long long {
+    i -= off;
+    return i < n ? terms_order_rank(P.ocount[Z.counters + i], P.oq[Z.counters + i], C, O.metric, asc)
+                 : terms_order_rank(P.ocount_missing[rel], P.oq_missing[rel], C, O.metric, asc);
+  };
+  uint32_t nz = 0;
+  unsigned long long sum = 0;
+  for (uint32_t i = threadIdx.x; i < L; i += blockDim.x) {
+    const uint32_t c = count_at(i);
+    nz += c ? 1u : 0u;
+    sum += c;
+  }
+  nz = __reduce_add_sync(kFull, nz);
+  for (int d = 16; d; d >>= 1) sum += __shfl_xor_sync(kFull, sum, d);
+  if (lane == 0) { s_part[warp] = nz; s_wide[warp] = sum; }
+  __syncthreads();
+  uint32_t N = 0;
+  unsigned long long total = 0;
+  for (int w = 0; w < kWarps; ++w) { N += s_part[w]; total += s_wide[w]; }
+  if (N <= ss) return;  // (CTA-uniform) no cut: every entry kept, both scalars 0, as k_terms_select wrote them
+  __syncthreads();
+  unsigned long long prefix = 0, mask = 0;
+  uint32_t k = ss + 1u;  // the (segment_size + 1)-th largest rank: the first entry cut, at t_cut or below it
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    s_hist[threadIdx.x] = 0;
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < L; i += blockDim.x) {
+      if (!count_at(i)) continue;
+      const unsigned long long t = rank_at(i);
+      if ((t & mask) == prefix) atomicAdd(&s_hist[(t >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      uint32_t b = 255, acc = 0;
+      for (; acc + s_hist[b] < k; --b) acc += s_hist[b];
+      s_prefix = prefix | ((unsigned long long)b << shift);
+      s_k = k - acc;
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    k = s_k;
+    mask |= 255ull << shift;
+    __syncthreads();
+  }
+  // t_cut: the rank of the entry at position segment_size, the k-th (1-based, lowest keys first) of the entries at it; the entries
+  // kept are those above t_cut and the k - 1 lowest keys at it
+  const unsigned long long t_cut = prefix;
+  const uint32_t need = k - 1u;
+  uint32_t base_eq = 0, base_keep = 0;
+  unsigned long long kept = 0;
+  for (uint32_t i0 = 0; i0 < L; i0 += blockDim.x) {
+    const uint32_t i = i0 + threadIdx.x;
+    const uint32_t c = i < L ? count_at(i) : 0u;
+    const unsigned long long t = c ? rank_at(i) : 0ull;
+    const bool eq = c && t == t_cut;
+    uint32_t tot;
+    const uint32_t r_eq = base_eq + cta_scan_excl(eq ? 1u : 0u, s_part, tot);
+    base_eq += tot;
+    const bool keep = c && (t > t_cut || (eq && r_eq < need));
+    if (eq && r_eq == need) s_error = c;
+    const uint32_t at = base_keep + cta_scan_excl(keep ? 1u : 0u, s_part, tot);
+    base_keep += tot;
+    if (keep) {
+      P.t.res_key[Z.region + at] = key_at(i);
+      P.t.res_count[Z.region + at] = c;
+      kept += c;
+    }
+  }
+  for (int d = 16; d; d >>= 1) kept += __shfl_xor_sync(kFull, kept, d);
+  if (lane == 0) s_wide[warp] = kept;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long k_sum = 0;
+    for (int w = 0; w < kWarps; ++w) k_sum += s_wide[w];
+    P.t.res_n[rel] = base_keep;
+    P.t.res_other[rel] = total - k_sum;
+    P.t.res_error[rel] = s_error;
+  }
+}
+
+// One CTA per (query, segment) of a wave, after the cut: each kept key's counter becomes kTermsSlot | its index in the region (a
+// missing key outside the counters: mslot).  Counts are below 2^31, so a marked counter is told from a count by its top bit.
+__global__ void __launch_bounds__(kThreads) k_terms_mark(const TermsMetricsParams P) {
+  const uint32_t rel = blockIdx.x;
+  const TermsSeg Z = P.t.tsegs[P.t.seg_base + rel];
+  uint32_t* const cnt = P.t.counts + Z.counters;
+  const uint32_t n = P.t.res_n[rel];
+  for (uint32_t j = threadIdx.x; j < n; j += blockDim.x) {
+    const unsigned long long key = P.t.res_key[Z.region + j];
+    if (key - Z.base < (unsigned long long)Z.n_keys) cnt[key - Z.base] = kTermsSlot | j;
+    else P.mslot[rel] = kTermsSlot | j;
+  }
+}
+
+// The docs of mask m (the thread's 32-doc word at lo) all in one slot: per column as k_metrics adds them (one-value tiles and
+// missing copies included), reduced per warp and merged once per (warp, column) into the slot's parts p.  Called by whole warps.
+__device__ __forceinline__ void tm_uniform(tq_metric_part* p, const uint32_t m, const uint32_t lo, const MetricsSeg& z,
+                                           const unsigned long long* s_one, const uint32_t* s_has_one, uint32_t (*s_ni)[2]) {
+  if (!__any_sync(kFull, m)) return;
+  const uint32_t lane = threadIdx.x & 31u;
+#pragma unroll 1
+  for (uint32_t c = 0; c < z.n_columns; ++c) {
+    const MetricsCol& C = z.col[c];
+    MetricAcc a{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};
+    const uint32_t with = (C.flags & TQ_METRIC_EMPTY) ? 0u : C.present ? m & __ldg(C.present + (lo >> 5) + threadIdx.x) : m;
+    const uint32_t n = (uint32_t)__popc(with), miss = (uint32_t)__popc(m ^ with);
+    a.count = n;
+    if (!(C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY))) {
+      if (s_has_one[c]) {
+        if (n) metric_add(a, s_one[c], C.kind, n, s_ni[c]);
+      } else {
+        for (uint32_t w = with; w; w &= w - 1u)
+          metric_add(a, __ldg(C.values + lo + threadIdx.x * 32u + (uint32_t)(__ffs(w) - 1)), C.kind, 1u, s_ni[c]);
+      }
+    }
+    if ((C.flags & TQ_METRIC_MISSING) && miss) {
+      a.count += miss;
+      if (!(C.flags & TQ_METRIC_COUNT_ONLY)) metric_add(a, C.missing, C.kind, miss, s_ni[c]);
+    }
+    const uint32_t count = __reduce_add_sync(kFull, a.count);
+    const int q = __reduce_min_sync(kFull, a.q);
+    unsigned long long vlo = a.lo, vhi = a.hi;
+    double sum = a.sum, mag = a.mag;
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {
+      vlo = min(vlo, __shfl_xor_sync(kFull, vlo, d));
+      vhi = max(vhi, __shfl_xor_sync(kFull, vhi, d));
+      sum = __dadd_rn(sum, __shfl_xor_sync(kFull, sum, d));
+      mag = __dadd_rn(mag, __shfl_xor_sync(kFull, mag, d));
+    }
+    __syncwarp();
+    if (lane == 0) {
+      const uint32_t n_nan = s_ni[c][0], n_inf = s_ni[c][1];
+      s_ni[c][0] = s_ni[c][1] = 0;
+      hm_merge(p + c, count, n_nan, n_inf, vlo, vhi, sum, mag, q);
+    }
+    __syncwarp();
+  }
+}
+
+// One CTA per Count unit: the docs k_terms counted, each into the parts of its key's slot (docs of keys cut feed nothing).  The
+// docs without a value go to the missing key's slot, a tile whose values are all one kept key to that key's: both with tm_uniform.
+// Any other tile has each thread walk its word's matches: one gather of the key, one lookup of its counter, and per column
+// hm_collect.  The parts of a (query, segment) keeping kTermsMetricsSmemSlots entries or fewer accumulate in shared memory and are
+// merged into the global ones at exit.
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 2) k_terms_metrics(const TermsMetricsParams P) {
+  static_assert(sizeof(MetricsSeg) % 8u == 0 && sizeof(MetricsSeg) / 8u <= (uint32_t)kThreads, "one word of the descriptor per thread");
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  constexpr uint32_t kPerDoc = 0xFFFFFFFFu, kSkip = 0xFFFFFFFEu;  // s_slot: walk each doc; no doc with a value feeds a slot
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ MetricsSeg s_z;
+  __shared__ tq_metric_part s_parts[kTermsMetricsSmemSlots * kC];
+  __shared__ unsigned long long s_one[kC];
+  __shared__ uint32_t s_has_one[kC];
+  __shared__ uint32_t s_slot;
+  __shared__ uint32_t s_nan_inf[kWarps][kC][2];
+  const uint32_t unit = P.t.unit_base + blockIdx.x;
+  const Unit U = P.t.c.units[unit];
+  const CountSeg S = P.t.c.segs[U.qseg];
+  const TermsSeg Z = P.t.tsegs[U.qseg];
+  const uint32_t rel = U.qseg - P.t.seg_base, n_kept = P.t.res_n[rel];
+  const uint32_t* const cnt = P.t.counts + Z.counters;
+  if (threadIdx.x < sizeof(MetricsSeg) / 8u)
+    reinterpret_cast<unsigned long long*>(&s_z)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(P.msegs + U.qseg)[threadIdx.x];
+  if (threadIdx.x < kWarps * kC * 2u) (&s_nan_inf[0][0][0])[threadIdx.x] = 0;
+  const bool shared = n_kept <= kTermsMetricsSmemSlots;
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < n_kept * (uint32_t)(sizeof(tq_metric_part) / 8u) * kC; i += blockDim.x)
+      reinterpret_cast<unsigned long long*>(s_parts)[i] = 0ull;
+  uint32_t ms = 0;  // the missing key's slot (CTA-uniform)
+  if (Z.flags & kTermsMissing) ms = Z.missing - Z.base < (unsigned long long)Z.n_keys ? cnt[Z.missing - Z.base] : P.mslot[rel];
+  __syncthreads();
+  const uint32_t nc = s_z.n_columns;
+  const uint32_t wb = S.words_base, ng = P.t.c.words[wb], need = P.t.c.words[wb + 1u];
+  const uint32_t warp = threadIdx.x >> 5;
+  tq_metric_part* const gparts = P.parts + Z.region * kC;
+  tq_metric_part* const parts = shared ? s_parts : gparts;
+  uint32_t one = 0;
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      const SortTile T = Z.tiles[tile];
+      uint32_t slot = kSkip;
+      if ((T.flags & kSortTileValues) && T.best[0] == ~T.best[1]) {
+        const unsigned long long i = T.best[0] - Z.base;
+        const uint32_t c = i < (unsigned long long)Z.n_keys ? cnt[i] : 0u;
+        if (c & kTermsSlot) slot = c & ~kTermsSlot;
+      } else if (T.flags & kSortTileValues) {
+        slot = kPerDoc;
+      }
+      s_slot = slot;
+      one += slot < kSkip ? 1u : 0u;
+    }
+    if (threadIdx.x < nc) {  // (warp 0)
+      const MetricsCol& C = s_z.col[threadIdx.x];
+      uint32_t has = 0;
+      if (!(C.flags & (TQ_METRIC_COUNT_ONLY | TQ_METRIC_EMPTY))) {
+        const SortTile T = C.tiles[tile];
+        has = (T.flags & kSortTileValues) && T.best[0] == ~T.best[1] ? 1u : 0u;
+        s_one[threadIdx.x] = T.best[0];
+      }
+      s_has_one[threadIdx.x] = has;
+    }
+    match_tile<kMixed>(P.t.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    uint32_t with = Z.present ? bits & __ldg(Z.present + (lo >> 5) + threadIdx.x) : bits;
+    if (ms & kTermsSlot) tm_uniform(parts + (ms & ~kTermsSlot) * kC, bits ^ with, lo, s_z, s_one, s_has_one, s_nan_inf[warp]);
+    const uint32_t slot = s_slot;
+    if (slot < kSkip) {
+      tm_uniform(parts + slot * kC, with, lo, s_z, s_one, s_has_one, s_nan_inf[warp]);
+    } else if (slot == kPerDoc && with) {
+      uint32_t cw[kC];
+#pragma unroll
+      for (uint32_t c = 0; c < kC; ++c) {
+        const MetricsCol& C = s_z.col[c];
+        cw[c] = c >= nc || (C.flags & TQ_METRIC_EMPTY) ? 0u : C.present ? __ldg(C.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+      }
+      for (; with; with &= with - 1u) {
+        const uint32_t bit = (uint32_t)(__ffs(with) - 1), doc = lo + threadIdx.x * 32u + bit;
+        const uint32_t c = __ldg(cnt + (__ldg(Z.values + doc) - Z.base));  // (the counters cover every value of the visited tiles)
+        if (!(c & kTermsSlot)) continue;
+        tq_metric_part* const p = parts + (c & ~kTermsSlot) * kC;
+#pragma unroll
+        for (uint32_t k = 0; k < kC; ++k) {
+          if (k >= nc) break;
+          hm_collect(p + k, s_z.col[k], doc, (cw[k] >> bit) & 1u);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (shared)  // every non-empty (slot, column) into the global parts
+    for (uint32_t i = threadIdx.x; i < n_kept * kC; i += blockDim.x) {
+      const tq_metric_part& a = s_parts[i];
+      hm_merge(gparts + i, a.count, a.n_nan, a.n_inf, ~a.min_image, a.max_image, a.sum, a.magnitude,
+               (int)(0x7FFFFFFFu - (unsigned)a.quantum_exp));
+    }
+  if (threadIdx.x == 0) {
+    const uint32_t seen = U.end - U.begin;
+    if (seen) { atomicAdd(&P.tiles[0], (unsigned long long)seen); if (one) atomicAdd(&P.tiles[1], (unsigned long long)one); }
+  }
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

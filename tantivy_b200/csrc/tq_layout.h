@@ -371,6 +371,36 @@ struct HistMetricsParams {
   uint32_t unit_base, query_base;  // the wave's first unit and first query
 };
 
+// ---- metrics per term (k_terms_order, k_terms_select_metric, k_terms_mark, k_terms_metrics) ---------------------------------
+// The terms of k_terms / k_terms_select (TermsSeg, the unit windows, the counters) with the metric columns of the (query, segment)'s
+// MetricsSeg.  After the cut, k_terms_mark overwrites the counter of each kept key with kTermsSlot | its index in the (query,
+// segment)'s region (a missing key outside the counters gets its slot in `mslot`); k_terms_metrics feeds each counted doc to the
+// kMetricsMaxColumns tq_metric_parts of its key's slot (complemented as in k_hist_metrics), in shared memory when the (query,
+// segment) keeps kTermsMetricsSmemSlots or fewer entries.  A metric order (kTermsByMetric) first accumulates per key of the
+// window the ordering column's value count and its one quantity (the f64 sum, ~min image or max image) in `ocount` / `oq`, and the
+// column's part over every collected doc per query; k_terms_select_metric cuts on them.
+constexpr uint32_t kTermsByMetric = 16;  // TermsSeg::flags: the order is orders[query]
+constexpr uint32_t kTermsSlot = 0x80000000u;
+constexpr uint32_t kTermsMetricsSmemSlots = 128;
+constexpr uint32_t kTermsOrderSmemKeys = 1024;
+struct TermsOrder {  // tq_terms_metric_order of one query
+  uint32_t column, metric;
+};
+struct TermsMetricsParams {
+  TermsParams t;                  // the terms of the wave: counters, missing counters, kept entries and scalars
+  const MetricsSeg* msegs;        // parallel to t.c.segs
+  const TermsOrder* orders;       // [nq]
+  uint32_t* ocount;               // parallel to t.counts: the ordering column's values per key (metric orders), zeroed per wave
+  unsigned long long* oq;         // ... their sum (f64 bits), ~smallest or largest image
+  uint32_t* ocount_missing;       // [wave's (query, segment)s]: the same for a missing key outside the counters
+  unsigned long long* oq_missing;
+  tq_metric_part* order_parts;    // [nq]: the ordering column over every collected doc, complemented, zeroed once
+  uint32_t* mslot;                // [wave's (query, segment)s]: kTermsSlot | slot of a missing key outside the counters, or 0
+  tq_metric_part* parts;          // [wave's region][kMetricsMaxColumns], complemented, zeroed per wave
+  unsigned long long* tiles;      // [0] tiles k_terms_metrics saw, [1] of them with one kept key
+};
+static_assert(sizeof(TermsOrder) == 8, "terms order descriptor layout");
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

@@ -7,7 +7,7 @@ import os
 import numpy as np
 
 from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
-                   MetricsSpec, MetricsStats, HistMetricsStats, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
+                   MetricsSpec, MetricsStats, HistMetricsStats, TermsMetricsStats, TermsMetricOrder, TERMS_METRIC_ORDER_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
                    f32p, ptr, u8p, u32p, u64p)
 
@@ -35,6 +35,7 @@ def _load():
     lib.tq_get_terms_stats.argtypes = [vp, C.POINTER(TermsStats)]
     lib.tq_get_metrics_stats.argtypes = [vp, C.POINTER(MetricsStats)]
     lib.tq_get_hist_metrics_stats.argtypes = [vp, C.POINTER(HistMetricsStats)]
+    lib.tq_get_terms_metrics_stats.argtypes = [vp, C.POINTER(TermsMetricsStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -54,6 +55,8 @@ def _load():
     lib.tq_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(MetricsSpec), sz, C.POINTER(MetricPart), u64p]
     lib.tq_histogram_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), C.POINTER(MetricsSpec), sz, C.c_uint32,
                                                C.POINTER(C.c_int64), u64p, C.POINTER(MetricPart), u32p, u64p]
+    lib.tq_terms_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), C.POINTER(MetricsSpec), C.POINTER(TermsMetricOrder), sz,
+                                           C.c_uint32, u32p, u64p, u64p, C.POINTER(MetricPart), u32p, u64p, u64p, C.POINTER(MetricPart), u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -132,6 +135,16 @@ def _histogram_specs(specs, nq):
         col, kind, interval, offset = sp[:4]
         hard_min, hard_max = sp[4:6] if len(sp) > 4 else (-np.finfo(np.float64).max, np.finfo(np.float64).max)
         spec[i] = (col, _FAST_KIND.get(kind, kind), interval, offset, hard_min, hard_max)
+    return spec
+
+
+def _terms_specs(specs, nq):
+    """TERMS_SPEC_DTYPE rows of (column_id, target, order, segment_size[, missing_mode, missing_image]) tuples."""
+    spec = np.zeros(max(nq, 1), dtype=TERMS_SPEC_DTYPE)
+    for i, sp in enumerate(specs):
+        col, target, order, segment_size = sp[:4]
+        mode, image = sp[4:6] if len(sp) > 4 else (0, 0)
+        spec[i] = (col, target, order, segment_size, mode, 0, image)
     return spec
 
 
@@ -337,6 +350,7 @@ class Context:
         self.h = h
         self.device = device
         self._hist_metrics_stride = 0  # the widest row hist_metrics_batch has returned (its next first try)
+        self._terms_metrics_stride = 0  # the widest row terms_metrics_batch has returned (its next first try)
 
     def segment_register(self, segment_ord, field, max_doc, record_option, idx_body, fieldnorm=None, alive=None):
         idx_body = np.ascontiguousarray(idx_body, dtype=np.uint8)
@@ -441,11 +455,7 @@ class Context:
         specs = list(specs)
         if len(specs) != qb.nq:
             raise ValueError(f"one terms spec per query: {len(specs)} for {qb.nq} queries")
-        spec = np.zeros(max(qb.nq, 1), dtype=TERMS_SPEC_DTYPE)
-        for i, sp in enumerate(specs):
-            col, target, order, segment_size = sp[:4]
-            mode, image = sp[4:6] if len(sp) > 4 else (0, 0)
-            spec[i] = (col, target, order, segment_size, mode, 0, image)
+        spec = _terms_specs(specs, qb.nq)
         n = max(qb.nq, 1)
         while True:
             segs = np.empty((n, stride), dtype=np.uint32)  # (only the first n[q] entries of row q are written)
@@ -514,6 +524,52 @@ class Context:
             out = (pos[:qb.nq], counts[:qb.nq], parts[:qb.nq], nb[:qb.nq])
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def terms_metrics_batch(self, qb: QueryBatch, tspecs, mspecs, orders=None, count_hits=False, stride=None):
+        """A terms aggregation with metric sub-aggregations per query (tq_terms_metrics_batch) over sort columns; tspecs = one terms
+        spec per query as terms_batch takes them (target also TQ_TERMS_BY_METRIC), mspecs = one list of 1..4 metric columns per query
+        as metrics_batch takes them, orders = one (spec column, TQ_TERMS_ORDER_*) or None per query, read for TQ_TERMS_BY_METRIC
+        (tantivy_b200.terms_metrics turns requests into all three).  Returns (segment_ord, key, doc_count, parts, n, sum_other,
+        error_bound, order_part): row q holds the n[q] kept entries of query q ascending by (segment_ord, key image) as terms_batch
+        returns them, parts[q, j] the [TQ_METRICS_MAX_COLUMNS] METRIC_PART_DTYPE parts of entry j, and order_part[q] the ordering
+        column's part over every doc the query's terms collect (empty for the _count / _key orders) -- and with count_hits=True the
+        Count of every query as well.  Raises TqError with code -4 (TQ_ERR_UNSUPPORTED) when a (query, segment) is too wide for the
+        device.  `stride` is the row width tried first (default: the widest row this context has returned, at least 1024): a longer
+        row runs the batch again at its width, so a context serving the same table shapes runs each batch once."""
+        tspecs, mspecs = list(tspecs), list(mspecs)
+        orders = [None] * qb.nq if orders is None else list(orders)
+        if stride is None:
+            stride = max(1024, self._terms_metrics_stride)
+        if len(tspecs) != qb.nq or len(mspecs) != qb.nq or len(orders) != qb.nq:
+            raise ValueError(f"one terms spec, metrics spec and order per query: {len(tspecs)}, {len(mspecs)} and {len(orders)} for {qb.nq} queries")
+        tspec, mspec = _terms_specs(tspecs, qb.nq), _metrics_specs(mspecs, qb.nq)
+        order = np.zeros(max(qb.nq, 1), dtype=TERMS_METRIC_ORDER_DTYPE)
+        for i, o in enumerate(orders):
+            if o is not None:
+                order[i] = tuple(o)
+        order_ptr = order.ctypes.data_as(C.POINTER(TermsMetricOrder)) if any(o is not None for o in orders) else None  # (NULL: no order)
+        n = max(qb.nq, 1)
+        while True:
+            segs = np.empty((n, stride), dtype=np.uint32)  # (only the first n[q] entries of row q are written)
+            keys = np.empty((n, stride), dtype=np.uint64)
+            counts = np.empty((n, stride), dtype=np.uint64)
+            parts = np.empty((n, stride, TQ_METRICS_MAX_COLUMNS), dtype=METRIC_PART_DTYPE)
+            nb = np.zeros(n, dtype=np.uint32)
+            other = np.zeros(n, dtype=np.uint64)
+            error = np.zeros(n, dtype=np.uint64)
+            opart = np.zeros(n, dtype=METRIC_PART_DTYPE)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_terms_metrics_batch(self.h, qb.ptr, tspec.ctypes.data_as(C.POINTER(TermsSpec)), mspec.ctypes.data_as(C.POINTER(MetricsSpec)),
+                                            order_ptr, qb.nq, stride, ptr(segs, u32p), ptr(keys, u64p),
+                                            ptr(counts, u64p), parts.ctypes.data_as(C.POINTER(MetricPart)), ptr(nb, u32p), ptr(other, u64p),
+                                            ptr(error, u64p), opart.ctypes.data_as(C.POINTER(MetricPart)), ptr(hits, u64p))
+            if rc == -1 and int(nb.max()) > stride:  # TQ_ERR_INVALID_ARGUMENT with the row lengths: a wider row
+                stride = int(nb.max())
+                continue
+            _check(rc, self.h)
+            self._terms_metrics_stride = max(self._terms_metrics_stride, int(nb[:qb.nq].max(initial=0)))
+            out = (segs[:qb.nq], keys[:qb.nq], counts[:qb.nq], parts[:qb.nq], nb[:qb.nq], other[:qb.nq], error[:qb.nq], opart[:qb.nq])
+            return out + (hits[:qb.nq],) if count_hits else out
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -560,6 +616,9 @@ class Context:
         hm = HistMetricsStats()
         _check(LIB.tq_get_hist_metrics_stats(self.h, C.byref(hm)), self.h)
         out.update({name: getattr(hm, name) for name, _ in HistMetricsStats._fields_})
+        tm = TermsMetricsStats()
+        _check(LIB.tq_get_terms_metrics_stats(self.h, C.byref(tm)), self.h)
+        out.update({name: getattr(tm, name) for name, _ in TermsMetricsStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):

@@ -234,15 +234,19 @@ def finalize(req: TermsAggregation, merged):
     return res
 
 
-def cut_segment(entries, req: TermsAggregation):
+def cut_segment(entries, req: TermsAggregation, metric=None):
     """One segment's cut to segment_size (into_intermediate_bucket_result + cut_off_buckets, term_agg/mod.rs:1000-1111,
     1328-1353) of {image: doc_count}: (kept [(image, doc_count)] ascending, term_doc_count_before_cutoff, sum_other_doc_count).
-    Equal counts at the cut keep the lowest images, as the device does."""
+    Equal counts at the cut keep the lowest images, as the device does.  An order by a sub-aggregation takes metric = {image: the
+    segment's compute_metric_value(...).unwrap_or(0.0)}, compared as partial_cmp does (-0.0 equals +0.0), equal values again by
+    image ascending."""
     items = sorted((k, c) for k, c in entries.items() if c)
     if len(items) <= req.segment_size:
         return items, 0, 0
     if req.order_target == "_key":
         order = items if req.order == "asc" else items[::-1]
+    elif metric is not None:
+        order = sorted(items, key=lambda kc: (metric[kc[0]] if req.order == "asc" else -metric[kc[0]], kc[0]))
     else:
         order = sorted(items, key=lambda kc: (kc[1] if req.order == "asc" else -kc[1], kc[0]))
     return sorted(order[:req.segment_size]), order[req.segment_size][1], sum(c for _, c in order[req.segment_size:])
