@@ -278,6 +278,17 @@ typedef struct {
   uint64_t terms_metrics_waves;
 } tq_terms_metrics_stats;
 int tq_get_terms_metrics_stats(tq_ctx*, tq_terms_metrics_stats* out);
+/* Cumulative since ctx creation: tq_range_batch, with and without metrics.  Device time of k_range or k_range_metrics over all
+ * waves, their CTAs (one per unit of up to eight 8192-doc tiles), the 8192-doc tiles the units came to and of those the ones in one
+ * bucket (the tile's smallest and largest image in one range: its matches added without reading a value).  A struct of its own,
+ * so that the other stats keep their layouts. */
+typedef struct {
+  float range_ms;
+  uint64_t units_range;
+  uint64_t range_tiles_seen;
+  uint64_t range_tiles_one_bucket;
+} tq_range_stats;
+int tq_get_range_stats(tq_ctx*, tq_range_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -569,6 +580,31 @@ int tq_terms_metrics_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec
                            const tq_terms_metric_order* orders, size_t nq, uint32_t out_stride, uint32_t* out_segment_ord,
                            uint64_t* out_key, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
                            uint64_t* out_sum_other, uint64_t* out_error_bound, tq_metric_part* out_order_part, uint64_t* out_hits);
+
+/* A range aggregation (`range`, bucket/range.rs), with or without metric sub-aggregations, synchronous like tq_count_batch, over
+ * the docs tq_count_batch counts.  rspecs[q] is query q's buckets in image space, as extend_validate_ranges leaves them: starts
+ * strictly ascending from 0, bucket b holding the images in [starts[b], starts[b + 1]) and the last one every image from its start
+ * up (get_bucket_pos: the end is never tested).  A doc without a value is not collected.  Row q (out_stride buckets apart) holds
+ * every bucket of query q, empty ones included, in start order: out_doc_count[q * out_stride + b] over all its segments and, with
+ * mspecs (exactly as in tq_metrics_batch), out_parts[(q * out_stride + b) * TQ_METRICS_MAX_COLUMNS + c] the bucket's tq_metric_part
+ * of column c (parts past n_columns are written empty), with tq_metrics_batch's merge rules and guard, applied per (bucket, column)
+ * by the caller.  mspecs NULL: doc counts only, and out_parts must be NULL.  out_hits may be NULL; else out_hits[q] =
+ * tq_count_batch's answer for query q.  With mspecs, queries whose accumulators exceed the ctx's TQ_HIST_METRICS_BUDGET (in
+ * (bucket, column) accumulators) run in consecutive waves.  TQ_OP_PHRASE returns TQ_ERR_UNSUPPORTED, a segment without a column
+ * TQ_ERR_NOT_FOUND; out_stride below some n_buckets, n_buckets outside 1 .. TQ_RANGE_MAX_BUCKETS, starts not strictly ascending
+ * or starts[0] != 0, out_parts NULL with mspecs (or not NULL without) and the metrics spec errors of tq_metrics_batch
+ * TQ_ERR_INVALID_ARGUMENT.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The run holds its columns as tq_sort_batch does. */
+#define TQ_RANGE_MAX_BUCKETS 128u
+typedef struct {
+  uint32_t column_id;                     /* a column of tq_sort_column_register */
+  uint32_t n_buckets;                     /* 1 .. TQ_RANGE_MAX_BUCKETS, after extension */
+  uint64_t starts[TQ_RANGE_MAX_BUCKETS];  /* strictly ascending images, starts[0] == 0 */
+} tq_range_spec;
+#ifdef __cplusplus
+static_assert(sizeof(tq_range_spec) == 1032, "range ABI layout");
+#endif
+int tq_range_batch(tq_ctx*, const tq_query* queries, const tq_range_spec* rspecs, const tq_metrics_spec* mspecs, size_t nq,
+                   uint32_t out_stride, uint64_t* out_doc_count, tq_metric_part* out_parts, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

@@ -17,3 +17,5 @@ from . import hist_metrics  # noqa: E402  (histograms with metric sub-aggregatio
 from .hist_metrics import HistMetricsRefused  # noqa: E402
 from . import terms_metrics  # noqa: E402  (terms with metric sub-aggregations: request and result side)
 from .terms_metrics import TermsMetricsRefused  # noqa: E402
+from . import ranges  # noqa: E402  (range aggregations, with or without metric sub-aggregations: request and result side)
+from .ranges import RangeRefused  # noqa: E402

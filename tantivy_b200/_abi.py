@@ -237,6 +237,23 @@ TERMS_METRIC_ORDER_DTYPE = np.dtype([("column", "<u4"), ("metric", "<u4")])
 assert TERMS_METRIC_ORDER_DTYPE.itemsize == C.sizeof(TermsMetricOrder) == 8
 
 
+TQ_RANGE_MAX_BUCKETS = 128
+
+
+class RangeSpec(C.Structure):
+    """tq_range_spec — the column and the strictly ascending bucket starts (images, starts[0] == 0) of one query's range."""
+    _fields_ = [("column_id", C.c_uint32), ("n_buckets", C.c_uint32), ("starts", C.c_uint64 * TQ_RANGE_MAX_BUCKETS)]
+
+
+RANGE_SPEC_DTYPE = np.dtype([("column_id", "<u4"), ("n_buckets", "<u4"), ("starts", "<u8", (TQ_RANGE_MAX_BUCKETS,))])
+assert RANGE_SPEC_DTYPE.itemsize == C.sizeof(RangeSpec) == 1032
+
+
+class RangeStats(C.Structure):
+    """tq_range_stats — the cumulative counters of tq_range_batch (tq_get_range_stats)."""
+    _fields_ = [("range_ms", C.c_float), ("units_range", C.c_uint64), ("range_tiles_seen", C.c_uint64), ("range_tiles_one_bucket", C.c_uint64)]
+
+
 def ptr(arr, typ):
     """numpy array -> ctypes pointer (array must stay alive while the pointer is used)."""
     if arr is None:

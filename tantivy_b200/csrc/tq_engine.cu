@@ -439,6 +439,16 @@ int tq_get_terms_metrics_stats(tq_ctx* c, tq_terms_metrics_stats* out) {
   return TQ_OK;
 }
 
+int tq_get_range_stats(tq_ctx* c, tq_range_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->range_ms = (float)c->range_ms;
+  out->units_range = c->range_units;
+  out->range_tiles_seen = c->range_tiles_seen;
+  out->range_tiles_one_bucket = c->range_tiles_one_bucket;
+  return TQ_OK;
+}
+
 int tq_segment_register(tq_ctx* c, uint32_t segment_ord, uint32_t field, uint32_t max_doc, int record_option,
                         const uint8_t* idx_body, size_t idx_len, const uint8_t* fieldnorm, size_t fieldnorm_len,
                         const uint8_t* alive_bitset, size_t alive_len) {
@@ -1820,23 +1830,33 @@ static bool unit_images(const SortColumn& col, const Unit& u, unsigned long long
 // segment) its column and bounds after normalize_histogram_req's collapse (hsegs, cols), per unit the first and last pos its tiles'
 // values in bounds can take (uwin; first > last: none), and the query's dense range [base, base + len) (compute_dense_range,
 // histogram.rs:751-769, over the visited tiles only).  A range above max_bins is TQ_ERR_UNSUPPORTED.
+// The registered column column_id of each (query, segment) plan_count added from s0, into cols.  `what` names the query in the
+// errors: a segment without the column is TQ_ERR_NOT_FOUND, one whose max_doc differs TQ_ERR_INVALID_ARGUMENT.
+static int find_columns(tq_ctx* c, uint32_t column_id, const CountPlan& cp, size_t s0, const char* what, std::vector<const SortColumn*>& cols) {
+  cols.clear();
+  for (size_t si = s0; si < cp.segs.size(); ++si) {
+    auto it = c->sort_columns.find({column_id, cp.segment_ords[si]});
+    if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, std::string(what) + " names a segment without the column (tq_sort_column_register)");
+    const SortColumn& col = it->second;
+    if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+    cols.push_back(&col);
+  }
+  return TQ_OK;
+}
+
 static int plan_hist_query(tq_ctx* c, const tq_histogram_spec& sp, size_t qi, const CountPlan& cp, size_t s0, size_t u0, uint32_t max_bins,
                            std::vector<HistSeg>& hsegs, std::vector<const SortColumn*>& cols, std::vector<std::pair<long long, long long>>& uwin,
                            long long& base, uint64_t& len) {
-  cols.clear();
-  for (size_t si = s0; si < cp.segs.size(); ++si) {
-    auto it = c->sort_columns.find({sp.column_id, cp.segment_ords[si]});
-    if (it == c->sort_columns.end()) return fail(TQ_ERR_NOT_FOUND, "a histogram query names a segment without the column (tq_sort_column_register)");
-    const SortColumn& col = it->second;
-    if (col.tiles.size() != (cp.segs[si].max_doc + kTileDocs - 1) / kTileDocs) return fail(TQ_ERR_INVALID_ARGUMENT, "column and segment differ in max_doc");
+  int rc = find_columns(c, sp.column_id, cp, s0, "a histogram query", cols);
+  if (rc != TQ_OK) return rc;
+  for (const SortColumn* col : cols) {
     // normalize_histogram_req: the hard bounds collapse to every finite value when the segment's column lies inside them
     double lo = sp.hard_min, hi = sp.hard_max;
-    if (col.min_image <= col.max_image && hist_value(col.min_image, sp.kind) >= lo && hist_value(col.max_image, sp.kind) <= hi) {
+    if (col->min_image <= col->max_image && hist_value(col->min_image, sp.kind) >= lo && hist_value(col->max_image, sp.kind) <= hi) {
       lo = -DBL_MAX;
       hi = DBL_MAX;
     }
-    hsegs.push_back(HistSeg{col.d_values, col.d_present, col.d_tiles, lo, hi});
-    cols.push_back(&col);
+    hsegs.push_back(HistSeg{col->d_values, col->d_present, col->d_tiles, lo, hi});
   }
   // per unit: the buckets of its tiles' values, clipped to its segment's bounds; the query's dense range (compute_dense_range,
   // histogram.rs:751-769, over the visited tiles only) is their union
@@ -2374,6 +2394,28 @@ int tq_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_metrics_spec* 
 }
 
 // ---- metrics per histogram bucket ----------------------------------------------------------------------------
+// Waves of consecutive queries whose accumulators (kMetricsMaxColumns per counter) fit the budget (a query above it runs alone),
+// query qi holding n_bins[qi] counters: at[qi] is its first counter and row_at[qi] its first row entry in its wave, its row holding
+// min(row_cap, n_bins[qi]) entries.
+struct Wave { size_t q0, q1; uint64_t counters, rows; };
+static std::vector<Wave> plan_waves(const std::vector<uint32_t>& n_bins, uint64_t budget, uint32_t row_cap, std::vector<unsigned long long>& at,
+                                    std::vector<unsigned long long>& row_at) {
+  std::vector<Wave> waves;
+  at.assign(n_bins.size(), 0);
+  row_at.assign(n_bins.size(), 0);
+  for (size_t qi = 0; qi < n_bins.size(); ++qi) {
+    if (waves.empty() || (waves.back().counters && (waves.back().counters + n_bins[qi]) * kMetricsMaxColumns > budget))
+      waves.push_back(Wave{qi, qi, 0, 0});
+    Wave& w = waves.back();
+    at[qi] = w.counters;
+    row_at[qi] = w.rows;
+    w.q1 = qi + 1;
+    w.counters += n_bins[qi];
+    w.rows += std::min<uint64_t>(row_cap, n_bins[qi]);
+  }
+  return waves;
+}
+
 int tq_histogram_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_metrics_spec* mspecs, size_t nq,
                                uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
                                uint64_t* out_hits) {
@@ -2435,23 +2477,16 @@ int tq_histogram_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_hist
     for (uint32_t col : b->held_columns) ++c->sort_users[col];
   }
   if (cp.units.empty()) return TQ_OK;
-  // waves of consecutive queries whose accumulators (kC per bucket) fit the budget (a query above it runs alone); counters and rows
-  // relative to the wave.  A query's row holds min(out_stride, n_bins) entries (it has at most n_bins non-empty buckets), so a
-  // wave's rows, on the device and in pinned memory, are bounded by its counters and the budget as well.
-  struct Wave { size_t q0, q1; uint64_t counters, rows; };
-  std::vector<Wave> waves;
-  std::vector<unsigned long long> row_at(nq);
+  // A query's row holds min(out_stride, n_bins) entries (it has at most n_bins non-empty buckets), so a wave's rows, on the device
+  // and in pinned memory, are bounded by its counters and the budget as well.
+  std::vector<uint32_t> bins(nq);
+  for (size_t qi = 0; qi < nq; ++qi) bins[qi] = hq[qi].n_bins;
+  std::vector<unsigned long long> at, row_at;
+  const std::vector<Wave> waves = plan_waves(bins, c->hist_metrics_budget, out_stride, at, row_at);
+  for (size_t qi = 0; qi < nq; ++qi) hq[qi].counters = at[qi];
   uint64_t max_counters = 0, max_rows = 0;
   size_t max_queries = 0;
-  for (size_t qi = 0; qi < nq; ++qi) {
-    if (waves.empty() || (waves.back().counters && (waves.back().counters + hq[qi].n_bins) * kC > c->hist_metrics_budget))
-      waves.push_back(Wave{qi, qi, 0, 0});
-    Wave& w = waves.back();
-    hq[qi].counters = w.counters;
-    row_at[qi] = w.rows;
-    w.q1 = qi + 1;
-    w.counters += hq[qi].n_bins;
-    w.rows += std::min<uint64_t>(out_stride, hq[qi].n_bins);
+  for (const Wave& w : waves) {
     max_counters = std::max(max_counters, w.counters);
     max_rows = std::max(max_rows, w.rows);
     max_queries = std::max(max_queries, w.q1 - w.q0);
@@ -2825,6 +2860,181 @@ int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_sp
     c->terms_metrics_waves += waves.size();
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride: out_n holds how many");
+  return TQ_OK;
+}
+
+// ---- range of a fast field ------------------------------------------------------------------------------------
+// A range spec's bucket count and starts (TQ_ERR_INVALID_ARGUMENT).
+static int check_range_spec(const tq_range_spec& r, uint32_t out_stride) {
+  if (r.n_buckets < 1 || r.n_buckets > TQ_RANGE_MAX_BUCKETS) return fail(TQ_ERR_INVALID_ARGUMENT, "range spec: n_buckets must be 1..128");
+  if (r.starts[0] != 0) return fail(TQ_ERR_INVALID_ARGUMENT, "range spec: starts[0] must be 0");
+  for (uint32_t b = 1; b < r.n_buckets; ++b)
+    if (r.starts[b] <= r.starts[b - 1]) return fail(TQ_ERR_INVALID_ARGUMENT, "range spec: starts must be strictly ascending");
+  if (out_stride < r.n_buckets) return fail(TQ_ERR_INVALID_ARGUMENT, "out_stride must hold every bucket of a range");
+  return TQ_OK;
+}
+
+int tq_range_batch(tq_ctx* c, const tq_query* queries, const tq_range_spec* rspecs, const tq_metrics_spec* mspecs, size_t nq,
+                   uint32_t out_stride, uint64_t* out_doc_count, tq_metric_part* out_parts, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !rspecs || !out_doc_count)) || (mspecs == nullptr) != (out_parts == nullptr))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null (out_parts goes with mspecs)");
+  TQ_CUDA(cudaSetDevice(c->device));
+  constexpr uint32_t kC = kMetricsMaxColumns;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "ranges of phrase queries are not on the device path");
+    int rc = check_range_spec(rspecs[qi], out_stride);
+    if (rc == TQ_OK && mspecs) rc = check_metrics_spec(mspecs[qi]);
+    if (rc != TQ_OK) return rc;
+  }
+  const tq_metric_part empty{0ull, 0ull, 0ull, ~0ull, 0ull, 0.0, 0.0, INT32_MAX, 0u};
+  for (size_t qi = 0; qi < nq; ++qi) {
+    for (size_t i = qi * (size_t)out_stride; i < (qi + 1) * (size_t)out_stride; ++i) {
+      out_doc_count[i] = 0;
+      for (uint32_t k = 0; mspecs && k < kC; ++k) out_parts[i * kC + k] = empty;
+    }
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<RangeSeg> rsegs;      // parallel to cp.segs
+  std::vector<MetricsSeg> msegs;    // parallel to cp.segs, with mspecs
+  std::vector<RangeQuery> rq(nq);
+  std::vector<HistUnit> windows;    // parallel to cp.units
+  std::vector<unsigned long long> starts;  // every query's starts, back to back
+  std::vector<size_t> start_at(nq), q_unit(nq + 1);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_range_spec& r = rspecs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      rc = find_columns(c, r.column_id, cp, s0, "a range query", cols);
+      if (rc != TQ_OK) return rc;
+      for (const SortColumn* col : cols) rsegs.push_back(RangeSeg{col->d_values, col->d_present, col->d_tiles});
+      if (mspecs) {
+        rc = plan_metrics_segs(c, mspecs[qi], cp, s0, out_hits != nullptr, msegs);
+        if (rc != TQ_OK) return rc;
+      }
+      windows.insert(windows.end(), cp.units.size() - u0, HistUnit{0u, r.n_buckets});  // (no per-unit window: every bucket)
+      start_at[qi] = starts.size();
+      starts.insert(starts.end(), r.starts, r.starts + r.n_buckets);
+      rq[qi] = RangeQuery{nullptr, 0ull, r.n_buckets, out_hits ? kRangeHits : 0u};
+    }
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      b->held_columns.push_back(rspecs[qi].column_id);
+      if (mspecs) hold_metric_columns(b, mspecs[qi]);
+    }
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // counters: without metrics every query's at once; with metrics in waves of accumulators that fit the budget
+  std::vector<Wave> waves;
+  if (mspecs) {
+    std::vector<uint32_t> bins(nq);
+    for (size_t qi = 0; qi < nq; ++qi) bins[qi] = rq[qi].n_bins;
+    std::vector<unsigned long long> at, row_at;
+    waves = plan_waves(bins, c->hist_metrics_budget, out_stride, at, row_at);
+    for (size_t qi = 0; qi < nq; ++qi) rq[qi].counters = at[qi];
+  } else {
+    waves.push_back(Wave{0, nq, 0, 0});
+    for (size_t qi = 0; qi < nq; ++qi) { rq[qi].counters = waves[0].counters; waves[0].counters += rq[qi].n_bins; }
+  }
+  uint64_t max_counters = 0;
+  for (const Wave& w : waves) max_counters = std::max(max_counters, w.counters);
+  // descriptors: one H2D copy (the queries point into the starts); scratch: hits | tile counters, then one wave's doc counters |
+  // accumulators, read back as they are (the rows are dense)
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(rsegs), o_m = st.add(msegs),
+               o_q = st.add(rq), o_h = st.add(windows), o_st = st.add(starts);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  for (size_t qi = 0; qi < nq; ++qi) rq[qi].starts = st.on_device<const unsigned long long>(o_st) + start_at[qi];
+  st.copy();
+  const size_t part_row = (size_t)kC * sizeof(tq_metric_part);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(32), head_bytes = off;
+  const size_t r_counters = take(max_counters * 8), r_acc = take(mspecs ? max_counters * part_row : 0), wave_bytes = off - head_bytes;
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  const CountParams cparams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                            reinterpret_cast<unsigned long long*>(d + r_hits)};
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  const uint8_t* h = b->res_pin.p;
+  const size_t p_acc = r_acc - head_bytes;
+  float ms_total = 0;
+  for (const Wave& w : waves) {
+    const size_t ua = q_unit[w.q0], ub = q_unit[w.q1];
+    TQ_CUDA(cudaMemsetAsync(d + r_counters, 0, w.counters * 8, b->stream));
+    if (mspecs) TQ_CUDA(cudaMemsetAsync(d + r_acc, 0, w.counters * part_row, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    if (ub > ua && mspecs) {
+      RangeMetricsParams P{};
+      P.c = cparams;
+      P.rsegs = st.on_device<const RangeSeg>(o_z);
+      P.msegs = st.on_device<const MetricsSeg>(o_m);
+      P.queries = st.on_device<const RangeQuery>(o_q);
+      P.windows = st.on_device<const HistUnit>(o_h);
+      P.counts = reinterpret_cast<unsigned long long*>(d + r_counters);
+      P.parts = reinterpret_cast<tq_metric_part*>(d + r_acc);
+      P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+      P.unit_base = (uint32_t)ua;
+      (cp.mixed ? k_range_metrics<true> : k_range_metrics<false>)<<<(unsigned)(ub - ua), kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    } else if (ub > ua) {
+      RangeParams P{};
+      P.c = cparams;
+      P.rsegs = st.on_device<const RangeSeg>(o_z);
+      P.queries = st.on_device<const RangeQuery>(o_q);
+      P.windows = st.on_device<const HistUnit>(o_h);
+      P.counts = reinterpret_cast<unsigned long long*>(d + r_counters);
+      P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+      (cp.mixed ? k_range<true> : k_range<false>)<<<(unsigned)(ub - ua), kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + r_counters, w.counters * 8, cudaMemcpyDeviceToHost, b->stream));
+    if (mspecs) TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + p_acc, d + r_acc, w.counters * part_row, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    const unsigned long long* counts = reinterpret_cast<const unsigned long long*>(h);
+    const tq_metric_part* parts = reinterpret_cast<const tq_metric_part*>(h + p_acc);
+    for (size_t qi = w.q0; qi < w.q1; ++qi) {
+      const size_t dst = qi * (size_t)out_stride;
+      memcpy(out_doc_count + dst, counts + rq[qi].counters, (size_t)rq[qi].n_bins * 8);
+      for (size_t i = 0; mspecs && i < (size_t)rq[qi].n_bins * kC; ++i) out_parts[dst * kC + i] = uncomplement(parts[rq[qi].counters * kC + i]);
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  unsigned long long tiles[2];
+  memcpy(tiles, h + r_tiles, 16);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->range_ms += ms_total;
+    c->range_units += cp.units.size();
+    c->range_tiles_seen += tiles[0];
+    c->range_tiles_one_bucket += tiles[1];
+  }
   return TQ_OK;
 }
 

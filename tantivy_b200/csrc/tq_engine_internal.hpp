@@ -254,6 +254,9 @@ struct tq_ctx {
   // ... and of the terms-with-metrics runs (terms_metrics_ms, units, tiles seen / with one kept key, waves)
   double terms_metrics_ms = 0;
   uint64_t terms_metrics_units = 0, terms_metrics_tiles_seen = 0, terms_metrics_tiles_one_key = 0, terms_metrics_waves = 0;
+  // ... and of the range runs, with and without metrics (range_ms, units, tiles seen / in one bucket)
+  double range_ms = 0;
+  uint64_t range_units = 0, range_tiles_seen = 0, range_tiles_one_bucket = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;

@@ -1427,7 +1427,7 @@ __global__ void __launch_bounds__(kThreads) k_sort_final(const SortParams P) {
 // atomicAdd per non-zero bucket at exit), else global.  A timestamp unit of eight tiles spans a few minutes of the column, so even a
 // query of many thousand buckets counts on chip.
 
-// The body of k_hist and k_terms: one CTA per Count unit counts its matching docs by key into its window of counters.  K is the
+// The body of k_hist, k_terms and k_range: one CTA per Count unit counts its matching docs by key into its window of counters.  K is the
 // key policy, static functions over the (query, segment)'s descriptor Z, the query's Q and the unit's window W (from the origin
 // `base`): the one key of a tile with values, if it has one (every value of the tile, matching or not, has it: the tile's matches are added without a gather;
 // ~0u: none), whether a value is counted and the index of its counter, and whether matching docs without a value are counted as
@@ -1522,11 +1522,14 @@ struct HistKeys {
   typedef double Value;
   typedef unsigned long long Counter;
   static constexpr bool kMissing = false;
-  static __device__ __forceinline__ HistSeg seg(const HistParams& P, const Unit& U) { return P.hsegs[U.qseg]; }
-  static __device__ __forceinline__ HistQuery query(const HistParams& P, const CountSeg& S, const HistSeg&) { return P.queries[S.query]; }
-  static __device__ __forceinline__ HistUnit window(const HistParams& P, uint32_t unit) { return P.hunits[unit]; }
+  // (Params: HistParams for k_hist, HistMetricsParams for k_hist_metrics)
+  template <class Params> static __device__ __forceinline__ HistSeg seg(const Params& P, const Unit& U) { return P.hsegs[U.qseg]; }
+  template <class Params> static __device__ __forceinline__ HistQuery query(const Params& P, const CountSeg& S, const HistSeg&) { return P.queries[S.query]; }
+  template <class Params> static __device__ __forceinline__ HistUnit window(const Params& P, uint32_t unit) { return P.hunits[unit]; }
   static __device__ __forceinline__ long long base(const HistSeg&, const HistQuery& Q, const HistUnit& W) { return Q.base + (long long)W.first; }
-  static __device__ __forceinline__ Counter* counts(const HistParams& P, const HistSeg&, const HistQuery& Q, const HistUnit& W) { return P.counts + Q.counters + W.first; }
+  template <class Params> static __device__ __forceinline__ Counter* counts(const Params& P, const HistSeg&, const HistQuery& Q, const HistUnit& W) { return P.counts + Q.counters + W.first; }
+  // the window's first counter in the wave (k_hist_metrics: its parts are kMetricsMaxColumns per counter)
+  static __device__ __forceinline__ unsigned long long slot(const HistSeg&, const HistQuery& Q, const HistUnit& W) { return Q.counters + W.first; }
   // one bucket: the tile's smallest and largest values both in bounds and in one bucket (pos is monotone in the image)
   static __device__ __forceinline__ void one(const SortTile T, const HistSeg& Z, const HistQuery& Q, const HistUnit& W, const long long base, uint32_t& idx) {
     const double vmin = hist_value(~T.best[1], Q.kind), vmax = hist_value(T.best[0], Q.kind);
@@ -1606,6 +1609,53 @@ struct TermsKeys {
 template <bool kMixed>
 __global__ void __launch_bounds__(kThreads, 4) k_terms(const TermsParams P) {
   count_unit_keys<TermsKeys, kMixed>(P, P.unit_base + blockIdx.x);
+}
+
+// ---- range of a fast field (AggregationCollector: range, bucket/range.rs) -------------------------------------------------
+// The docs Count counts, each with a value counted in range bucket b = the last start <= its image (get_bucket_pos: a binary search
+// over the starts, the end never tested), through count_unit_keys.  The image alone decides the bucket: no conversion, no division.
+// A tile whose smallest and largest images land in one bucket adds its matches there without a gather; a doc without a value is not
+// collected (range has no `missing`).  The window is the query's whole bucket list.
+struct RangeKeys {
+  typedef RangeSeg Seg;
+  typedef RangeQuery Query;
+  typedef uint32_t Base;  // (0: the window starts at the query's first bucket)
+  typedef unsigned long long Value;
+  typedef unsigned long long Counter;
+  static constexpr bool kMissing = false;
+  // (Params: RangeParams for k_range, RangeMetricsParams for k_range_metrics)
+  template <class Params> static __device__ __forceinline__ RangeSeg seg(const Params& P, const Unit& U) { return P.rsegs[U.qseg]; }
+  template <class Params> static __device__ __forceinline__ RangeQuery query(const Params& P, const CountSeg& S, const RangeSeg&) { return P.queries[S.query]; }
+  template <class Params> static __device__ __forceinline__ HistUnit window(const Params& P, uint32_t unit) { return P.windows[unit]; }
+  static __device__ __forceinline__ uint32_t base(const RangeSeg&, const RangeQuery&, const HistUnit&) { return 0u; }
+  template <class Params> static __device__ __forceinline__ Counter* counts(const Params& P, const RangeSeg&, const RangeQuery& Q, const HistUnit&) { return P.counts + Q.counters; }
+  static __device__ __forceinline__ unsigned long long slot(const RangeSeg&, const RangeQuery& Q, const HistUnit&) { return Q.counters; }
+  // upper bound over the starts (through the read-only cache): the last b with starts[b] <= v; starts[0] == 0, so always one.  At
+  // most 7 steps for kRangeMaxBins buckets.
+  static __device__ __forceinline__ uint32_t bucket(const unsigned long long v, const RangeQuery& Q) {
+    uint32_t lo = 0, n = Q.n_bins;
+    while (n > 1u) {
+      const uint32_t half = n >> 1;
+      if (__ldg(Q.starts + lo + half) <= v) lo += half;
+      n -= half;
+    }
+    return lo;
+  }
+  // one bucket: the tile's smallest and largest images in the same one (the bucket is monotone in the image)
+  static __device__ __forceinline__ void one(const SortTile T, const RangeSeg&, const RangeQuery& Q, const HistUnit&, uint32_t, uint32_t& idx) {
+    const uint32_t b = bucket(~T.best[1], Q);
+    if (b == bucket(T.best[0], Q)) idx = b;
+  }
+  static __device__ __forceinline__ unsigned long long value(unsigned long long v, const RangeQuery&) { return v; }
+  static __device__ __forceinline__ bool counted(unsigned long long, const RangeSeg&) { return true; }
+  static __device__ __forceinline__ unsigned long long index(unsigned long long v, const RangeQuery& Q, uint32_t) { return bucket(v, Q); }
+  static __device__ __forceinline__ bool hits(const RangeQuery& Q) { return Q.flags & kRangeHits; }
+};
+
+// (4 CTAs per SM: the search is a few compares and loads, and the 64 registers hold the loop without spilling)
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 4) k_range(const RangeParams P) {
+  count_unit_keys<RangeKeys, kMixed>(P, blockIdx.x);
 }
 
 // Exclusive CTA-wide prefix sum of v (fields packed in v add independently while each total fits its field); *total = the sum.
@@ -1983,8 +2033,10 @@ __device__ __forceinline__ void hm_doc(Docs* docs, tq_metric_part* parts, const 
   }
 }
 
-template <bool kMixed>
-__global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsParams P) {
+// The body of k_hist_metrics and k_range_metrics, over the key policy K of count_unit_keys (its seg, query, window, base, counts,
+// one, value, counted, index and hits, and slot: the window's first counter, whose parts are kMetricsMaxColumns per counter).
+template <class K, bool kMixed, class Params>
+__device__ __forceinline__ void metrics_unit_keys(const Params& P) {
   static_assert(kTileDocs / 32u == (uint32_t)kThreads, "one 32-doc word of a tile per thread");
   static_assert(sizeof(MetricsSeg) % 8u == 0 && sizeof(MetricsSeg) / 8u <= (uint32_t)kThreads, "one word of the descriptor per thread");
   constexpr uint32_t kC = kMetricsMaxColumns;
@@ -2004,9 +2056,9 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
   const uint32_t unit = P.unit_base + blockIdx.x;
   const Unit U = P.c.units[unit];
   const CountSeg S = P.c.segs[U.qseg];
-  const HistSeg Z = P.hsegs[U.qseg];
-  const HistQuery Q = P.queries[S.query];
-  const HistUnit W = P.hunits[unit];
+  const typename K::Seg Z = K::seg(P, U);
+  const typename K::Query Q = K::query(P, S, Z);
+  const HistUnit W = K::window(P, unit);
   if (threadIdx.x < sizeof(MetricsSeg) / 8u)
     reinterpret_cast<unsigned long long*>(&s_z)[threadIdx.x] = reinterpret_cast<const unsigned long long*>(P.msegs + U.qseg)[threadIdx.x];
   if (threadIdx.x < 2u * kC) (&s_nan_inf[0][0])[threadIdx.x] = 0;
@@ -2020,9 +2072,9 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
   const uint32_t nc = s_z.n_columns;
   const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const long long base = Q.base + (long long)W.first;  // pos of the window's first bucket
-  unsigned long long* const gdocs = P.counts + Q.counters + W.first;
-  tq_metric_part* const gparts = P.parts + (Q.counters + W.first) * kC;
+  const typename K::Base base = K::base(Z, Q, W);  // the key of the window's first bucket
+  unsigned long long* const gdocs = K::counts(P, Z, Q, W);
+  tq_metric_part* const gparts = P.parts + K::slot(Z, Q, W) * kC;
   MetricAcc acc[kC];
 #pragma unroll
   for (uint32_t c = 0; c < kC; ++c) acc[c] = MetricAcc{~0ull, 0ull, 0.0, 0.0, 0u, 0u, INT32_MAX};
@@ -2096,7 +2148,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
     if (threadIdx.x == 0) {
       const SortTile T = Z.tiles[tile];
       uint32_t idx = 0xFFFFFFFFu;
-      if (W.n_bins && (T.flags & kSortTileValues)) HistKeys::one(T, Z, Q, W, base, idx);
+      if (W.n_bins && (T.flags & kSortTileValues)) K::one(T, Z, Q, W, base, idx);
       s_bucket = idx;
       one += idx != 0xFFFFFFFFu ? 1u : 0u;
     }
@@ -2151,9 +2203,9 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
         }
         for (; hw; hw &= hw - 1u) {
           const uint32_t bit = (uint32_t)(__ffs(hw) - 1), doc = lo + threadIdx.x * 32u + bit;
-          const double val = hist_value(__ldg(Z.values + doc), Q.kind);
-          if (!(val >= Z.lo && val <= Z.hi)) continue;  // HistogramBounds::contains (NaN never passes)
-          const unsigned long long idx = (unsigned long long)(hist_pos(val, Q.offset, Q.interval) - base);
+          const typename K::Value val = K::value(__ldg(Z.values + doc), Q);
+          if (!K::counted(val, Z)) continue;
+          const unsigned long long idx = K::index(val, Q, base);
           if (idx >= W.n_bins) continue;  // (never: the window covers every counted value of the unit's tiles)
           if (shared) hm_doc(s_docs + idx, s_parts + idx * kC, s_z, cw, doc, bit);
           else hm_doc(gdocs + idx, gparts + idx * kC, s_z, cw, doc, bit);
@@ -2181,7 +2233,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
   if (lane == 0) { s_part[warp] = total; s_rdocs[warp] = flushed_shared; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (Q.flags & kHistHits) {
+    if (K::hits(Q)) {
       unsigned long long hits = 0;
       for (int w = 0; w < kWarps; ++w) hits += s_part[w];
       if (hits) atomicAdd(&P.c.counts[S.query], hits);
@@ -2193,6 +2245,19 @@ __global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsP
     if (fs) atomicAdd(&P.tiles[2], fs);
     if (flushed_global) atomicAdd(&P.tiles[3], (unsigned long long)flushed_global);
   }
+}
+
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 2) k_hist_metrics(const HistMetricsParams P) {
+  metrics_unit_keys<HistKeys, kMixed>(P);
+}
+
+// The docs k_range counts, each feeding the metric columns of the (query, segment)'s MetricsSeg in its range bucket: the body of
+// k_hist_metrics over RangeKeys.  The window is the query's whole bucket list, so its accumulators always live in shared memory; the
+// wave's accumulators are the query's dense rows, which the host reads back and uncomplements (no compaction kernel).
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 2) k_range_metrics(const RangeMetricsParams P) {
+  metrics_unit_keys<RangeKeys, kMixed>(P);
 }
 
 // One CTA per query of the wave: its non-empty buckets in ascending pos into its row (the prefix sum of k_hist_final; at most

@@ -371,6 +371,46 @@ struct HistMetricsParams {
   uint32_t unit_base, query_base;  // the wave's first unit and first query
 };
 
+// ---- range of a fast field (k_range, k_range_metrics) ---------------------------------------------------------------------
+// Doc counts per range bucket b = the last start <= image (get_bucket_pos, range.rs) of the docs Count counts, and with metrics one
+// tq_metric_part per (bucket, column) as in k_hist_metrics.  A query's counters are its n_bins buckets, every one of them (the rows
+// are dense), and every unit's window is the query's whole bucket list (kRangeMaxBins <= kHistMetricsSmemBins <= kHistSmemBins:
+// always on chip).  With metrics, queries run in waves whose accumulators fit the ctx's budget, and counters are relative to the wave.
+constexpr uint32_t kRangeMaxBins = 128;  // TQ_RANGE_MAX_BUCKETS
+static_assert(kRangeMaxBins <= kHistMetricsSmemBins && kRangeMaxBins <= kHistSmemBins, "a range window always lives in shared memory");
+struct RangeSeg {  // the column of one (query, segment), parallel to CountParams::segs
+  const unsigned long long* values;  // [max_doc] u64 images
+  const uint32_t* present;           // bitset in the alive layout (null: every doc has a value)
+  const SortTile* tiles;             // the column's per-tile bounds
+};
+struct RangeQuery {
+  const unsigned long long* starts;  // [n_bins] strictly ascending images, starts[0] == 0 (device)
+  unsigned long long counters;       // first counter of the query
+  uint32_t n_bins;                   // 1 .. kRangeMaxBins
+  uint32_t flags;                    // kRangeHits: the query's Count is asked for as well
+};
+constexpr uint32_t kRangeHits = 1;
+struct RangeParams {
+  CountParams c;                // structure words, (query, segment) pairs, units and hit counters: the Count plan
+  const RangeSeg* rsegs;        // parallel to c.segs
+  const RangeQuery* queries;    // [nq]
+  const HistUnit* windows;      // parallel to c.units: {0, n_bins} of the unit's query
+  unsigned long long* counts;   // every query's counters, zeroed before the run
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them counted as one bucket
+};
+struct RangeMetricsParams {
+  CountParams c;                // structure words, (query, segment) pairs, units and hit counters: the Count plan of the batch
+  const RangeSeg* rsegs;        // parallel to c.segs
+  const MetricsSeg* msegs;      // parallel to c.segs: the metric columns
+  const RangeQuery* queries;    // [nq]: counters relative to the wave
+  const HistUnit* windows;      // parallel to c.units
+  unsigned long long* counts;   // the wave's doc counters, zeroed before it
+  tq_metric_part* parts;        // [wave's counters][kMetricsMaxColumns], zeroed before the wave (complemented as in k_hist_metrics)
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them in one bucket, [2] buckets flushed from shared, [3] runs flushed to global
+  uint32_t unit_base;           // the wave's first unit
+};
+static_assert(sizeof(RangeSeg) == 24 && sizeof(RangeQuery) == 24, "range descriptor layout");
+
 // ---- metrics per term (k_terms_order, k_terms_select_metric, k_terms_mark, k_terms_metrics) ---------------------------------
 // The terms of k_terms / k_terms_select (TermsSeg, the unit windows, the counters) with the metric columns of the (query, segment)'s
 // MetricsSeg.  After the cut, k_terms_mark overwrites the counter of each kept key with kTermsSlot | its index in the (query,

@@ -9,7 +9,7 @@ import numpy as np
 from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
                    MetricsSpec, MetricsStats, HistMetricsStats, TermsMetricsStats, TermsMetricOrder, TERMS_METRIC_ORDER_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
-                   f32p, ptr, u8p, u32p, u64p)
+                   RANGE_SPEC_DTYPE, RangeSpec, RangeStats, TQ_RANGE_MAX_BUCKETS, f32p, ptr, u8p, u32p, u64p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -36,6 +36,7 @@ def _load():
     lib.tq_get_metrics_stats.argtypes = [vp, C.POINTER(MetricsStats)]
     lib.tq_get_hist_metrics_stats.argtypes = [vp, C.POINTER(HistMetricsStats)]
     lib.tq_get_terms_metrics_stats.argtypes = [vp, C.POINTER(TermsMetricsStats)]
+    lib.tq_get_range_stats.argtypes = [vp, C.POINTER(RangeStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -57,6 +58,8 @@ def _load():
                                                C.POINTER(C.c_int64), u64p, C.POINTER(MetricPart), u32p, u64p]
     lib.tq_terms_metrics_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), C.POINTER(MetricsSpec), C.POINTER(TermsMetricOrder), sz,
                                            C.c_uint32, u32p, u64p, u64p, C.POINTER(MetricPart), u32p, u64p, u64p, C.POINTER(MetricPart), u64p]
+    lib.tq_range_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(RangeSpec), C.POINTER(MetricsSpec), sz, C.c_uint32, u64p, C.POINTER(MetricPart),
+                                   u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -158,6 +161,19 @@ def _metrics_specs(specs, nq):
             flags, image = (tuple(col[2:4]) + (0, 0))[:2]
             spec[i]["columns"][j] = (col[0], col[1], flags, 0, image)
     return spec
+
+def _range_specs(specs, nq):
+    """RANGE_SPEC_DTYPE rows of (column_id, starts) tuples: starts the bucket starts in image space, ascending from 0."""
+    spec = np.zeros(max(nq, 1), dtype=RANGE_SPEC_DTYPE)
+    for i, (col, starts) in enumerate(specs):
+        starts = [int(x) for x in starts]
+        if len(starts) > TQ_RANGE_MAX_BUCKETS:
+            raise ValueError(f"query {i}: a range has at most {TQ_RANGE_MAX_BUCKETS} buckets, got {len(starts)}")
+        spec[i]["column_id"] = col
+        spec[i]["n_buckets"] = len(starts)
+        spec[i]["starts"][:len(starts)] = np.array(starts, dtype=np.uint64)
+    return spec
+
 
 def fast_value_to_u64(values, kind):
     """The u64 image of fast-field values (MonotonicallyMappableToU64, common/src/lib.rs), what tq_sort_column_register takes:
@@ -524,6 +540,31 @@ class Context:
             out = (pos[:qb.nq], counts[:qb.nq], parts[:qb.nq], nb[:qb.nq])
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def range_batch(self, qb: QueryBatch, rspecs, mspecs=None, count_hits=False):
+        """A range aggregation per query (tq_range_batch) over sort columns, with or without metric sub-aggregations; rspecs = one
+        (column_id, starts) per query, starts the query's 1..TQ_RANGE_MAX_BUCKETS bucket starts in image space, strictly ascending
+        from 0 (tantivy_b200.ranges turns requests into them); mspecs = None, or one list of 1..4 metric columns per query as
+        metrics_batch takes them.  Returns (doc_count, parts) -- and with count_hits=True the Count of every query as well: row q
+        holds every bucket of query q in start order, doc_count[q, b] over all its segments and parts[q, b] its
+        [TQ_METRICS_MAX_COLUMNS] METRIC_PART_DTYPE parts (None without mspecs).  Rows are max(n_buckets) wide; entries past a
+        query's own buckets are zero."""
+        rspecs = list(rspecs)
+        if len(rspecs) != qb.nq or (mspecs is not None and len(list(mspecs)) != qb.nq):
+            raise ValueError(f"one range spec (and metrics spec, if any) per query for {qb.nq} queries")
+        rspec = _range_specs(rspecs, qb.nq)
+        mspec = _metrics_specs(list(mspecs), qb.nq) if mspecs is not None else None
+        stride = int(rspec["n_buckets"][:qb.nq].max(initial=1))
+        n = max(qb.nq, 1)
+        counts = np.zeros((n, stride), dtype=np.uint64)
+        parts = np.zeros((n, stride, TQ_METRICS_MAX_COLUMNS), dtype=METRIC_PART_DTYPE) if mspec is not None else None
+        hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+        _check(LIB.tq_range_batch(self.h, qb.ptr, rspec.ctypes.data_as(C.POINTER(RangeSpec)),
+                                  mspec.ctypes.data_as(C.POINTER(MetricsSpec)) if mspec is not None else None, qb.nq, stride,
+                                  ptr(counts, u64p), parts.ctypes.data_as(C.POINTER(MetricPart)) if parts is not None else None,
+                                  ptr(hits, u64p)), self.h)
+        out = (counts[:qb.nq], parts[:qb.nq] if parts is not None else None)
+        return out + (hits[:qb.nq],) if count_hits else out
+
     def terms_metrics_batch(self, qb: QueryBatch, tspecs, mspecs, orders=None, count_hits=False, stride=None):
         """A terms aggregation with metric sub-aggregations per query (tq_terms_metrics_batch) over sort columns; tspecs = one terms
         spec per query as terms_batch takes them (target also TQ_TERMS_BY_METRIC), mspecs = one list of 1..4 metric columns per query
@@ -619,6 +660,9 @@ class Context:
         tm = TermsMetricsStats()
         _check(LIB.tq_get_terms_metrics_stats(self.h, C.byref(tm)), self.h)
         out.update({name: getattr(tm, name) for name, _ in TermsMetricsStats._fields_})
+        rs = RangeStats()
+        _check(LIB.tq_get_range_stats(self.h, C.byref(rs)), self.h)
+        out.update({name: getattr(rs, name) for name, _ in RangeStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
