@@ -288,10 +288,15 @@ int tq_ctx_create(int device, tq_ctx** out) {
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
   c->tile_scratch_mb = env_u32("TQ_TILE_SCRATCH_MB", (uint32_t)(total_bytes / 8 >> 20));
-  c->tile_sample_div = env_u32("TQ_TILE_SAMPLE_DIV", 32);    // share of the tiles in the sample launch (0/1: none)
+  // share of the tiles in the sample launch (0/1: none).  1/64: the running threshold of the exact launches raises what the
+  // samples leave within a few tiles, so a sample launch over twice the tiles costs more than its better seed saves (DESIGN §6)
+  c->tile_sample_div = env_u32("TQ_TILE_SAMPLE_DIV", 64);
   c->tile_round_div1 = env_u32("TQ_TILE_ROUND_DIV1", 8);     // the exact launches end at 1/8, 1/2 and all of a segment's tiles
   c->tile_round_div2 = env_u32("TQ_TILE_ROUND_DIV2", 2);
-  c->tile_light_max = env_u32("TQ_TILE_LIGHT_MAX", 96);      // essential postings up to which a (query, tile) pair is evaluated posting by posting
+  // essential postings up to which a (query, tile) pair is evaluated posting by posting.  Above it a pair takes one of the
+  // CTA's two window warps while its other six wait at the barrier after B3; B2 deals the postings of a pair of a few hundred
+  // to all eight warps, so only the largest pairs are worth a window (DESIGN §6)
+  c->tile_light_max = env_u32("TQ_TILE_LIGHT_MAX", 384);
   c->tile_counters = env_u32("TQ_TILE_COUNTERS", 0);         // diagnostics (tile_counters of tq_stats)
   c->tile_ops = env_u32("TQ_TILE_OPS", 7);                  // bit 0 term, 1 AND, 2 OR
   c->tile_cand_floor = env_u32("TQ_TILE_CAND_FLOOR", 32768);  // smallest candidate region of a tile query (test hook: tiny regions overflow)

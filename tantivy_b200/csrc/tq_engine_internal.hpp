@@ -268,7 +268,7 @@ struct tq_ctx {
   uint32_t terms_metrics_budget;  // (kept entry, column) parts one tq_terms_metrics_batch wave may hold
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
-  uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 32, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 96, tile_counters = 0;
+  uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 64, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 384, tile_counters = 0;
   uint32_t tile_ops = 7;  // bit per TQ_OP_*: which query shapes the tile engine takes
   uint32_t tile_seg_cap_hook = 0;
   uint32_t tile_windows = 0;
