@@ -289,6 +289,24 @@ typedef struct {
   uint64_t range_tiles_one_bucket;
 } tq_range_stats;
 int tq_get_range_stats(tq_ctx*, tq_range_stats* out);
+/* Cumulative since ctx creation: tq_terms_histogram_batch.  Device time of its kernels over all waves (k_terms, k_terms_select,
+ * k_terms_mark, k_terms_hist, k_terms_hist_final), their CTAs, the 8192-doc tiles k_terms_hist came to, and of those the ones whose
+ * docs with a key all hold one kept key (no key gather), the ones whose histogram values are all in bounds and in one bucket (no
+ * value gather), and the ones with both (each warp's matches added to one cell), the waves, and the k_terms_hist units that counted
+ * in shared memory (their window of kept slots × buckets fits 8192 cells) and in the wave's grid.  A struct of its own, so that the
+ * other stats keep their layouts. */
+typedef struct {
+  float terms_hist_ms;
+  uint64_t units_terms_hist;
+  uint64_t terms_hist_tiles_seen;
+  uint64_t terms_hist_tiles_one_key;
+  uint64_t terms_hist_tiles_one_bucket;
+  uint64_t terms_hist_tiles_both;
+  uint64_t terms_hist_waves;
+  uint64_t terms_hist_units_shared;
+  uint64_t terms_hist_units_global;
+} tq_terms_hist_stats;
+int tq_get_terms_hist_stats(tq_ctx*, tq_terms_hist_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -605,6 +623,29 @@ static_assert(sizeof(tq_range_spec) == 1032, "range ABI layout");
 #endif
 int tq_range_batch(tq_ctx*, const tq_query* queries, const tq_range_spec* rspecs, const tq_metrics_spec* mspecs, size_t nq,
                    uint32_t out_stride, uint64_t* out_doc_count, tq_metric_part* out_parts, uint64_t* out_hits);
+
+/* A terms aggregation whose only sub-aggregation is a histogram / date_histogram (one `terms` over one `histogram`, the fused
+ * collector of term_histogram.rs), synchronous like tq_count_batch, over the docs tq_count_batch counts.  tspecs[q] is query q's
+ * terms exactly as in tq_terms_batch (TQ_TERMS_BY_METRIC is TQ_ERR_INVALID_ARGUMENT), hspecs[q] its histogram exactly as in
+ * tq_histogram_batch.  Every doc the terms count under a key, the missing key's included, feeds that key's histogram: it counts in
+ * bucket pos when it has a histogram value inside the (query, segment)'s bounds, as tq_histogram_batch counts.
+ *   Rows.  Row q (out_stride entries apart) holds query q's kept entries over all its segments, ascending by (segment_ord, key), with
+ *   the doc counts, out_sum_other and out_error_bound exactly as tq_terms_batch writes them (a segment this context evaluates only
+ *   part of is not cut).  The cells of all queries follow one another in one array, query by query and entry by entry in row order:
+ *   entry i's non-empty buckets are cells out_cell_first[i] .. + out_cell_n[i] (absolute indices), out_cell_pos (i64) and
+ *   out_cell_count in ascending pos, and out_cells[q] counts query q's.  When some out_n[q] > out_stride or the cells of all
+ *   queries exceed cell_capacity, every out_n and out_cells is written and the call returns TQ_ERR_INVALID_ARGUMENT: retry with a
+ *   larger stride or capacity.  out_hits may be NULL; else out_hits[q] = tq_count_batch's answer.
+ *   Limits.  Those of tq_terms_batch and tq_histogram_batch (2^20 keys in a segment, 2^20 buckets in a query), and a (query,
+ *   segment) whose grid -- kept entries (every entry of a partial segment) times its bucket span -- exceeds the ctx's cell budget
+ *   (TQ_TERMS_HIST_BUDGET at ctx creation, in u32 cells, at most 2^28) returns TQ_ERR_UNSUPPORTED naming the query.  Queries run
+ *   in waves whose counters fit TQ_TERMS_COUNTER_BUDGET and whose grids fit TQ_TERMS_HIST_BUDGET.
+ *   Errors.  Those of tq_terms_batch and tq_histogram_batch.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The run holds its
+ *   columns as tq_sort_batch does. */
+int tq_terms_histogram_batch(tq_ctx*, const tq_query* queries, const tq_terms_spec* tspecs, const tq_histogram_spec* hspecs, size_t nq,
+                             uint32_t out_stride, uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n,
+                             uint64_t* out_sum_other, uint64_t* out_error_bound, uint64_t cell_capacity, uint64_t* out_cell_first,
+                             uint32_t* out_cell_n, int64_t* out_cell_pos, uint64_t* out_cell_count, uint32_t* out_cells, uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

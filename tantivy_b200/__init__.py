@@ -19,3 +19,5 @@ from . import terms_metrics  # noqa: E402  (terms with metric sub-aggregations: 
 from .terms_metrics import TermsMetricsRefused  # noqa: E402
 from . import ranges  # noqa: E402  (range aggregations, with or without metric sub-aggregations: request and result side)
 from .ranges import RangeRefused  # noqa: E402
+from . import terms_hist  # noqa: E402  (terms with one histogram sub-aggregation: request and result side)
+from .terms_hist import TermsHistRefused  # noqa: E402

@@ -254,6 +254,13 @@ class RangeStats(C.Structure):
     _fields_ = [("range_ms", C.c_float), ("units_range", C.c_uint64), ("range_tiles_seen", C.c_uint64), ("range_tiles_one_bucket", C.c_uint64)]
 
 
+class TermsHistStats(C.Structure):
+    """tq_terms_hist_stats — the cumulative counters of tq_terms_histogram_batch (tq_get_terms_hist_stats)."""
+    _fields_ = [("terms_hist_ms", C.c_float), ("units_terms_hist", C.c_uint64), ("terms_hist_tiles_seen", C.c_uint64),
+                ("terms_hist_tiles_one_key", C.c_uint64), ("terms_hist_tiles_one_bucket", C.c_uint64), ("terms_hist_tiles_both", C.c_uint64),
+                ("terms_hist_waves", C.c_uint64), ("terms_hist_units_shared", C.c_uint64), ("terms_hist_units_global", C.c_uint64)]
+
+
 def ptr(arr, typ):
     """numpy array -> ctypes pointer (array must stay alive while the pointer is used)."""
     if arr is None:

@@ -284,6 +284,9 @@ int tq_ctx_create(int device, tq_ctx** out) {
   c->terms_counter_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_COUNTER_BUDGET", 1u << 26));
   c->hist_metrics_budget = std::max<uint32_t>(1u, env_u32("TQ_HIST_METRICS_BUDGET", 1u << 22));
   c->terms_metrics_budget = std::max<uint32_t>(1u, env_u32("TQ_TERMS_METRICS_BUDGET", 1u << 22));
+  // histogram cells per wave of tq_terms_histogram_batch (64 MB of grid, 128 MB of cell list); test hook: a small budget runs a
+  // batch in many waves and refuses a wide (query, segment)
+  c->terms_hist_budget = std::min<uint32_t>(1u << 28, std::max<uint32_t>(1u, env_u32("TQ_TERMS_HIST_BUDGET", 1u << 24)));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -441,6 +444,21 @@ int tq_get_terms_metrics_stats(tq_ctx* c, tq_terms_metrics_stats* out) {
   out->terms_metrics_tiles_seen = c->terms_metrics_tiles_seen;
   out->terms_metrics_tiles_one_key = c->terms_metrics_tiles_one_key;
   out->terms_metrics_waves = c->terms_metrics_waves;
+  return TQ_OK;
+}
+
+int tq_get_terms_hist_stats(tq_ctx* c, tq_terms_hist_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->terms_hist_ms = (float)c->terms_hist_ms;
+  out->units_terms_hist = c->terms_hist_units;
+  out->terms_hist_tiles_seen = c->terms_hist_tiles_seen;
+  out->terms_hist_tiles_one_key = c->terms_hist_tiles_one_key;
+  out->terms_hist_tiles_one_bucket = c->terms_hist_tiles_one_bucket;
+  out->terms_hist_tiles_both = c->terms_hist_tiles_both;
+  out->terms_hist_units_shared = c->terms_hist_units_shared;
+  out->terms_hist_units_global = c->terms_hist_units_global;
+  out->terms_hist_waves = c->terms_hist_waves;
   return TQ_OK;
 }
 
@@ -2610,6 +2628,30 @@ static tq_metric_part uncomplement(tq_metric_part p) {
   return p;
 }
 
+// Waves of consecutive terms queries whose counters fit counter_budget and whose per-query load q_extra (the metric parts or the
+// histogram cells of their kept entries) fits extra_budget; a query above either runs alone (a wave holding neither yet takes any).  Shifts each TermsSeg's counters and
+// region to be relative to its wave; a wave's `extra` is where each query's load starts, in at[qi].
+struct TermsWave { size_t q0, q1; uint64_t counters, region, extra; };
+static std::vector<TermsWave> plan_terms_waves(const std::vector<uint64_t>& q_counters, const std::vector<uint64_t>& q_region,
+                                               const std::vector<uint64_t>& q_extra, uint64_t counter_budget, uint64_t extra_budget,
+                                               const std::vector<size_t>& q_seg, std::vector<TermsSeg>& tsegs, std::vector<uint64_t>* at = nullptr) {
+  std::vector<TermsWave> waves;
+  if (at) at->assign(q_counters.size(), 0);
+  for (size_t qi = 0; qi < q_counters.size(); ++qi) {
+    if (waves.empty() || ((waves.back().counters || waves.back().extra) && (waves.back().counters + q_counters[qi] > counter_budget ||
+                                                                            waves.back().extra + q_extra[qi] > extra_budget)))
+      waves.push_back(TermsWave{qi, qi, 0, 0, 0});
+    TermsWave& w = waves.back();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) { tsegs[si].counters += w.counters; tsegs[si].region += w.region; }
+    if (at) (*at)[qi] = w.extra;
+    w.q1 = qi + 1;
+    w.counters += q_counters[qi];
+    w.region += q_region[qi];
+    w.extra += q_extra[qi];
+  }
+  return waves;
+}
+
 int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* tspecs, const tq_metrics_spec* mspecs,
                            const tq_terms_metric_order* orders, size_t nq, uint32_t out_stride, uint32_t* out_segment_ord,
                            uint64_t* out_key, uint64_t* out_doc_count, tq_metric_part* out_parts, uint32_t* out_n,
@@ -2692,20 +2734,15 @@ int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_sp
   if (cp.units.empty()) return TQ_OK;
   // waves of consecutive queries whose counters fit the counter budget and whose kept entries' parts fit the metrics budget (a query
   // above either runs alone); counters and regions relative to the wave
-  struct Wave { size_t q0, q1; uint64_t counters, region; bool by_metric; };
-  std::vector<Wave> waves;
+  std::vector<uint64_t> q_parts(nq);
+  for (size_t qi = 0; qi < nq; ++qi) q_parts[qi] = q_region[qi] * kC;
+  std::vector<TermsWave> waves = plan_terms_waves(q_counters, q_region, q_parts, c->terms_counter_budget, c->terms_metrics_budget, q_seg, tsegs);
   uint64_t max_counters = 0, max_region = 0;
   size_t max_segs = 0;
-  for (size_t qi = 0; qi < nq; ++qi) {
-    if (waves.empty() || (waves.back().counters && (waves.back().counters + q_counters[qi] > c->terms_counter_budget ||
-                                                    (waves.back().region + q_region[qi]) * kC > c->terms_metrics_budget)))
-      waves.push_back(Wave{qi, qi, 0, 0, false});
-    Wave& w = waves.back();
-    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) { tsegs[si].counters += w.counters; tsegs[si].region += w.region; }
-    w.q1 = qi + 1;
-    w.counters += q_counters[qi];
-    w.region += q_region[qi];
-    w.by_metric = w.by_metric || tspecs[qi].target == TQ_TERMS_BY_METRIC;
+  std::vector<bool> wave_by_metric(waves.size(), false);
+  for (size_t wi = 0; wi < waves.size(); ++wi) {
+    const TermsWave& w = waves[wi];
+    for (size_t qi = w.q0; qi < w.q1; ++qi) wave_by_metric[wi] = wave_by_metric[wi] || tspecs[qi].target == TQ_TERMS_BY_METRIC;
     max_counters = std::max(max_counters, w.counters);
     max_region = std::max(max_region, w.region);
     max_segs = std::max(max_segs, q_seg[w.q1] - q_seg[w.q0]);
@@ -2761,27 +2798,29 @@ int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_sp
   float ms_total = 0;
   uint64_t ctas = 0;
   const uint8_t* h = b->res_pin.p;
-  for (const Wave& w : waves) {
+  for (size_t wi = 0; wi < waves.size(); ++wi) {
+    const TermsWave& w = waves[wi];
+    const bool by_metric = wave_by_metric[wi];
     const size_t sa = q_seg[w.q0], sb = q_seg[w.q1], ua = q_unit[w.q0], ub = q_unit[w.q1];
     if (sa == sb) continue;
     P.t.unit_base = (uint32_t)ua;
     P.t.seg_base = (uint32_t)sa;
     TQ_CUDA(cudaMemsetAsync(d + r_missing, 0, r_counters + w.counters * 4 - r_missing, b->stream));  // missing .. counters
     TQ_CUDA(cudaMemsetAsync(d + r_parts, 0, w.region * part_row, b->stream));
-    if (w.by_metric) TQ_CUDA(cudaMemsetAsync(d + r_ocount, 0, r_oq + w.counters * 8 - r_ocount, b->stream));
+    if (by_metric) TQ_CUDA(cudaMemsetAsync(d + r_ocount, 0, r_oq + w.counters * 8 - r_ocount, b->stream));
     TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
     const unsigned nu = (unsigned)(ub - ua), ns = (unsigned)(sb - sa);
     if (nu) {
       (cp.mixed ? k_terms<true> : k_terms<false>)<<<nu, kThreads, 0, b->stream>>>(P.t);
       TQ_CUDA(cudaGetLastError());
-      if (w.by_metric) {
+      if (by_metric) {
         (cp.mixed ? k_terms_order<true> : k_terms_order<false>)<<<nu, kThreads, 0, b->stream>>>(P);
         TQ_CUDA(cudaGetLastError());
       }
     }
     k_terms_select<<<ns, kThreads, 0, b->stream>>>(P.t);
     TQ_CUDA(cudaGetLastError());
-    if (w.by_metric) {
+    if (by_metric) {
       k_terms_select_metric<<<ns, kThreads, 0, b->stream>>>(P);
       TQ_CUDA(cudaGetLastError());
     }
@@ -2792,7 +2831,7 @@ int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_sp
       TQ_CUDA(cudaGetLastError());
     }
     TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
-    ctas += (w.by_metric ? 3u : 2u) * (uint64_t)nu + (w.by_metric ? 3u : 2u) * (uint64_t)ns;
+    ctas += (by_metric ? 3u : 2u) * (uint64_t)nu + (by_metric ? 3u : 2u) * (uint64_t)ns;
     TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + head_bytes, r_key - head_bytes + w.region * 8, cudaMemcpyDeviceToHost, b->stream));
     TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_count - head_bytes), d + r_count, w.region * 4, cudaMemcpyDeviceToHost, b->stream));
     TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_parts - head_bytes), d + r_parts, w.region * part_row, cudaMemcpyDeviceToHost, b->stream));
@@ -2865,6 +2904,304 @@ int tq_terms_metrics_batch(tq_ctx* c, const tq_query* queries, const tq_terms_sp
     c->terms_metrics_waves += waves.size();
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride: out_n holds how many");
+  return TQ_OK;
+}
+
+// ---- histogram per term --------------------------------------------------------------------------------------
+int tq_terms_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_terms_spec* tspecs, const tq_histogram_spec* hspecs, size_t nq,
+                             uint32_t out_stride, uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n,
+                             uint64_t* out_sum_other, uint64_t* out_error_bound, uint64_t cell_capacity, uint64_t* out_cell_first,
+                             uint32_t* out_cell_n, int64_t* out_cell_pos, uint64_t* out_cell_count, uint32_t* out_cells, uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !tspecs || !hspecs || !out_n || !out_sum_other || !out_error_bound || !out_cells ||
+                    (out_stride && (!out_segment_ord || !out_key || !out_doc_count || !out_cell_first || !out_cell_n)) ||
+                    (cell_capacity && (!out_cell_pos || !out_cell_count)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const tq_terms_spec& sp = tspecs[qi];
+    const tq_histogram_spec& hs = hspecs[qi];
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "terms of phrase queries are not on the device path");
+    if (sp.target > TQ_TERMS_BY_KEY || sp.order > TQ_ORDER_ASC || sp.missing_mode > TQ_TERMS_MISSING_AFTER_MAX || !sp.segment_size)
+      return fail(TQ_ERR_INVALID_ARGUMENT, "terms spec: target, order, missing mode or segment_size");
+    if (hs.kind > TQ_FAST_DATE) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram kind");
+    if (!(hs.interval > 0.0) || !std::isfinite(hs.interval)) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram interval must be finite and > 0");
+  }
+  for (size_t qi = 0; qi < nq; ++qi) {
+    out_n[qi] = out_cells[qi] = 0;
+    out_sum_other[qi] = out_error_bound[qi] = 0;
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<TermsSeg> tsegs;      // parallel to cp.segs
+  std::vector<HistSeg> hsegs;       // parallel to cp.segs
+  std::vector<TermsHistSeg> gsegs;  // parallel to cp.segs
+  std::vector<HistUnit> windows;    // parallel to cp.units: the unit's keys
+  std::vector<HistUnit> hunits;     // parallel to cp.units: the unit's buckets
+  std::vector<HistQuery> hq(nq);
+  std::vector<size_t> q_seg(nq + 1), q_unit(nq + 1);
+  std::vector<uint64_t> q_counters(nq, 0), q_region(nq, 0), q_cells(nq, 0);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<unsigned long long, unsigned long long>> uwin;
+    std::vector<std::pair<long long, long long>> hwin;  // per unit of the query: its first and last pos (first > last: none)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_terms_spec& sp = tspecs[qi];
+      const tq_histogram_spec& hs = hspecs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_seg[qi] = s0;
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      const uint32_t flags = (out_hits ? kTermsHits : 0u) | (sp.missing_mode != TQ_TERMS_MISSING_NONE ? kTermsMissing : 0u) |
+                             (sp.target == TQ_TERMS_BY_KEY ? kTermsByKey : 0u) | (sp.order == TQ_ORDER_ASC ? kTermsAsc : 0u);
+      rc = plan_terms_query(c, sp, qi, flags, cp, s0, u0, tsegs, windows, cols, uwin, q_counters[qi], q_region[qi]);
+      if (rc != TQ_OK) return rc;
+      long long qbase = 0;
+      uint64_t qlen = 0;
+      rc = plan_hist_query(c, hs, qi, cp, s0, u0, kHistMaxBins, hsegs, cols, hwin, qbase, qlen);
+      if (rc != TQ_OK) return rc;
+      // per (query, segment): the union of its units' buckets, then each unit's window relative to its first
+      std::vector<std::pair<long long, long long>> sspan(cp.segs.size() - s0, {1, 0});
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const auto& w = hwin[ui - u0];
+        if (w.first > w.second) continue;
+        auto& s = sspan[cp.units[ui].qseg - s0];
+        s = s.first > s.second ? w : std::make_pair(std::min(s.first, w.first), std::max(s.second, w.second));
+      }
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        const auto& s = sspan[si - s0];
+        const TermsSeg& z = tsegs[si];
+        const uint32_t span = s.first <= s.second ? (uint32_t)(s.second - s.first + 1) : 0u;
+        const uint64_t rows = std::min<uint64_t>(z.segment_size, (uint64_t)z.n_keys + ((z.flags & kTermsMissing) ? 1u : 0u));
+        if (rows * span > c->terms_hist_budget)
+          return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": the histogram cells of its entries in a segment exceed the device budget (take the CPU path)");
+        gsegs.push_back(TermsHistSeg{q_cells[qi], span ? s.first : 0ll, span, 0u});
+        q_cells[qi] += rows * span;
+      }
+      if (q_cells[qi] > (1ull << 31))
+        return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": the histogram cells of its entries exceed 2^31 (take the CPU path)");
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const auto& w = hwin[ui - u0];
+        hunits.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - gsegs[cp.units[ui].qseg].base), (uint32_t)(w.second - w.first + 1)}
+                                             : HistUnit{0u, 0u});
+      }
+      hq[qi] = HistQuery{hs.interval, hs.offset, 0ll, 0ull, 0u, hs.kind, 0u, 0u};
+    }
+    q_seg[nq] = cp.segs.size();
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      b->held_columns.push_back(tspecs[qi].column_id);
+      b->held_columns.push_back(hspecs[qi].column_id);
+    }
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // waves of consecutive queries whose counters fit the counter budget and whose grids fit the cell budget (a query above either
+  // runs alone); counters, regions and grids relative to the wave
+  std::vector<uint64_t> at;
+  const std::vector<TermsWave> waves = plan_terms_waves(q_counters, q_region, q_cells, c->terms_counter_budget, c->terms_hist_budget, q_seg, tsegs, &at);
+  for (size_t qi = 0; qi < nq; ++qi)
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) gsegs[si].grid += at[qi];
+  uint64_t max_counters = 0, max_region = 0, max_cells = 0;
+  size_t max_segs = 0;
+  for (const TermsWave& w : waves) {
+    max_counters = std::max(max_counters, w.counters);
+    max_region = std::max(max_region, w.region);
+    max_cells = std::max(max_cells, w.extra);
+    max_segs = std::max(max_segs, q_seg[w.q1] - q_seg[w.q0]);
+  }
+  // descriptors: one H2D copy; scratch: hits | tile counters, then one wave's per-(query, segment) results | kept entries | their
+  // first cells | the cursor | the cell list, then the wave's accumulators: missing counters and slots | counters | the grid
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(tsegs), o_h = st.add(windows),
+               o_hz = st.add(hsegs), o_q = st.add(hq), o_g = st.add(gsegs), o_hu = st.add(hunits);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_ttiles = take(16), r_tiles = take(48), head_bytes = off;
+  const size_t r_n = take(max_segs * 4), r_other = take(max_segs * 8), r_err = take(max_segs * 8), r_key = take(max_region * 8),
+               r_count = take(max_region * 4), r_first = take(max_region * 4), r_total = take(max_segs * 4), r_cursor = take(8),
+               r_cpos = take(max_cells * 4), r_ccount = take(max_cells * 4), wave_bytes = off - head_bytes;
+  const size_t r_missing = take(max_segs * 4), r_mslot = take(max_segs * 4), r_counters = take(max_counters * 4), r_grid = take(max_cells * 4);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  TermsHistParams P{};
+  P.t.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                      reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.t.tsegs = st.on_device<const TermsSeg>(o_z);
+  P.t.windows = st.on_device<const HistUnit>(o_h);
+  P.t.counts = reinterpret_cast<uint32_t*>(d + r_counters);
+  P.t.missing = reinterpret_cast<uint32_t*>(d + r_missing);
+  P.t.tiles = reinterpret_cast<unsigned long long*>(d + r_ttiles);
+  P.t.res_key = reinterpret_cast<unsigned long long*>(d + r_key);
+  P.t.res_count = reinterpret_cast<uint32_t*>(d + r_count);
+  P.t.res_n = reinterpret_cast<uint32_t*>(d + r_n);
+  P.t.res_other = reinterpret_cast<unsigned long long*>(d + r_other);
+  P.t.res_error = reinterpret_cast<unsigned long long*>(d + r_err);
+  P.hsegs = st.on_device<const HistSeg>(o_hz);
+  P.queries = st.on_device<const HistQuery>(o_q);
+  P.gsegs = st.on_device<const TermsHistSeg>(o_g);
+  P.hunits = st.on_device<const HistUnit>(o_hu);
+  P.mslot = reinterpret_cast<const uint32_t*>(d + r_mslot);
+  P.grid = reinterpret_cast<uint32_t*>(d + r_grid);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  P.cell_first = reinterpret_cast<uint32_t*>(d + r_first);
+  P.cell_pos = reinterpret_cast<uint32_t*>(d + r_cpos);
+  P.cell_count = reinterpret_cast<uint32_t*>(d + r_ccount);
+  P.cell_total = reinterpret_cast<uint32_t*>(d + r_total);
+  P.cursor = reinterpret_cast<unsigned long long*>(d + r_cursor);
+  TermsMetricsParams M{};  // k_terms_mark's view: the terms and the missing key's slot
+  M.mslot = reinterpret_cast<uint32_t*>(d + r_mslot);
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  // per (query, segment): its kept entries (ascending key) with their non-empty cells, and its scalars, gathered wave by wave
+  struct Entry { unsigned long long key; uint32_t count; std::vector<std::pair<long long, uint32_t>> cells; };
+  std::vector<std::vector<Entry>> kept(cp.segs.size());
+  std::vector<uint64_t> seg_other(cp.segs.size()), seg_err(cp.segs.size());
+  float ms_total = 0;
+  uint64_t ctas = 0;
+  const uint8_t* h = b->res_pin.p;
+  auto hp = [&](size_t r) { return h + (r - head_bytes); };
+  for (const TermsWave& w : waves) {
+    const size_t sa = q_seg[w.q0], sb = q_seg[w.q1], ua = q_unit[w.q0], ub = q_unit[w.q1];
+    if (sa == sb) continue;
+    P.t.unit_base = (uint32_t)ua;
+    P.t.seg_base = (uint32_t)sa;
+    M.t = P.t;
+    TQ_CUDA(cudaMemsetAsync(d + r_missing, 0, r_counters + w.counters * 4 - r_missing, b->stream));  // missing .. counters
+    TQ_CUDA(cudaMemsetAsync(d + r_grid, 0, w.extra * 4, b->stream));
+    TQ_CUDA(cudaMemsetAsync(d + r_cursor, 0, 8, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    const unsigned nu = (unsigned)(ub - ua), ns = (unsigned)(sb - sa);
+    if (nu) {
+      (cp.mixed ? k_terms<true> : k_terms<false>)<<<nu, kThreads, 0, b->stream>>>(P.t);
+      TQ_CUDA(cudaGetLastError());
+    }
+    k_terms_select<<<ns, kThreads, 0, b->stream>>>(P.t);
+    TQ_CUDA(cudaGetLastError());
+    k_terms_mark<<<ns, kThreads, 0, b->stream>>>(M);
+    TQ_CUDA(cudaGetLastError());
+    if (nu) {
+      (cp.mixed ? k_terms_hist<true> : k_terms_hist<false>)<<<nu, kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    k_terms_hist_final<<<ns, kThreads, 0, b->stream>>>(P);
+    TQ_CUDA(cudaGetLastError());
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    ctas += 2u * (uint64_t)nu + 3u * (uint64_t)ns;
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + head_bytes, r_key - head_bytes + w.region * 8, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_count - head_bytes), d + r_count, w.region * 4, cudaMemcpyDeviceToHost, b->stream));
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_first - head_bytes), d + r_first, r_cpos - r_first, cudaMemcpyDeviceToHost, b->stream));  // first cells .. cursor
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    unsigned long long n_cells;
+    memcpy(&n_cells, hp(r_cursor), 8);
+    if (n_cells) {  // the cell list, only as long as it is
+      TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_cpos - head_bytes), d + r_cpos, n_cells * 4, cudaMemcpyDeviceToHost, b->stream));
+      TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_ccount - head_bytes), d + r_ccount, n_cells * 4, cudaMemcpyDeviceToHost, b->stream));
+      TQ_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    for (size_t si = sa; si < sb; ++si) {
+      const size_t rel = si - sa;
+      uint32_t n, total;
+      memcpy(&n, hp(r_n) + rel * 4, 4);
+      memcpy(&total, hp(r_total) + rel * 4, 4);
+      memcpy(&seg_other[si], hp(r_other) + rel * 8, 8);
+      memcpy(&seg_err[si], hp(r_err) + rel * 8, 8);
+      kept[si].resize(n);
+      uint32_t seg_first = 0;
+      if (n) memcpy(&seg_first, hp(r_first) + tsegs[si].region * 4, 4);
+      for (uint32_t j = 0; j < n; ++j) {
+        const size_t e = tsegs[si].region + j;
+        Entry& x = kept[si][j];
+        memcpy(&x.key, hp(r_key) + e * 8, 8);
+        memcpy(&x.count, hp(r_count) + e * 4, 4);
+        uint32_t first, end = seg_first + total;
+        memcpy(&first, hp(r_first) + e * 4, 4);
+        if (j + 1 < n) memcpy(&end, hp(r_first) + (e + 1) * 4, 4);
+        x.cells.resize(end - first);
+        for (uint32_t k = first; k < end; ++k) {
+          uint32_t pos, count;
+          memcpy(&pos, hp(r_cpos) + (size_t)k * 4, 4);
+          memcpy(&count, hp(r_ccount) + (size_t)k * 4, 4);
+          x.cells[k - first] = {gsegs[si].base + (long long)pos, count};
+        }
+      }
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  unsigned long long tiles[6];
+  memcpy(tiles, h + r_tiles, 48);
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  // rows: each query's segments by segment_ord, each in ascending key; cells: each entry's in ascending pos, in row order, the
+  // queries' cells one after the other
+  bool fits = true;
+  std::vector<size_t> by_ord;
+  uint64_t nc = 0;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    by_ord.clear();
+    for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) by_ord.push_back(si);
+    std::sort(by_ord.begin(), by_ord.end(), [&](size_t x, size_t y) { return cp.segment_ords[x] < cp.segment_ords[y]; });
+    uint32_t n = 0;
+    const uint64_t nc0 = nc;
+    for (size_t si : by_ord) {
+      out_sum_other[qi] += seg_other[si];
+      out_error_bound[qi] += seg_err[si];
+      for (const Entry& e : kept[si]) {
+        if (n < out_stride) {
+          const size_t at = qi * (size_t)out_stride + n;
+          out_segment_ord[at] = cp.segment_ords[si];
+          out_key[at] = e.key;
+          out_doc_count[at] = e.count;
+          out_cell_first[at] = nc;
+          out_cell_n[at] = (uint32_t)e.cells.size();
+        }
+        for (const auto& cell : e.cells) {
+          if (nc < cell_capacity) {
+            out_cell_pos[nc] = cell.first;
+            out_cell_count[nc] = cell.second;
+          }
+          ++nc;
+        }
+        ++n;
+      }
+    }
+    out_n[qi] = n;
+    out_cells[qi] = (uint32_t)(nc - nc0);
+    fits = fits && n <= out_stride;
+  }
+  fits = fits && nc <= cell_capacity;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->terms_hist_ms += ms_total;
+    c->terms_hist_units += ctas;
+    c->terms_hist_tiles_seen += tiles[0];
+    c->terms_hist_tiles_one_key += tiles[1];
+    c->terms_hist_tiles_one_bucket += tiles[2];
+    c->terms_hist_tiles_both += tiles[3];
+    c->terms_hist_units_shared += tiles[4];
+    c->terms_hist_units_global += tiles[5];
+    c->terms_hist_waves += waves.size();
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride, or the cells exceed cell_capacity: out_n and out_cells hold how many");
   return TQ_OK;
 }
 

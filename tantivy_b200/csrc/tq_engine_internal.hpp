@@ -257,6 +257,11 @@ struct tq_ctx {
   // ... and of the range runs, with and without metrics (range_ms, units, tiles seen / in one bucket)
   double range_ms = 0;
   uint64_t range_units = 0, range_tiles_seen = 0, range_tiles_one_bucket = 0;
+  // ... and of the terms-with-histogram runs (terms_hist_ms, units, tiles seen / with one kept key / in one bucket / both, waves,
+  // k_terms_hist units counting in shared memory / in the grid)
+  double terms_hist_ms = 0;
+  uint64_t terms_hist_units = 0, terms_hist_tiles_seen = 0, terms_hist_tiles_one_key = 0, terms_hist_tiles_one_bucket = 0,
+           terms_hist_tiles_both = 0, terms_hist_waves = 0, terms_hist_units_shared = 0, terms_hist_units_global = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;
@@ -266,6 +271,7 @@ struct tq_ctx {
   uint32_t terms_counter_budget;  // u32 counters one tq_terms_batch wave may hold
   uint32_t hist_metrics_budget;   // (bucket, column) accumulators one tq_histogram_metrics_batch wave may hold
   uint32_t terms_metrics_budget;  // (kept entry, column) parts one tq_terms_metrics_batch wave may hold
+  uint32_t terms_hist_budget;     // u32 (kept entry, bucket) cells one tq_terms_histogram_batch wave may hold
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 64, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 384, tile_counters = 0;

@@ -2760,6 +2760,159 @@ __global__ void __launch_bounds__(kThreads, 2) k_terms_metrics(const TermsMetric
   }
 }
 
+// ---- histogram per term (terms with one histogram sub-aggregation: collect_terms_with_docs, term_histogram.rs) ---------------
+// One CTA per Count unit, after k_terms_mark: the docs k_terms counted, each with a histogram value in its (query, segment)'s
+// bounds counted in cell (slot of its key, pos); docs of keys cut count nowhere, docs without a key go to the missing key's slot.
+// Per tile, thread 0 reads both columns' SortTile: a tile whose values all hold one kept key skips the key gather, a tile whose
+// histogram values are all in bounds and in one bucket (HistKeys::one) skips the value gather, and a tile with both adds each warp's
+// count of matching docs with both values to one cell.  A unit whose window (kept slots × its buckets) fits kTermsHistSmemCells
+// counts in shared memory (one u32 atomic per doc) and adds its non-zero cells to the grid at exit; a wider one counts in the grid.
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 3) k_terms_hist(const TermsHistParams P) {
+  constexpr uint32_t kPerDoc = 0xFFFFFFFFu, kSkip = 0xFFFFFFFEu;  // s_slot: look each doc's key up; no doc with a key is counted
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ uint32_t s_cells[kTermsHistSmemCells];
+  __shared__ uint32_t s_slot, s_bucket;
+  const uint32_t unit = P.t.unit_base + blockIdx.x;
+  const Unit U = P.t.c.units[unit];
+  const uint32_t rel = U.qseg - P.t.seg_base, n_kept = P.t.res_n[rel];
+  const HistUnit W = P.hunits[unit];
+  if (!n_kept || !W.n_bins) return;  // (CTA-uniform: nothing of the unit can be counted)
+  const CountSeg S = P.t.c.segs[U.qseg];
+  const TermsSeg Z = P.t.tsegs[U.qseg];
+  const HistSeg H = P.hsegs[U.qseg];
+  const HistQuery Q = P.queries[S.query];
+  const TermsHistSeg G = P.gsegs[U.qseg];
+  const uint32_t* const cnt = P.t.counts + Z.counters;
+  const long long base = G.base + (long long)W.first;  // pos of the window's first bucket
+  const bool shared = n_kept * W.n_bins <= kTermsHistSmemCells;  // (n_kept * n_bins <= the grid budget < 2^32)
+  uint32_t* const gcells = P.grid + G.grid + W.first;
+  uint32_t* const cells = shared ? s_cells : gcells;
+  const uint32_t row = shared ? W.n_bins : G.span;  // cell (slot, b) of the window: cells[slot * row + b]
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < n_kept * W.n_bins; i += blockDim.x) s_cells[i] = 0;
+  uint32_t ms = kSkip;  // the missing key's slot (CTA-uniform)
+  if (Z.flags & kTermsMissing) {
+    const uint32_t c = Z.missing - Z.base < (unsigned long long)Z.n_keys ? cnt[Z.missing - Z.base] : P.mslot[rel];
+    if (c & kTermsSlot) ms = c & ~kTermsSlot;
+  }
+  const uint32_t wb = S.words_base, ng = P.t.c.words[wb], need = P.t.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u;
+  uint32_t n_one_key = 0, n_one_bucket = 0, n_both = 0;
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      const SortTile T = Z.tiles[tile];
+      uint32_t slot = kSkip;
+      if ((T.flags & kSortTileValues) && T.best[0] == ~T.best[1]) {
+        const unsigned long long i = T.best[0] - Z.base;
+        const uint32_t c = i < (unsigned long long)Z.n_keys ? cnt[i] : 0u;
+        if (c & kTermsSlot) slot = c & ~kTermsSlot;
+      } else if (T.flags & kSortTileValues) {
+        slot = kPerDoc;
+      }
+      const SortTile V = H.tiles[tile];
+      uint32_t b = 0xFFFFFFFFu;
+      if (V.flags & kSortTileValues) HistKeys::one(V, H, Q, W, base, b);
+      s_slot = slot;
+      s_bucket = b;
+      n_one_key += slot < kSkip ? 1u : 0u;
+      n_one_bucket += b != 0xFFFFFFFFu ? 1u : 0u;
+      n_both += slot < kSkip && b != 0xFFFFFFFFu ? 1u : 0u;
+    }
+    match_tile<kMixed>(P.t.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    const uint32_t kp = Z.present ? __ldg(Z.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+    const uint32_t hp = H.present ? __ldg(H.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+    const uint32_t slot = s_slot, b1 = s_bucket;
+    const uint32_t kd = slot == kSkip ? 0u : bits & kp & hp;  // matching docs with a key (that may be kept) and a histogram value
+    const uint32_t md = ms == kSkip ? 0u : bits & ~kp & hp;   // ... without a key, with a histogram value
+    if (b1 != 0xFFFFFFFFu) {  // every histogram value of the tile counts in bucket b1
+      const uint32_t nm = __reduce_add_sync(kFull, (uint32_t)__popc(md));
+      if (lane == 0 && nm) atomicAdd(&cells[ms * row + b1], nm);
+      if (slot < kSkip) {
+        const uint32_t nk = __reduce_add_sync(kFull, (uint32_t)__popc(kd));
+        if (lane == 0 && nk) atomicAdd(&cells[slot * row + b1], nk);
+      } else {
+        for (uint32_t w = kd; w; w &= w - 1u) {
+          const uint32_t c = __ldg(cnt + (__ldg(Z.values + lo + threadIdx.x * 32u + (uint32_t)(__ffs(w) - 1)) - Z.base));
+          if (c & kTermsSlot) atomicAdd(&cells[(c & ~kTermsSlot) * row + b1], 1u);
+        }
+      }
+    } else {
+      for (uint32_t w = kd | md; w; w &= w - 1u) {
+        const uint32_t bit = (uint32_t)(__ffs(w) - 1), doc = lo + threadIdx.x * 32u + bit;
+        uint32_t s = ms;
+        if ((kd >> bit) & 1u) {
+          s = slot;
+          if (slot == kPerDoc) {  // (the counters cover every value of the visited tiles)
+            const uint32_t c = __ldg(cnt + (__ldg(Z.values + doc) - Z.base));
+            if (!(c & kTermsSlot)) continue;
+            s = c & ~kTermsSlot;
+          }
+        }
+        const double val = HistKeys::value(__ldg(H.values + doc), Q);
+        if (!HistKeys::counted(val, H)) continue;
+        const unsigned long long b = HistKeys::index(val, Q, base);
+        if (b < W.n_bins) atomicAdd(&cells[s * row + (uint32_t)b], 1u);  // (always: the window covers every counted value)
+      }
+    }
+    __syncthreads();
+  }
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < n_kept * W.n_bins; i += blockDim.x)
+      if (s_cells[i]) atomicAdd(&gcells[(i / W.n_bins) * G.span + i % W.n_bins], s_cells[i]);
+  if (threadIdx.x == 0) {
+    const uint32_t seen = U.end - U.begin;
+    if (seen) atomicAdd(&P.tiles[0], (unsigned long long)seen);
+    if (n_one_key) atomicAdd(&P.tiles[1], (unsigned long long)n_one_key);
+    if (n_one_bucket) atomicAdd(&P.tiles[2], (unsigned long long)n_one_bucket);
+    if (n_both) atomicAdd(&P.tiles[3], (unsigned long long)n_both);
+    atomicAdd(&P.tiles[shared ? 4 : 5], 1ull);
+  }
+}
+
+// One CTA per (query, segment) of a wave: its non-empty cells, slot by slot in ascending pos, into the wave's cell list.  A first
+// pass counts them and takes their place in the list (one atomic on the cursor), a second writes them with a CTA-wide prefix sum
+// per 256 cells of the flat grid and records each slot's first cell (the cells before its row).
+__global__ void __launch_bounds__(kThreads) k_terms_hist_final(const TermsHistParams P) {
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ unsigned long long s_at;
+  const uint32_t rel = blockIdx.x;
+  const TermsSeg Z = P.t.tsegs[P.t.seg_base + rel];
+  const TermsHistSeg G = P.gsegs[P.t.seg_base + rel];
+  const uint32_t n_kept = P.t.res_n[rel];
+  const uint32_t n = n_kept * G.span;  // (<= the grid budget)
+  const uint32_t* const cells = P.grid + G.grid;
+  uint32_t nz = 0;
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) nz += cells[i] ? 1u : 0u;
+  uint32_t total;
+  cta_scan_excl(nz, s_part, total);
+  if (threadIdx.x == 0) {
+    s_at = total ? atomicAdd(P.cursor, (unsigned long long)total) : 0ull;
+    P.cell_total[rel] = total;
+  }
+  __syncthreads();
+  const uint32_t at = (uint32_t)s_at;  // (the wave's list holds at most its grid's cells)
+  uint32_t done = 0;
+  for (uint32_t i0 = 0; i0 < n; i0 += blockDim.x) {
+    const uint32_t i = i0 + threadIdx.x;
+    const uint32_t c = i < n ? cells[i] : 0u;
+    uint32_t tot;
+    const uint32_t ex = done + cta_scan_excl(c ? 1u : 0u, s_part, tot);
+    if (i < n && i % G.span == 0u) P.cell_first[Z.region + i / G.span] = at + ex;
+    if (c) {
+      P.cell_pos[at + ex] = i % G.span;
+      P.cell_count[at + ex] = c;
+    }
+    done += tot;
+  }
+  if (!G.span)
+    for (uint32_t j = threadIdx.x; j < n_kept; j += blockDim.x) P.cell_first[Z.region + j] = at;
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

@@ -441,6 +441,38 @@ struct TermsMetricsParams {
 };
 static_assert(sizeof(TermsOrder) == 8, "terms order descriptor layout");
 
+// ---- histogram per term (k_terms_hist, k_terms_hist_final) --------------------------------------------------------------------
+// The terms of k_terms / k_terms_select / k_terms_mark (TermsSeg, the unit windows, the counters marked with each kept key's slot)
+// with the histogram of HistSeg / HistQuery / HistUnit.  Each (query, segment) has a u32 cell grid of (its region's entries) rows ×
+// (its bucket span) columns; k_terms_hist counts each doc the terms count under a kept key, and whose histogram value is in bounds,
+// in cell (slot, pos - base).  A unit whose window (kept slots × its buckets) has kTermsHistSmemCells or fewer cells counts in
+// shared memory and adds its non-zero cells to the grid at exit.  k_terms_hist_final compacts each (query, segment)'s non-empty
+// cells, slot by slot in ascending pos, into the wave's cell list.  Queries run in waves whose grids fit the ctx's budget.
+constexpr uint32_t kTermsHistSmemCells = 8192;
+struct TermsHistSeg {  // the grid of one (query, segment), parallel to CountParams::segs
+  unsigned long long grid;  // its first cell in TermsHistParams::grid (relative to the wave)
+  long long base;           // pos of column 0
+  uint32_t span;            // columns per slot (0: no value of the segment's visited tiles passes its bounds)
+  uint32_t pad;
+};
+struct TermsHistParams {
+  TermsParams t;                // the terms of the wave: counters (kept keys marked), missing counters, kept entries and scalars
+  const HistSeg* hsegs;         // parallel to t.c.segs: the histogram column and bounds
+  const HistQuery* queries;     // [nq]: interval, offset and kind of the query's histogram
+  const TermsHistSeg* gsegs;    // parallel to t.c.segs
+  const HistUnit* hunits;       // parallel to t.c.units: the unit's buckets, relative to its (query, segment)'s base
+  const uint32_t* mslot;        // [wave's (query, segment)s]: kTermsSlot | slot of a missing key outside the counters, or 0
+  uint32_t* grid;               // the wave's cells, zeroed before it
+  unsigned long long* tiles;    // [0] tiles seen, [1] of them with one kept key, [2] in one bucket, [3] both; units counting [4] in
+                                // shared memory, [5] in the grid
+  uint32_t* cell_first;         // [wave's region]: first cell of the entry in the wave's cell list (k_terms_hist_final)
+  uint32_t* cell_pos;           // the wave's cell list: pos - base of the (query, segment)
+  uint32_t* cell_count;
+  uint32_t* cell_total;         // [wave's (query, segment)s]: their non-empty cells
+  unsigned long long* cursor;   // cells the wave's list holds
+};
+static_assert(sizeof(TermsHistSeg) == 24, "terms histogram descriptor layout");
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

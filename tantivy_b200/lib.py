@@ -9,7 +9,7 @@ import numpy as np
 from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
                    MetricsSpec, MetricsStats, HistMetricsStats, TermsMetricsStats, TermsMetricOrder, TERMS_METRIC_ORDER_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
-                   RANGE_SPEC_DTYPE, RangeSpec, RangeStats, TQ_RANGE_MAX_BUCKETS, f32p, ptr, u8p, u32p, u64p)
+                   RANGE_SPEC_DTYPE, RangeSpec, RangeStats, TermsHistStats, TQ_RANGE_MAX_BUCKETS, f32p, ptr, u8p, u32p, u64p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -37,6 +37,7 @@ def _load():
     lib.tq_get_hist_metrics_stats.argtypes = [vp, C.POINTER(HistMetricsStats)]
     lib.tq_get_terms_metrics_stats.argtypes = [vp, C.POINTER(TermsMetricsStats)]
     lib.tq_get_range_stats.argtypes = [vp, C.POINTER(RangeStats)]
+    lib.tq_get_terms_hist_stats.argtypes = [vp, C.POINTER(TermsHistStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -60,6 +61,8 @@ def _load():
                                            C.c_uint32, u32p, u64p, u64p, C.POINTER(MetricPart), u32p, u64p, u64p, C.POINTER(MetricPart), u64p]
     lib.tq_range_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(RangeSpec), C.POINTER(MetricsSpec), sz, C.c_uint32, u64p, C.POINTER(MetricPart),
                                    u64p]
+    lib.tq_terms_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), C.POINTER(HistogramSpec), sz, C.c_uint32, u32p, u64p,
+                                             u64p, u32p, u64p, u64p, C.c_uint64, u64p, u32p, C.POINTER(C.c_int64), u64p, u32p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -367,6 +370,7 @@ class Context:
         self.device = device
         self._hist_metrics_stride = 0  # the widest row hist_metrics_batch has returned (its next first try)
         self._terms_metrics_stride = 0  # the widest row terms_metrics_batch has returned (its next first try)
+        self._terms_hist_sizes = (0, 0)  # the widest row and the most cells terms_hist_batch has returned (its next first try)
 
     def segment_register(self, segment_ord, field, max_doc, record_option, idx_body, fieldnorm=None, alive=None):
         idx_body = np.ascontiguousarray(idx_body, dtype=np.uint8)
@@ -611,6 +615,52 @@ class Context:
             out = (segs[:qb.nq], keys[:qb.nq], counts[:qb.nq], parts[:qb.nq], nb[:qb.nq], other[:qb.nq], error[:qb.nq], opart[:qb.nq])
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def terms_hist_batch(self, qb: QueryBatch, tspecs, hspecs, count_hits=False, stride=None, cell_capacity=None):
+        """A terms aggregation whose only sub-aggregation is a histogram, per query (tq_terms_histogram_batch) over sort columns;
+        tspecs = one terms spec per query as terms_batch takes them, hspecs = one histogram spec per query as histogram_batch takes
+        them (tantivy_b200.terms_hist turns requests into both).  Returns (segment_ord, key, doc_count, n, sum_other, error_bound,
+        cell_first, cell_n, cell_pos, cell_count, n_cells): row q holds the n[q] kept entries of query q as terms_batch returns them,
+        and entry j's non-empty buckets are cells cell_first[q, j] .. + cell_n[q, j] of the one cell array (pos, doc_count),
+        ascending pos; n_cells[q] counts query q's cells -- and with count_hits=True the Count of every query as well.  Raises TqError
+        with code -4 (TQ_ERR_UNSUPPORTED) when a (query, segment) is too wide for the device.  `stride` / `cell_capacity` are the
+        sizes tried first (default: the widest row and the most cells this context has returned, at least 1024 / 65536): larger
+        results run the batch again at their sizes."""
+        tspecs, hspecs = list(tspecs), list(hspecs)
+        if len(tspecs) != qb.nq or len(hspecs) != qb.nq:
+            raise ValueError(f"one terms and one histogram spec per query: {len(tspecs)} and {len(hspecs)} for {qb.nq} queries")
+        if stride is None:
+            stride = max(1024, self._terms_hist_sizes[0])
+        if cell_capacity is None:
+            cell_capacity = max(65536, self._terms_hist_sizes[1])
+        tspec, hspec = _terms_specs(tspecs, qb.nq), _histogram_specs(hspecs, qb.nq)
+        n = max(qb.nq, 1)
+        while True:
+            segs = np.empty((n, stride), dtype=np.uint32)  # (only the first n[q] entries of row q, and sum(n_cells) cells, are written)
+            keys = np.empty((n, stride), dtype=np.uint64)
+            counts = np.empty((n, stride), dtype=np.uint64)
+            first = np.empty((n, stride), dtype=np.uint64)
+            ncell = np.empty((n, stride), dtype=np.uint32)
+            pos = np.empty(cell_capacity, dtype=np.int64)
+            ccount = np.empty(cell_capacity, dtype=np.uint64)
+            nb = np.zeros(n, dtype=np.uint32)
+            nc = np.zeros(n, dtype=np.uint32)
+            other = np.zeros(n, dtype=np.uint64)
+            error = np.zeros(n, dtype=np.uint64)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_terms_histogram_batch(self.h, qb.ptr, tspec.ctypes.data_as(C.POINTER(TermsSpec)), hspec.ctypes.data_as(C.POINTER(HistogramSpec)),
+                                              qb.nq, stride, ptr(segs, u32p), ptr(keys, u64p), ptr(counts, u64p), ptr(nb, u32p), ptr(other, u64p),
+                                              ptr(error, u64p), cell_capacity, ptr(first, u64p), ptr(ncell, u32p),
+                                              pos.ctypes.data_as(C.POINTER(C.c_int64)), ptr(ccount, u64p), ptr(nc, u32p), ptr(hits, u64p))
+            total = int(nc.sum(dtype=np.uint64))
+            if rc == -1 and (int(nb.max()) > stride or total > cell_capacity):  # TQ_ERR_INVALID_ARGUMENT with the lengths: larger sizes
+                stride, cell_capacity = max(stride, int(nb.max())), max(cell_capacity, total)
+                continue
+            _check(rc, self.h)
+            self._terms_hist_sizes = (max(self._terms_hist_sizes[0], int(nb[:qb.nq].max(initial=0))), max(self._terms_hist_sizes[1], total))
+            out = (segs[:qb.nq], keys[:qb.nq], counts[:qb.nq], nb[:qb.nq], other[:qb.nq], error[:qb.nq], first[:qb.nq], ncell[:qb.nq],
+                   pos[:total], ccount[:total], nc[:qb.nq])
+            return out + (hits[:qb.nq],) if count_hits else out
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -663,6 +713,9 @@ class Context:
         rs = RangeStats()
         _check(LIB.tq_get_range_stats(self.h, C.byref(rs)), self.h)
         out.update({name: getattr(rs, name) for name, _ in RangeStats._fields_})
+        th = TermsHistStats()
+        _check(LIB.tq_get_terms_hist_stats(self.h, C.byref(th)), self.h)
+        out.update({name: getattr(th, name) for name, _ in TermsHistStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):

@@ -211,24 +211,32 @@ def _key_order(k):
     return (_RANK[k[0]], k[1])
 
 
-def finalize(req: TermsAggregation, merged):
-    """IntermediateTermBucketResult::into_final_result (intermediate_agg_result.rs:869-961) of merge()'s result: min_doc_count,
-    the order (equal counts by key ascending, where the reference leaves them unspecified), the cut to size."""
-    entries, other, error = merged
-    buckets = [(k, c) for k, c in entries.items() if c >= req.min_doc_count]
+def ordered_buckets(req: TermsAggregation, counts):
+    """The final buckets' keys of {key: doc_count}: min_doc_count, the order (`_count` or `_key`; equal counts by key ascending,
+    where the reference leaves them unspecified), the cut to size.  Returns ([(key, doc_count)] kept, doc count of the cut)."""
+    buckets = [(k, c) for k, c in counts.items() if c >= req.min_doc_count]
     if req.order_target == "_key":
         buckets.sort(key=lambda b: _key_order(b[0]), reverse=req.order == "desc")
     else:
         buckets.sort(key=lambda b: _key_order(b[0]))
         buckets.sort(key=lambda b: b[1], reverse=req.order == "desc")
-    cut = sum(c for _, c in buckets[req.size:])
-    out = []
-    for k, c in buckets[:req.size]:
-        e = {"key": _final_key(k)[1], "doc_count": c}
-        if k[0] == "bool":
-            e["key_as_string"] = "true" if k[1] else "false"
-        out.append(e)
-    res = {"buckets": out, "sum_other_doc_count": other + cut}
+    return buckets[:req.size], sum(c for _, c in buckets[req.size:])
+
+
+def bucket_entry(key, count):
+    """One final terms bucket {"key", "doc_count"[, "key_as_string"]} of an intermediate key."""
+    e = {"key": _final_key(key)[1], "doc_count": count}
+    if key[0] == "bool":
+        e["key_as_string"] = "true" if key[1] else "false"
+    return e
+
+
+def finalize(req: TermsAggregation, merged):
+    """IntermediateTermBucketResult::into_final_result (intermediate_agg_result.rs:869-961) of merge()'s result: ordered_buckets,
+    each as bucket_entry."""
+    entries, other, error = merged
+    kept, cut = ordered_buckets(req, entries)
+    res = {"buckets": [bucket_entry(k, c) for k, c in kept], "sum_other_doc_count": other + cut}
     if req.show_term_doc_count_error:
         res["doc_count_error_upper_bound"] = error
     return res
