@@ -307,6 +307,25 @@ typedef struct {
   uint64_t terms_hist_units_global;
 } tq_terms_hist_stats;
 int tq_get_terms_hist_stats(tq_ctx*, tq_terms_hist_stats* out);
+/* Cumulative since ctx creation: tq_histogram_terms_batch.  Device time of its kernels over all waves (k_hist_terms,
+ * k_hist_terms_final), their CTAs, the 8192-doc tiles k_hist_terms came to, and of those the ones whose values all hold one key (no
+ * key gather), the ones whose histogram values are all in bounds and in one bucket (no value gather), and the ones with both (each
+ * warp's matches added to one cell), the k_hist_terms units that counted in shared memory (their window of buckets × keys fits 8192
+ * cells) and in the wave's grid, the (segment, bucket) rows cut on the device, and the waves.  A struct of its own, so that the
+ * other stats keep their layouts. */
+typedef struct {
+  float hist_terms_ms;
+  uint64_t units_hist_terms;
+  uint64_t hist_terms_tiles_seen;
+  uint64_t hist_terms_tiles_one_key;
+  uint64_t hist_terms_tiles_one_bucket;
+  uint64_t hist_terms_tiles_both;
+  uint64_t hist_terms_units_shared;
+  uint64_t hist_terms_units_global;
+  uint64_t hist_terms_rows_cut;
+  uint64_t hist_terms_waves;
+} tq_hist_terms_stats;
+int tq_get_hist_terms_stats(tq_ctx*, tq_hist_terms_stats* out);
 
 /* Uploads one field of one segment to HBM (copied; caller keeps ownership of its mmap).
  * idx_body    = the field's sub-file of the `.idx` composite, INCLUDING the 8-byte
@@ -646,6 +665,32 @@ int tq_terms_histogram_batch(tq_ctx*, const tq_query* queries, const tq_terms_sp
                              uint32_t out_stride, uint32_t* out_segment_ord, uint64_t* out_key, uint64_t* out_doc_count, uint32_t* out_n,
                              uint64_t* out_sum_other, uint64_t* out_error_bound, uint64_t cell_capacity, uint64_t* out_cell_first,
                              uint32_t* out_cell_n, int64_t* out_cell_pos, uint64_t* out_cell_count, uint32_t* out_cells, uint64_t* out_hits);
+
+/* A histogram / date_histogram whose only sub-aggregation is a terms (one `histogram` over one `terms`: the sub-aggregation branch
+ * of SegmentHistogramCollector::collect, one HashMapTermBuckets per bucket), synchronous like tq_count_batch, over the docs
+ * tq_count_batch counts.  hspecs[q] is query q's histogram exactly as in tq_histogram_batch, tspecs[q] its terms exactly as in
+ * tq_terms_batch (TQ_TERMS_BY_METRIC is TQ_ERR_INVALID_ARGUMENT).  Every doc the histogram counts in bucket pos -- it has a histogram
+ * value inside the (query, segment)'s bounds -- feeds that bucket's terms: under its image, under the missing key, or (without a
+ * value and without a missing key) under none.  Each (segment, bucket) is cut to segment_size on its own as tq_terms_batch cuts a
+ * segment (a segment this context evaluates only part of is not cut).
+ *   Rows.  Row q (out_stride buckets apart) holds query q's non-empty buckets in ascending pos: out_pos (i64) and out_doc_count as
+ *   tq_histogram_batch writes them, out_sum_other and out_error_bound summed over the segments, and its kept entries
+ *   out_entry_first (an absolute index) .. + out_entry_n.  The entries of all queries follow one another in one array, query by query
+ *   and bucket by bucket in row order, each bucket's by (segment_ord, image): out_entry_segment_ord, out_entry_key (the image) and
+ *   out_entry_count; out_entries[q] counts query q's.  When some out_n[q] > out_stride or the entries of all queries exceed
+ *   entry_capacity, every out_n and out_entries is written and the call returns TQ_ERR_INVALID_ARGUMENT: retry with a larger stride
+ *   or capacity.  out_hits may be NULL; else out_hits[q] = tq_count_batch's answer.
+ *   Limits.  Those of tq_terms_batch and tq_histogram_batch (2^20 keys in a segment, 2^20 buckets in a query), and a (query,
+ *   segment) whose grid -- its bucket span times (its key span + 1) -- exceeds the ctx's cell budget (TQ_HIST_TERMS_BUDGET at ctx
+ *   creation, in u32 cells, default 2^24, at most 2^28) returns TQ_ERR_UNSUPPORTED naming the query.  Queries run in waves whose
+ *   grids fit that budget.
+ *   Errors.  Those of tq_histogram_batch and tq_terms_batch.  k, thresholds and TQ_QUERY_COUNT_HITS are ignored.  The run holds its
+ *   columns as tq_sort_batch does. */
+int tq_histogram_terms_batch(tq_ctx*, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_terms_spec* tspecs, size_t nq,
+                             uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, uint64_t* out_sum_other, uint64_t* out_error_bound,
+                             uint64_t* out_entry_first, uint32_t* out_entry_n, uint32_t* out_n, uint64_t entry_capacity,
+                             uint32_t* out_entry_segment_ord, uint64_t* out_entry_key, uint64_t* out_entry_count, uint32_t* out_entries,
+                             uint64_t* out_hits);
 
 /* The same split in three so that callers can keep inputs/outputs device resident:
  * prepare = host planning + H2D of descriptors + block-table builds (cached per term),

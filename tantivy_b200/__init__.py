@@ -21,3 +21,5 @@ from . import ranges  # noqa: E402  (range aggregations, with or without metric 
 from .ranges import RangeRefused  # noqa: E402
 from . import terms_hist  # noqa: E402  (terms with one histogram sub-aggregation: request and result side)
 from .terms_hist import TermsHistRefused  # noqa: E402
+from . import hist_terms  # noqa: E402  (a histogram with one terms sub-aggregation: request and result side)
+from .hist_terms import HistTermsRefused  # noqa: E402

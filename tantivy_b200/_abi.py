@@ -261,6 +261,14 @@ class TermsHistStats(C.Structure):
                 ("terms_hist_waves", C.c_uint64), ("terms_hist_units_shared", C.c_uint64), ("terms_hist_units_global", C.c_uint64)]
 
 
+class HistTermsStats(C.Structure):
+    """tq_hist_terms_stats — the cumulative counters of tq_histogram_terms_batch (tq_get_hist_terms_stats)."""
+    _fields_ = [("hist_terms_ms", C.c_float), ("units_hist_terms", C.c_uint64), ("hist_terms_tiles_seen", C.c_uint64),
+                ("hist_terms_tiles_one_key", C.c_uint64), ("hist_terms_tiles_one_bucket", C.c_uint64), ("hist_terms_tiles_both", C.c_uint64),
+                ("hist_terms_units_shared", C.c_uint64), ("hist_terms_units_global", C.c_uint64), ("hist_terms_rows_cut", C.c_uint64),
+                ("hist_terms_waves", C.c_uint64)]
+
+
 def ptr(arr, typ):
     """numpy array -> ctypes pointer (array must stay alive while the pointer is used)."""
     if arr is None:

@@ -287,6 +287,9 @@ int tq_ctx_create(int device, tq_ctx** out) {
   // histogram cells per wave of tq_terms_histogram_batch (64 MB of grid, 128 MB of cell list); test hook: a small budget runs a
   // batch in many waves and refuses a wide (query, segment)
   c->terms_hist_budget = std::min<uint32_t>(1u << 28, std::max<uint32_t>(1u, env_u32("TQ_TERMS_HIST_BUDGET", 1u << 24)));
+  // (bucket, key) cells per wave and per (query, segment) of tq_histogram_terms_batch (64 MB of grid, 128 MB each of entry scratch
+  // and entry list); test hook: a small budget runs a batch in many waves and refuses a wide (query, segment)
+  c->hist_terms_budget = std::min<uint32_t>(1u << 28, std::max<uint32_t>(1u, env_u32("TQ_HIST_TERMS_BUDGET", 1u << 24)));
   c->tile = env_u32("TQ_TILE", 1);                          // unions take the shared-decode tile engine (tq_tile.cuh); 0 = per-query kernels only
   // (doc, score) pairs one batch may materialise: an eighth of the device memory (10 GB on an 80 GB H100), so that the
   // four batches bench.py keeps prepared fit next to the index; queries past the budget run on the per-query kernels
@@ -459,6 +462,22 @@ int tq_get_terms_hist_stats(tq_ctx* c, tq_terms_hist_stats* out) {
   out->terms_hist_units_shared = c->terms_hist_units_shared;
   out->terms_hist_units_global = c->terms_hist_units_global;
   out->terms_hist_waves = c->terms_hist_waves;
+  return TQ_OK;
+}
+
+int tq_get_hist_terms_stats(tq_ctx* c, tq_hist_terms_stats* out) {
+  if (!c || !out) return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  std::lock_guard<std::mutex> g(c->mu);
+  out->hist_terms_ms = (float)c->hist_terms_ms;
+  out->units_hist_terms = c->hist_terms_units;
+  out->hist_terms_tiles_seen = c->hist_terms_tiles_seen;
+  out->hist_terms_tiles_one_key = c->hist_terms_tiles_one_key;
+  out->hist_terms_tiles_one_bucket = c->hist_terms_tiles_one_bucket;
+  out->hist_terms_tiles_both = c->hist_terms_tiles_both;
+  out->hist_terms_units_shared = c->hist_terms_units_shared;
+  out->hist_terms_units_global = c->hist_terms_units_global;
+  out->hist_terms_rows_cut = c->hist_terms_rows_cut;
+  out->hist_terms_waves = c->hist_terms_waves;
   return TQ_OK;
 }
 
@@ -3202,6 +3221,287 @@ int tq_terms_histogram_batch(tq_ctx* c, const tq_query* queries, const tq_terms_
     c->terms_hist_waves += waves.size();
   }
   if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a terms row has more entries than out_stride, or the cells exceed cell_capacity: out_n and out_cells hold how many");
+  return TQ_OK;
+}
+
+// ---- terms per histogram bucket ----------------------------------------------------------------------------------
+int tq_histogram_terms_batch(tq_ctx* c, const tq_query* queries, const tq_histogram_spec* hspecs, const tq_terms_spec* tspecs, size_t nq,
+                             uint32_t out_stride, int64_t* out_pos, uint64_t* out_doc_count, uint64_t* out_sum_other, uint64_t* out_error_bound,
+                             uint64_t* out_entry_first, uint32_t* out_entry_n, uint32_t* out_n, uint64_t entry_capacity,
+                             uint32_t* out_entry_segment_ord, uint64_t* out_entry_key, uint64_t* out_entry_count, uint32_t* out_entries,
+                             uint64_t* out_hits) {
+  if (!c || (nq && (!queries || !tspecs || !hspecs || !out_n || !out_entries ||
+                    (out_stride && (!out_pos || !out_doc_count || !out_sum_other || !out_error_bound || !out_entry_first || !out_entry_n)) ||
+                    (entry_capacity && (!out_entry_segment_ord || !out_entry_key || !out_entry_count)))))
+    return fail(TQ_ERR_INVALID_ARGUMENT, "null");
+  TQ_CUDA(cudaSetDevice(c->device));
+  for (size_t qi = 0; qi < nq; ++qi) {
+    const tq_terms_spec& sp = tspecs[qi];
+    const tq_histogram_spec& hs = hspecs[qi];
+    if (queries[qi].op == TQ_OP_PHRASE) return fail(TQ_ERR_UNSUPPORTED, "histograms of phrase queries are not on the device path");
+    if (sp.target > TQ_TERMS_BY_KEY || sp.order > TQ_ORDER_ASC || sp.missing_mode > TQ_TERMS_MISSING_AFTER_MAX || !sp.segment_size)
+      return fail(TQ_ERR_INVALID_ARGUMENT, "terms spec: target, order, missing mode or segment_size");
+    if (hs.kind > TQ_FAST_DATE) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram kind");
+    if (!(hs.interval > 0.0) || !std::isfinite(hs.interval)) return fail(TQ_ERR_INVALID_ARGUMENT, "histogram interval must be finite and > 0");
+  }
+  for (size_t qi = 0; qi < nq; ++qi) {
+    out_n[qi] = out_entries[qi] = 0;
+    if (out_hits) out_hits[qi] = 0;
+  }
+  if (!nq) return TQ_OK;
+  tq_batch* b = acquire_batch(c);
+  if (!b) return fail(TQ_ERR_CUDA, "stream/event creation failed");
+  struct Guard { tq_batch* b; ~Guard() { tq_batch_destroy(b); } } guard{b};
+  CountPlan cp;
+  std::vector<TermsSeg> tsegs;      // parallel to cp.segs
+  std::vector<HistSeg> hsegs;       // parallel to cp.segs
+  std::vector<HistTermsSeg> gsegs;  // parallel to cp.segs
+  std::vector<HistUnit> windows;    // parallel to cp.units: the unit's keys
+  std::vector<HistUnit> hunits;     // parallel to cp.units: the unit's buckets
+  std::vector<HistQuery> hq(nq);
+  std::vector<size_t> q_seg(nq + 1), q_unit(nq + 1);
+  std::vector<uint64_t> q_counters(nq, 0), q_region(nq, 0), q_cells(nq, 0), q_rows(nq, 0);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    TableScope table_scope{c};
+    uint64_t built = 0, unused = 0;
+    std::vector<const tq_term_seg*> order;
+    std::vector<const SortColumn*> cols;
+    std::vector<std::pair<unsigned long long, unsigned long long>> uwin;
+    std::vector<std::pair<long long, long long>> hwin;  // per unit of the query: its first and last pos (first > last: none)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      const tq_terms_spec& sp = tspecs[qi];
+      const tq_histogram_spec& hs = hspecs[qi];
+      const size_t s0 = cp.segs.size(), u0 = cp.units.size();
+      q_seg[qi] = s0;
+      q_unit[qi] = u0;
+      int rc = plan_count(c, queries[qi], (uint32_t)qi, order, cp, &unused, true);
+      if (rc != TQ_OK) return rc;
+      const uint32_t flags = (out_hits ? kTermsHits : 0u) | (sp.missing_mode != TQ_TERMS_MISSING_NONE ? kTermsMissing : 0u) |
+                             (sp.target == TQ_TERMS_BY_KEY ? kTermsByKey : 0u) | (sp.order == TQ_ORDER_ASC ? kTermsAsc : 0u);
+      uint64_t counters = 0, region = 0;  // (the key windows only: no k_terms counters here)
+      rc = plan_terms_query(c, sp, qi, flags, cp, s0, u0, tsegs, windows, cols, uwin, counters, region);
+      if (rc != TQ_OK) return rc;
+      long long qbase = 0;
+      uint64_t qlen = 0;
+      rc = plan_hist_query(c, hs, qi, cp, s0, u0, kHistMaxBins, hsegs, cols, hwin, qbase, qlen);
+      if (rc != TQ_OK) return rc;
+      // per (query, segment): the union of its units' buckets (its rows), then each unit's window relative to its first
+      std::vector<std::pair<long long, long long>> sspan(cp.segs.size() - s0, {1, 0});
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const auto& w = hwin[ui - u0];
+        if (w.first > w.second) continue;
+        auto& s = sspan[cp.units[ui].qseg - s0];
+        s = s.first > s.second ? w : std::make_pair(std::min(s.first, w.first), std::max(s.second, w.second));
+      }
+      for (size_t si = s0; si < cp.segs.size(); ++si) {
+        const auto& s = sspan[si - s0];
+        const TermsSeg& z = tsegs[si];
+        const uint32_t span = s.first <= s.second ? (uint32_t)(s.second - s.first + 1) : 0u, ncol = z.n_keys + 1u;
+        if ((uint64_t)span * ncol > c->hist_terms_budget)
+          return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": the (bucket, key) cells of a segment exceed the device budget (take the CPU path)");
+        // the missing key: inside the keys it counts in its own column, outside them in column n_keys, one more entry before or
+        // after the keys in key order; without one, column n_keys counts the docs without a value for the doc count alone
+        const bool missing = z.flags & kTermsMissing, inside = missing && z.missing - z.base < (unsigned long long)z.n_keys;
+        const bool extra = missing && !inside;
+        gsegs.push_back(HistTermsSeg{q_cells[qi], span ? s.first : 0ll, span, ncol, inside ? (uint32_t)(z.missing - z.base) : z.n_keys,
+                                     z.n_keys + (extra ? 1u : 0u), extra && z.missing < z.base ? 1u : 0u, (uint32_t)q_rows[qi]});
+        q_cells[qi] += (uint64_t)span * ncol;
+        q_rows[qi] += span;
+      }
+      if (q_cells[qi] > (1ull << 31))
+        return fail(TQ_ERR_UNSUPPORTED, "query " + std::to_string(qi) + ": its (bucket, key) cells exceed 2^31 (take the CPU path)");
+      for (size_t ui = u0; ui < cp.units.size(); ++ui) {
+        const auto& w = hwin[ui - u0];
+        hunits.push_back(w.first <= w.second ? HistUnit{(uint32_t)(w.first - gsegs[cp.units[ui].qseg].base), (uint32_t)(w.second - w.first + 1)}
+                                             : HistUnit{0u, 0u});
+      }
+      hq[qi] = HistQuery{hs.interval, hs.offset, 0ll, 0ull, 0u, hs.kind, 0u, 0u};
+    }
+    q_seg[nq] = cp.segs.size();
+    q_unit[nq] = cp.units.size();
+    int rc = flush_builds(c, &built);
+    if (rc != TQ_OK) return rc;
+    hold_segments(c, b, queries, nq);  // (the segments, their filter views and the columns stay until the rows are in)
+    for (size_t qi = 0; qi < nq; ++qi) {
+      b->held_columns.push_back(tspecs[qi].column_id);
+      b->held_columns.push_back(hspecs[qi].column_id);
+    }
+    std::sort(b->held_columns.begin(), b->held_columns.end());
+    b->held_columns.erase(std::unique(b->held_columns.begin(), b->held_columns.end()), b->held_columns.end());
+    for (uint32_t col : b->held_columns) ++c->sort_users[col];
+  }
+  if (cp.units.empty()) return TQ_OK;
+  // waves of consecutive queries whose grids fit the cell budget (a query above it runs alone); grids and rows relative to the wave
+  std::vector<uint64_t> at;
+  const std::vector<TermsWave> waves = plan_terms_waves(q_counters, q_region, q_cells, 1u, c->hist_terms_budget, q_seg, tsegs, &at);
+  uint64_t max_cells = 0, max_rows = 0;
+  std::vector<uint64_t> wave_rows(waves.size(), 0);
+  for (size_t wi = 0; wi < waves.size(); ++wi) {
+    const TermsWave& w = waves[wi];
+    uint64_t rows = 0;
+    for (size_t qi = w.q0; qi < w.q1; ++qi) {
+      for (size_t si = q_seg[qi]; si < q_seg[qi + 1]; ++si) {
+        gsegs[si].grid += at[qi];
+        gsegs[si].row += (uint32_t)rows;
+      }
+      rows += q_rows[qi];
+    }
+    wave_rows[wi] = rows;
+    max_cells = std::max(max_cells, w.extra);
+    max_rows = std::max(max_rows, rows);
+  }
+  // descriptors: one H2D copy; scratch: hits | tile counters, then one wave's cursors | rows | entries (read back), then its entry
+  // scratch and its grid
+  Staging st;
+  const size_t o_w = st.add(cp.words), o_s = st.add(cp.segs), o_u = st.add(cp.units), o_z = st.add(tsegs), o_k = st.add(windows),
+               o_hz = st.add(hsegs), o_q = st.add(hq), o_g = st.add(gsegs), o_hu = st.add(hunits);
+  TQ_CUDA(st.reserve(b->pin, b->dev));
+  st.copy();
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off = align256(off + bytes); return at; };
+  const size_t r_hits = take(nq * 8), r_tiles = take(56), head_bytes = off;
+  const size_t r_cursor = take(24), r_orows = take(max_rows * sizeof(HistTermsRow)), r_oents = take(max_cells * sizeof(HistTermsEntry)),
+               wave_bytes = off - head_bytes;
+  const size_t r_ents = take(max_cells * sizeof(HistTermsEntry)), r_grid = take(max_cells * 4);
+  TQ_CUDA(b->scratch.ensure(off));
+  TQ_CUDA(b->res_pin.ensure(std::max(head_bytes, wave_bytes)));
+  uint8_t* const d = b->scratch.p;
+  HistTermsParams P{};
+  P.c = CountParams{c->d_lists, st.on_device<const uint32_t>(o_w), st.on_device<const CountSeg>(o_s), st.on_device<const Unit>(o_u),
+                    reinterpret_cast<unsigned long long*>(d + r_hits)};
+  P.tsegs = st.on_device<const TermsSeg>(o_z);
+  P.windows = st.on_device<const HistUnit>(o_k);
+  P.hsegs = st.on_device<const HistSeg>(o_hz);
+  P.queries = st.on_device<const HistQuery>(o_q);
+  P.gsegs = st.on_device<const HistTermsSeg>(o_g);
+  P.hunits = st.on_device<const HistUnit>(o_hu);
+  P.grid = reinterpret_cast<uint32_t*>(d + r_grid);
+  P.ents = reinterpret_cast<HistTermsEntry*>(d + r_ents);
+  P.out_rows = reinterpret_cast<HistTermsRow*>(d + r_orows);
+  P.out_ents = reinterpret_cast<HistTermsEntry*>(d + r_oents);
+  P.cursor = reinterpret_cast<unsigned long long*>(d + r_cursor);
+  P.tiles = reinterpret_cast<unsigned long long*>(d + r_tiles);
+  TQ_CUDA(cudaMemcpyAsync(b->dev.p, b->pin.p, st.bytes, cudaMemcpyHostToDevice, b->stream));
+  TQ_CUDA(cudaMemsetAsync(d, 0, head_bytes, b->stream));  // hits, tile counters
+  // per query: each (segment, non-empty bucket) with its kept entries (image, doc count) in ascending image, gathered wave by wave
+  struct SegRow { long long pos; uint32_t segment_ord, doc_count, n; uint64_t other, error; size_t e0; };
+  std::vector<std::vector<SegRow>> q_rows_out(nq);
+  std::vector<std::pair<unsigned long long, uint32_t>> ents;
+  float ms_total = 0;
+  uint64_t ctas = 0;
+  const uint8_t* h = b->res_pin.p;
+  auto hp = [&](size_t r) { return h + (r - head_bytes); };
+  int n_sm = 132;
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device);
+  for (size_t wi = 0; wi < waves.size(); ++wi) {
+    const TermsWave& w = waves[wi];
+    const size_t sa = q_seg[w.q0], sb = q_seg[w.q1], ua = q_unit[w.q0], ub = q_unit[w.q1];
+    if (sa == sb) continue;
+    P.unit_base = (uint32_t)ua;
+    P.seg_base = (uint32_t)sa;
+    P.n_segs = (uint32_t)(sb - sa);
+    P.n_rows = (uint32_t)wave_rows[wi];
+    TQ_CUDA(cudaMemsetAsync(d + r_grid, 0, w.extra * 4, b->stream));
+    TQ_CUDA(cudaMemsetAsync(d + r_cursor, 0, 24, b->stream));
+    TQ_CUDA(cudaEventRecord(b->ev_k0, b->stream));
+    const unsigned nu = (unsigned)(ub - ua);
+    const unsigned nf = (unsigned)std::min<uint64_t>((wave_rows[wi] + kWarps - 1) / kWarps, (uint64_t)n_sm * 8u);
+    if (nu) {
+      (cp.mixed ? k_hist_terms<true> : k_hist_terms<false>)<<<nu, kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    if (nf) {
+      k_hist_terms_final<<<nf, kThreads, 0, b->stream>>>(P);
+      TQ_CUDA(cudaGetLastError());
+    }
+    TQ_CUDA(cudaEventRecord(b->ev_k1, b->stream));
+    ctas += (uint64_t)nu + nf;
+    TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d + head_bytes, 24, cudaMemcpyDeviceToHost, b->stream));  // cursors
+    TQ_CUDA(cudaStreamSynchronize(b->stream));
+    unsigned long long cur[3];
+    memcpy(cur, hp(r_cursor), 24);
+    // the output lists, only as long as they are
+    if (cur[2]) TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_orows - head_bytes), d + r_orows, cur[2] * sizeof(HistTermsRow), cudaMemcpyDeviceToHost, b->stream));
+    if (cur[1]) TQ_CUDA(cudaMemcpyAsync(b->res_pin.p + (r_oents - head_bytes), d + r_oents, cur[1] * sizeof(HistTermsEntry), cudaMemcpyDeviceToHost, b->stream));
+    if (cur[1] || cur[2]) TQ_CUDA(cudaStreamSynchronize(b->stream));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, b->ev_k0, b->ev_k1);
+    ms_total += ms;
+    const HistTermsRow* rows_h = reinterpret_cast<const HistTermsRow*>(hp(r_orows));
+    const HistTermsEntry* ents_h = reinterpret_cast<const HistTermsEntry*>(hp(r_oents));
+    for (unsigned long long j = 0; j < cur[2]; ++j) {
+      const HistTermsRow& x = rows_h[j];
+      const size_t si = sa + x.seg;
+      const TermsSeg& z = tsegs[si];
+      const HistTermsSeg& g = gsegs[si];
+      q_rows_out[cp.segs[si].query].push_back(SegRow{g.base + (long long)x.pos, cp.segment_ords[si], x.doc_count, x.n, x.other, x.error, ents.size()});
+      for (uint32_t k = 0; k < x.n; ++k) {
+        const HistTermsEntry& e = ents_h[(size_t)x.first + k];
+        const uint32_t i = g.mfirst ? (e.key ? e.key - 1u : z.n_keys) : e.key;  // (its column)
+        ents.emplace_back(i < z.n_keys ? z.base + i : z.missing, e.count);
+      }
+    }
+  }
+  TQ_CUDA(cudaMemcpyAsync(b->res_pin.p, d, head_bytes, cudaMemcpyDeviceToHost, b->stream));
+  TQ_CUDA(cudaStreamSynchronize(b->stream));
+  unsigned long long tiles[7];
+  memcpy(tiles, h + r_tiles, 56);
+  if (out_hits) memcpy(out_hits, h + r_hits, nq * 8);
+  // rows: each query's buckets in ascending pos, the segments' parts summed; entries: each bucket's by (segment_ord, image), in
+  // row order, the queries' entries one after the other
+  bool fits = true;
+  uint64_t ne = 0;
+  for (size_t qi = 0; qi < nq; ++qi) {
+    std::vector<SegRow>& rs = q_rows_out[qi];
+    std::sort(rs.begin(), rs.end(), [](const SegRow& x, const SegRow& y) { return x.pos != y.pos ? x.pos < y.pos : x.segment_ord < y.segment_ord; });
+    uint32_t n = 0;
+    const uint64_t ne0 = ne;
+    for (size_t i = 0; i < rs.size();) {
+      size_t j = i;
+      uint64_t doc = 0, other = 0, error = 0, first = ne;
+      for (; j < rs.size() && rs[j].pos == rs[i].pos; ++j) {
+        doc += rs[j].doc_count;
+        other += rs[j].other;
+        error += rs[j].error;
+        for (uint32_t k = 0; k < rs[j].n; ++k, ++ne)
+          if (ne < entry_capacity) {
+            out_entry_segment_ord[ne] = rs[j].segment_ord;
+            out_entry_key[ne] = ents[rs[j].e0 + k].first;
+            out_entry_count[ne] = ents[rs[j].e0 + k].second;
+          }
+      }
+      if (n < out_stride) {
+        const size_t a = qi * (size_t)out_stride + n;
+        out_pos[a] = rs[i].pos;
+        out_doc_count[a] = doc;
+        out_sum_other[a] = other;
+        out_error_bound[a] = error;
+        out_entry_first[a] = first;
+        out_entry_n[a] = (uint32_t)(ne - first);
+      }
+      ++n;
+      i = j;
+    }
+    out_n[qi] = n;
+    out_entries[qi] = (uint32_t)(ne - ne0);
+    fits = fits && n <= out_stride;
+  }
+  fits = fits && ne <= entry_capacity;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->hist_terms_ms += ms_total;
+    c->hist_terms_units += ctas;
+    c->hist_terms_tiles_seen += tiles[0];
+    c->hist_terms_tiles_one_key += tiles[1];
+    c->hist_terms_tiles_one_bucket += tiles[2];
+    c->hist_terms_tiles_both += tiles[3];
+    c->hist_terms_units_shared += tiles[4];
+    c->hist_terms_units_global += tiles[5];
+    c->hist_terms_rows_cut += tiles[6];
+    c->hist_terms_waves += waves.size();
+  }
+  if (!fits) return fail(TQ_ERR_INVALID_ARGUMENT, "a histogram row has more buckets than out_stride, or the entries exceed entry_capacity: out_n and out_entries hold how many");
   return TQ_OK;
 }
 

@@ -262,6 +262,11 @@ struct tq_ctx {
   double terms_hist_ms = 0;
   uint64_t terms_hist_units = 0, terms_hist_tiles_seen = 0, terms_hist_tiles_one_key = 0, terms_hist_tiles_one_bucket = 0,
            terms_hist_tiles_both = 0, terms_hist_waves = 0, terms_hist_units_shared = 0, terms_hist_units_global = 0;
+  // ... and of the histogram-with-terms runs (hist_terms_ms, CTAs, tiles seen / with one key / in one bucket / both, k_hist_terms
+  // units counting in shared memory / in the grid, rows cut on the device, waves)
+  double hist_terms_ms = 0;
+  uint64_t hist_terms_units = 0, hist_terms_tiles_seen = 0, hist_terms_tiles_one_key = 0, hist_terms_tiles_one_bucket = 0,
+           hist_terms_tiles_both = 0, hist_terms_units_shared = 0, hist_terms_units_global = 0, hist_terms_rows_cut = 0, hist_terms_waves = 0;
   cudaStream_t build_stream = nullptr;
   tq::host::PinBuf build_pin;
   tq::host::DevBuf build_dev;
@@ -272,6 +277,7 @@ struct tq_ctx {
   uint32_t hist_metrics_budget;   // (bucket, column) accumulators one tq_histogram_metrics_batch wave may hold
   uint32_t terms_metrics_budget;  // (kept entry, column) parts one tq_terms_metrics_batch wave may hold
   uint32_t terms_hist_budget;     // u32 (kept entry, bucket) cells one tq_terms_histogram_batch wave may hold
+  uint32_t hist_terms_budget;     // u32 (bucket, key) cells one tq_histogram_terms_batch wave, and one (query, segment), may hold
   unsigned long long* d_counters = nullptr;  // [0..8) k_or_strip windows by route and bytes read, [8..16) k_tile diagnostics, [16..24) k_tile cycles by stage,
                                              // [24..28) k_tile B2 union postings by exit
   uint32_t tile = 1, tile_scratch_mb = 24576, tile_sample_div = 64, tile_round_div1 = 8, tile_round_div2 = 2, tile_light_max = 384, tile_counters = 0;

@@ -2913,6 +2913,267 @@ __global__ void __launch_bounds__(kThreads) k_terms_hist_final(const TermsHistPa
     for (uint32_t j = threadIdx.x; j < n_kept; j += blockDim.x) P.cell_first[Z.region + j] = at;
 }
 
+// ---- terms per histogram bucket (a histogram whose only sub-aggregation is a terms: SegmentHistogramCollector::collect's
+// sub-aggregation branch, histogram.rs:490-505, into one HashMapTermBuckets per bucket) -------------------------------------------
+// One CTA per Count unit: each matching doc with a histogram value in its (query, segment)'s bounds counted in cell (its bucket, its
+// key's column) -- the image's offset from the segment's key base, or the column of a doc without a value.  Per tile, thread 0 reads
+// both columns' SortTile: a tile whose values all hold one image skips the key gather, a tile whose histogram values are all in bounds
+// and in one bucket (HistKeys::one) skips the value gather, and a tile with both adds each warp's count to one cell.  A unit whose
+// window (its buckets × its keys + 1) fits kTermsHistSmemCells counts in shared memory and adds its non-zero cells to the grid at
+// exit; a wider one counts in the grid.  With kTermsHits the unit's matches are added to its query's Count.  (Apart from
+// k_terms_hist: that kernel looks each key's slot up in the cut's counters, this one takes the key's offset and feeds no cut, and the
+// two share only match_tile and HistKeys.)
+template <bool kMixed>
+__global__ void __launch_bounds__(kThreads, 3) k_hist_terms(const HistTermsParams P) {
+  constexpr uint32_t kNone = 0xFFFFFFFFu;
+  __shared__ uint32_t s_acc[kTileDocs / 32u], s_tmp[kTileDocs / 32u];
+  __shared__ uint32_t s_cnt[kMixed ? kTileDocs / 4u : 1u];
+  __shared__ uint32_t s_cells[kTermsHistSmemCells];
+  __shared__ uint32_t s_part[kWarps];
+  __shared__ uint32_t s_key, s_bucket;
+  const uint32_t unit = P.unit_base + blockIdx.x;
+  const Unit U = P.c.units[unit];
+  const TermsSeg Z = P.tsegs[U.qseg];
+  const HistUnit W = P.hunits[unit], K = P.windows[unit];
+  const bool hits = Z.flags & kTermsHits;
+  if (!W.n_bins && !hits) return;  // (CTA-uniform: no value of the unit is in bounds, and its Count is not asked for)
+  const CountSeg S = P.c.segs[U.qseg];
+  const HistSeg H = P.hsegs[U.qseg];
+  const HistQuery Q = P.queries[S.query];
+  const HistTermsSeg G = P.gsegs[U.qseg];
+  const long long base = G.base + (long long)W.first;  // pos of the window's first bucket
+  const uint32_t kw = K.n_bins + 1u;                  // the window's columns: the unit's keys, then the docs without a value
+  const bool shared = W.n_bins * kw <= kTermsHistSmemCells;  // (W.n_bins * kw <= the (query, segment)'s grid <= its budget < 2^32)
+  uint32_t* const gcells = P.grid + G.grid + (unsigned long long)W.first * G.cols;
+  auto cell = [&](uint32_t b, uint32_t k) -> uint32_t* {  // cell (bucket b, column k) of the window
+    return shared ? &s_cells[b * kw + k] : &gcells[(size_t)b * G.cols + (k == K.n_bins ? G.mcol : K.first + k)];
+  };
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins * kw; i += blockDim.x) s_cells[i] = 0;
+  const unsigned long long kbase = Z.base + K.first;  // image of the window's column 0
+  const uint32_t wb = S.words_base, ng = P.c.words[wb], need = P.c.words[wb + 1u];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  uint32_t total = 0, n_one_key = 0, n_one_bucket = 0, n_both = 0;
+  for (uint32_t tile = U.begin; tile < U.end; ++tile) {
+    const uint32_t lo = tile * kTileDocs, hi = min(lo + kTileDocs, S.max_doc);
+    if (threadIdx.x == 0) {
+      uint32_t k1 = kNone, b1 = kNone;
+      const SortTile T = Z.tiles[tile];
+      if ((T.flags & kSortTileValues) && T.best[0] == ~T.best[1] && T.best[0] - kbase < K.n_bins) k1 = (uint32_t)(T.best[0] - kbase);
+      const SortTile V = H.tiles[tile];
+      if (W.n_bins && (V.flags & kSortTileValues)) HistKeys::one(V, H, Q, W, base, b1);
+      s_key = k1;
+      s_bucket = b1;
+      n_one_key += k1 != kNone ? 1u : 0u;
+      n_one_bucket += b1 != kNone ? 1u : 0u;
+      n_both += k1 != kNone && b1 != kNone ? 1u : 0u;
+    }
+    match_tile<kMixed>(P.c, S.alive, wb, ng, need, lo, hi, s_acc, s_tmp, s_cnt, [&](uint32_t w, uint32_t bits) { s_acc[w] = bits; });
+    __syncthreads();
+    const uint32_t bits = s_acc[threadIdx.x];
+    total += (uint32_t)__popc(bits);
+    const uint32_t kp = Z.present ? __ldg(Z.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+    const uint32_t hp = H.present ? __ldg(H.present + (lo >> 5) + threadIdx.x) : 0xFFFFFFFFu;
+    const uint32_t k1 = s_key, b1 = s_bucket;
+    const uint32_t dd = W.n_bins ? bits & hp : 0u;  // matching docs with a histogram value
+    if (b1 != kNone) {  // every histogram value of the tile counts in bucket b1
+      const uint32_t nm = __reduce_add_sync(kFull, (uint32_t)__popc(dd & ~kp));
+      if (lane == 0 && nm) atomicAdd(cell(b1, K.n_bins), nm);
+      if (k1 != kNone) {
+        const uint32_t nk = __reduce_add_sync(kFull, (uint32_t)__popc(dd & kp));
+        if (lane == 0 && nk) atomicAdd(cell(b1, k1), nk);
+      } else {
+        for (uint32_t w = dd & kp; w; w &= w - 1u)
+          atomicAdd(cell(b1, (uint32_t)(__ldg(Z.values + lo + threadIdx.x * 32u + (uint32_t)(__ffs(w) - 1)) - kbase)), 1u);
+      }
+    } else {
+      for (uint32_t w = dd; w; w &= w - 1u) {
+        const uint32_t bit = (uint32_t)(__ffs(w) - 1), doc = lo + threadIdx.x * 32u + bit;
+        const double val = HistKeys::value(__ldg(H.values + doc), Q);
+        if (!HistKeys::counted(val, H)) continue;
+        const unsigned long long b = HistKeys::index(val, Q, base);
+        if (b >= W.n_bins) continue;  // (never: the window covers every counted value)
+        const uint32_t k = !((kp >> bit) & 1u) ? K.n_bins : k1 != kNone ? k1 : (uint32_t)(__ldg(Z.values + doc) - kbase);
+        atomicAdd(cell((uint32_t)b, k), 1u);
+      }
+    }
+    __syncthreads();
+  }
+  if (shared)
+    for (uint32_t i = threadIdx.x; i < W.n_bins * kw; i += blockDim.x)
+      if (s_cells[i]) {
+        const uint32_t k = i % kw;
+        atomicAdd(&gcells[(size_t)(i / kw) * G.cols + (k == K.n_bins ? G.mcol : K.first + k)], s_cells[i]);
+      }
+  if (hits) {
+    total = __reduce_add_sync(kFull, total);
+    if (lane == 0) s_part[warp] = total;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (hits) {
+      unsigned long long sum = 0;
+      for (int w = 0; w < kWarps; ++w) sum += s_part[w];
+      if (sum) atomicAdd(&P.c.counts[S.query], sum);
+    }
+    const uint32_t seen = U.end - U.begin;
+    if (seen) atomicAdd(&P.tiles[0], (unsigned long long)seen);
+    if (n_one_key) atomicAdd(&P.tiles[1], (unsigned long long)n_one_key);
+    if (n_one_bucket) atomicAdd(&P.tiles[2], (unsigned long long)n_one_bucket);
+    if (n_both) atomicAdd(&P.tiles[3], (unsigned long long)n_both);
+    if (W.n_bins) atomicAdd(&P.tiles[shared ? 4 : 5], 1ull);
+  }
+}
+
+// One warp per bucket row of a wave, grid-striding over the wave's rows (a row's (query, segment) found by a binary search over their
+// first rows); rows leave in any order, each with its (query, segment), and the host orders them by pos.  Per row:
+//   A. its doc count (every cell) and entries (the non-zero entry cells); a row without docs writes nothing;
+//   B. a row of a whole segment with more than segment_size entries (partial segments have segment_size above their keys): its
+//      entries in key order into the wave's scratch (one ballot per 32 columns, its place taken with one atomic), then §3.7's cut
+//      over them alone -- by count, a warp's radix select (4 passes of 8 bits, a 256-bin histogram per warp) finds the count t of
+//      the segment_size-th entry and keeps the entries above it and the lowest keys at it; by key, the first or last segment_size
+//      -- compacted in place, with term_doc_count_before_cutoff and sum_other_doc_count, and copied to the entry list;
+//   C. any other row: its entries in key order straight into the entry list, both scalars 0.
+// The grid is read twice (A, then B or C) and only kept entries are written to the list the host copies back.
+__global__ void __launch_bounds__(kThreads) k_hist_terms_final(const HistTermsParams P) {
+  __shared__ uint32_t s_hist[kWarps][256];
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
+  uint32_t* const hist = s_hist[warp];
+  uint32_t n_cut = 0;
+  for (uint32_t g = blockIdx.x * kWarps + warp; g < P.n_rows; g += gridDim.x * kWarps) {
+    uint32_t lo = 0, n = P.n_segs;  // the last (query, segment) of the wave whose first row is <= g
+    while (n > 1u) {
+      const uint32_t half = n >> 1;
+      if (P.gsegs[P.seg_base + lo + half].row <= g) lo += half;
+      n -= half;
+    }
+    const TermsSeg Z = P.tsegs[P.seg_base + lo];
+    const HistTermsSeg G = P.gsegs[P.seg_base + lo];
+    const uint32_t r = g - G.row;  // (< G.span: a (query, segment) without rows has the next one's first row)
+    const uint32_t* const row = P.grid + G.grid + (size_t)r * G.cols;
+    const uint32_t L = G.n_entries, ss = Z.segment_size, nc = G.cols;
+    const bool all_entries = L == nc;  // (else column nc - 1 is not an entry: docs without a value and without a missing key)
+    auto col_of = [&](uint32_t i) -> uint32_t { return G.mfirst ? (i ? i - 1u : nc - 1u) : i; };
+    // A
+    uint32_t doc = 0, N = 0;
+    for (uint32_t i = lane; i < nc; i += 32u) {
+      const uint32_t v = row[i];
+      doc += v;
+      N += v && (i + 1u < nc || all_entries) ? 1u : 0u;
+    }
+    doc = __reduce_add_sync(kFull, doc);
+    N = __reduce_add_sync(kFull, N);
+    if (!doc) continue;  // (warp-uniform)
+    const bool cut = N > ss;
+    unsigned long long at = 0;  // the row's entries: in the scratch when it is cut, else in the list
+    if (lane == 0 && N) at = atomicAdd(&P.cursor[cut ? 0 : 1], (unsigned long long)N);
+    at = __shfl_sync(kFull, at, 0);
+    HistTermsEntry* const E = (cut ? P.ents : P.out_ents) + at;
+    unsigned long long sum = 0;
+    uint32_t k_at = 0;
+    for (uint32_t i0 = 0; N && i0 < L; i0 += 32u) {
+      const uint32_t i = i0 + lane;
+      const uint32_t v = i < L ? row[col_of(i)] : 0u;
+      const uint32_t m = __ballot_sync(kFull, v != 0u);
+      if (v) E[k_at + (uint32_t)__popc(m & lt)] = HistTermsEntry{i, v};
+      k_at += (uint32_t)__popc(m);
+      sum += v;
+    }
+    uint32_t kept = N, first = (uint32_t)at;  // (the wave's lists hold at most its grid's cells)
+    unsigned long long other = 0, error = 0;
+    if (cut) {
+      __syncwarp();
+      const bool asc = Z.flags & kTermsAsc, by_key = Z.flags & kTermsByKey;
+      auto rank = [&](uint32_t c) -> uint32_t { return asc ? ~c : c; };  // larger first
+      uint32_t t_cut = 0, need = 0, err_t = 0;
+      if (!by_key) {
+        uint32_t prefix = 0, mask = 0, k = ss, n_eq = 0;
+        for (int shift = 24; shift >= 0; shift -= 8) {
+          for (uint32_t j = lane; j < 256u; j += 32u) hist[j] = 0;
+          __syncwarp();
+          for (uint32_t j = lane; j < N; j += 32u) {
+            const uint32_t t = rank(E[j].count);
+            if ((t & mask) == prefix) atomicAdd(&hist[(t >> shift) & 255u], 1u);
+          }
+          __syncwarp();
+          // the bin of the k-th largest: lane l holds bins [8l, 8l + 8); a suffix sum over the lanes finds the one it falls in
+          uint32_t s = 0;
+#pragma unroll
+          for (uint32_t j = 0; j < 8u; ++j) s += hist[lane * 8u + j];
+          uint32_t suf = s;
+#pragma unroll
+          for (uint32_t d = 1; d < 32u; d <<= 1) {
+            const uint32_t y = __shfl_down_sync(kFull, suf, d);
+            if (lane + d < 32u) suf += y;
+          }
+          const bool mine = suf >= k && suf - s < k;  // (one lane: the suffix sums rise to the entries matching the prefix >= k)
+          const uint32_t who = (uint32_t)(__ffs(__ballot_sync(kFull, mine)) - 1);
+          uint32_t b = 0, acc = 0;
+          if (mine) {
+            acc = suf - s;
+            for (b = lane * 8u + 7u; acc + hist[b] < k; --b) acc += hist[b];
+          }
+          b = __shfl_sync(kFull, b, who);
+          acc = __shfl_sync(kFull, acc, who);
+          n_eq = hist[b];
+          prefix |= b << shift;
+          k -= acc;
+          mask |= 255u << shift;
+          __syncwarp();
+        }
+        t_cut = prefix;
+        need = k;  // entries at t_cut to keep, the lowest keys first
+        // term_doc_count_before_cutoff: t_cut itself when more entries tie at it, else the largest t below it
+        uint32_t below = 0;
+        if (n_eq <= need)
+          for (uint32_t j = lane; j < N; j += 32u) {
+            const uint32_t t = rank(E[j].count);
+            if (t < t_cut) below = max(below, t);
+          }
+        err_t = rank(n_eq > need ? t_cut : __reduce_max_sync(kFull, below));
+      }
+      // the kept entries, compacted in place in key order; by key: the entry ranks kept and the rank whose count is reported
+      const uint32_t r0 = by_key && !asc ? N - ss : 0u, r_err = by_key ? (asc ? ss : N - ss - 1u) : 0xFFFFFFFFu;
+      uint32_t eq_seen = 0, err_c = 0;
+      unsigned long long kept_sum = 0;
+      kept = 0;
+      for (uint32_t j0 = 0; j0 < N; j0 += 32u) {
+        const uint32_t j = j0 + lane;
+        const HistTermsEntry e = j < N ? E[j] : HistTermsEntry{0u, 0u};
+        const uint32_t t = rank(e.count);
+        const bool eq = j < N && !by_key && t == t_cut;
+        const uint32_t me = __ballot_sync(kFull, eq);
+        const bool keep = j < N && (by_key ? j - r0 < ss : (t > t_cut || (eq && eq_seen + (uint32_t)__popc(me & lt) < need)));
+        eq_seen += (uint32_t)__popc(me);
+        if (j == r_err) err_c = e.count;
+        const uint32_t km = __ballot_sync(kFull, keep);
+        __syncwarp();  // (every lane has read its entry before any is overwritten)
+        if (keep) E[kept + (uint32_t)__popc(km & lt)] = e;
+        kept += (uint32_t)__popc(km);
+        kept_sum += keep ? e.count : 0u;
+      }
+      for (int d = 16; d; d >>= 1) {
+        sum += __shfl_xor_sync(kFull, sum, d);
+        kept_sum += __shfl_xor_sync(kFull, kept_sum, d);
+      }
+      other = sum - kept_sum;
+      error = by_key ? __reduce_max_sync(kFull, err_c) : err_t;
+      unsigned long long to = 0;
+      if (lane == 0) to = atomicAdd(&P.cursor[1], (unsigned long long)kept);
+      to = __shfl_sync(kFull, to, 0);
+      __syncwarp();
+      for (uint32_t j = lane; j < kept; j += 32u) P.out_ents[to + j] = E[j];
+      first = (uint32_t)to;
+      ++n_cut;
+    }
+    if (lane == 0) {
+      const unsigned long long o = atomicAdd(&P.cursor[2], 1ull);
+      P.out_rows[o] = HistTermsRow{r, doc, kept, first, lo, 0u, other, error};
+    }
+  }
+  if (lane == 0 && n_cut) atomicAdd(&P.tiles[6], (unsigned long long)n_cut);
+}
+
 // The docs a filtered query (TQ_QUERY_FILTER) may collect in one (segment, field): alive AND [doc_lo, doc_hi) AND filter, as 32-bit
 // words of the alive layout (FilterCollector over the collection loop that skips deleted docs, filter_collector_wrapper.rs:160-199,
 // collector/mod.rs:186-221).  alive null: no deletes.  doc_hi <= max_doc, so the bits at and beyond max_doc come out clear.

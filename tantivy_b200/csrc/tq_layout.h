@@ -473,6 +473,52 @@ struct TermsHistParams {
 };
 static_assert(sizeof(TermsHistSeg) == 24, "terms histogram descriptor layout");
 
+// ---- terms per histogram bucket (k_hist_terms, k_hist_terms_final) ----------------------------------------------------------
+// The histogram of HistSeg / HistQuery / HistUnit with the terms key windows of TermsSeg (no k_terms counters).  Each (query,
+// segment) has a u32 grid of (its bucket span) rows × (n_keys + 1) columns: column k counts the docs of image base + k, column
+// n_keys the docs without a value (the missing key when it lies outside the keys, else nothing); a missing key inside the keys
+// counts in its own column.  k_hist_terms counts each matching doc whose histogram value is in bounds in cell (pos - base, column):
+// a row's cells sum to the histogram's doc count.  A unit whose window (its buckets × its keys + 1) fits kTermsHistSmemCells
+// counts in shared memory.  k_hist_terms_final, a warp per row, compacts each row's entries once, cuts each row of a whole segment
+// with more than segment_size entries by a warp's radix select over them, and writes the non-empty rows with their kept entries.
+struct HistTermsSeg {  // the grid of one (query, segment), parallel to CountParams::segs
+  unsigned long long grid;  // its first cell in HistTermsParams::grid (relative to the wave)
+  long long base;           // pos of row 0
+  uint32_t span;            // rows (0: no value of the segment's visited tiles passes its bounds)
+  uint32_t cols;            // n_keys + 1
+  uint32_t mcol;            // the column of a doc without a value
+  uint32_t n_entries;       // entry columns in key order: n_keys, plus 1 for a missing key outside the keys
+  uint32_t mfirst;          // 1: that missing key sorts before the keys (entry 0 is column n_keys)
+  uint32_t row;             // its first row in HistTermsParams::rows (relative to the wave)
+};
+// One non-empty bucket row of a (query, segment) (seg: its index in the wave): its pos - base, doc count, kept entries (first: in
+// the wave's entry list) and scalars.
+struct HistTermsRow {
+  uint32_t pos, doc_count, n, first, seg, pad;
+  unsigned long long other, error;
+};
+// One entry: its index in key order (HistTermsSeg) and doc count.
+struct HistTermsEntry { uint32_t key, count; };
+struct HistTermsParams {
+  CountParams c;                 // structure words, (query, segment) pairs, units and hit counters: the Count plan of the batch
+  const TermsSeg* tsegs;         // parallel to c.segs: the terms column, key base and count, missing key, segment_size, flags
+  const HistUnit* windows;       // parallel to c.units: the unit's keys, relative to its TermsSeg's base
+  const HistSeg* hsegs;          // parallel to c.segs: the histogram column and bounds
+  const HistQuery* queries;      // [nq]: interval, offset and kind of the query's histogram
+  const HistTermsSeg* gsegs;     // parallel to c.segs
+  const HistUnit* hunits;        // parallel to c.units: the unit's buckets, relative to its (query, segment)'s base
+  uint32_t* grid;                // the wave's cells, zeroed before it
+  HistTermsEntry* ents;          // the entries of the wave's rows that are cut (k_hist_terms_final's scratch)
+  HistTermsRow* out_rows;        // the wave's non-empty rows, in any order
+  HistTermsEntry* out_ents;      // their kept entries, row by row
+  unsigned long long* cursor;    // [0] ents, [1] out_ents, [2] out_rows held
+  unsigned long long* tiles;     // [0] tiles seen, [1] of them with one key, [2] in one bucket, [3] both; units counting [4] in
+                                 // shared memory, [5] in the grid; [6] rows cut
+  uint32_t unit_base, seg_base;  // the wave's first unit and first (query, segment)
+  uint32_t n_segs, n_rows;       // the wave's (query, segment)s and rows
+};
+static_assert(sizeof(HistTermsSeg) == 40 && sizeof(HistTermsRow) == 40 && sizeof(HistTermsEntry) == 8, "histogram terms descriptor layout");
+
 // ---- the tile engine (tq_tile.cuh) --------------------------------------------------------------------------------------
 
 constexpr uint32_t kTile = 1024;            // docs per tile

@@ -9,7 +9,7 @@ import numpy as np
 from ._abi import (HISTOGRAM_SPEC_DTYPE, METRIC_PART_DTYPE, METRICS_SPEC_DTYPE, SORT_SPEC_DTYPE, TERMS_SPEC_DTYPE, TQ_METRICS_MAX_COLUMNS, MetricPart,
                    MetricsSpec, MetricsStats, HistMetricsStats, TermsMetricsStats, TermsMetricOrder, TERMS_METRIC_ORDER_DTYPE, TQ_FAST_BOOL, TQ_FAST_DATE, TQ_FAST_F64, TQ_FAST_I64, TQ_FAST_U64,
                    TQ_ORDER_ASC, TQ_ORDER_DESC, HistogramSpec, HistogramStats, Query, QueryBatch, SortSpec, Stats, TermSeg, TermsSpec, TermsStats,
-                   RANGE_SPEC_DTYPE, RangeSpec, RangeStats, TermsHistStats, TQ_RANGE_MAX_BUCKETS, f32p, ptr, u8p, u32p, u64p)
+                   RANGE_SPEC_DTYPE, RangeSpec, RangeStats, TermsHistStats, HistTermsStats, TQ_RANGE_MAX_BUCKETS, f32p, ptr, u8p, u32p, u64p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("TANTIVY_B200_LIB") or os.path.join(_HERE, "_lib", "libtantivy_b200.so")  # (override: A/B builds)
@@ -38,6 +38,7 @@ def _load():
     lib.tq_get_terms_metrics_stats.argtypes = [vp, C.POINTER(TermsMetricsStats)]
     lib.tq_get_range_stats.argtypes = [vp, C.POINTER(RangeStats)]
     lib.tq_get_terms_hist_stats.argtypes = [vp, C.POINTER(TermsHistStats)]
+    lib.tq_get_hist_terms_stats.argtypes = [vp, C.POINTER(HistTermsStats)]
     lib.tq_segment_register.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, u8p, sz, u8p, sz, u8p, sz]
     lib.tq_segment_register_positions.argtypes = [vp, C.c_uint32, C.c_uint32, u8p, sz]
     lib.tq_segment_unregister.argtypes = [vp, C.c_uint32, C.c_uint32]
@@ -63,6 +64,8 @@ def _load():
                                    u64p]
     lib.tq_terms_histogram_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(TermsSpec), C.POINTER(HistogramSpec), sz, C.c_uint32, u32p, u64p,
                                              u64p, u32p, u64p, u64p, C.c_uint64, u64p, u32p, C.POINTER(C.c_int64), u64p, u32p, u64p]
+    lib.tq_histogram_terms_batch.argtypes = [vp, C.POINTER(Query), C.POINTER(HistogramSpec), C.POINTER(TermsSpec), sz, C.c_uint32,
+                                             C.POINTER(C.c_int64), u64p, u64p, u64p, u64p, u32p, u32p, C.c_uint64, u32p, u64p, u64p, u32p, u64p]
     lib.tq_batch_run.argtypes = [vp]
     lib.tq_batch_run_phase.argtypes = [vp, C.c_int]
     lib.tq_batch_phases.argtypes = [vp]
@@ -371,6 +374,7 @@ class Context:
         self._hist_metrics_stride = 0  # the widest row hist_metrics_batch has returned (its next first try)
         self._terms_metrics_stride = 0  # the widest row terms_metrics_batch has returned (its next first try)
         self._terms_hist_sizes = (0, 0)  # the widest row and the most cells terms_hist_batch has returned (its next first try)
+        self._hist_terms_sizes = (0, 0)  # the widest row and the most entries hist_terms_batch has returned (its next first try)
 
     def segment_register(self, segment_ord, field, max_doc, record_option, idx_body, fieldnorm=None, alive=None):
         idx_body = np.ascontiguousarray(idx_body, dtype=np.uint8)
@@ -661,6 +665,52 @@ class Context:
                    pos[:total], ccount[:total], nc[:qb.nq])
             return out + (hits[:qb.nq],) if count_hits else out
 
+    def hist_terms_batch(self, qb: QueryBatch, hspecs, tspecs, count_hits=False, stride=None, entry_capacity=None):
+        """A histogram whose only sub-aggregation is a terms, per query (tq_histogram_terms_batch) over sort columns; hspecs = one
+        histogram spec per query as histogram_batch takes them, tspecs = one terms spec per query as terms_batch takes them
+        (tantivy_b200.hist_terms turns requests into both).  Returns (pos, doc_count, sum_other, error_bound, entry_first, entry_n,
+        n, entry_segment_ord, entry_key, entry_count, n_entries): row q holds the n[q] non-empty buckets of query q in ascending pos,
+        and bucket j's kept entries are entries entry_first[q, j] .. + entry_n[q, j] of the one entry array (segment_ord, image,
+        doc_count), by (segment_ord, image); n_entries[q] counts query q's entries -- and with count_hits=True the Count of every
+        query as well.  Raises TqError with code -4 (TQ_ERR_UNSUPPORTED) when a (query, segment) is too wide for the device.
+        `stride` / `entry_capacity` are the sizes tried first (default: the widest row and the most entries this context has
+        returned, at least 1024 / 65536): larger results run the batch again at their sizes."""
+        hspecs, tspecs = list(hspecs), list(tspecs)
+        if len(tspecs) != qb.nq or len(hspecs) != qb.nq:
+            raise ValueError(f"one histogram and one terms spec per query: {len(hspecs)} and {len(tspecs)} for {qb.nq} queries")
+        if stride is None:
+            stride = max(1024, self._hist_terms_sizes[0])
+        if entry_capacity is None:
+            entry_capacity = max(65536, self._hist_terms_sizes[1])
+        hspec, tspec = _histogram_specs(hspecs, qb.nq), _terms_specs(tspecs, qb.nq)
+        n = max(qb.nq, 1)
+        while True:
+            pos = np.empty((n, stride), dtype=np.int64)  # (only the first n[q] buckets of row q, and sum(n_entries) entries, are written)
+            docs = np.empty((n, stride), dtype=np.uint64)
+            other = np.empty((n, stride), dtype=np.uint64)
+            error = np.empty((n, stride), dtype=np.uint64)
+            first = np.empty((n, stride), dtype=np.uint64)
+            nent = np.empty((n, stride), dtype=np.uint32)
+            eseg = np.empty(entry_capacity, dtype=np.uint32)
+            ekey = np.empty(entry_capacity, dtype=np.uint64)
+            ecount = np.empty(entry_capacity, dtype=np.uint64)
+            nb = np.zeros(n, dtype=np.uint32)
+            ne = np.zeros(n, dtype=np.uint32)
+            hits = np.zeros(n, dtype=np.uint64) if count_hits else None
+            rc = LIB.tq_histogram_terms_batch(self.h, qb.ptr, hspec.ctypes.data_as(C.POINTER(HistogramSpec)), tspec.ctypes.data_as(C.POINTER(TermsSpec)),
+                                              qb.nq, stride, pos.ctypes.data_as(C.POINTER(C.c_int64)), ptr(docs, u64p), ptr(other, u64p),
+                                              ptr(error, u64p), ptr(first, u64p), ptr(nent, u32p), ptr(nb, u32p), entry_capacity, ptr(eseg, u32p),
+                                              ptr(ekey, u64p), ptr(ecount, u64p), ptr(ne, u32p), ptr(hits, u64p))
+            total = int(ne.sum(dtype=np.uint64))
+            if rc == -1 and (int(nb.max()) > stride or total > entry_capacity):  # TQ_ERR_INVALID_ARGUMENT with the lengths: larger sizes
+                stride, entry_capacity = max(stride, int(nb.max())), max(entry_capacity, total)
+                continue
+            _check(rc, self.h)
+            self._hist_terms_sizes = (max(self._hist_terms_sizes[0], int(nb[:qb.nq].max(initial=0))), max(self._hist_terms_sizes[1], total))
+            out = (pos[:qb.nq], docs[:qb.nq], other[:qb.nq], error[:qb.nq], first[:qb.nq], nent[:qb.nq], nb[:qb.nq], eseg[:total],
+                   ekey[:total], ecount[:total], ne[:qb.nq])
+            return out + (hits[:qb.nq],) if count_hits else out
+
     def search_batch(self, batch: QueryBatch, out=None):
         stride, scores, segs, docs, counts = out or batch.alloc_out()
         _check(LIB.tq_search_batch(self.h, batch.ptr, batch.nq, stride, ptr(scores, f32p), ptr(segs, u32p), ptr(docs, u32p),
@@ -716,6 +766,9 @@ class Context:
         th = TermsHistStats()
         _check(LIB.tq_get_terms_hist_stats(self.h, C.byref(th)), self.h)
         out.update({name: getattr(th, name) for name, _ in TermsHistStats._fields_})
+        ht = HistTermsStats()
+        _check(LIB.tq_get_hist_terms_stats(self.h, C.byref(ht)), self.h)
+        out.update({name: getattr(ht, name) for name, _ in HistTermsStats._fields_})
         return out
 
     def merge_topk_dev(self, n_lists, nq, stride, k, scores, segs, docs, counts, out_scores, out_segs, out_docs, out_counts):
