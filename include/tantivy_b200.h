@@ -705,7 +705,12 @@ int tq_batch_run(tq_batch*);
  * zero-extended to int64; 0 = no bound yet) to a DEVICE array; the caller takes the element-wise MAX over all shards
  * (e.g. ncclAllReduce) and hands it back with tq_batch_thresholds_import_dev.  Every shard then prunes against the best
  * bound any shard found: a valid lower bound of the global k-th score (SURVEY.md §8e "broadcast the running global
- * threshold").  tq_batch_run == all phases in order. */
+ * threshold").  tq_batch_run == all phases in order.
+ * A run is in progress from its first phase until its last one has been enqueued.  Meanwhile tq_batch_run finishes it (it
+ * starts at the next phase of the run), tq_batch_run_phase with any other phase returns TQ_ERR_INVALID_ARGUMENT and keeps the
+ * run where it was, and every result entry point (tq_batch_fetch, tq_batch_fetch_hits, tq_batch_results_dev,
+ * tq_batch_results_copy_dev, tq_batch_results_pack_dev, tq_batch_results_pack_dev_async) returns TQ_ERR_INVALID_ARGUMENT and
+ * changes nothing: the rows of an earlier run are no longer the batch's answer, and this run's are not there yet. */
 int tq_batch_phases(tq_batch*);
 int tq_batch_run_phase(tq_batch*, int phase);
 int tq_batch_thresholds_export_dev(tq_batch*, int64_t* keys_dev);
@@ -726,13 +731,15 @@ int tq_batch_fetch(tq_batch*, uint32_t out_stride, float* out_scores, uint32_t* 
  * phase); like tq_batch_fetch it resolves an overflowed run first.  Every run counts from zero.  The tile engine counts from the
  * postings the run has already decoded; queries on the per-query kernels are counted by the Count kernels in the same run. */
 int tq_batch_fetch_hits(tq_batch*, uint64_t* out_hits);
-/* Device pointers of the result rows of a finished run: row stride = k_max of the batch. */
+/* Device pointers of the result rows of a finished run (none in progress, see tq_batch_phases): row stride = k_max of the batch. */
 int tq_batch_results_dev(tq_batch*, const float** scores_dev, const uint32_t** segment_ord_dev,
                          const uint32_t** doc_dev, const uint32_t** count_dev, uint32_t* stride);
 /* Copies the result rows of a finished run into caller-owned DEVICE buffers (row stride = k_max of
  * the batch), e.g. torch tensors about to be all-gathered over NCCL. */
 int tq_batch_results_copy_dev(tq_batch*, float* scores_dev, uint32_t* segment_ord_dev, uint32_t* doc_dev,
                               uint32_t* count_dev);
+/* Allowed at any point, also between two phases of a run: it waits for all work of the batch on both of its streams before its
+ * segments, filters, columns and buffers are let go. */
 void tq_batch_destroy(tq_batch*);
 
 /* Cross-GPU merge_fruits (sort_key_top_collector.rs:76-95): merges `n_lists` result sets

@@ -1272,6 +1272,12 @@ void tq_batch_destroy(tq_batch* b) {
   if (!b) return;
   cudaSetDevice(b->ctx->device);
   cudaStreamSynchronize(b->stream);
+  // a run abandoned after phase 0 may still have k_phrase / the Count kernels on the second stream, reading this batch's
+  // descriptors and writing its scratch: the next owner of the pooled buffers must not start before they end
+  if (b->side_pending) {
+    cudaStreamSynchronize(b->side);
+    b->side_pending = false;
+  }
   b->next_phase = 0;
   b->ran = false;
   std::lock_guard<std::mutex> g(b->ctx->mu);
@@ -1472,10 +1478,12 @@ static int finalize_run(tq_batch* b) {
   return rc;
 }
 
-// The start of every result entry point: the batch has run and the outputs are there; then the batch's device, and with
-// `finalize` the run waited for and, if it overflowed, repeated (finalize_run).
+// The start of every result entry point: the batch has run, no later run is in progress and the outputs are there; then the
+// batch's device, and with `finalize` the run waited for and, if it overflowed, repeated (finalize_run).  Between the phases of
+// a second run the rows and flags are still the first run's, and finalize_run would mark the run in progress as repaired.
 static int results_ready(tq_batch* b, bool have_outputs, bool finalize) {
   if (!b || !b->ran) return fail(TQ_ERR_INVALID_ARGUMENT, "batch has not run");
+  if (b->next_phase != 0) return fail(TQ_ERR_INVALID_ARGUMENT, "a run is in progress: finish its phases");
   if (!have_outputs) return fail(TQ_ERR_INVALID_ARGUMENT, "null output");
   TQ_CUDA(cudaSetDevice(b->ctx->device));
   return finalize ? finalize_run(b) : TQ_OK;

@@ -180,6 +180,7 @@ int tq_multi_search_batch(tq_multi* m, const tq_query* queries, size_t nq, uint3
   std::vector<std::vector<uint32_t>> keys(nd, std::vector<uint32_t>(rows));  // [device][query][kmax] best keys so far
   std::vector<long long> bound(std::max<size_t>(nq, 1), 0);                   // exact k-th best of the union, per query
   std::vector<int> rcs(nd, TQ_OK);
+  std::vector<char> aborted(nd, 0);  // the worker stopped only because another device failed
   std::vector<std::string> errs(nd);
   HostBarrier bar(nd);
   bool abort_all = false;
@@ -210,7 +211,7 @@ int tq_multi_search_batch(tq_multi* m, const tq_query* queries, size_t nq, uint3
           bound[q] = (long long)all[k - 1];
         }
       });
-      if (abort_all) { if (rc == TQ_OK) rc = TQ_ERR_CUDA; break; }
+      if (abort_all) { if (rc == TQ_OK) { rc = TQ_ERR_CUDA; aborted[d] = 1; } break; }
       if (rc == TQ_OK && cudaMemcpyAsync(d_bound, bound.data(), nq * 8, cudaMemcpyHostToDevice, stream) != cudaSuccess) rc = fail(TQ_ERR_CUDA, "bound import");
       if (rc == TQ_OK && nq) rc = tq_batch_thresholds_import_dev(b, reinterpret_cast<const int64_t*>(d_bound));
     }
@@ -224,8 +225,11 @@ int tq_multi_search_batch(tq_multi* m, const tq_query* queries, size_t nq, uint3
   std::vector<std::thread> th;
   for (int d = 0; d < nd; ++d) th.emplace_back(worker, d);
   for (auto& t : th) t.join();
+  // the error of a device whose own call failed, not of the devices that stopped for it
   for (int d = 0; d < nd; ++d)
-    if (rcs[d] != TQ_OK) return refuse(m, rcs[d], errs[d]);
+    if (rcs[d] != TQ_OK && !aborted[d]) return refuse(m, rcs[d], errs[d]);
+  for (int d = 0; d < nd; ++d)
+    if (rcs[d] != TQ_OK) return refuse(m, rcs[d], "a device stopped the search without an error of its own");
   // merge_fruits: (score desc, segment_ord asc, doc asc), keep k (top_score_collector.rs:591-600)
   struct Row { float s; uint32_t g, d; };
   std::vector<Row> all;
