@@ -331,7 +331,7 @@ int tq_ctx_create(int device, tq_ctx** out) {
   if (err == cudaSuccess) err = cudaFuncSetAttribute(k_or_strip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)strip_smem_bytes(kMaxCached));
   // k_tile's occupancy is bound by shared memory: ask for the largest carveout so that the SM's full 228 KB is there to share
   for (auto kern : kTileKernels) {
-    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileMaxSmem);
     if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
   }
   if (err != cudaSuccess) { delete c; return fail(TQ_ERR_CUDA, cudaGetErrorString(err)); }
@@ -1089,14 +1089,14 @@ static int lay_out(tq_ctx* c, tq_batch* b, BatchPlan& pl) {
     TP.max_queries = (gs.max_queries + 1u) & ~1u;
     // per-tile work list: about two (query, essential clause) entries per query, more for wide unions; a tile that needs more
     // takes another round of routing + expansion
-    TP.seg_cap = std::min<uint32_t>(4096u, std::max<uint32_t>(256u, std::max<uint32_t>(2u, gs.max_clauses / 4u) * TP.max_queries));
+    TP.seg_cap = std::min<uint32_t>(kTileMaxWorkList, std::max<uint32_t>(256u, std::max<uint32_t>(2u, gs.max_clauses / 4u) * TP.max_queries));
     if (c->tile_seg_cap_hook) TP.seg_cap = c->tile_seg_cap_hook;
     TP.light_max = c->tile_light_max;
-    TP.cl_cap = gs.max_clause_words <= 16384u ? ((gs.max_clause_words + 3u) & ~3u) : 0u;
+    TP.cl_cap = gs.max_clause_words <= kTileMaxStagedClauses ? ((gs.max_clause_words + 3u) & ~3u) : 0u;
     TP.n_win = c->tile_windows ? std::min<uint32_t>(c->tile_windows, kTileWarps) : kTileExactWindows;
     run.smem = tile_smem_bytes(gs.p_cap, gs.max_slots, TP.max_big, TP.max_queries, TP.seg_cap, TP.cl_cap, TP.n_win);
     c->tile_smem_last = run.smem;
-    if (run.smem > 200u * 1024u) return fail(TQ_ERR_UNSUPPORTED, "tile group needs more shared memory than an SM has");
+    if (run.smem > kTileMaxSmem) return fail(TQ_ERR_UNSUPPORTED, "tile group needs more shared memory than an SM has");
     int ctas = 0;
     run.union_only = gs.union_only;
     // (the exact instance the group runs without TQ_TILE_COUNTERS: the counters instances are built for 3 CTAs per SM)

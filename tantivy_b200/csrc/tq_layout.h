@@ -648,6 +648,14 @@ TQ_HD constexpr size_t tile_smem_bytes(uint32_t p_cap, uint32_t max_slots, uint3
                                        uint32_t cl_cap, uint32_t n_win) {
   return tile_smem_layout(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win).end;
 }
+constexpr uint32_t kTileMaxSmem = 200u * 1024u;  // dynamic shared memory of a k_tile CTA (an H100 allows 227 KB)
+constexpr uint32_t kTileMaxWorkList = 4096u;     // TileParams::seg_cap
+// A group's clause words are staged in shared memory when its largest segment has at most this many; above it every segment
+// reads them from global memory.  The bound keeps the largest layout the planner can produce -- any p_cap up to the repeat's
+// kTileMaxPairs -- within kTileMaxSmem, so a group that was admitted is never refused for its shared memory.
+constexpr uint32_t kTileMaxStagedClauses = 12288u;
+static_assert(tile_smem_bytes(kTileMaxPairs, kTileMaxSlots, kTileMaxBig, kTileMaxQueries, kTileMaxWorkList, kTileMaxStagedClauses,
+                              kTileWarps) <= kTileMaxSmem, "the largest k_tile group with staged clause words exceeds its shared memory");
 
 // k_count_tiles
 constexpr uint8_t kTileQueryCount = 8;      // TQuery::flags bit 3: count the query's hits (k_tile does not read it)

@@ -228,6 +228,15 @@ BOOL_BRANCHES = {"empty_must", "msm_gt_n", "msm_eq_n", "optional_with_must", "op
                  "required_disjunction", "exclude_1", "exclude_many", "groups4_sequential", "groups4_intersection"}
 
 
+def tile_smem_bytes(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win):
+    """tile_smem_bytes (csrc/tq_layout.h) restated: TileQ 16 B, TileSeg 4 B, TileTQ 8 B, kTile = 1024, stage-A scratch 264 words.
+    Takes numpy arrays as well as ints."""
+    union = np.maximum(max_queries * 16 + np.maximum(seg_cap * 4, (2 * 64 + 8 * 17) * 4), n_win * 1024 * 4)
+    union = (union + 15) & ~15
+    return (p_cap * 4 + union + max_slots * 12 + max_big * 128 + max_queries * 8 + max_big * 64 + p_cap * 2 + max_queries * 2 +
+            cl_cap * 2 + 64)
+
+
 def hits(result, i=0):
     scores, segs, docs, counts = result
     n = int(counts[i])

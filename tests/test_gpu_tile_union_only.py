@@ -13,7 +13,7 @@ import tantivy_b200 as T  # noqa: E402
 from oracle import tq_oracle as O  # noqa: E402
 from tantivy_b200._abi import TQ_OP_AND, TQ_OP_OR, TQ_OP_TERM, TQ_RECORD_BASIC, TQ_TERM_IGNORE_FREQ, QueryBatch  # noqa: E402
 from tests import score_model as M  # noqa: E402
-from tests.helpers import hits, make_query  # noqa: E402
+from tests.helpers import hits, make_query, tile_smem_bytes  # noqa: E402
 from tests.test_gpu_parity import (DOC_RANGE_CUTS, TILE_OVERFLOW_HOOKS, TILE_PATH_HOOKS, _ctx_with_env, _tile_queries,  # noqa: E402
                                    assert_same)
 from tests.test_gpu_scoring_edges import _segment, _variants, large, small, wide  # noqa: E402,F401  (fixtures)
@@ -510,14 +510,6 @@ def test_rows_do_not_depend_on_the_batch(pool, pool_ctx):
 
 
 # ---- the largest group the planner admits ---------------------------------------------------------------------------------
-def _tile_smem_bytes(p_cap, max_slots, max_big, max_queries, seg_cap, cl_cap, n_win):
-    """tile_smem_bytes (csrc/tq_tile.cuh) restated: TileQ 16 B, TileSeg 4 B, TileTQ 8 B, kTile = 1024, stage-A scratch 264 words."""
-    union = max(max_queries * 16 + max(seg_cap * 4, (2 * 64 + 8 * 17) * 4), n_win * 1024 * 4)
-    union = (union + 15) & ~15
-    return (p_cap * 4 + union + max_slots * 12 + max_big * 128 + max_queries * 8 + max_big * 64 + p_cap * 2 + max_queries * 2 +
-            cl_cap * 2 + 64)
-
-
 def test_largest_union_group_launches():
     """1024 eight-term unions on one segment over 4096 distinct lists (kTileMaxSlots), 64 of them dense (kTileMaxBig), with the
     lists' densities summing to near the tile pair buffer's limit: one group, on the union-only instance, within the shared
@@ -543,7 +535,7 @@ def test_largest_union_group_launches():
     p_cap = (int(min(12288.0, max(1024.0, total * 1024 * 1.25 + 192.0))) + 63) & ~63
     n_big = sum(1 for t in range(n_terms) if ix.term_info[0][t][0] * 1024 >= 6 * max_doc)
     assert n_big >= 64
-    want_smem = _tile_smem_bytes(p_cap, n_terms, 64, 1024, 2048, 8192, 2)
+    want_smem = tile_smem_bytes(p_cap, n_terms, 64, 1024, 2048, 8192, 2)
     oi = O.OracleIndex()
     ix.register(oi, segment_base=base)
     qb = QueryBatch(qs)
